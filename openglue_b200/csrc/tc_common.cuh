@@ -58,6 +58,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > (1u << 24)) asm volatile("trap;");
   }
 }
+// The same bound without the trap, for code after setmaxnreg.inc: a trap anywhere in that code makes ptxas allocate the whole
+// kernel at its launch-bound register count (spills, serialized wgmmas).  A timeout sets `timed_out` and returns, and later
+// waits return at once; the caller hands the flag to a role that may trap.
+__device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, uint32_t& timed_out) {
+  if (timed_out || mbar_try_wait(bar, parity)) return;
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 24)) { timed_out = 1; return; }
+  }
+}
 
 // ----------------------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* m) {
@@ -88,6 +98,16 @@ inline int& pdl_mode() {
   static int v = [] { const char* e = getenv("OG_PDL"); return e ? atoi(e) : 1; }();
   return v;
 }
+
+// ----------------------------------------------------------------------------- warp specialization
+// setmaxnreg moves registers between the warpgroups of a CTA (every warp of the warpgroup executes it; N a multiple of 8 in
+// [24, 256]): a TMA producer warpgroup gives registers back, consumer warpgroups take them for larger fragments.
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// Named barriers among `count` threads of whole warps (id 0 is __syncthreads): arrive does not wait, sync waits until `count`
+// threads have arrived or synced on `id`.
+__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // ----------------------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes with the 128-byte swizzle (what TMA
