@@ -5,12 +5,17 @@
 //   3xFP16 (F16LinearArgs): B_hi / B_lo are fp16 with a power-of-two weight scale sW (w_meta[0]); A is scaled on the fly by
 //                           sA = f16_scale_for(max of the producers' amax slots) and split into fp16 hi / lo; alpha / (sA sW)
 //                           undoes both scales exactly (see tc_common.cuh for the range argument).
-// Per CTA: a 128 x 128 output tile, two consumer warpgroups of 64 rows each.  Per K block (32 tf32 or 64 fp16 elements) TMA
-// stages the raw fp32 A tile and the B_hi / B_lo tiles (128-byte swizzled rows) into a ring of mbarrier-guarded stages; thread 0
-// refills a stage once all eight warps have released it.  Each warp reads its A fragment out of shared memory, splits it into
-// hi / lo registers, and the warpgroup issues wgmma with A from registers and B from shared memory.  The wgmma accumulator holds
-// at most CHUNK K blocks (K = 64 tf32 / 128 fp16) before it is folded into a register accumulator with round-to-nearest adds,
-// so long reductions are not carried by the tensor core's own accumulation alone.
+// Persistent and warp-specialized: min(tiles, SMs) CTAs walk the 128 x 128 output tiles in a static schedule (tile = blockIdx.x +
+// i gridDim.x over (batch item, row tile, column tile), column tile fastest, so the CTAs resident at one time share each A row
+// block through L2).  Warpgroup 0 is the producer: it gives its registers back (setmaxnreg) and one thread stages, per K block
+// (32 tf32 or 64 fp16 elements), the raw fp32 A tile and the B_hi / B_lo tiles (128-byte swizzled rows) by TMA into a ring of
+// mbarrier-guarded stages, running ahead across tile boundaries so the next tile's first stages load during the epilogue.
+// Warpgroups 1 and 2 own 64 rows of a tile each: a warp reads its A fragment out of shared memory and splits it into hi / lo
+// registers, and the warpgroup issues wgmma with A from registers and B from shared memory.  The two consumers take turns to
+// issue (a ping-pong over two named barriers), and each splits the A fragment of block kb + 1 while its wgmmas of block kb run,
+// so the splits, folds and epilogues of one consumer run under the other's MMAs.  The wgmma accumulator holds at most CHUNK K
+// blocks (K = 64 tf32 / 128 fp16) before it is folded into a register accumulator with round-to-nearest adds, so long
+// reductions are not carried by the tensor core's own accumulation alone.
 #pragma once
 #include "tc_common.cuh"
 #include <algorithm>
@@ -60,18 +65,30 @@ struct F16LinearArgs {
 };
 
 namespace tcf {
-constexpr int BM = 128, BN = 128, THREADS = 256;
+constexpr int BM = 128, BN = 128, THREADS = 384;         // TMA producer warpgroup + two consumer warpgroups
 template <bool F16> struct Cfg {
   static constexpr int KB = F16 ? 64 : 32;                // K elements per block: one 128-byte row of B
   static constexpr int A_BOXES = F16 ? 2 : 1;             // [128 rows x 32 fp32] TMA boxes of A per block
   static constexpr int A_BYTES = A_BOXES * BM * 128;
   static constexpr int B_TILE = BN * 128;                 // B_hi (or B_lo) part of a stage
   static constexpr int STAGE = A_BYTES + 2 * B_TILE;
-  static constexpr int STAGES = F16 ? 3 : 4;              // 192 KB of the 227 KB a block may use
+  static constexpr int STAGES = F16 ? 3 : 4;              // 192 KB
   static constexpr int CHUNK = 2;                         // K blocks per wgmma accumulator chunk
   static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE + 128;
+  // The attention kernel and the GEMMs share the 196 KB shared-memory configuration (193 KB + the 1 KB an SM reserves per
+  // block): a kernel that needs the 228 KB configuration moves the SMs there, and the kernels around it run slower.
+  static_assert(SMEM_BYTES + 1024 <= 196 * 1024, "shared-memory configuration of the attention and GEMM kernels");
 };
+// output tile `tile` of the static schedule: column tile fastest, then row tile, then batch item
+__host__ __device__ __forceinline__ void tile_origin(int tile, int tiles_n, int tiles_m, int& n0, int& m0, int& bz) {
+  const int rt = tile / tiles_n;
+  n0 = (tile - rt * tiles_n) * BN;
+  bz = rt / tiles_m;
+  m0 = (rt - bz * tiles_m) * BM;
+}
 }  // namespace tcf
+
+__host__ __device__ inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // fp32 element (r, c) of a [rows x 32] fp32 tile written by TMA with the 128-byte swizzle
 __device__ __forceinline__ const float* sw128_f32(const uint8_t* tile, int r, int c) {
@@ -81,6 +98,28 @@ __device__ __forceinline__ const float* sw128_f32(const uint8_t* tile, int r, in
 __device__ __forceinline__ void store_half_pair(__half* p, uint32_t v, bool both) {
   if (both) *reinterpret_cast<uint32_t*>(p) = v;
   else *p = __ushort_as_half((unsigned short)(v & 0xffffu));
+}
+// the first n (< 8) 16-bit elements of v, element 0 at p
+__device__ __forceinline__ void store_b16_run(__half* p, uint4 v, int n) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (i < n) p[i] = __ushort_as_half((unsigned short)(i & 1 ? w[i >> 1] >> 16 : w[i >> 1] & 0xffffu));
+}
+
+// Lane t of a quad holds w[j] = 16-bit elements (8j + 2t, 8j + 2t + 1) of one row (element 0 in the low half), j = 0..15.  Returns
+// the elements 8 (4q + t) .. 8 (4q + t) + 7 of that row: two rounds of exchanges within the quad (whole quads must take part).
+__device__ __forceinline__ uint4 quad_gather_b16(const uint32_t (&w)[16], int q, int t) {
+  const uint32_t x0 = w[4 * q], x1 = w[4 * q + 1], x2 = w[4 * q + 2], x3 = w[4 * q + 3];
+  const bool odd = t & 1, upper = t & 2;
+  // lanes t, t ^ 1: the even lane collects blocks 4q / 4q + 2, the odd lane blocks 4q + 1 / 4q + 3, four elements each
+  const uint32_t r0 = __shfl_xor_sync(0xffffffffu, odd ? x0 : x1, 1), r1 = __shfl_xor_sync(0xffffffffu, odd ? x2 : x3, 1);
+  const uint2 p0 = odd ? make_uint2(r0, x1) : make_uint2(x0, r0);  // block 4q + (t & 1), elements 4 (t >> 1) .. + 3
+  const uint2 p1 = odd ? make_uint2(r1, x3) : make_uint2(x2, r1);  // block 4q + 2 + (t & 1)
+  // lanes t, t ^ 2: the lower pair completes block 4q + t from p0, the upper pair from p1
+  const uint2 sd = upper ? p0 : p1;
+  const uint32_t s0 = __shfl_xor_sync(0xffffffffu, sd.x, 2), s1 = __shfl_xor_sync(0xffffffffu, sd.y, 2);
+  return upper ? make_uint4(s0, s1, p1.x, p1.y) : make_uint4(p0.x, p0.y, s0, s1);
 }
 
 template <class Args>
@@ -93,20 +132,21 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
   constexpr bool F16 = std::is_same<Args, F16LinearArgs>::value;
   using C = Cfg<F16>;
   constexpr int S = C::STAGES;
+  constexpr int TURN = 1;                                    // named barriers TURN + consumer
   launch_dependents();
   extern __shared__ uint8_t og_lin_smem_raw[];
   uint8_t* smem = align_smem_1024(og_lin_smem_raw);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * C::STAGE);
   uint64_t* empty = full + S;
+  volatile uint32_t* timeout_flag = reinterpret_cast<uint32_t*>(empty + S);   // a consumer's wait on `full` timed out
 
-  const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM, bz = blockIdx.z;
   const int K = a.k1 + a.k2, nkb = cdiv(K, C::KB);
-  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int abz = a.strideA ? bz : 0, a2bz = a.strideA2 ? bz : 0;
-  const int brow = n0 + bz * a.b_rows_per_batch;
+  const int tiles_n = cdiv(a.nout, BN), tiles_m = cdiv(a.rows, BM), ntiles = tiles_n * tiles_m * a.batch;
+  const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
+    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
+    *timeout_flag = 0;
     fence_barrier_init();
     prefetch_tensormap(&map_a); prefetch_tensormap(&map_a2);
     prefetch_tensormap(&map_bhi); prefetch_tensormap(&map_blo);
@@ -114,21 +154,41 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
   __syncthreads();
   grid_dependency_wait();                                    // A, the amax slots and the residual come from previous kernels
 
-  auto issue = [&](int kb) {                                 // thread 0 only
-    const int s = kb % S;
-    uint8_t* st = smem + s * C::STAGE;
-    mbar_arrive_expect_tx(&full[s], C::STAGE);               // out-of-bounds box parts arrive as zeros and count in full
+  if (wg == 0) {                                             // ---- producer
+    setmaxnreg_dec<24>();
+    if (threadIdx.x == 0) {
+      uint32_t it = 0;                                       // K blocks staged so far (over all tiles of this CTA)
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        int n0, m0, bz;
+        tile_origin(tile, tiles_n, tiles_m, n0, m0, bz);
+        const int abz = a.strideA ? bz : 0, a2bz = a.strideA2 ? bz : 0;
+        const int brow = n0 + bz * a.b_rows_per_batch;
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % S;
+          if (it >= S) mbar_wait(&empty[s], (it / S - 1) & 1);
+          uint8_t* st = smem + s * C::STAGE;
+          mbar_arrive_expect_tx(&full[s], C::STAGE);         // out-of-bounds box parts arrive as zeros and count in full
 #pragma unroll
-    for (int j = 0; j < C::A_BOXES; ++j) {
-      const int k = kb * C::KB + 32 * j;
-      if (k < a.k1 || !a.A2) tma_load_3d(st + j * BM * 128, &map_a, &full[s], k, m0, abz);
-      else                   tma_load_3d(st + j * BM * 128, &map_a2, &full[s], k - a.k1, m0, a2bz);
+          for (int j = 0; j < C::A_BOXES; ++j) {
+            const int k = kb * C::KB + 32 * j;
+            if (k < a.k1 || !a.A2) tma_load_3d(st + j * BM * 128, &map_a, &full[s], k, m0, abz);
+            else                   tma_load_3d(st + j * BM * 128, &map_a2, &full[s], k - a.k1, m0, a2bz);
+          }
+          tma_load_2d(st + C::A_BYTES, &map_bhi, &full[s], kb * C::KB, brow);
+          tma_load_2d(st + C::A_BYTES + C::B_TILE, &map_blo, &full[s], kb * C::KB, brow);
+        }
+      }
+      mbar_wait(&empty[(it - 1) % S], ((it - 1) / S) & 1);   // both consumers are done with the last stage
+      if (*timeout_flag) asm volatile("trap;");
     }
-    tma_load_2d(st + C::A_BYTES, &map_bhi, &full[s], kb * C::KB, brow);
-    tma_load_2d(st + C::A_BYTES + C::B_TILE, &map_blo, &full[s], kb * C::KB, brow);
-  };
-  if (threadIdx.x == 0)
-    for (int kb = 0; kb < S && kb < nkb; ++kb) issue(kb);
+    return;
+  }
+  // ---- consumers.  Their waits on `full` are bounded without a trap (mbar_wait_flag): a trap anywhere after setmaxnreg.inc
+  // makes ptxas allocate the whole kernel at its launch-bound register count, with spills and serialized wgmmas.  A timeout is
+  // handed to the producer thread, which traps after the last release.
+  setmaxnreg_inc<240>();
+  const int c = wg - 1, tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int r0 = c * 64 + warp * 16 + g;                     // tile rows of this thread: r0, r0 + 8
 
   // operand scales of the fp16 form (every thread derives the same values from the same device scalars)
   float s_a = 1.f, amax_a = 0.f;
@@ -136,31 +196,37 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
 #pragma unroll
     for (int i = 0; i < 3; ++i) if (a.amax_in[i]) amax_a = fmaxf(amax_a, __ldcg(a.amax_in[i]));
     s_a = f16_scale_for(amax_a);
+    if (blockIdx.x == 0 && threadIdx.x == 128) {             // one thread of the grid publishes the output scales
+      if (a.nkinds > 1) {
+        for (int kk = 0; kk < a.nkinds; ++kk) {
+          const float* w2 = a.w_meta + 4 * kk;
+          const float so = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(w2 + 1), __ldg(w2 + 2)));
+          if (a.kind0 + kk == 1 && a.scale_out) *a.scale_out = so;
+          if (a.kind0 + kk == 2 && a.scale_out_v) *a.scale_out_v = so;
+        }
+      } else if (!a.Y && a.scale_out) {
+        *a.scale_out = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(a.w_meta + 1), __ldg(a.w_meta + 2)));
+      }
+    }
   }
 
   float racc[64], acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) { racc[i] = 0.f; acc[i] = 0.f; }
-  const int r0 = wg * 64 + warp * 16 + g;                    // tile rows of this thread: r0, r0 + 8
+  uint32_t ahi0[4][4], alo0[4][4], ahi1[4][4], alo1[4][4];  // A fragments of two K blocks: split one while the other's wgmmas run
+  uint32_t it = 0, timed_out = 0;
 
-#pragma unroll 1
-  for (int kb = 0; kb < nkb; ++kb) {
-    if (threadIdx.x == 0 && kb >= 1 && kb - 1 + S < nkb) {
-      mbar_wait(&empty[(kb - 1) % S], ((kb - 1) / S) & 1);
-      issue(kb - 1 + S);
-    }
-    const int s = kb % S;
-    mbar_wait(&full[s], (kb / S) & 1);
+  // waits for stage `it_` and splits this warp's A fragment of it
+  auto split_a = [&](uint32_t it_, uint32_t (&ahi)[4][4], uint32_t (&alo)[4][4]) {
+    const int s = it_ % S;
+    mbar_wait_flag(&full[s], (it_ / S) & 1, timed_out);
     const uint8_t* st = smem + s * C::STAGE;
-    uint32_t ahi[4][4], alo[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       if constexpr (F16) {
         const uint8_t* box = st + (kk >> 1) * BM * 128;
-        const int c = (kk & 1) * 16 + 2 * t;
+        const int col = (kk & 1) * 16 + 2 * t;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {                        // q: (row r0 | r0 + 8) x (column c | c + 8)
-          const float2 v = *reinterpret_cast<const float2*>(sw128_f32(box, r0 + (q & 1) * 8, c + (q >> 1) * 8));
+        for (int q = 0; q < 4; ++q) {                        // q: (row r0 | r0 + 8) x (column col | col + 8)
+          const float2 v = *reinterpret_cast<const float2*>(sw128_f32(box, r0 + (q & 1) * 8, col + (q >> 1) * 8));
           split_f16x2(v.x * s_a, v.y * s_a, ahi[kk][q], alo[kk][q]);
           if (a.swap_halves) { ahi[kk][q] = __byte_perm(ahi[kk][q], 0, 0x1032); alo[kk][q] = __byte_perm(alo[kk][q], 0, 0x1032); }
         }
@@ -169,125 +235,228 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
         for (int q = 0; q < 4; ++q) split_tf32(*sw128_f32(st, r0 + (q & 1) * 8, 8 * kk + t + (q >> 1) * 4), ahi[kk][q], alo[kk][q]);
       }
     }
-    const uint32_t bhi = smem_u32(st + C::A_BYTES), blo = bhi + C::B_TILE;
-    fence_operands(acc);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const uint64_t dhi = make_wgdesc_sw128(bhi + kk * 32), dlo = make_wgdesc_sw128(blo + kk * 32);
-      const int acc0 = (kb % C::CHUNK != 0 || kk) ? 1 : 0;
-      if constexpr (F16) {
-        wgmma_f16_m64n128(acc, alo[kk], dhi, acc0);
-        wgmma_f16_m64n128(acc, ahi[kk], dlo, 1);
-        wgmma_f16_m64n128(acc, ahi[kk], dhi, 1);
-      } else {
-        wgmma_tf32_m64n128(acc, alo[kk], dhi, acc0);
-        wgmma_tf32_m64n128(acc, ahi[kk], dlo, 1);
-        wgmma_tf32_m64n128(acc, ahi[kk], dhi, 1);
-      }
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_operands(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);                   // this warp is done with the stage (A reads and its wgmmas)
-    if (kb % C::CHUNK == C::CHUNK - 1 || kb == nkb - 1) {
-#pragma unroll
-      for (int i = 0; i < 64; ++i) racc[i] += acc[i];
-    }
-  }
+  };
 
-  // ---- epilogue: thread holds rows r0 / r0 + 8, columns n0 + 8j + 2t (+1), j = 0..15
-  if constexpr (F16) {
-    const float s_w = __ldg(a.w_meta);
-    int okind = a.Y ? 1 : (a.Yh ? 2 : 3), kidx = 0, ocols = a.nout;
-    float alpha_t = a.alpha / (s_a * s_w), sos = 1.f;
-    const float* wm = a.w_meta;
-    if (a.nkinds > 1) {
-      kidx = n0 / a.kind_cols; okind = a.kind0 + kidx + 1; ocols = a.kind_cols;
-      wm = a.w_meta + 4 * kidx;
-      alpha_t = a.alpha / (s_a * __ldg(wm));
-    }
-    if (okind != 1) sos = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(wm + 1), __ldg(wm + 2)));
-    if (blockIdx.x == 0 && blockIdx.y == 0 && bz == 0 && threadIdx.x == 0) {
-      if (a.nkinds > 1) {
-        for (int kk = 0; kk < a.nkinds; ++kk) {
-          const float* w2 = a.w_meta + 4 * kk;
-          const float so = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(w2 + 1), __ldg(w2 + 2)));
-          if (a.kind0 + kk == 1 && a.scale_out) *a.scale_out = so;
-          if (a.kind0 + kk == 2 && a.scale_out_v) *a.scale_out_v = so;
-        }
-      } else if (okind != 1 && a.scale_out) {
-        *a.scale_out = sos;
-      }
-    }
-    float tmax = 0.f;
+  // consumer 0 takes the first turn; consumer 1 skips its last hand-over, so both barriers end balanced
+  if (c == 1) named_bar_arrive(TURN + 0, 256);
+#pragma unroll 1
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int n0, m0, bz;
+    tile_origin(tile, tiles_n, tiles_m, n0, m0, bz);
+    const bool last_tile = tile + (int)gridDim.x >= ntiles;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int grow = m0 + r0 + 8 * h;
-      if (grow >= a.rows) continue;
+    for (int i = 0; i < 64; ++i) racc[i] = 0.f;
+
+    // one K block in this consumer's turn: its wgmmas from (ahi, alo), then the split of the next block into (nhi, nlo)
+    auto mma_block = [&](int kb, const uint32_t (&ahi)[4][4], const uint32_t (&alo)[4][4], uint32_t (&nhi)[4][4],
+                         uint32_t (&nlo)[4][4]) {
+      const int s = it % S;
+      const bool last = last_tile && kb == nkb - 1;
+      if (last && timed_out) *timeout_flag = 1;              // published before the turn barrier, which orders it before the last release
+      const uint32_t bhi = smem_u32(smem + s * C::STAGE + C::A_BYTES), blo = bhi + C::B_TILE;
+      named_bar_sync(TURN + c, 256);
+      fence_operands(acc);
+      wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = n0 + 8 * j + 2 * t, oc = col - kidx * ocols;
-        if (col >= a.nout) continue;
-        const bool two = col + 1 < a.nout;
-        float y0 = fmaf(racc[4 * j + 2 * h], alpha_t, a.bias ? __ldg(a.bias + col) : 0.f);
-        float y1 = two ? fmaf(racc[4 * j + 2 * h + 1], alpha_t, a.bias ? __ldg(a.bias + col + 1) : 0.f) : 0.f;
-        if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
-        if (okind == 1) {
-          const int64_t o = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy + oc;
-          if (a.R) {
-            const float* rr = a.R + (int64_t)bz * a.strideR + (int64_t)grow * a.ldr + oc;
-            y0 += rr[0];
-            if (two) y1 += rr[1];
-          }
-          if (two) *reinterpret_cast<float2*>(a.Y + o) = make_float2(y0, y1);
-          else a.Y[o] = y0;
-          tmax = fmaxf(tmax, fmaxf(fabsf(y0), fabsf(y1)));
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t dhi = make_wgdesc_sw128(bhi + kk * 32), dlo = make_wgdesc_sw128(blo + kk * 32);
+        const int acc0 = (kb % C::CHUNK != 0 || kk) ? 1 : 0;
+        if constexpr (F16) {
+          wgmma_f16_m64n128(acc, alo[kk], dhi, acc0);
+          wgmma_f16_m64n128(acc, ahi[kk], dlo, 1);
+          wgmma_f16_m64n128(acc, ahi[kk], dhi, 1);
         } else {
-          uint32_t hv, lv;
-          split_f16x2(y0 * sos, y1 * sos, hv, lv);
-          if (okind == 2) {
-            const int64_t o = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy + oc;
-            store_half_pair(a.Yh + o, hv, two);
-            store_half_pair(a.Yl + o, lv, two);
-          } else {
-            const int64_t o = (int64_t)bz * a.strideYt + grow + (int64_t)oc * a.ldyt;
-            a.Yth[o] = __ushort_as_half((unsigned short)(hv & 0xffffu)); a.Ytl[o] = __ushort_as_half((unsigned short)(lv & 0xffffu));
-            if (two) { a.Yth[o + a.ldyt] = __ushort_as_half((unsigned short)(hv >> 16)); a.Ytl[o + a.ldyt] = __ushort_as_half((unsigned short)(lv >> 16)); }
+          wgmma_tf32_m64n128(acc, alo[kk], dhi, acc0);
+          wgmma_tf32_m64n128(acc, ahi[kk], dlo, 1);
+          wgmma_tf32_m64n128(acc, ahi[kk], dhi, 1);
+        }
+      }
+      wgmma_commit();
+      if (!(last && c == 1)) named_bar_arrive(TURN + (c ^ 1), 256);
+      if (kb + 1 < nkb) split_a(it + 1, nhi, nlo);
+      wgmma_wait<0>();
+      fence_operands(acc);
+      if (tid == 0) mbar_arrive(&empty[s]);                  // this warpgroup's reads of the stage are done
+      if (kb % C::CHUNK == C::CHUNK - 1 || kb == nkb - 1) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) racc[i] += acc[i];
+      }
+      ++it;
+    };
+    split_a(it, ahi0, alo0);
+#pragma unroll 1
+    for (int kb = 0; kb < nkb; kb += 2) {
+      mma_block(kb, ahi0, alo0, ahi1, alo1);
+      if (kb + 1 < nkb) mma_block(kb + 1, ahi1, alo1, ahi0, alo0);
+    }
+
+    // ---- epilogue: thread holds rows r0 / r0 + 8, columns n0 + 8j + 2t (+1), j = 0..15
+    if constexpr (F16) {
+      const float s_w = __ldg(a.w_meta);
+      int okind = a.Y ? 1 : (a.Yh ? 2 : 3), kidx = 0, ocols = a.nout;
+      float alpha_t = a.alpha / (s_a * s_w), sos = 1.f;
+      const float* wm = a.w_meta;
+      if (a.nkinds > 1) {
+        kidx = n0 / a.kind_cols; okind = a.kind0 + kidx + 1; ocols = a.kind_cols;
+        wm = a.w_meta + 4 * kidx;
+        alpha_t = a.alpha / (s_a * __ldg(wm));
+      }
+      if (okind != 1) sos = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(wm + 1), __ldg(wm + 2)));
+      float tmax = 0.f;
+      if (okind == 1) {
+        // Every load of the epilogue is issued before its first store: the compiler may not move a load across a store to a
+        // pointer that could alias it, and loads interleaved with the stores expose one memory latency per 8-column block.
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int grow = m0 + r0 + 8 * h;
+          if (grow >= a.rows) continue;
+          const float* rrow = a.R ? a.R + (int64_t)bz * a.strideR + (int64_t)grow * a.ldr : nullptr;
+#pragma unroll
+          for (int jh = 0; jh < 16; jh += 8) {
+            // bias and residual of columns n0 + 8 (jh + i / 2) + 2t + (i % 2), loaded before the stores (R may be Y: each
+            // element is read and written by this thread only)
+            float bv[16], rv[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              const int col = n0 + 8 * (jh + (i >> 1)) + 2 * t + (i & 1);
+              const bool in = col < a.nout;
+              bv[i] = a.bias && in ? __ldg(a.bias + col) : 0.f;
+              rv[i] = rrow && in ? rrow[col] : 0.f;
+            }
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = jh + jj;
+              const int col = n0 + 8 * j + 2 * t;
+              if (col >= a.nout) continue;
+              const bool two = col + 1 < a.nout;
+              float y0 = fmaf(racc[4 * j + 2 * h], alpha_t, bv[2 * jj]);
+              float y1 = two ? fmaf(racc[4 * j + 2 * h + 1], alpha_t, bv[2 * jj + 1]) : 0.f;
+              if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+              const int64_t o = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy + col;
+              if (a.R) {
+                y0 += rv[2 * jj];
+                if (two) y1 += rv[2 * jj + 1];
+              }
+              if (two) *reinterpret_cast<float2*>(a.Y + o) = make_float2(y0, y1);
+              else a.Y[o] = y0;
+              tmax = fmaxf(tmax, fmaxf(fabsf(y0), fabsf(y1)));
+            }
+          }
+        }
+      } else {
+        // fp16 hi / lo operands: every element is computed first (also rows / columns past the tensor, which are not stored), so
+        // that whole warps take part in the shuffles that regroup them into 16-byte runs
+        uint32_t hv[2][16], lv[2][16];                       // [row r0 | r0 + 8][j]: columns n0 + 8j + 2t, +1 (element 0 low)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = n0 + 8 * j + 2 * t;
+          const bool two = col + 1 < a.nout;
+          const float b0 = a.bias && col < a.nout ? __ldg(a.bias + col) : 0.f;
+          const float b1 = a.bias && two ? __ldg(a.bias + col + 1) : 0.f;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float y0 = fmaf(racc[4 * j + 2 * h], alpha_t, b0);
+            float y1 = two ? fmaf(racc[4 * j + 2 * h + 1], alpha_t, b1) : 0.f;
+            if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+            split_f16x2(y0 * sos, y1 * sos, hv[h][j], lv[h][j]);
+          }
+        }
+        if (okind == 2) {
+          const bool wide = a.ldy % 8 == 0 && a.strideY % 8 == 0 && al16(a.Yh) && al16(a.Yl);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int grow = m0 + r0 + 8 * h;
+            const int64_t orow = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy - kidx * ocols;
+            if (wide) {
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {                  // this thread stores columns n0 + 8 (4q + t) .. + 7
+                const uint4 vh = quad_gather_b16(hv[h], q, t), vl = quad_gather_b16(lv[h], q, t);
+                const int col = n0 + 8 * (4 * q + t);
+                if (grow >= a.rows || col >= a.nout) continue;
+                if (col + 8 <= a.nout) {
+                  *reinterpret_cast<uint4*>(a.Yh + orow + col) = vh;
+                  *reinterpret_cast<uint4*>(a.Yl + orow + col) = vl;
+                } else {
+                  store_b16_run(a.Yh + orow + col, vh, a.nout - col);
+                  store_b16_run(a.Yl + orow + col, vl, a.nout - col);
+                }
+              }
+            } else if (grow < a.rows) {
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+                const int col = n0 + 8 * j + 2 * t;
+                if (col >= a.nout) continue;
+                store_half_pair(a.Yh + orow + col, hv[h][j], col + 1 < a.nout);
+                store_half_pair(a.Yl + orow + col, lv[h][j], col + 1 < a.nout);
+              }
+            }
+          }
+        } else {
+          // V^T: the lanes of a warp hold 16 rows of a column, two 16-byte runs.  Gathering such runs in one lane (an 8 x 8 exchange)
+          // made each store touch 32 columns, 32 rows of V^T that lie ldyt apart, and measured 3x slower than these stores.
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int grow = m0 + r0 + 8 * h;
+            if (grow < a.rows) {
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+                const int col = n0 + 8 * j + 2 * t;
+                if (col >= a.nout) continue;
+                const int64_t o = (int64_t)bz * a.strideYt + grow + (int64_t)(col - kidx * ocols) * a.ldyt;
+                a.Yth[o] = __ushort_as_half((unsigned short)(hv[h][j] & 0xffffu)); a.Ytl[o] = __ushort_as_half((unsigned short)(lv[h][j] & 0xffffu));
+                if (col + 1 < a.nout) {
+                  a.Yth[o + a.ldyt] = __ushort_as_half((unsigned short)(hv[h][j] >> 16));
+                  a.Ytl[o + a.ldyt] = __ushort_as_half((unsigned short)(lv[h][j] >> 16));
+                }
+              }
+            }
           }
         }
       }
-    }
-    if (okind == 1 && a.amax_out) {
-      tmax = warp_max(tmax);
-      if (lane == 0 && tmax > 0.f) atomic_amax(a.amax_out, tmax);
-    }
-  } else {
+      if (okind == 1 && a.amax_out) {
+        tmax = warp_max(tmax);
+        if (lane == 0 && tmax > 0.f) atomic_amax(a.amax_out, tmax);
+      }
+    } else {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int grow = m0 + r0 + 8 * h;
-      if (grow >= a.rows) continue;
-      const float* Rrow = a.R ? a.R + (int64_t)bz * a.strideR + (int64_t)grow * a.ldr : nullptr;
-      const int64_t yoff = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy;
-      const int64_t ytoff = (int64_t)bz * a.strideYt + grow;
+      for (int h = 0; h < 2; ++h) {
+        const int grow = m0 + r0 + 8 * h;
+        if (grow >= a.rows) continue;
+        const float* rrow = a.R ? a.R + (int64_t)bz * a.strideR + (int64_t)grow * a.ldr : nullptr;
+        const int64_t yoff = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy;
+        const int64_t ytoff = (int64_t)bz * a.strideYt + grow;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+        for (int jh = 0; jh < 16; jh += 8) {
+          // loads first, as in the fp16 form: bias, rscale and residual of columns n0 + 8 (jh + i / 2) + 2t + (i % 2)
+          float bv[16], sv[16], rv[16];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int c = n0 + 8 * j + 2 * t + e;
-          if (c >= a.nout) continue;
-          float v = racc[4 * j + 2 * h + e] * a.alpha;
-          if (a.bias) v += __ldg(a.bias + c);
-          if (a.relu) v = fmaxf(v, 0.f);
-          if (Rrow) { const float rv = Rrow[c]; v = a.rscale ? fmaf(__ldg(a.rscale + c), rv, v) : (v + rv); }
-          uint32_t vh = 0, vl = 0;
-          if (a.Yhi || a.Ythi) split_tf32(v, vh, vl);
-          if (a.Y) a.Y[yoff + c] = v;
-          if (a.Yhi) { a.Yhi[yoff + c] = __uint_as_float(vh); a.Ylo[yoff + c] = __uint_as_float(vl); }
-          const int64_t o = ytoff + (int64_t)c * a.ldyt;
-          if (a.Yt) a.Yt[o] = v;
-          if (a.Ythi) { a.Ythi[o] = __uint_as_float(vh); a.Ytlo[o] = __uint_as_float(vl); }
+          for (int i = 0; i < 16; ++i) {
+            const int col = n0 + 8 * (jh + (i >> 1)) + 2 * t + (i & 1);
+            const bool in = col < a.nout;
+            bv[i] = a.bias && in ? __ldg(a.bias + col) : 0.f;
+            sv[i] = rrow && a.rscale && in ? __ldg(a.rscale + col) : 0.f;
+            rv[i] = rrow && in ? rrow[col] : 0.f;
+          }
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = jh + jj;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = n0 + 8 * j + 2 * t + e;
+              if (col >= a.nout) continue;
+              float v = racc[4 * j + 2 * h + e] * a.alpha;
+              if (a.bias) v += bv[2 * jj + e];
+              if (a.relu) v = fmaxf(v, 0.f);
+              if (rrow) { const float r = rv[2 * jj + e]; v = a.rscale ? fmaf(sv[2 * jj + e], r, v) : (v + r); }
+              uint32_t vh = 0, vl = 0;
+              if (a.Yhi || a.Ythi) split_tf32(v, vh, vl);
+              if (a.Y) a.Y[yoff + col] = v;
+              if (a.Yhi) { a.Yhi[yoff + col] = __uint_as_float(vh); a.Ylo[yoff + col] = __uint_as_float(vl); }
+              const int64_t o = ytoff + (int64_t)col * a.ldyt;
+              if (a.Yt) a.Yt[o] = v;
+              if (a.Ythi) { a.Ythi[o] = __uint_as_float(vh); a.Ytlo[o] = __uint_as_float(vl); }
+            }
+          }
         }
       }
     }
@@ -316,7 +485,9 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
   if (attr_set.once())
     OG_CUDA(cudaFuncSetAttribute(linear_sm90_kernel<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(cdiv(a.nout, BN), cdiv(a.rows, BM), a.batch);
+  const int tiles = cdiv(a.nout, BN) * cdiv(a.rows, BM) * a.batch;
+  const int sms = device_info().ok ? device_info().sm_count : 132;
+  cfg.gridDim = dim3(std::min(tiles, sms));                 // persistent: each CTA walks tiles blockIdx.x + i gridDim.x
   cfg.blockDim = dim3(THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = stream;
@@ -328,8 +499,6 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
   launch_counter()++;
   return OG_OK;
 }
-
-inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // Bhi/Blo: [b_total_rows, K] row-major fp32 (tf32-exact values), row stride ldb.  A concatenated second operand needs k1 % 32 == 0
 // (a K block comes from one of the two tensors).
