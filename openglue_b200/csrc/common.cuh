@@ -50,11 +50,16 @@ inline const DeviceInfo& device_info() {
   }
   return d;
 }
-// One flag per device for "cudaFuncSetAttribute done": declare `static DeviceFlags f;` next to the launch and test f.once().
+// One flag per device for "cudaFuncSetAttribute done": declare `static DeviceFlags f;` next to the launch and test f.once(),
+// or test f.pending() and call f.mark() once the attribute call succeeded (a failed call is then retried on the next launch).
 struct DeviceFlags {
   bool set[OG_MAX_DEVICES] = {};
   bool once() { const int dev = current_device(); if (set[dev]) return false; set[dev] = true; return true; }
+  bool pending() const { return !set[current_device()]; }
+  void mark() { set[current_device()] = true; }
 };
+// Dynamic shared memory one block may opt in to on sm_90 (cudaDevAttrMaxSharedMemoryPerBlockOptin: 227 KB of the SM's 228 KB)
+constexpr size_t OG_SMEM_OPTIN_MAX = 227 * 1024;
 
 __host__ __device__ inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }

@@ -400,7 +400,7 @@ constexpr int SINK_L2_RESIDENT_MB = 0;   // of the 50 MB L2
 constexpr int SINK_L2_PREFETCH_ROWS = 0;
 
 template <int V, int W, int SLOTS>
-inline size_t sinkhorn_smem(int mpad) {
+constexpr size_t sinkhorn_smem(int mpad) {
   constexpr int C = 128 * V, G = SINK_WARPS / W;
   return ((size_t)(W * C + 4) + (size_t)G * mpad + (size_t)SINK_WARPS * SLOTS * C) * sizeof(float) +
          (size_t)SINK_WARPS * SLOTS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float2) + 128;
@@ -455,10 +455,12 @@ inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
 
 template <int V, int W, int SLOTS>
 inline int sinkhorn_launch_v(SinkArgs a, const SinkPlan& p, cudaStream_t stream) {
+  constexpr size_t smem_max = sinkhorn_smem<V, W, SLOTS>(128 * V * W + 4);     // largest request of this instantiation: m = 128 V W
+  static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "sinkhorn_kernel: shared memory beyond what one block may opt in to");
   static DeviceFlags attr_set;
-  if (attr_set.once()) {                 // largest request of this instantiation: m = 128 V W
-    OG_CUDA(cudaFuncSetAttribute(sinkhorn_kernel<V, W, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)sinkhorn_smem<V, W, SLOTS>(128 * V * W + 4)));
+  if (attr_set.pending()) {
+    OG_CUDA(cudaFuncSetAttribute(sinkhorn_kernel<V, W, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    attr_set.mark();
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.B * a.SP);

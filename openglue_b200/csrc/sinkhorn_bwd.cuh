@@ -368,9 +368,33 @@ __global__ void __launch_bounds__(256) sinkb_dustbin_kernel(const float* __restr
 // history the forward pass records for the backward pass: u [B][T][n+1] then v [B][T+1][m+1]
 inline int64_t sinkhorn_hist_floats(int B, int n, int m, int T) { return (int64_t)B * T * (n + 1) + (int64_t)B * (T + 1) * (m + 1); }
 
+template <int V, int W, int SLOTS>
+constexpr size_t sinkhorn_bwd_smem(int mpad) {
+  constexpr int C = 128 * V, G = SINK_WARPS / W;
+  return ((size_t)3 * (W * C + 4) + (size_t)G * mpad + (size_t)SINK_WARPS * SLOTS * C) * sizeof(float) +
+         (size_t)SINK_WARPS * SLOTS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float) + 128;
+}
+
+// The backward sweep keeps three column vectors in shared memory where the forward keeps one, so it has its own instantiation per
+// column band: the same V and W as the forward, but ONE ring slot per warp for 2048 < m <= 4096 (two slots would need 246 KB, more
+// than a block may opt in to).  Two CTAs per SM only while two blocks (each with the 1 KB the runtime reserves) fit in 227 KB.
+// The instantiation, the occupancy (and with it the strip decomposition) and the workspace size all come from this plan.
+inline int sinkhorn_bwd_plan(int B, int n, int m, SinkPlan* p) {
+  p->mpad = (int)align_up(m + 1, 4);
+  if (m <= 512)       { p->V = 4;  p->W = 1; p->slots = 2; p->smem = sinkhorn_bwd_smem<4, 1, 2>(p->mpad); }
+  else if (m <= 1024) { p->V = 4;  p->W = 2; p->slots = 2; p->smem = sinkhorn_bwd_smem<4, 2, 2>(p->mpad); }
+  else if (m <= 2048) { p->V = 8;  p->W = 2; p->slots = 2; p->smem = sinkhorn_bwd_smem<8, 2, 2>(p->mpad); }
+  else if (m <= 4096) { p->V = 16; p->W = 2; p->slots = 1; p->smem = sinkhorn_bwd_smem<16, 2, 1>(p->mpad); }
+  else if (m <= SINK_MAX_COLS) { p->V = 16; p->W = 4; p->slots = 1; p->smem = sinkhorn_bwd_smem<16, 4, 1>(p->mpad); }
+  else return fail(OG_EUNSUPPORTED, "sinkhorn_bwd: m = %d > %d columns not supported (swap the images)", m, SINK_MAX_COLS);
+  p->occ = (p->V <= 8 && 2 * (p->smem + 1024) <= OG_SMEM_OPTIN_MAX) ? 2 : 1;     // (__launch_bounds__: 2 CTAs only for V <= 8)
+  sinkhorn_decompose(p, B, n);
+  return OG_OK;
+}
+
 inline int64_t sinkhorn_bwd_workspace_bytes(int B, int n, int m, int T) {
   SinkPlan p;
-  if (sinkhorn_plan(B, n, m, &p) != OG_OK) return -1;
+  if (sinkhorn_bwd_plan(B, n, m, &p) != OG_OK) return -1;
   const int64_t sp_max = std::max(p.SP, 32), nrs = cdiv(n + 1, SINKB_RS_ROWS);
   int64_t f = 0;
   f += align_up((int64_t)B * (n + 1), 64) + align_up((int64_t)B * (m + 1), 64);                 // ubar_init, vbar_init
@@ -382,18 +406,17 @@ inline int64_t sinkhorn_bwd_workspace_bytes(int B, int n, int m, int T) {
 
 template <int V, int W, int SLOTS>
 inline int sinkhorn_bwd_launch_v(SinkBwdArgs a, const SinkPlan& p, cudaStream_t stream) {
-  constexpr int C = 128 * V, G = SINK_WARPS / W;
-  auto smem_for = [](int mpad) {
-    return ((size_t)3 * (W * C + 4) + (size_t)G * mpad + (size_t)SINK_WARPS * SLOTS * C) * sizeof(float) +
-           (size_t)SINK_WARPS * SLOTS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float) + 128;
-  };
+  constexpr size_t smem_max = sinkhorn_bwd_smem<V, W, SLOTS>(128 * V * W + 4);     // largest request of this instantiation: m = 128 V W
+  static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "sinkhorn_bwd_kernel: shared memory beyond what one block may opt in to");
   static DeviceFlags attr_set;
-  if (attr_set.once())
-    OG_CUDA(cudaFuncSetAttribute(sinkhorn_bwd_kernel<V, W, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_for(128 * V * W + 4)));
+  if (attr_set.pending()) {
+    OG_CUDA(cudaFuncSetAttribute(sinkhorn_bwd_kernel<V, W, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    attr_set.mark();
+  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.B * a.SP);
   cfg.blockDim = dim3(SINK_WARPS * 32);
-  cfg.dynamicSmemBytes = smem_for(p.mpad);
+  cfg.dynamicSmemBytes = p.smem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeCooperative;
@@ -409,12 +432,8 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
                                const float* hist, const float* G, float* dZ, float* ddustbin, void* ws, int64_t ws_bytes,
                                cudaStream_t stream) {
   SinkPlan p;
-  int rc = sinkhorn_plan(B, n, m, &p);
+  int rc = sinkhorn_bwd_plan(B, n, m, &p);
   if (rc != OG_OK) return rc;
-  {  // three column vectors instead of one in shared memory: two CTAs per SM only while 2 x smem still fits
-    const size_t smem = ((size_t)3 * (p.W * 128 * p.V + 4) + (size_t)(SINK_WARPS / p.W) * p.mpad + (size_t)SINK_WARPS * p.slots * 128 * p.V) * 4 + 1024;
-    if (p.occ == 2 && 2 * (smem + 1024) > 227 * 1024) { p.occ = 1; sinkhorn_decompose(&p, B, n); }
-  }
   if (ws_bytes < sinkhorn_bwd_workspace_bytes(B, n, m, iters)) return fail(OG_EWORKSPACE, "sinkhorn_bwd: workspace too small");
   if (lds % 4 != 0 || lds < m || (reinterpret_cast<uintptr_t>(S) & 15) || strideS % 4 != 0)
     return fail(OG_EINVAL, "sinkhorn_bwd: S rows must be 16-byte aligned (lds %% 4 == 0, lds >= m)");
@@ -466,7 +485,7 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
       if (p.V == 4 && p.W == 1)       rc = sinkhorn_bwd_launch_v<4, 1, 2>(g, p, stream);
       else if (p.V == 4)              rc = sinkhorn_bwd_launch_v<4, 2, 2>(g, p, stream);
       else if (p.V == 8)              rc = sinkhorn_bwd_launch_v<8, 2, 2>(g, p, stream);
-      else if (p.W == 2)              rc = sinkhorn_bwd_launch_v<16, 2, 2>(g, p, stream);
+      else if (p.W == 2)              rc = sinkhorn_bwd_launch_v<16, 2, 1>(g, p, stream);
       else                            rc = sinkhorn_bwd_launch_v<16, 4, 1>(g, p, stream);
       if (rc != OG_OK) return rc;
     }
