@@ -131,47 +131,58 @@ static og_linear_args lin(const float* A, int64_t lda, int k, const float* W, co
   return a;
 }
 
-static TcLinearArgs to_tc_args(const og_linear_args& a) {
-  TcLinearArgs t;
+// The fields of the tensor-core GEMM arguments (TcLinearArgs or F16LinearArgs) that come from og_linear_args; the split and
+// fp16 outputs and the fp16 operand scales are the caller's.  The fp16 form has no rscale or fp32 transposed output.
+template <class T> static T gemm_args(const og_linear_args& a) {
+  T t;
   memset(&t, 0, sizeof(t));
   t.A = a.A; t.lda = a.lda; t.strideA = a.strideA; t.A2 = a.A2; t.lda2 = a.lda2; t.strideA2 = a.strideA2;
   t.k1 = a.k1; t.k2 = a.k2;
   t.b_rows_per_batch = a.strideW ? (int)(a.strideW / a.ldw) : 0;
   t.bias = a.bias; t.rows = a.rows; t.nout = a.nout; t.batch = a.batch; t.alpha = a.alpha; t.relu = a.relu;
-  t.R = a.R; t.ldr = a.ldr; t.strideR = a.strideR; t.rscale = a.rscale;
-  t.Y = a.Y; t.ldy = a.ldy; t.strideY = a.strideY; t.Yt = a.Yt; t.ldyt = a.ldyt; t.strideYt = a.strideYt;
+  t.R = a.R; t.ldr = a.ldr; t.strideR = a.strideR;
+  t.Y = a.Y; t.ldy = a.ldy; t.strideY = a.strideY; t.ldyt = a.ldyt; t.strideYt = a.strideYt;
+  if constexpr (std::is_same<T, TcLinearArgs>::value) { t.rscale = a.rscale; t.Yt = a.Yt; }
   return t;
+}
+
+// Launches the tensor-core GEMM t = gemm_args(a) + the caller's fields on the weight split Bhi / Blo (a.W's layout); an
+// untileable shape fails with "who: why".
+template <class T, class BT>
+static int linear_sm90_run(const og_linear_args& a, const T& t, const BT* Bhi, const BT* Blo, const char* who, const char* why,
+                           cudaStream_t s) {
+  if (a.strideW && a.strideW % a.ldw != 0) return fail(OG_EUNSUPPORTED, "%s: strideW must be a multiple of ldw", who);
+  if (!linear_sm90_eligible(t, Bhi, Blo, a.ldw)) return fail(OG_EUNSUPPORTED, "%s: %s", who, why);
+  // rows the B tensor map may touch: the LAST batch item only owns nout rows (a map declared over b_rows_per_batch * batch rows
+  // would let a 128-row TMA box read past the end of a head-sliced or exactly-sized operand; rows beyond the map are zero-filled)
+  const int64_t brows = a.strideW ? (int64_t)t.b_rows_per_batch * (a.batch - 1) + a.nout : a.nout;
+  return linear_sm90_launch(t, Bhi, Blo, a.ldw, brows, s);
 }
 
 // Split-output request for the tensor-core path (the fp32 CUDA-core path ignores it).
 struct SplitOut { float *Yhi = nullptr, *Ylo = nullptr, *Ythi = nullptr, *Ytlo = nullptr; };
 
 static int linear_tc_run(const og_linear_args& a, const float* Whi, const float* Wlo, const SplitOut& so, cudaStream_t s) {
-  TcLinearArgs t = to_tc_args(a);
+  TcLinearArgs t = gemm_args<TcLinearArgs>(a);
   t.Yhi = so.Yhi; t.Ylo = so.Ylo; t.Ythi = so.Ythi; t.Ytlo = so.Ytlo;
-  if (a.strideW && a.strideW % a.ldw != 0) return fail(OG_EUNSUPPORTED, "linear_tc: strideW must be a multiple of ldw");
-  if (!linear_tc_eligible(t, Whi, Wlo, a.ldw))
-    return fail(OG_EUNSUPPORTED, "linear_tc: needs K >= 32, K %% 4 == 0, k1 %% 32 == 0 with a second operand and 16-byte aligned rows");
-  // rows the B tensor map may touch: the LAST batch item only owns nout rows (a map declared over b_rows_per_batch * batch rows
-  // would let a 128-row TMA box read past the end of a head-sliced or exactly-sized operand; rows beyond the map are zero-filled)
-  const int64_t brows = a.strideW ? (int64_t)t.b_rows_per_batch * (a.batch - 1) + a.nout : a.nout;
-  return linear_tc_launch(t, Whi, Wlo, a.ldw, brows, s);
+  return linear_sm90_run(a, t, Whi, Wlo, "linear_tc",
+                         "needs K >= 32, K % 4 == 0, k1 % 32 == 0 with a second operand and 16-byte aligned rows", s);
 }
 
 // Kernel selection for one linear layer: the wgmma 3xTF32 GEMM when asked for and the shape is tileable,
 // otherwise the fp32 CUDA-core kernel (tiny K such as the 3-channel keypoint-encoder input).
 static int linear_dispatch(const og_linear_args& a, int precision, cudaStream_t s, const float* Whi = nullptr,
                            const float* Wlo = nullptr, const SplitOut& so = SplitOut()) {
-  if (precision == OG_PREC_TF32X3 && Whi && Wlo) {
-    TcLinearArgs t = to_tc_args(a);
-    if (linear_tc_eligible(t, Whi, Wlo, a.ldw)) return linear_tc_run(a, Whi, Wlo, so, s);
-  }
+  if (precision == OG_PREC_TF32X3 && Whi && Wlo && linear_sm90_eligible(gemm_args<TcLinearArgs>(a), Whi, Wlo, a.ldw))
+    return linear_tc_run(a, Whi, Wlo, so, s);
   if (so.Yhi || so.Ythi) return fail(OG_EUNSUPPORTED, "split outputs need the tensor-core path");
   return linear_simt_launch(a, s);
 }
 
-// exact fp32 attention (CUDA cores); the tensor-core forms take pre-split operands and have their own entry points
-static int attention_fp32(const AttnArgs& a, int head_dim, cudaStream_t s) { return attention_simt_launch(a, head_dim, s); }
+// floats of W a GEMM reads: batch weight blocks strideW apart, the last of them nout rows of ldw
+static int64_t weight_floats(const og_linear_args& a) {
+  return (a.batch > 1 && a.strideW) ? (int64_t)(a.batch - 1) * a.strideW + (int64_t)a.nout * a.ldw : (int64_t)a.nout * a.ldw;
+}
 
 }  // namespace og
 
@@ -266,19 +277,16 @@ int og_linear_tc_fwd(const og_linear_args* a, const float* Whi, const float* Wlo
 // W footprint in floats), the exact fp32 CUDA-core kernel otherwise
 int64_t og_linear_auto_scratch_floats(const og_linear_args* a) {
   if (!a || a->nout <= 0 || a->ldw <= 0 || a->batch <= 0) return -1;
-  const int64_t wf = (a->batch > 1 && a->strideW) ? (int64_t)(a->batch - 1) * a->strideW + (int64_t)a->nout * a->ldw : (int64_t)a->nout * a->ldw;
-  return 2 * align_up(wf, 64);
+  return 2 * align_up(weight_floats(*a), 64);
 }
 int og_linear_auto_fwd(const og_linear_args* a, int precision, float* split_scratch, void* stream) {
   OG_CHECK_ARG(a && a->A && a->W && (a->Y || a->Yt), "linear_auto: null pointer");
   OG_CHECK_ARG(a->rows > 0 && a->nout > 0 && a->batch > 0 && a->k1 > 0 && a->k2 >= 0, "linear_auto: bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
   if (precision != OG_PREC_FP32 && split_scratch && (!a->strideW || a->strideW % a->ldw == 0)) {
-    const int64_t half = og_linear_auto_scratch_floats(a) / 2;
-    const int64_t wf = (a->batch > 1 && a->strideW) ? (int64_t)(a->batch - 1) * a->strideW + (int64_t)a->nout * a->ldw : (int64_t)a->nout * a->ldw;
-    float* hi = split_scratch; float* lo = split_scratch + half;
-    TcLinearArgs t = to_tc_args(*a);
-    if (linear_tc_eligible(t, hi, lo, a->ldw) && (reinterpret_cast<uintptr_t>(a->W) & 15) == 0) {
+    const int64_t wf = weight_floats(*a);
+    float* hi = split_scratch; float* lo = split_scratch + align_up(wf, 64);
+    if (linear_sm90_eligible(gemm_args<TcLinearArgs>(*a), hi, lo, a->ldw) && (reinterpret_cast<uintptr_t>(a->W) & 15) == 0) {
       split_tf32_kernel<<<(unsigned)((wf + 255) / 256), 256, 0, st>>>(a->W, hi, lo, wf);
       OG_LAUNCH_CHECK("split_tf32_kernel");
       launch_counter()++;
@@ -310,7 +318,7 @@ int og_attention_fwd(const float* q, int64_t ldq, int64_t strideq, const float* 
   (void)precision;                                   // raw fp32 operands: always the exact kernel (see the header)
   AttnArgs a{q, ldq, strideq, k, ldk, stridek, v, ldv, stridev, out, ldo, strideo, batch, nq, nk, num_heads,
              (float)pow((double)head_dim, -0.5)};
-  return attention_fp32(a, head_dim, (cudaStream_t)stream);
+  return attention_simt_launch(a, head_dim, (cudaStream_t)stream);
 }
 
 int og_attention_tc_fwd(const float* q, int64_t ldq, int64_t strideq, const float* khi, const float* klo, int64_t ldk,
@@ -591,8 +599,7 @@ int og_sp_select(const int* cand_idx, const float* cand_score, const int* count,
   int n2 = 1;
   while (n2 < max_count) n2 <<= 1;
   const int smem = 2 * n2 * 4;
-  static DeviceFlags attr_set;
-  if (attr_set.once()) OG_CUDA(cudaFuncSetAttribute(sp_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * SP_MAX_CAND * 4));
+  if (const int rc = smem_opt_in<sp_select_kernel>(2 * SP_MAX_CAND * 4)) return rc;
   sp_select_kernel<<<B, 1024, smem, (cudaStream_t)stream>>>(cand_idx, cand_score, count, n_out, mode, cap, W, out_cap, kpts, scores);
   OG_LAUNCH_CHECK("sp_select_kernel");
   launch_counter()++;
@@ -673,222 +680,176 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
   }
 
   // ---- attentional GNN (attention_gnn.py:58-93) ----
-  auto attend = [&](int qrow0, int nq, int krow0, int nk, int batch) -> int {
-    // q from qkv[:, 0:d] of rows qrow0.., k/v from qkv[:, d:3d] of rows krow0..; out -> o rows qrow0..
-    AttnArgs a{w.qkv + (int64_t)qrow0 * 3 * d, 3 * d, (int64_t)nq * 3 * d,
-               w.qkv + (int64_t)krow0 * 3 * d + d, 3 * d, (int64_t)nk * 3 * d,
-               w.qkv + (int64_t)krow0 * 3 * d + 2 * d, 3 * d, (int64_t)nk * 3 * d,
-               w.o + (int64_t)qrow0 * d, d, (int64_t)nq * d, batch, nq, nk, H, (float)pow((double)dh, -0.5)};
-    return attention_fp32(a, dh, st);
-  };
-  auto mlp = [&](int l, int row0, int rows) -> int {
-    // x <- x + W2 . relu(W1 . [x ; o] + b1) + b2     (out_proj and BN folded into W1 / W2 on the host)
-    float* xr = w.x + (int64_t)row0 * d;
-    og_linear_args a = lin(xr, d, d, Wp + L.fc1_w[l], Wp + L.fc1_b[l], rows, 2 * d, w.hid + (int64_t)row0 * 2 * d, 2 * d);
-    a.A2 = w.o + (int64_t)row0 * d; a.lda2 = d; a.k2 = d; a.ldw = 2 * d; a.relu = 1;
-    int r = linear_dispatch(a, prec, st, WH(L.fc1_w[l]), WL(L.fc1_w[l]));
-    if (r != OG_OK) return r;
-    og_linear_args c2 = lin(w.hid + (int64_t)row0 * 2 * d, 2 * d, 2 * d, Wp + L.fc2_w[l], Wp + L.fc2_b[l], rows, d, xr, d);
-    c2.R = xr; c2.ldr = d;
-    return linear_dispatch(c2, prec, st, WH(L.fc2_w[l]), WL(L.fc2_w[l]));
-  };
-  auto project = [&](int l, int row0, int rows, int wrow0, int nout) -> int {
-    // qkv[rows, wrow0 : wrow0 + nout] = x[rows] . Wqkv[wrow0 : wrow0 + nout]^T + b
-    og_linear_args a = lin(w.x + (int64_t)row0 * d, d, d, Wp + L.qkv_w[l] + (int64_t)wrow0 * d, Wp + L.qkv_b[l] + wrow0,
-                           rows, nout, w.qkv + (int64_t)row0 * 3 * d + wrow0, 3 * d);
-    return linear_dispatch(a, prec, st, WH(L.qkv_w[l] + (int64_t)wrow0 * d), WL(L.qkv_w[l] + (int64_t)wrow0 * d));
-  };
-  // Tensor-core attention path (OG_PREC_TF32X3, Dh in {32, 64}): the projection GEMM writes Q as fp32, K split
-  // hi/lo keypoint-major and V split hi/lo channel-major (= the reference's own [B, d, M] layout), which are
-  // exactly the operand layouts csrc/attention_sm90.cuh stages with TMA.
-  const bool tca_ok = tcp && (dh == 32 || dh == 64);
-  auto project_tc = [&](int l, int qrow0, int nq_rows, int srow0, int ns, int sbatch) -> int {
-    // q rows [qrow0, +nq_rows);  k / v from source rows [srow0, +sbatch*ns) (sbatch sequences of ns keypoints)
-    int r;
-    og_linear_args aq = lin(w.x + (int64_t)qrow0 * d, d, d, Wp + L.qkv_w[l], Wp + L.qkv_b[l], nq_rows, d,
-                            w.q + (int64_t)qrow0 * d, d);
-    if ((r = linear_dispatch(aq, prec, st, WH(L.qkv_w[l]), WL(L.qkv_w[l]))) != OG_OK) return r;
-    og_linear_args ak = lin(w.x + (int64_t)srow0 * d, d, d, Wp + L.qkv_w[l] + (int64_t)d * d, Wp + L.qkv_b[l] + d,
-                            sbatch * ns, d, nullptr, d);
-    SplitOut sk; sk.Yhi = w.khi + (int64_t)srow0 * d; sk.Ylo = w.klo + (int64_t)srow0 * d;
-    if ((r = linear_dispatch(ak, prec, st, WH(L.qkv_w[l] + (int64_t)d * d), WL(L.qkv_w[l] + (int64_t)d * d), sk)) != OG_OK) return r;
-    const int64_t ldv = (srow0 == 0) ? w.ldn : w.ldm;
-    const int64_t voff = (srow0 == 0) ? 0 : (int64_t)B * d * w.ldn;
-    og_linear_args av = lin(w.x + (int64_t)srow0 * d, d, d, Wp + L.qkv_w[l] + 2 * (int64_t)d * d, Wp + L.qkv_b[l] + 2 * d,
-                            ns, d, nullptr, d);
-    av.batch = sbatch; av.strideA = (int64_t)ns * d; av.ldyt = ldv; av.strideYt = (int64_t)d * ldv;
-    SplitOut sv; sv.Ythi = w.vthi + voff; sv.Ytlo = w.vtlo + voff;
-    return linear_dispatch(av, prec, st, WH(L.qkv_w[l] + 2 * (int64_t)d * d), WL(L.qkv_w[l] + 2 * (int64_t)d * d), sv);
-  };
-  auto attend_tc = [&](int qrow0, int nq, int krow0, int nk, int batch) -> int {
-    const int64_t ldv = (krow0 == 0) ? w.ldn : w.ldm;
-    const int64_t voff = (krow0 == 0) ? 0 : (int64_t)B * d * w.ldn;
-    TcAttnArgs a{w.q + (int64_t)qrow0 * d, d, (int64_t)nq * d, w.o + (int64_t)qrow0 * d, d, (int64_t)nq * d,
-                 batch, nq, nk, H, d, (float)pow((double)dh, -0.5)};
-    return attention_tc_launch(a, w.khi + (int64_t)krow0 * d, w.klo + (int64_t)krow0 * d, d, w.vthi + voff, w.vtlo + voff,
-                               ldv, dh, st);
-  };
-  // ---- fp16 hi/lo form of the GNN (OG_PREC_FP16X3; csrc/linear_sm90.cuh, csrc/attention_sm90.cuh) ----
-  // Every activation tensor has a device slot with its tracked amax (fp32 tensors) or the scale it was written with (fp16
+  // One layer schedule for three forms of attention.  They differ in how the projection writes Q / K / V, how attention reads
+  // them and how the GEMMs get their operand scales:
+  //   FP32: Q | K | V interleaved in qkv [R, 3d], exact attention on CUDA cores (fp32, d < 32 or head_dim not in {32, 64});
+  //   TF32: Q fp32, K split hi/lo keypoint-major and V split hi/lo channel-major (= the reference's own [B, d, M] layout), which
+  //         are exactly the operand layouts csrc/attention_sm90.cuh stages with TMA;
+  //   F16:  the same layouts in fp16 hi/lo, every operand scaled from device slots (below).
+  enum class Att { FP32, TF32, F16 };
+  const Att att = f16p ? Att::F16 : (tcp && (dh == 32 || dh == 64)) ? Att::TF32 : Att::FP32;
+  // `count` sequences of `len` keypoints from row `row0` on, of image `img` (2: both)
+  struct Seqs { int row0, len, count, img; int rows() const { return len * count; } };
+  const Seqs img[2] = {{0, n, B, 0}, {R0, m, B, 1}};
+  const Seqs all{0, R, 1, 2};                                // every row at once, for the GEMMs only
+  // Granularity of a self layer with n != m, which each form keeps as it is:
+  //   FP32 projects both images in one launch (its GEMMs see rows, not sequences);
+  //   F16 runs the MLP per image, so that each image keeps its own amax slot: one shared slot would change the fp16 scales.
+  const bool project_all_rows = att == Att::FP32, mlp_per_image = att == Att::F16;
+  // V^T of image 0 (or of both images when n == m) at offset 0 with rows ldn apart, V^T of image 1 after it with rows ldm apart
+  auto vt_ld = [&](const Seqs& kv) { return kv.row0 == 0 ? w.ldn : w.ldm; };
+  auto vt_off = [&](const Seqs& kv) { return kv.row0 == 0 ? 0 : (int64_t)B * d * w.ldn; };
+
+  // F16: every activation tensor has a device slot with its tracked amax (fp32 tensors) or the scale it was written with (fp16
   // K / V^T); a consumer derives its operand scale from the producers' slots, so no scale ever passes through the host.
   int nslot = 0;
   auto new_slot = [&]() -> float* { return w.slots + (nslot < w.nslots - 1 ? nslot++ : w.nslots - 1); };
-  float *sx0 = nullptr, *sx1 = nullptr;                      // amax slots of the current x0 / x1
+  float* sx[2] = {};                                         // amax slots of the current x0 / x1
+  struct SeqSlots { float *q, *k, *v, *o; } ss[2] = {};      // of the last projection of image 0 (or both images) / image 1
+  auto xslot = [&](const Seqs& g, int i) { return g.img == 2 ? sx[i] : i == 0 ? sx[g.img] : nullptr; };   // amax of x's rows g
   __half* kh16 = reinterpret_cast<__half*>(w.khi); __half* kl16 = reinterpret_cast<__half*>(w.klo);
   __half* vth16 = reinterpret_cast<__half*>(w.vthi); __half* vtl16 = reinterpret_cast<__half*>(w.vtlo);
-  if (f16p) {
+  if (att == Att::F16) {
     OG_CUDA(cudaMemsetAsync(w.slots, 0, (size_t)w.nslots * 4, st));
-    sx0 = sx1 = new_slot();
+    sx[0] = sx[1] = new_slot();
     const int64_t nx = (int64_t)R * d;
-    amax_kernel<<<(unsigned)std::min<int64_t>((nx + 2047) / 2048, 1184), 256, 0, st>>>(w.x, nx, sx0);
+    amax_kernel<<<(unsigned)std::min<int64_t>((nx + 2047) / 2048, 1184), 256, 0, st>>>(w.x, nx, sx[0]);
     OG_LAUNCH_CHECK("amax_kernel");
     launch_counter()++;
   }
-  auto M16 = [&](int l, int t) { return meta16 + ((int64_t)l * 5 + t) * 4; };
-  auto gemm16 = [&](const float* A, int64_t lda, int k1, const float* A2, int64_t lda2, int k2, int64_t woff, const float* bias,
-                    int rows, int nout, const float* am0, const float* am1, const float* am2, const float* meta) {
-    F16LinearArgs g;
-    memset(&g, 0, sizeof(g));
-    g.A = A; g.lda = lda; g.k1 = k1; g.A2 = A2; g.lda2 = lda2; g.k2 = k2; g.bias = bias; g.rows = rows; g.nout = nout; g.batch = 1;
-    g.alpha = 1.f; g.amax_in[0] = am0; g.amax_in[1] = am1; g.amax_in[2] = am2; g.w_meta = meta;
-    (void)woff;
+  // the fp16 GEMM of `a`: operand amax slots am0 .. am2 (of A, A2) and the meta of weight t of layer l (og_pack_f16)
+  auto args16 = [&](const og_linear_args& a, float* am0, float* am1, float* am2, int l, int t) {
+    F16LinearArgs g = gemm_args<F16LinearArgs>(a);
+    g.amax_in[0] = am0; g.amax_in[1] = am1; g.amax_in[2] = am2; g.w_meta = meta16 + ((int64_t)l * 5 + t) * 4;
     return g;
   };
-  auto run16 = [&](const F16LinearArgs& g, int64_t woff) -> int {
-    const int K = g.k1 + g.k2;
-    if (!linear_f16_eligible(g, W16h + woff, W16l + woff, K)) return fail(OG_EUNSUPPORTED, "forward: a layer is not tileable by the fp16 GEMM");
-    return linear_f16_launch(g, W16h + woff, W16l + woff, K, g.nout, st);
+  auto run16 = [&](const og_linear_args& a, const F16LinearArgs& g, int64_t woff) {
+    return linear_sm90_run(a, g, W16h + woff, W16l + woff, "forward", "a layer is not tileable by the fp16 GEMM", st);
   };
-  struct SeqSlots { float *q, *k, *v, *o; };
-  // Q / K / V projections.  d % 128 == 0 (every shipped config): the projections that share their input run as ONE launch over the
-  // stacked weights (linear_f16.cuh OUTK 4) - Q | K | V in a self layer (same keypoints), K | V in a cross layer (+ Q on its own).
-  const int fuse_qkv = fuse_qkv_mode();
-  auto project_f16 = [&](int l, int qrow0, int nq_rows, int srow0, int ns, int sbatch, float* aq0, float* aq1, float* as0, float* as1,
-                         SeqSlots& ss) -> int {
+  // F16 with d % 128 == 0 (every shipped config): the projections that share their input run as ONE launch over the stacked
+  // weights (F16LinearArgs::nkinds): Q | K | V in a self layer (same keypoints), K | V in a cross layer (+ Q on its own).
+  const bool fuse_qkv = fuse_qkv_mode() && d % tcf::BN == 0;
+
+  // Q of the rows q, K and V of the rows kv (q itself in a self layer)
+  auto project = [&](int l, const Seqs& q, const Seqs& kv) -> int {
+    const bool self = q.row0 == kv.row0;
+    const int64_t wq = L.qkv_w[l], bq = L.qkv_b[l], dd = (int64_t)d * d;
+    const float* xq = w.x + (int64_t)q.row0 * d;
+    const float* xkv = w.x + (int64_t)kv.row0 * d;
     int r;
-    ss.q = new_slot(); ss.k = new_slot(); ss.v = new_slot(); ss.o = new_slot();
-    const int64_t ldv = (srow0 == 0) ? w.ldn : w.ldm;
-    const int64_t voff = (srow0 == 0) ? 0 : (int64_t)B * d * w.ldn;
-    const bool fuse = fuse_qkv && d % tcf::BN == 0;
-    const bool same_src = qrow0 == srow0 && nq_rows == sbatch * ns;
-    if (!(fuse && same_src)) {
-      F16LinearArgs gq = gemm16(w.x + (int64_t)qrow0 * d, d, d, nullptr, 0, 0, L.qkv_w[l], Wp + L.qkv_b[l], nq_rows, d, aq0, aq1, nullptr, M16(l, 0));
-      gq.Y = w.q + (int64_t)qrow0 * d; gq.ldy = d; gq.amax_out = ss.q;
-      if ((r = run16(gq, L.qkv_w[l])) != OG_OK) return r;
+    if (att == Att::FP32) {       // qkv[g, c0 : c0 + nout] = x[g] . Wqkv[c0 : c0 + nout]^T + b: Q | K | V in one launch in a self layer
+      auto part = [&](const Seqs& g, int c0, int nout) {
+        og_linear_args a = lin(w.x + (int64_t)g.row0 * d, d, d, Wp + wq + (int64_t)c0 * d, Wp + bq + c0, g.rows(), nout,
+                               w.qkv + (int64_t)g.row0 * 3 * d + c0, 3 * d);
+        return linear_dispatch(a, prec, st, WH(wq + (int64_t)c0 * d), WL(wq + (int64_t)c0 * d));
+      };
+      if (self) return part(q, 0, 3 * d);
+      return (r = part(q, 0, d)) != OG_OK ? r : part(kv, d, 2 * d);
     }
-    if (fuse) {
-      const int k0 = same_src ? 0 : 1, nk_ = 3 - k0;
-      F16LinearArgs g = gemm16(w.x + (int64_t)srow0 * d, d, d, nullptr, 0, 0, 0, Wp + L.qkv_b[l] + k0 * d, ns, nk_ * d, as0, as1, nullptr, M16(l, k0));
-      g.batch = sbatch; g.strideA = (int64_t)ns * d;
-      g.nkinds = nk_; g.kind0 = k0; g.kind_cols = d;
-      g.ldy = d; g.strideY = (int64_t)ns * d;
-      if (k0 == 0) { g.Y = w.q + (int64_t)srow0 * d; g.amax_out = ss.q; }
-      g.Yh = kh16 + (int64_t)srow0 * d; g.Yl = kl16 + (int64_t)srow0 * d; g.scale_out = ss.k;
-      g.Yth = vth16 + voff; g.Ytl = vtl16 + voff; g.ldyt = ldv; g.strideYt = (int64_t)d * ldv; g.scale_out_v = ss.v;
-      return run16(g, L.qkv_w[l] + (int64_t)k0 * d * d);
+    const int64_t ldv = vt_ld(kv), voff = vt_off(kv);
+    og_linear_args aq = lin(xq, d, d, Wp + wq, Wp + bq, q.rows(), d, w.q + (int64_t)q.row0 * d, d);
+    og_linear_args ak = lin(xkv, d, d, Wp + wq + dd, Wp + bq + d, kv.rows(), d, nullptr, d);
+    og_linear_args av = lin(xkv, d, d, Wp + wq + 2 * dd, Wp + bq + 2 * d, kv.len, d, nullptr, d);   // V^T batched per sequence
+    av.batch = kv.count; av.strideA = (int64_t)kv.len * d; av.ldyt = ldv; av.strideYt = (int64_t)d * ldv;
+    if (att == Att::TF32) {
+      SplitOut sk, sv;
+      sk.Yhi = w.khi + (int64_t)kv.row0 * d; sk.Ylo = w.klo + (int64_t)kv.row0 * d;
+      sv.Ythi = w.vthi + voff; sv.Ytlo = w.vtlo + voff;
+      if ((r = linear_dispatch(aq, prec, st, WH(wq), WL(wq))) != OG_OK) return r;
+      if ((r = linear_dispatch(ak, prec, st, WH(wq + dd), WL(wq + dd), sk)) != OG_OK) return r;
+      return linear_dispatch(av, prec, st, WH(wq + 2 * dd), WL(wq + 2 * dd), sv);
     }
-    F16LinearArgs gk = gemm16(w.x + (int64_t)srow0 * d, d, d, nullptr, 0, 0, 0, Wp + L.qkv_b[l] + d, sbatch * ns, d, as0, as1, nullptr, M16(l, 1));
-    gk.Yh = kh16 + (int64_t)srow0 * d; gk.Yl = kl16 + (int64_t)srow0 * d; gk.ldy = d; gk.scale_out = ss.k;
-    if ((r = run16(gk, L.qkv_w[l] + (int64_t)d * d)) != OG_OK) return r;
-    F16LinearArgs gv = gemm16(w.x + (int64_t)srow0 * d, d, d, nullptr, 0, 0, 0, Wp + L.qkv_b[l] + 2 * d, ns, d, as0, as1, nullptr, M16(l, 2));
-    gv.batch = sbatch; gv.strideA = (int64_t)ns * d; gv.Yth = vth16 + voff; gv.Ytl = vtl16 + voff; gv.ldyt = ldv; gv.strideYt = (int64_t)d * ldv;
-    gv.scale_out = ss.v;
-    return run16(gv, L.qkv_w[l] + 2 * (int64_t)d * d);
+    SeqSlots& s = ss[q.img == 1];
+    s = {new_slot(), new_slot(), new_slot(), new_slot()};
+    if (!(fuse_qkv && self)) {
+      F16LinearArgs gq = args16(aq, xslot(q, 0), xslot(q, 1), nullptr, l, 0);
+      gq.amax_out = s.q;
+      if ((r = run16(aq, gq, wq)) != OG_OK) return r;
+    }
+    if (fuse_qkv) {
+      const int k0 = self ? 0 : 1, nk = 3 - k0;
+      og_linear_args a = lin(xkv, d, d, Wp + wq + k0 * dd, Wp + bq + k0 * d, kv.len, nk * d, k0 == 0 ? w.q + (int64_t)kv.row0 * d : nullptr, d);
+      a.batch = kv.count; a.strideA = a.strideY = (int64_t)kv.len * d; a.ldyt = ldv; a.strideYt = (int64_t)d * ldv;
+      F16LinearArgs g = args16(a, xslot(kv, 0), xslot(kv, 1), nullptr, l, k0);
+      g.nkinds = nk; g.kind0 = k0; g.kind_cols = d;
+      if (k0 == 0) g.amax_out = s.q;
+      g.Yh = kh16 + (int64_t)kv.row0 * d; g.Yl = kl16 + (int64_t)kv.row0 * d; g.scale_out = s.k;
+      g.Yth = vth16 + voff; g.Ytl = vtl16 + voff; g.scale_out_v = s.v;
+      return run16(a, g, wq + k0 * dd);
+    }
+    F16LinearArgs gk = args16(ak, xslot(kv, 0), xslot(kv, 1), nullptr, l, 1);
+    gk.Yh = kh16 + (int64_t)kv.row0 * d; gk.Yl = kl16 + (int64_t)kv.row0 * d; gk.scale_out = s.k;
+    if ((r = run16(ak, gk, wq + dd)) != OG_OK) return r;
+    F16LinearArgs gv = args16(av, xslot(kv, 0), xslot(kv, 1), nullptr, l, 2);
+    gv.Yth = vth16 + voff; gv.Ytl = vtl16 + voff; gv.scale_out = s.v;
+    return run16(av, gv, wq + 2 * dd);
   };
-  auto attend_f16 = [&](int qrow0, int nq, int krow0, int nk, int batch, const SeqSlots& ss) -> int {
-    const int64_t ldv = (krow0 == 0) ? w.ldn : w.ldm;
-    const int64_t voff = (krow0 == 0) ? 0 : (int64_t)B * d * w.ldn;
-    TcAttnArgs a{w.q + (int64_t)qrow0 * d, d, (int64_t)nq * d, w.o + (int64_t)qrow0 * d, d, (int64_t)nq * d,
-                 batch, nq, nk, H, d, (float)pow((double)dh, -0.5)};
-    F16AttnScales sc{ss.q, ss.k, ss.v, ss.o, 0};
-    return attention_f16_launch(a, sc, kh16 + (int64_t)krow0 * d, kl16 + (int64_t)krow0 * d, d, vth16 + voff, vtl16 + voff, ldv, dh, st);
+
+  // o[q] = attention of the queries q over the keys / values kv
+  auto attend = [&](const Seqs& q, const Seqs& kv) -> int {
+    const float scale = (float)pow((double)dh, -0.5);
+    if (att == Att::FP32) {
+      const float* qkv_q = w.qkv + (int64_t)q.row0 * 3 * d;
+      const float* qkv_kv = w.qkv + (int64_t)kv.row0 * 3 * d;
+      AttnArgs a{qkv_q, 3 * d, (int64_t)q.len * 3 * d, qkv_kv + d, 3 * d, (int64_t)kv.len * 3 * d, qkv_kv + 2 * d, 3 * d,
+                 (int64_t)kv.len * 3 * d, w.o + (int64_t)q.row0 * d, d, (int64_t)q.len * d, q.count, q.len, kv.len, H, scale};
+      return attention_simt_launch(a, dh, st);
+    }
+    const int64_t ldv = vt_ld(kv), voff = vt_off(kv), k0 = (int64_t)kv.row0 * d;
+    TcAttnArgs a{w.q + (int64_t)q.row0 * d, d, (int64_t)q.len * d, w.o + (int64_t)q.row0 * d, d, (int64_t)q.len * d,
+                 q.count, q.len, kv.len, H, d, scale};
+    if (att == Att::TF32) return attention_tc_launch(a, w.khi + k0, w.klo + k0, d, w.vthi + voff, w.vtlo + voff, ldv, dh, st);
+    const SeqSlots& s = ss[q.img == 1];
+    return attention_f16_launch(a, F16AttnScales{s.q, s.k, s.v, s.o, 0}, kh16 + k0, kl16 + k0, d, vth16 + voff, vtl16 + voff, ldv, dh, st);
   };
-  auto mlp_f16 = [&](int l, int row0, int rows, float* ax0, float* ax1, float* ao, float** sx_new) -> int {
+
+  // x[g] <- x[g] + W2 . relu(W1 . [x[g] ; o[g]] + b1) + b2     (out_proj and BN folded into W1 / W2 on the host)
+  auto mlp = [&](int l, const Seqs& g) -> int {
+    float* xr = w.x + (int64_t)g.row0 * d;
+    float* hr = w.hid + (int64_t)g.row0 * 2 * d;
+    og_linear_args a1 = lin(xr, d, d, Wp + L.fc1_w[l], Wp + L.fc1_b[l], g.rows(), 2 * d, hr, 2 * d);
+    a1.A2 = w.o + (int64_t)g.row0 * d; a1.lda2 = d; a1.k2 = d; a1.ldw = 2 * d; a1.relu = 1;
+    og_linear_args a2 = lin(hr, 2 * d, 2 * d, Wp + L.fc2_w[l], Wp + L.fc2_b[l], g.rows(), d, xr, d);
+    a2.R = xr; a2.ldr = d;
+    int r;
+    if (att != Att::F16) {
+      if ((r = linear_dispatch(a1, prec, st, WH(L.fc1_w[l]), WL(L.fc1_w[l]))) != OG_OK) return r;
+      return linear_dispatch(a2, prec, st, WH(L.fc2_w[l]), WL(L.fc2_w[l]));
+    }
+    // F16: [x ; o] scaled by the slots of x and of the attention output, the hidden layer by the amax fc1 tracked
     float* sh = new_slot();
     float* sn = new_slot();
-    float* xr = w.x + (int64_t)row0 * d;
-    F16LinearArgs g1 = gemm16(xr, d, d, w.o + (int64_t)row0 * d, d, d, 0, Wp + L.fc1_b[l], rows, 2 * d, ax0, ax1, ao, M16(l, 3));
-    g1.relu = 1; g1.Y = w.hid + (int64_t)row0 * 2 * d; g1.ldy = 2 * d; g1.amax_out = sh;
-    int r = run16(g1, L.fc1_w[l]);
-    if (r != OG_OK) return r;
-    F16LinearArgs g2 = gemm16(w.hid + (int64_t)row0 * 2 * d, 2 * d, 2 * d, nullptr, 0, 0, 0, Wp + L.fc2_b[l], rows, d, sh, nullptr, nullptr, M16(l, 4));
-    g2.R = xr; g2.ldr = d; g2.Y = xr; g2.ldy = d; g2.amax_out = sn;
-    *sx_new = sn;
-    return run16(g2, L.fc2_w[l]);
+    F16LinearArgs g1 = args16(a1, xslot(g, 0), xslot(g, 1), ss[g.img == 1].o, l, 3);
+    g1.amax_out = sh;
+    if ((r = run16(a1, g1, L.fc1_w[l])) != OG_OK) return r;
+    F16LinearArgs g2 = args16(a2, sh, nullptr, nullptr, l, 4);
+    g2.amax_out = sn;
+    if ((r = run16(a2, g2, L.fc2_w[l])) != OG_OK) return r;
+    if (g.img != 1) sx[0] = sn;
+    if (g.img != 0) sx[1] = sn;
+    return OG_OK;
   };
+
   for (int l = 0; l < cfg->num_layers; ++l) {
-    if (f16p) {
-      SeqSlots ss;
-      float* sn = nullptr;
-      if (l % 2 == 0) {                                    // self
-        if (n == m) {
-          if ((rc = project_f16(l, 0, R, 0, n, 2 * B, sx0, sx1, sx0, sx1, ss)) != OG_OK) return rc;
-          if ((rc = attend_f16(0, n, 0, n, 2 * B, ss)) != OG_OK) return rc;
-          if ((rc = mlp_f16(l, 0, R, sx0, sx1, ss.o, &sn)) != OG_OK) return rc;
-          sx0 = sx1 = sn;
-        } else {
-          SeqSlots s1;
-          if ((rc = project_f16(l, 0, R0, 0, n, B, sx0, nullptr, sx0, nullptr, ss)) != OG_OK) return rc;
-          if ((rc = attend_f16(0, n, 0, n, B, ss)) != OG_OK) return rc;
-          if ((rc = project_f16(l, R0, R1, R0, m, B, sx1, nullptr, sx1, nullptr, s1)) != OG_OK) return rc;
-          if ((rc = attend_f16(R0, m, R0, m, B, s1)) != OG_OK) return rc;
-          float *sa = nullptr, *sb = nullptr;
-          if ((rc = mlp_f16(l, 0, R0, sx0, nullptr, ss.o, &sa)) != OG_OK) return rc;
-          if ((rc = mlp_f16(l, R0, R1, sx1, nullptr, s1.o, &sb)) != OG_OK) return rc;
-          sx0 = sa; sx1 = sb;
-        }
-      } else {                                             // cross: SEQUENTIAL (attention_gnn.py:74-77)
-        if ((rc = project_f16(l, 0, R0, R0, m, B, sx0, nullptr, sx1, nullptr, ss)) != OG_OK) return rc;
-        if ((rc = attend_f16(0, n, R0, m, B, ss)) != OG_OK) return rc;
-        if ((rc = mlp_f16(l, 0, R0, sx0, nullptr, ss.o, &sn)) != OG_OK) return rc;
-        sx0 = sn;
-        if ((rc = project_f16(l, R0, R1, 0, n, B, sx1, nullptr, sx0, nullptr, ss)) != OG_OK) return rc;     // k, v of the UPDATED image 0
-        if ((rc = attend_f16(R0, m, 0, n, B, ss)) != OG_OK) return rc;
-        if ((rc = mlp_f16(l, R0, R1, sx1, nullptr, ss.o, &sn)) != OG_OK) return rc;
-        sx1 = sn;
+    if (l % 2 == 1) {                                      // cross: SEQUENTIAL (attention_gnn.py:74-77)
+      for (int i = 0; i < 2; ++i) {                        // image 1's K / V come from the UPDATED image 0
+        if ((rc = project(l, img[i], img[1 - i])) != OG_OK) return rc;
+        if ((rc = attend(img[i], img[1 - i])) != OG_OK) return rc;
+        if ((rc = mlp(l, img[i])) != OG_OK) return rc;
       }
-      continue;
-    }
-    if (tca_ok) {
-      if (l % 2 == 0) {                                    // self
-        if (n == m) {
-          if ((rc = project_tc(l, 0, R, 0, n, 2 * B)) != OG_OK) return rc;
-          if ((rc = attend_tc(0, n, 0, n, 2 * B)) != OG_OK) return rc;
-        } else {
-          if ((rc = project_tc(l, 0, R0, 0, n, B)) != OG_OK) return rc;
-          if ((rc = attend_tc(0, n, 0, n, B)) != OG_OK) return rc;
-          if ((rc = project_tc(l, R0, R1, R0, m, B)) != OG_OK) return rc;
-          if ((rc = attend_tc(R0, m, R0, m, B)) != OG_OK) return rc;
-        }
-        if ((rc = mlp(l, 0, R)) != OG_OK) return rc;
-      } else {                                             // cross: SEQUENTIAL (attention_gnn.py:74-77)
-        if ((rc = project_tc(l, 0, R0, R0, m, B)) != OG_OK) return rc;
-        if ((rc = attend_tc(0, n, R0, m, B)) != OG_OK) return rc;
-        if ((rc = mlp(l, 0, R0)) != OG_OK) return rc;
-        if ((rc = project_tc(l, R0, R1, 0, n, B)) != OG_OK) return rc;     // k, v of the UPDATED image 0
-        if ((rc = attend_tc(R0, m, 0, n, B)) != OG_OK) return rc;
-        if ((rc = mlp(l, R0, R1)) != OG_OK) return rc;
+    } else if (n == m) {                                   // self: both images as one batch of 2B sequences
+      const Seqs both{0, n, 2 * B, 2};
+      if ((rc = project(l, both, both)) != OG_OK) return rc;
+      if ((rc = attend(both, both)) != OG_OK) return rc;
+      if ((rc = mlp(l, both)) != OG_OK) return rc;
+    } else {                                               // self: one image at a time
+      if (project_all_rows && (rc = project(l, all, all)) != OG_OK) return rc;
+      for (int i = 0; i < 2; ++i) {
+        if (!project_all_rows && (rc = project(l, img[i], img[i])) != OG_OK) return rc;
+        if ((rc = attend(img[i], img[i])) != OG_OK) return rc;
       }
-      continue;
-    }
-    if (l % 2 == 0) {                                      // self: both images, shared weights, independent
-      if ((rc = project(l, 0, R, 0, 3 * d)) != OG_OK) return rc;
-      if (n == m) {
-        if ((rc = attend(0, n, 0, n, 2 * B)) != OG_OK) return rc;
-      } else {
-        if ((rc = attend(0, n, 0, n, B)) != OG_OK) return rc;
-        if ((rc = attend(R0, m, R0, m, B)) != OG_OK) return rc;
-      }
-      if ((rc = mlp(l, 0, R)) != OG_OK) return rc;
-    } else {                                               // cross: SEQUENTIAL (attention_gnn.py:74-77)
-      if ((rc = project(l, 0, R0, 0, d)) != OG_OK) return rc;            // q of image 0
-      if ((rc = project(l, R0, R1, d, 2 * d)) != OG_OK) return rc;       // k, v of image 1
-      if ((rc = attend(0, n, R0, m, B)) != OG_OK) return rc;
-      if ((rc = mlp(l, 0, R0)) != OG_OK) return rc;
-      if ((rc = project(l, R0, R1, 0, d)) != OG_OK) return rc;           // q of image 1
-      if ((rc = project(l, 0, R0, d, 2 * d)) != OG_OK) return rc;        // k, v of the UPDATED image 0
-      if ((rc = attend(R0, m, 0, n, B)) != OG_OK) return rc;
-      if ((rc = mlp(l, R0, R1)) != OG_OK) return rc;
+      for (int i = 0; i < (mlp_per_image ? 2 : 1); ++i)
+        if ((rc = mlp(l, mlp_per_image ? img[i] : all)) != OG_OK) return rc;
     }
   }
 
@@ -998,22 +959,12 @@ int og_linear_f16_fwd(const og_linear_args* a, const void* Wh16, const void* Wl1
   OG_CHECK_ARG(a && a->A && Wh16 && Wl16 && w_meta && a_amax, "linear_f16: null pointer");
   OG_CHECK_ARG(a->rows > 0 && a->nout > 0 && a->batch > 0 && a->k1 > 0 && a->k2 >= 0, "linear_f16: bad sizes");
   OG_CHECK_ARG(!a->rscale && !a->Yt, "linear_f16: rscale / fp32 transposed outputs are not part of the fp16 form");
-  F16LinearArgs g;
-  memset(&g, 0, sizeof(g));
-  g.A = a->A; g.lda = a->lda; g.strideA = a->strideA; g.A2 = a->A2; g.lda2 = a->lda2; g.strideA2 = a->strideA2; g.k1 = a->k1; g.k2 = a->k2;
-  if (a->strideW && a->strideW % a->ldw != 0) return fail(OG_EUNSUPPORTED, "linear_f16: strideW must be a multiple of ldw");
-  g.b_rows_per_batch = a->strideW ? (int)(a->strideW / a->ldw) : 0;
-  g.bias = a->bias; g.rows = a->rows; g.nout = a->nout; g.batch = a->batch; g.alpha = a->alpha; g.relu = a->relu;
-  g.R = a->R; g.ldr = a->ldr; g.strideR = a->strideR;
-  g.Y = a->Y; g.ldy = a->ldy; g.strideY = a->strideY;
+  F16LinearArgs g = gemm_args<F16LinearArgs>(*a);
   g.Yh = static_cast<__half*>(Yh); g.Yl = static_cast<__half*>(Yl);
-  g.Yth = static_cast<__half*>(Yth); g.Ytl = static_cast<__half*>(Ytl); g.ldyt = a->ldyt; g.strideYt = a->strideYt;
+  g.Yth = static_cast<__half*>(Yth); g.Ytl = static_cast<__half*>(Ytl);
   g.amax_in[0] = a_amax; g.w_meta = w_meta; g.amax_out = amax_out; g.scale_out = scale_out; g.swap_halves = swap_halves;
-  const __half* bh = static_cast<const __half*>(Wh16); const __half* bl = static_cast<const __half*>(Wl16);
-  if (!linear_f16_eligible(g, bh, bl, a->ldw))
-    return fail(OG_EUNSUPPORTED, "linear_f16: needs K >= 64, 16-byte aligned rows, exactly one output kind (Y | Yh,Yl | Yth,Ytl)");
-  const int64_t brows = a->strideW ? (int64_t)g.b_rows_per_batch * (a->batch - 1) + a->nout : a->nout;
-  return linear_f16_launch(g, bh, bl, a->ldw, brows, (cudaStream_t)stream);
+  return linear_sm90_run(*a, g, static_cast<const __half*>(Wh16), static_cast<const __half*>(Wl16), "linear_f16",
+                         "needs K >= 64, 16-byte aligned rows, exactly one output kind (Y | Yh,Yl | Yth,Ytl)", (cudaStream_t)stream);
 }
 
 int og_attention_f16_fwd(const float* q, int64_t ldq, int64_t strideq, const float* q_amax, const void* khi, const void* klo,

@@ -137,11 +137,7 @@ inline int attention_simt_launch(const AttnArgs& a, int head_dim, cudaStream_t s
 #define OG_ATTN_CASE(DH_)                                                                        \
   case DH_: {                                                                                    \
     constexpr int smem = (DH_ * (ATQ + ATK) + ATK * DH_ + ATK * ATQ) * (int)sizeof(float);       \
-    static DeviceFlags attr_set;                                                                \
-    if (attr_set.once()) {                                                                             \
-      OG_CUDA(cudaFuncSetAttribute(attention_simt_kernel<DH_>,                                   \
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, smem));          \
-    }                                                                                            \
+    if (const int rc = smem_opt_in<attention_simt_kernel<DH_>>(smem)) return rc;                 \
     attention_simt_kernel<DH_><<<grid, 256, smem, stream>>>(a);                                  \
   } break;
   switch (head_dim) {

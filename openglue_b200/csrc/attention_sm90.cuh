@@ -471,21 +471,9 @@ inline int attention_sm90_launch(const TcAttnArgs& a, const F16AttnScales& sc, c
     if ((rc = tc::make_tmap_2d(&mvh, vthi, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
     if ((rc = tc::make_tmap_2d(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
   }
-  static DeviceFlags attr_set;
-  if (attr_set.once())
-    OG_CUDA(cudaFuncSetAttribute(attention_sm90_kernel<DH, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(cdiv(a.nq, BM), a.num_heads, a.batch);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = tc::pdl_mode() ? 1 : 0;
-  OG_CUDA(cudaLaunchKernelEx(&cfg, attention_sm90_kernel<DH, F16>, mkh, mkl, mvh, mvl, a, sc));
-  launch_counter()++;
-  return OG_OK;
+  if ((rc = smem_opt_in<attention_sm90_kernel<DH, F16>>(C::SMEM_BYTES)) != OG_OK) return rc;
+  return tc::pdl_launch(attention_sm90_kernel<DH, F16>, dim3(cdiv(a.nq, BM), a.num_heads, a.batch), dim3(C::THREADS), C::SMEM_BYTES,
+                        stream, mkh, mkl, mvh, mvl, a, sc);
 }
 
 inline bool attention_tc_eligible(int head_dim, int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo) {

@@ -30,7 +30,7 @@ inline int fail(int code, const char* fmt, ...) {
 inline int& launch_counter() { static thread_local int c = 0; return c; }
 
 // Per-device state (a process may drive several GPUs: MatchingCore(device=...), .to(dev)): the capability cache and the
-// "function attribute already set" flags are indexed by the CURRENT device, never process-global.
+// "function attribute already set" flags (smem_opt_in) are indexed by the CURRENT device, never process-global.
 constexpr int OG_MAX_DEVICES = 64;
 inline int current_device() { int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= OG_MAX_DEVICES) dev = 0; return dev; }
 
@@ -50,16 +50,20 @@ inline const DeviceInfo& device_info() {
   }
   return d;
 }
-// One flag per device for "cudaFuncSetAttribute done": declare `static DeviceFlags f;` next to the launch and test f.once(),
-// or test f.pending() and call f.mark() once the attribute call succeeded (a failed call is then retried on the next launch).
-struct DeviceFlags {
-  bool set[OG_MAX_DEVICES] = {};
-  bool once() { const int dev = current_device(); if (set[dev]) return false; set[dev] = true; return true; }
-  bool pending() const { return !set[current_device()]; }
-  void mark() { set[current_device()] = true; }
-};
 // Dynamic shared memory one block may opt in to on sm_90 (cudaDevAttrMaxSharedMemoryPerBlockOptin: 227 KB of the SM's 228 KB)
 constexpr size_t OG_SMEM_OPTIN_MAX = 227 * 1024;
+// Opts Kernel in to `bytes` of dynamic shared memory, once per device.  The flag is keyed on the kernel itself (every template
+// instantiation has its own) and set only after the call succeeded, so a failed opt-in is retried on the next launch.
+template <auto Kernel>
+inline int smem_opt_in(int bytes) {
+  static bool done[OG_MAX_DEVICES] = {};
+  bool& d = done[current_device()];
+  if (!d) {
+    OG_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    d = true;
+  }
+  return OG_OK;
+}
 
 __host__ __device__ inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }

@@ -481,37 +481,26 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
     if ((rc = tc::make_tmap_2d(&mh, Bhi, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
     if ((rc = tc::make_tmap_2d(&ml, Blo, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
   }
-  static DeviceFlags attr_set;
-  if (attr_set.once())
-    OG_CUDA(cudaFuncSetAttribute(linear_sm90_kernel<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-  cudaLaunchConfig_t cfg = {};
+  if ((rc = smem_opt_in<linear_sm90_kernel<Args>>(C::SMEM_BYTES)) != OG_OK) return rc;
   const int tiles = cdiv(a.nout, BN) * cdiv(a.rows, BM) * a.batch;
   const int sms = device_info().ok ? device_info().sm_count : 132;
-  cfg.gridDim = dim3(std::min(tiles, sms));                 // persistent: each CTA walks tiles blockIdx.x + i gridDim.x
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = tc::pdl_mode() ? 1 : 0;
-  OG_CUDA(cudaLaunchKernelEx(&cfg, linear_sm90_kernel<Args>, ma, ma2, mh, ml, a));
-  launch_counter()++;
-  return OG_OK;
+  // persistent: each CTA walks tiles blockIdx.x + i gridDim.x
+  return tc::pdl_launch(linear_sm90_kernel<Args>, dim3(std::min(tiles, sms)), dim3(THREADS), C::SMEM_BYTES, stream, ma, ma2, mh, ml, a);
 }
+// The two operand forms, instantiated next to the template: where the kernels sit in the binary (and so a cuobjdump -sass
+// comparison of two builds) does not depend on where the host code first launches them.
+template int linear_sm90_launch(const TcLinearArgs&, const float*, const float*, int64_t, int64_t, cudaStream_t);
+template int linear_sm90_launch(const F16LinearArgs&, const __half*, const __half*, int64_t, int64_t, cudaStream_t);
 
 // Bhi/Blo: [b_total_rows, K] row-major fp32 (tf32-exact values), row stride ldb.  A concatenated second operand needs k1 % 32 == 0
 // (a K block comes from one of the two tensors).
-inline bool linear_tc_eligible(const TcLinearArgs& a, const float* Bhi, const float* Blo, int64_t ldb) {
+inline bool linear_sm90_eligible(const TcLinearArgs& a, const float* Bhi, const float* Blo, int64_t ldb) {
   const int K = a.k1 + a.k2;
   return K >= 32 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && al16(a.A) &&
          (!a.A2 || (a.k1 % 32 == 0 && a.lda2 % 4 == 0 && a.strideA2 % 4 == 0 && al16(a.A2))) && ldb % 4 == 0 && al16(Bhi) && al16(Blo);
 }
-inline int linear_tc_launch(const TcLinearArgs& a, const float* Bhi, const float* Blo, int64_t ldb, int64_t b_total_rows, cudaStream_t stream) {
-  return linear_sm90_launch(a, Bhi, Blo, ldb, b_total_rows, stream);
-}
 
-inline bool linear_f16_eligible(const F16LinearArgs& a, const __half* Bh, const __half* Bl, int64_t ldb) {
+inline bool linear_sm90_eligible(const F16LinearArgs& a, const __half* Bh, const __half* Bl, int64_t ldb) {
   const int K = a.k1 + a.k2;
   if (!(K >= 64 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && al16(a.A) && ldb % 8 == 0 && al16(Bh) && al16(Bl))) return false;
   if (a.A2 && (a.k1 % 32 != 0 || a.lda2 % 4 != 0 || a.strideA2 % 4 != 0 || !al16(a.A2))) return false;
@@ -526,9 +515,6 @@ inline bool linear_f16_eligible(const F16LinearArgs& a, const __half* Bh, const 
   if (a.Yh && !(a.Yl && a.ldy % 2 == 0 && a.strideY % 2 == 0 && al16(a.Yh) && al16(a.Yl) && !a.R && a.scale_out)) return false;
   if (a.Yth && !(a.Ytl && !a.R && (a.scale_out || a.scale_out_v))) return false;
   return true;
-}
-inline int linear_f16_launch(const F16LinearArgs& a, const __half* Bh, const __half* Bl, int64_t ldb, int64_t b_total_rows, cudaStream_t stream) {
-  return linear_sm90_launch(a, Bh, Bl, ldb, b_total_rows, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

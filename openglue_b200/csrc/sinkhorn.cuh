@@ -457,11 +457,7 @@ template <int V, int W, int SLOTS>
 inline int sinkhorn_launch_v(SinkArgs a, const SinkPlan& p, cudaStream_t stream) {
   constexpr size_t smem_max = sinkhorn_smem<V, W, SLOTS>(128 * V * W + 4);     // largest request of this instantiation: m = 128 V W
   static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "sinkhorn_kernel: shared memory beyond what one block may opt in to");
-  static DeviceFlags attr_set;
-  if (attr_set.pending()) {
-    OG_CUDA(cudaFuncSetAttribute(sinkhorn_kernel<V, W, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-    attr_set.mark();
-  }
+  if (const int rc = smem_opt_in<sinkhorn_kernel<V, W, SLOTS>>((int)smem_max)) return rc;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.B * a.SP);
   cfg.blockDim = dim3(SINK_WARPS * 32);

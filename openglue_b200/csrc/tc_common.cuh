@@ -98,6 +98,22 @@ inline int& pdl_mode() {
   static int v = [] { const char* e = getenv("OG_PDL"); return e ? atoi(e) : 1; }();
   return v;
 }
+// kernel<<<grid, block, smem, stream>>>(args...), as a programmatic dependent launch unless pdl_mode() is 0
+template <class... Params, class... Args>
+inline int pdl_launch(void (*kernel)(Params...), dim3 grid, dim3 block, int smem, cudaStream_t stream, const Args&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl_mode() ? 1 : 0;
+  OG_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
+  launch_counter()++;
+  return OG_OK;
+}
 
 // ----------------------------------------------------------------------------- warp specialization
 // setmaxnreg moves registers between the warpgroups of a CTA (every warp of the warpgroup executes it; N a multiple of 8 in

@@ -208,7 +208,7 @@ def test_attention_f16_many_tiles(B, H, nq, nk, pair):
 @pytest.mark.gpu
 @pytest.mark.parametrize('batch,n,m', [(2, 330, 197), (1, 256, 256), (3, 64, 1)])
 def test_fused_projections_are_bit_identical(batch, n, m):
-    """One launch over the stacked Q | K | V (self) or K | V (cross) weights (linear_f16.cuh OUTK 4) computes the same tiles with the
+    """One launch over the stacked Q | K | V (self) or K | V (cross) weights (linear_sm90.cuh, F16LinearArgs::nkinds) computes the same tiles with the
     same arithmetic as one launch per projection: the whole path's outputs must not change by a single bit."""
     import torch
     from openglue_b200 import SuperGlue, _cabi
