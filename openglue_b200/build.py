@@ -32,19 +32,6 @@ def _stale() -> bool:
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_variant(out: str, defines: list[str]) -> str:
-    """A/B build: the same sources with extra -D switches into another file (load it with OG_LIB=<path>)."""
-    flags = [f for f in NVCC_FLAGS if f != '--use_fast_math=false']
-    cmd = [_nvcc(), *flags, *[f'-D{d}' for d in defines], '-o', out, *[os.path.join(CSRC, s) for s in SOURCES], '-lcudart']
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError(f'nvcc failed ({res.returncode}): {" ".join(cmd)}')
-    with open(out + '.log', 'w') as f:
-        f.write(' '.join(cmd) + '\n' + res.stdout + res.stderr)
-    return out
-
-
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not _stale():
         return LIB
@@ -61,8 +48,4 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 
 if __name__ == '__main__':
-    if '--variant' in sys.argv:                     # python -m openglue_b200.build --variant out.so DEFINE=1 DEFINE2=0 ...
-        i = sys.argv.index('--variant')
-        print(build_variant(sys.argv[i + 1], sys.argv[i + 2:]))
-        sys.exit(0)
     print(build(force='--force' in sys.argv, verbose='--verbose' in sys.argv))

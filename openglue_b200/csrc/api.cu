@@ -303,13 +303,6 @@ int og_split_tf32(const float* src, float* hi, float* lo, int64_t n, void* strea
   return OG_OK;
 }
 
-#ifdef OG_TRACE
-int og_trace_read(long long* host_out) {     // debug build only
-  OG_CUDA(cudaMemcpyFromSymbol(host_out, og_trace_buf, sizeof(long long) * 2 * 16 * 256));
-  return OG_OK;
-}
-#endif
-
 int og_attention_fwd(const float* q, int64_t ldq, int64_t strideq, const float* k, int64_t ldk, int64_t stridek,
                      const float* v, int64_t ldv, int64_t stridev, float* out, int64_t ldo, int64_t strideo,
                      int batch, int nq, int nk, int num_heads, int head_dim, int precision, void* stream) {

@@ -7,13 +7,6 @@
 #include "../../include/openglue_b200.h"
 
 namespace og {
-#ifdef OG_TRACE
-// debug build only (-DOG_TRACE, read back with og_trace_read): event timestamps of CTAs 0 and 1
-__device__ long long og_trace_buf[2 * 16 * 256];
-#define OG_TRACE_EVT(ev, idx) do { if (blockIdx.x < 2 && blockIdx.y == 0 && blockIdx.z == 0 && (idx) < 256) og_trace_buf[blockIdx.x * 4096 + (ev) * 256 + (idx)] = clock64(); } while (0)
-#else
-#define OG_TRACE_EVT(ev, idx) do { } while (0)
-#endif
 
 // thread-local error message (og_last_error)
 inline char* err_buf() { static thread_local char buf[512] = {0}; return buf; }

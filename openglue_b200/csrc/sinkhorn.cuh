@@ -18,15 +18,20 @@
 // warp -> CTA (shared memory) -> grid (per-strip partials in global memory, double buffered),
 // with one grid-wide barrier per iteration; every CTA of a pair then rebuilds v redundantly
 // in a fixed order (deterministic, no atomics on data).
+//
+// The backward pass (sinkhorn_bwd.cuh) sweeps the same strips in the same way, so the pieces both kernels are made of live
+// here: the strip geometry (SinkStrip), the bulk-copy row ring (SinkRowRing), the exchange among the warps of a row
+// (sink_row_exchange), the column reduction (sink_column_reduce), the plan (band table, occupancy, strips) and the launcher.
 #pragma once
 #include "common.cuh"
+#include "tc_common.cuh"
 #include <math_constants.h>
 #include <algorithm>
-#include <stdlib.h>
 
 namespace og {
 
 struct SinkArgs {
+  static constexpr bool kBackward = false;
   const float* S; int64_t lds, strideS;
   const float* dustbin;
   int B, n, m, iters;
@@ -39,12 +44,12 @@ struct SinkArgs {
   int SP, rows_per_strip, mpad;
   float* hist_u;                         // optional [B][iters][n+1]: u_t of every iteration  (kept for the backward pass,
   float* hist_v;                         // optional [B][iters+1][m+1]: v_t, row 0 = v_0 = 0   csrc/sinkhorn_bwd.cuh)
-  int res_q16;                           // fraction (Q16) of the rows that are loaded with the L2 evict_last policy (see sink_policy)
-  int pf_rows;                           // L2 prefetch distance beyond the ring, in rows of a group (0 = off)
 };
 
 constexpr int SINK_WARPS = 8;
 constexpr int64_t SINK_BARRIER_BYTES = 256 * 128;     // one 128-byte line per pair of a launch (<= SM count pairs)
+constexpr int SINK_MAX_COLS = 8192;
+constexpr int SINK_MAX_STRIPS = 32;                    // strips per pair at most (the strip-partial workspace is sized for it)
 constexpr float LOG2E_F = 1.4426950408889634f;
 
 __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int target) {
@@ -59,48 +64,6 @@ __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int
     __threadfence();
   }
   __syncthreads();
-}
-
-// --- shared-memory row ring fed by bulk async copies (TMA 1-D): decouples HBM latency from the math ---
-
-__device__ __forceinline__ uint32_t sink_smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void sink_mbar_init(uint64_t* bar) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sink_smem_u32(bar)) : "memory");
-}
-// L2 residency: the score matrix is read `iters` + 1 times and never written, but at the headline shape (16 pairs x 2048^2 x 4 B
-// = 268 MB) it is five times the 50 MB L2, and with plain LRU-like replacement a cyclic sweep over it hits nothing.  So a FIXED subset - the first res_rows rows of every strip, ~RES_MB in total - is loaded with
-// the evict_last policy and everything else with evict_first: the subset stays in L2 across the iterations and only the rest
-// streams from HBM.  The subset is INTERLEAVED with the streamed rows (round k of a strip is kept iff floor((k+1) f) != floor(k f)):
-// with a contiguous block of resident rows every CTA would sit in its L2 phase at the same time and leave HBM idle, then all
-// stream together.  The final pass reads every row with evict_first, which hands
-// the lines back to the kernels that follow.
-__device__ __forceinline__ uint64_t sink_policy(bool keep) {
-  uint64_t p;
-  if (keep) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  else      asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void sink_row_copy(float* dst, const float* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sink_smem_u32(bar)), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-               ::"r"(sink_smem_u32(dst)), "l"(src), "r"(bytes), "r"(sink_smem_u32(bar)), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void sink_row_copy(float* dst, const float* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sink_smem_u32(bar)), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(sink_smem_u32(dst)), "l"(src), "r"(bytes), "r"(sink_smem_u32(bar)) : "memory");
-}
-// L2 prefetch of a row segment that the ring will ask for a few rows later: the 2-deep ring covers ~2 row times, about the loaded
-// HBM latency; a segment that is already in L2 when its bulk copy is issued arrives in a fraction of that
-__device__ __forceinline__ void sink_row_prefetch(const float* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void sink_mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok = 0;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(sink_smem_u32(bar)), "r"(parity) : "memory");
-  } while (!ok);
 }
 
 // fp32 pairs: Hopper has no packed fp32 arithmetic, so each pair operation is two scalar round-to-nearest operations (the
@@ -124,144 +87,232 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
 }
 
 // V: float4s per lane of a warp's column segment (C = 128 V columns);  W: warps that share one row (a row group covers
-// W C columns; the warps exchange (max, sum) of their segments through shared memory and one named barrier per row);
-// SLOTS: ring depth per warp.  Configurations with V <= 8 need <= 128 registers and <= 106 KB of shared memory: two CTAs
-// per SM, so one CTA streams while the other sits in its per-iteration reduction / barrier phase.
+// W C columns; the warps exchange what they know of their segments through shared memory and one named barrier per row);
+// G = SINK_WARPS / W row groups = rows in progress per CTA.  A warp works on rows r0 + grp, r0 + grp + G, ... of its strip
+// [r0, r1) (row n is the dustbin row), columns [c0, c0 + C) of each.
+template <int V, int W>
+struct SinkStrip {
+  static constexpr int C = 128 * V, MC = W * C, G = SINK_WARPS / W;
+  int b, strip, tid, lane, grp, sub, c0, r0, r1;
+  template <class Args>
+  __device__ __forceinline__ explicit SinkStrip(const Args& a) {
+    b = blockIdx.x / a.SP; strip = blockIdx.x % a.SP;
+    tid = threadIdx.x; lane = tid & 31;
+    grp = (tid >> 5) / W; sub = (tid >> 5) % W;
+    c0 = sub * C;
+    r0 = strip * a.rows_per_strip;
+    r1 = min(r0 + a.rows_per_strip, a.n + 1);
+  }
+};
+
+// One warp's slice of the shared-memory row ring, fed by bulk async copies (TMA 1-D) so that HBM latency overlaps the math of
+// the rows before: SLOTS segments of C floats, one mbarrier each.  Every sweep visits the warp's rows in the same order;
+// `consumed` counts the real rows taken so far and gives each its slot and phase.  EVICT_FIRST loads with the L2 evict_first
+// policy (the forward pass): at the headline shape the score matrix is five times the 50 MB L2 and is swept cyclically, so
+// its lines would hit nothing and only push out those of the kernels that follow.
+template <int V, int W, int SLOTS, bool EVICT_FIRST, class Args>
+struct SinkRowRing {
+  static constexpr int C = 128 * V, G = SINK_WARPS / W;
+  float* slot;                                         // [SLOTS][C]
+  uint64_t* bar;                                       // [SLOTS]
+  const Args& a;
+  const float* seg;                                    // this warp's column segment of row 0 of the pair
+  int first, end_real, c0, lane;                       // first row of the warp; rows >= end_real do not exist in memory
+  uint32_t bytes, consumed;                            // bytes of a segment: 0 when it lies beyond the last column
+  bool full;                                           // the whole segment lies inside the row (warp-uniform)
+  float dz;                                            // the dustbin score divided by reg, Z = M / reg
+  uint64_t policy;
+
+  __device__ __forceinline__ SinkRowRing(const Args& args, const SinkStrip<V, W>& s, float* ring, uint64_t* bars) : a(args) {
+    const int warp = s.grp * W + s.sub;
+    slot = ring + warp * SLOTS * C;
+    bar = bars + warp * SLOTS;
+    seg = a.S + (int64_t)s.b * a.strideS + s.c0;
+    first = s.r0 + s.grp;
+    end_real = min(s.r1, a.n);
+    c0 = s.c0; lane = s.lane;
+    const int seg_cols = min(a.m, c0 + C) - c0;        // <= 0: this warp's segment lies beyond the last column
+    bytes = seg_cols > 0 ? (uint32_t)(((seg_cols + 3) / 4) * 16) : 0u;     // <= 4 * (lds - c0): inside the padded row
+    full = seg_cols == C;
+    consumed = 0;
+    dz = (a.reg == 1.0f) ? __ldg(a.dustbin) : __fdiv_rn(__ldg(a.dustbin), a.reg);
+    if (lane == 0) {
+      for (int sl = 0; sl < SLOTS; ++sl) tc::mbar_init(&bar[sl], 1);
+      tc::fence_barrier_init();
+    }
+    if (EVICT_FIRST) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(policy));
+  }
+
+  __device__ __forceinline__ void copy(uint32_t sl, int row) {
+    tc::mbar_arrive_expect_tx(&bar[sl], bytes);
+    const float* src = seg + (int64_t)row * a.lds;
+    if (EVICT_FIRST)
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                   ::"r"(tc::smem_u32(slot + sl * C)), "l"(src), "r"(bytes), "r"(tc::smem_u32(&bar[sl])), "l"(policy) : "memory");
+    else
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                   ::"r"(tc::smem_u32(slot + sl * C)), "l"(src), "r"(bytes), "r"(tc::smem_u32(&bar[sl])) : "memory");
+  }
+
+  // Starts the copies of the first SLOTS rows of the next sweep.  Called only when a sweep follows: copies nobody waits for
+  // could still be writing into shared memory when the CTA exits.
+  __device__ __forceinline__ void prime() {
+    if (lane == 0 && bytes) {
+      for (int sl = 0; sl < SLOTS; ++sl) {
+        const int row = first + sl * G;
+        if (row < end_real) copy((consumed + sl) % SLOTS, row);
+      }
+    }
+  }
+
+  // This warp's segment of row `row` in registers (columns >= m zero, divided by reg), and the slot refilled with the row SLOTS
+  // ahead.  The dustbin row is the constant dustbin score.
+  __device__ __forceinline__ void take(int row, float4 (&z)[V]) {
+    if (row >= a.n) {
+#pragma unroll
+      for (int k = 0; k < V; ++k) z[k] = make_float4(dz, dz, dz, dz);
+      return;
+    }
+    if (!bytes) {
+#pragma unroll
+      for (int k = 0; k < V; ++k) z[k] = make_float4(0.f, 0.f, 0.f, 0.f);     // the kernels mask these columns
+      return;
+    }
+    const uint32_t sl = consumed % SLOTS, ph = (consumed / SLOTS) & 1;
+    while (!tc::mbar_try_wait(&bar[sl], ph)) {}
+    const float4* src = reinterpret_cast<const float4*>(slot + sl * C);
+    if (full) {                                        // no masks (the common case)
+#pragma unroll
+      for (int k = 0; k < V; ++k) z[k] = src[lane + 32 * k];
+    } else {
+#pragma unroll
+      for (int k = 0; k < V; ++k) {
+        const int idx = lane + 32 * k;
+        const int c = c0 + 4 * idx;
+        const int m = a.m;
+        float4 q = (c < m) ? src[idx] : make_float4(0.f, 0.f, 0.f, 0.f);
+        if (c < m && c + 3 >= m) {                     // the float4 that straddles column m: its tail is row padding (any bits)
+          if (c + 1 >= m) q.y = 0.f;
+          if (c + 2 >= m) q.z = 0.f;
+          q.w = 0.f;
+        }
+        z[k] = q;
+      }
+    }
+    ++consumed;
+    __syncwarp();                                      // every lane has its part of the row in registers
+    const int nxt = row + SLOTS * G;
+    if (lane == 0 && nxt < end_real) copy(sl, nxt);
+    if (a.reg != 1.0f) {
+      const float reg = a.reg;
+#pragma unroll
+      for (int k = 0; k < V; ++k) {
+        z[k].x = __fdiv_rn(z[k].x, reg); z[k].y = __fdiv_rn(z[k].y, reg);
+        z[k].z = __fdiv_rn(z[k].z, reg); z[k].w = __fdiv_rn(z[k].w, reg);
+      }
+    }
+  }
+};
+
+// The W warps of a row group publish one value each (`mine`) and meet at the group's named barrier; the returned W values are
+// in warp order, the same in every warp.  The buffer xr [2][G][W] alternates halves row by row (rowpar), so a warp that runs
+// ahead into the next row cannot overwrite values another warp has yet to read.
+template <int V, int W, class X>
+__device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkStrip<V, W>& s, uint32_t& rowpar) {
+  X* x = xr + (rowpar * SinkStrip<V, W>::G + s.grp) * W;
+  if (s.lane == 0) x[s.sub] = mine;
+  asm volatile("bar.sync %0, %1;" ::"r"(1 + s.grp), "n"(W * 32) : "memory");
+  rowpar ^= 1u;
+  return x;
+}
+
+// Column sums of sweep `k` (0, 1, ... in launch order): warp (cacc: this warp's segment; cacc_m: the dustbin column, counted by
+// segment 0) -> CTA (red [G][mpad]: the row groups' warps own disjoint columns of their row) -> this strip's partial in global
+// memory (buffer k & 1 of two) -> barrier among the SP CTAs of the pair -> every CTA of the pair rebuilds the sums in the same
+// fixed order (bitwise identical across CTAs) and calls update(j, sum) for j < m and update(MC, sum) for the dustbin column.
+template <int V, int W, class Args, class Update>
+__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
+                                                   float cacc_m, int k, Update update) {
+  const int m = a.m;
+  float* myred = red + s.grp * a.mpad;
+#pragma unroll
+  for (int q = 0; q < V; ++q) {
+    const int c = s.c0 + 4 * (s.lane + 32 * q);
+    if (c < m) *reinterpret_cast<float4*>(myred + c) = cacc[q];     // entries >= m are zero
+  }
+  __syncthreads();                                    // (a) all float4 column sums are in `red`
+  if (s.sub == 0 && s.lane == 0) myred[m] = cacc_m;   // column m = dustbin column (may overlap a float4 tail)
+  __syncthreads();
+  const int64_t buf = (int64_t)(k & 1) * a.B * a.SP + (int64_t)s.b * a.SP;
+  float* part = a.partial + (buf + s.strip) * a.mpad;
+  for (int j = s.tid; j <= m; j += blockDim.x) {
+    float sum = 0.f;
+#pragma unroll
+    for (int w = 0; w < SinkStrip<V, W>::G; ++w) sum += red[w * a.mpad + j];
+    part[j] = sum;
+  }
+  // only the SP CTAs of this pair exchange data: a per-pair barrier (own 128-byte line) lets the pairs drift apart,
+  // so HBM keeps streaming for the other pairs while one pair sits in its reduction / barrier phase
+  grid_barrier(a.barrier + 32 * s.b, (unsigned int)(k + 1) * (unsigned int)a.SP);
+  const float* pb = a.partial + buf * a.mpad;
+  // float4 columns, all SP loads of a thread in flight together (this phase is pure L2 latency: every CTA of the pair waits on it)
+  for (int j4 = s.tid; 4 * j4 <= m; j4 += blockDim.x) {
+    float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 8
+    for (int sp = 0; sp < a.SP; ++sp) {
+      const float4 q = __ldcg(reinterpret_cast<const float4*>(pb + (int64_t)sp * a.mpad) + j4);
+      c.x += q.x; c.y += q.y; c.z += q.z; c.w += q.w;
+    }
+    const float cc[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int j = 4 * j4 + e;
+      if (j < m) update(j, cc[e]);
+      else if (j == m) update(SinkStrip<V, W>::MC, cc[e]);
+    }
+  }
+  __syncthreads();
+}
+
+// SLOTS: ring depth per warp.  Configurations with V <= 8 need <= 128 registers and <= 106 KB of shared memory: two CTAs per
+// SM, so one CTA streams while the other sits in its per-iteration reduction / barrier phase.
 template <int V, int W, int SLOTS>
 __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_kernel(SinkArgs a) {
   extern __shared__ __align__(128) float og_sink_smem[];
-  constexpr int C = 128 * V;                           // columns of one warp's segment = floats per ring slot
-  constexpr int MC = W * C;                            // columns a row group covers (m <= MC)
-  constexpr int G = SINK_WARPS / W;                    // row groups = rows in progress per CTA
+  using Strip = SinkStrip<V, W>;
+  constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G;
   float* v_s = og_sink_smem;                           // [MC + 4]  v_j for j < m, -inf for m <= j < MC (masks the padding
                                                        //           columns in the sweep without per-element selects), v_s[MC] = v_dustbin
   float* red = og_sink_smem + MC + 4;                  // [G][mpad]
   float* ring = red + G * a.mpad;                      // [SINK_WARPS][SLOTS][C]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);   // [SINK_WARPS][SLOTS]
   float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS * SLOTS);             // [2][G][W] (max, sum) of a segment
-  const int b = blockIdx.x / a.SP, strip = blockIdx.x % a.SP;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int grp = warp / W, sub = warp % W;
-  const int c0 = sub * C;                              // first column of this warp's segment
-  const int n = a.n, m = a.m;
-  const int r0 = strip * a.rows_per_strip;
-  const int r1 = min(r0 + a.rows_per_strip, n + 1);
-  const int r1_real = min(r1, n);                      // rows that exist in memory (the dustbin row does not)
-  const float* __restrict__ Sb = a.S + (int64_t)b * a.strideS;
-  const bool unit_reg = (a.reg == 1.0f);
-  const float dz = unit_reg ? __ldg(a.dustbin) : __fdiv_rn(__ldg(a.dustbin), a.reg);   // Z = M / reg
+  const Strip s(a);
+  const int n = a.n, m = a.m, c0 = s.c0, lane = s.lane, sub = s.sub;
   const float a_reg = expf(a.norm), a_last = expf(a.log_a_last);
-  const int seg_cols = min(m, c0 + C) - c0;            // <= 0: this warp's segment lies beyond the last column
-  const bool has_seg = seg_cols > 0;
-  const bool seg_full = seg_cols == C;                 // warp-uniform
-  const uint32_t seg_bytes = has_seg ? (uint32_t)(((seg_cols + 3) / 4) * 16) : 0u;     // <= 4 * (lds - c0): inside the padded row
-  float* my_ring = ring + warp * SLOTS * C;
-  uint64_t* my_bars = bars + warp * SLOTS;
+  SinkRowRing<V, W, SLOTS, true, SinkArgs> rows(a, s, ring, bars);
+  const float dz = rows.dz;
 
-  if (lane == 0) {
-    for (int sl = 0; sl < SLOTS; ++sl) sink_mbar_init(&my_bars[sl]);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  for (int j = tid; j < MC; j += blockDim.x) v_s[j] = (j < m) ? 0.f : -CUDART_INF_F;
-  if (tid == 0) v_s[MC] = 0.f;
+  for (int j = s.tid; j < MC; j += blockDim.x) v_s[j] = (j < m) ? 0.f : -CUDART_INF_F;
+  if (s.tid == 0) v_s[MC] = 0.f;
   __syncthreads();
 
-  uint32_t issued = 0, consumed = 0;                   // per-warp ring counters (real rows only)
-  const uint64_t pol_keep = sink_policy(true), pol_stream = sink_policy(false);
-  auto keep_row = [&](int row) {                       // does this row belong to the L2-resident subset?
-    const uint32_t k = (uint32_t)(row - r0) / (uint32_t)G;
-    return ((k + 1) * (uint32_t)a.res_q16 >> 16) != (k * (uint32_t)a.res_q16 >> 16);
-  };
-  bool last_sweep = (a.iters == 0);                    // the sweep being FETCHED is the final pass (set below)
-  auto prefetch_first = [&]() {                        // first SLOTS rows of this warp's group
-    if (lane == 0 && has_seg) {
-      for (int sl = 0; sl < SLOTS; ++sl) {
-        const int row = r0 + grp + sl * G;
-        if (row < r1_real) {
-          sink_row_copy(my_ring + (issued % SLOTS) * C, Sb + (int64_t)row * a.lds + c0, seg_bytes, &my_bars[issued % SLOTS],
-                        (!last_sweep && keep_row(row)) ? pol_keep : pol_stream);
-          ++issued;
-        }
-      }
-      for (int sl = SLOTS; sl < SLOTS + a.pf_rows; ++sl) {
-        const int row = r0 + grp + sl * G;
-        if (row < r1_real) sink_row_prefetch(Sb + (int64_t)row * a.lds + c0, seg_bytes);
-      }
-    }
-  };
-  // fetch this warp's segment of row `row` into registers (float4 k = pairs 2k, 2k+1); refill the slot with the row SLOTS ahead
-  auto take_row = [&](int row, f32x2 (&z)[2 * V]) {
-    if (row < n) {
-      if (has_seg) {
-        const uint32_t sl = consumed % SLOTS, ph = (consumed / SLOTS) & 1;
-        sink_mbar_wait(&my_bars[sl], ph);
-        const ulonglong2* src = reinterpret_cast<const ulonglong2*>(my_ring + sl * C);
-        if (seg_full) {                                // the whole segment lies inside the row: no masks (the common case)
-#pragma unroll
-          for (int k = 0; k < V; ++k) { const ulonglong2 q = src[lane + 32 * k]; z[2 * k] = q.x; z[2 * k + 1] = q.y; }
-        } else {
-#pragma unroll
-          for (int k = 0; k < V; ++k) {
-            const int idx = lane + 32 * k;
-            const int c = c0 + 4 * idx;
-            float4 q = (c < m) ? reinterpret_cast<const float4*>(src)[idx] : make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c < m && c + 3 >= m) {                 // the float4 that straddles column m: its tail is row padding (any bits)
-              if (c + 1 >= m) q.y = 0.f;
-              if (c + 2 >= m) q.z = 0.f;
-              q.w = 0.f;
-            }
-            z[2 * k] = pk2(q.x, q.y); z[2 * k + 1] = pk2(q.z, q.w);
-          }
-        }
-        ++consumed;
-        __syncwarp();                                  // every lane has its part of the row in registers
-        const int nxt = row + SLOTS * G;
-        if (lane == 0 && nxt < r1_real) {
-          sink_row_copy(my_ring + sl * C, Sb + (int64_t)nxt * a.lds + c0, seg_bytes, &my_bars[sl],
-                        (!last_sweep && keep_row(nxt)) ? pol_keep : pol_stream);
-          ++issued;
-        }
-        const int pfr = nxt + a.pf_rows * G;
-        if (lane == 0 && a.pf_rows > 0 && pfr < r1_real) sink_row_prefetch(Sb + (int64_t)pfr * a.lds + c0, seg_bytes);
-        if (!unit_reg) {
-#pragma unroll
-          for (int k = 0; k < 2 * V; ++k) {
-            float x, y; upk2(z[k], x, y);
-            z[k] = pk2(__fdiv_rn(x, a.reg), __fdiv_rn(y, a.reg));
-          }
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 2 * V; ++k) z[k] = 0ull;   // masked through v = -inf
-      }
-    } else {                                           // the dustbin row is the constant dustbin score
-#pragma unroll
-      for (int k = 0; k < 2 * V; ++k) z[k] = pk2(dz, dz);
-    }
-  };
-
-  prefetch_first();
+  rows.prime();
   uint32_t rowpar = 0;                                 // parity of the exchange buffer (alternates per row of the group)
   const f32x2 log2e2 = pk2(LOG2E_F, LOG2E_F);
   for (int it = 0; it < a.iters; ++it) {
-    if (tid == 0) OG_TRACE_EVT(0, it);
     f32x2 cacc[2 * V];
 #pragma unroll
     for (int k = 0; k < 2 * V; ++k) cacc[k] = 0ull;
     float cacc_m = 0.f;
     const float v_m = v_s[MC];
 
-    for (int row = r0 + grp; row < r1; row += G) {
+    for (int row = s.r0 + s.grp; row < s.r1; row += G) {
+      float4 q[V];
+      rows.take(row, q);
       f32x2 z[2 * V];
-#ifdef OG_TRACE
-      const int tr = (it == 20 && tid == 0) ? (row - r0) / G : 1 << 20;     // row timeline of warp 0 in iteration 20
-#define OG_SINK_ROW_EVT(e) OG_TRACE_EVT(e, tr)
-#else
-#define OG_SINK_ROW_EVT(e) do { } while (0)
-#endif
-      OG_SINK_ROW_EVT(5);
-      take_row(row, z);
-      OG_SINK_ROW_EVT(6);
+#pragma unroll
+      for (int k = 0; k < V; ++k) { z[2 * k] = pk2(q[k].x, q[k].y); z[2 * k + 1] = pk2(q[k].z, q[k].w); }
       // t = z + v, masked; maximum over this warp's segment (the dustbin column entry belongs to segment 0)
       const float t_m = dz + v_m;
       float mx = (sub == 0) ? t_m : -CUDART_INF_F;
@@ -273,7 +324,6 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
         mx = fmaxf(mx, fmaxf(fmaxf(x0, x1), fmaxf(x2, x3)));
       }
       mx = warp_max(mx);
-      OG_SINK_ROW_EVT(7);
       const float mxs = (mx == -CUDART_INF_F) ? 0.f : mx;               // an all-padding segment: e = 2^-inf = 0, not NaN
       const f32x2 mxs2 = pk2(mxs, mxs);
       f32x2 sum2a = 0ull, sum2b = 0ull;
@@ -286,12 +336,9 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
       float sa, sb; upk2(add2(sum2a, sum2b), sa, sb);
       const float e_m = (sub == 0) ? ex2_approx((t_m - mxs) * LOG2E_F) : 0.f;
       float s_i = warp_sum(sa + sb) + e_m;
-      OG_SINK_ROW_EVT(8);
       float mxg = mx, f_w = 1.f;
       if (W > 1) {                                     // combine the segments of the row: S = sum_w S_w 2^(mx_w - mx)
-        float2* x = xr + (rowpar * G + grp) * W;
-        if (lane == 0) x[sub] = make_float2(mx, s_i);
-        asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "n"(W * 32) : "memory");
+        const float2* x = sink_row_exchange(xr, make_float2(mx, s_i), s, rowpar);
         float2 p[W];
 #pragma unroll
         for (int w2 = 0; w2 < W; ++w2) { p[w2] = x[w2]; mxg = fmaxf(mxg, p[w2].x); }
@@ -299,94 +346,52 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
 #pragma unroll
         for (int w2 = 0; w2 < W; ++w2) s_i = fmaf(p[w2].y, ex2_approx((p[w2].x - mxg) * LOG2E_F), s_i);   // fixed order: identical in every warp
         f_w = ex2_approx((mx - mxg) * LOG2E_F);
-        rowpar ^= 1u;
       }
-      OG_SINK_ROW_EVT(9);
       const float w_i = __fdiv_rn((row < n) ? a_reg : a_last, s_i) * f_w;
       if ((it == a.iters - 1 || a.hist_u) && sub == 0 && lane == 0) {
         const float u_i = ((row < n) ? a.norm : a.log_a_last) - (mxg + logf(s_i));
-        if (it == a.iters - 1) a.u[(int64_t)b * (n + 1) + row] = u_i;
-        if (a.hist_u) a.hist_u[((int64_t)b * a.iters + it) * (n + 1) + row] = u_i;
+        if (it == a.iters - 1) a.u[(int64_t)s.b * (n + 1) + row] = u_i;
+        if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (n + 1) + row] = u_i;
       }
       const f32x2 w2 = pk2(w_i, w_i);
 #pragma unroll
       for (int k = 0; k < 2 * V; ++k) cacc[k] = fma2(z[k], w2, cacc[k]);
       cacc_m = fmaf(e_m, w_i, cacc_m);
-      OG_SINK_ROW_EVT(10);
     }
-    if (tid == 0) OG_TRACE_EVT(1, it);
-    last_sweep = (it == a.iters - 1);
-    prefetch_first();                                 // next sweep's (or the final pass's) first rows fly during the reduction
-    // warp -> CTA: a row group's warps own disjoint column segments of red[grp]
-    float* myred = red + grp * a.mpad;
+    rows.prime();                                      // next sweep's (or the final pass's) first rows fly during the reduction
+    float4 c4[V];
 #pragma unroll
-    for (int k = 0; k < V; ++k) {
-      const int c = c0 + 4 * (lane + 32 * k);
-      if (c < m) *reinterpret_cast<ulonglong2*>(myred + c) = make_ulonglong2(cacc[2 * k], cacc[2 * k + 1]);   // entries >= m are zero
-    }
-    __syncthreads();                                  // (a) all float4 column sums are in `red`
-    if (sub == 0 && lane == 0) myred[m] = cacc_m;     // column m = dustbin column (may overlap a float4 tail)
-    __syncthreads();
-    float* part = a.partial + ((int64_t)(it & 1) * a.B * a.SP + (int64_t)b * a.SP + strip) * a.mpad;
-    for (int j = tid; j <= m; j += blockDim.x) {
-      float s = 0.f;
-#pragma unroll
-      for (int w = 0; w < G; ++w) s += red[w * a.mpad + j];
-      part[j] = s;
-    }
-    // only the SP CTAs of this pair exchange data: a per-pair barrier (own 128-byte line) lets the pairs drift apart,
-    // so HBM keeps streaming for the other pairs while one pair sits in its reduction / barrier phase
-    if (tid == 0) OG_TRACE_EVT(2, it);
-    grid_barrier(a.barrier + 32 * b, (unsigned int)(it + 1) * (unsigned int)a.SP);
-    if (tid == 0) OG_TRACE_EVT(3, it);
-    // every CTA of the pair rebuilds v (fixed summation order => bitwise identical across CTAs)
-    const float* pb = a.partial + ((int64_t)(it & 1) * a.B * a.SP + (int64_t)b * a.SP) * a.mpad;
-    // float4 columns, all SP loads of a thread in flight together (this phase is pure L2 latency: every CTA of the pair waits on it)
-    for (int j4 = tid; 4 * j4 <= m; j4 += blockDim.x) {
-      float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 8
-      for (int s = 0; s < a.SP; ++s) {
-        const float4 q = __ldcg(reinterpret_cast<const float4*>(pb + (int64_t)s * a.mpad) + j4);
-        c.x += q.x; c.y += q.y; c.z += q.z; c.w += q.w;
-      }
-      const float cc[4] = {c.x, c.y, c.z, c.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int j = 4 * j4 + e;
-        if (j < m) v_s[j] = a.norm + v_s[j] - logf(cc[e]);
-        else if (j == m) v_s[MC] = a.log_b_last + v_s[MC] - logf(cc[e]);
-      }
-    }
-    __syncthreads();
-    if (tid == 0) OG_TRACE_EVT(4, it);
-    if (a.hist_v && strip == 0) {                     // every CTA of the pair holds the same v: one of them records it
-      float* hv = a.hist_v + ((int64_t)b * (a.iters + 1) + it + 1) * (m + 1);
-      for (int j = tid; j <= m; j += blockDim.x) hv[j] = (j < m) ? v_s[j] : v_s[MC];
+    for (int k = 0; k < V; ++k) { upk2(cacc[2 * k], c4[k].x, c4[k].y); upk2(cacc[2 * k + 1], c4[k].z, c4[k].w); }
+    sink_column_reduce(a, s, red, c4, cacc_m, it, [&](int j, float c) {
+      v_s[j] = ((j < MC) ? a.norm : a.log_b_last) + v_s[j] - logf(c);
+    });
+    if (a.hist_v && s.strip == 0) {                   // every CTA of the pair holds the same v: one of them records it
+      float* hv = a.hist_v + ((int64_t)s.b * (a.iters + 1) + it + 1) * (m + 1);
+      for (int j = s.tid; j <= m; j += blockDim.x) hv[j] = (j < m) ? v_s[j] : v_s[MC];
     }
   }
 
   // final pass: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111)
   {
     const float v_m = v_s[MC];
-    for (int row = r0 + grp; row < r1; row += G) {
-      f32x2 zp[2 * V];
-      take_row(row, zp);
+    for (int row = s.r0 + s.grp; row < s.r1; row += G) {
+      float4 z[V];
+      rows.take(row, z);
       float u_i = 0.f;
       if (a.iters > 0) {
-        if (lane == 0) u_i = __ldcg(a.u + (int64_t)b * (n + 1) + row);
+        if (lane == 0) u_i = __ldcg(a.u + (int64_t)s.b * (n + 1) + row);
         u_i = __shfl_sync(0xffffffffu, u_i, 0);
       }
-      float* out = a.scores + ((int64_t)b * (n + 1) + row) * (m + 1);
+      float* out = a.scores + ((int64_t)s.b * (n + 1) + row) * (m + 1);
 #pragma unroll
       for (int k = 0; k < V; ++k) {
         const int c = c0 + 4 * (lane + 32 * k);
         if (c < m) {
           const float4 vv = *reinterpret_cast<const float4*>(v_s + c);
-          float z0, z1, z2, z3; upk2(zp[2 * k], z0, z1); upk2(zp[2 * k + 1], z2, z3);
-          if (c + 0 < m) out[c + 0] = (z0 + u_i) + vv.x - a.norm;
-          if (c + 1 < m) out[c + 1] = (z1 + u_i) + vv.y - a.norm;
-          if (c + 2 < m) out[c + 2] = (z2 + u_i) + vv.z - a.norm;
-          if (c + 3 < m) out[c + 3] = (z3 + u_i) + vv.w - a.norm;
+          if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - a.norm;
+          if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - a.norm;
+          if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - a.norm;
+          if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - a.norm;
         }
       }
       if (sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - a.norm;
@@ -395,69 +400,65 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
 }
 
 struct SinkPlan { int V, W, slots, occ, SP, rows_per_strip, mpad, pairs_per_launch; size_t smem; };
-constexpr int SINK_MAX_COLS = 8192;
-constexpr int SINK_L2_RESIDENT_MB = 0;   // of the 50 MB L2
-constexpr int SINK_L2_PREFETCH_ROWS = 0;
 
-template <int V, int W, int SLOTS>
-constexpr size_t sinkhorn_smem(int mpad) {
-  constexpr int C = 128 * V, G = SINK_WARPS / W;
-  return ((size_t)(W * C + 4) + (size_t)G * mpad + (size_t)SINK_WARPS * SLOTS * C) * sizeof(float) +
-         (size_t)SINK_WARPS * SLOTS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float2) + 128;
+// Dynamic shared memory of one CTA: the column vectors of MC + 4 floats (forward: v; backward: cvec, vbar, wq), the row groups'
+// column sums [G][mpad], the row ring [SINK_WARPS][slots][C] and its mbarriers, the row exchange [2][G][W] (forward: (max, sum);
+// backward: a sum) and 128 bytes of slack.
+constexpr size_t sinkhorn_smem(bool backward, int V, int W, int slots, int mpad) {
+  const int C = 128 * V, G = SINK_WARPS / W, vecs = backward ? 3 : 1;
+  const size_t xbytes = backward ? sizeof(float) : sizeof(float2);
+  return ((size_t)vecs * (W * C + 4) + (size_t)G * mpad + (size_t)SINK_WARPS * slots * C) * sizeof(float) +
+         (size_t)SINK_WARPS * slots * sizeof(uint64_t) + (size_t)2 * G * W * xbytes + 128;
 }
 
-// strips per pair / pairs per cooperative launch for p->occ co-resident CTAs per SM
-inline void sinkhorn_decompose(SinkPlan* p, int B, int n) {
+// The instantiation, its shared memory, the occupancy and the strip decomposition of either pass.  Both passes use the same V and
+// W per column band; the backward keeps three column vectors in shared memory where the forward keeps one, so for
+// 2048 < m <= 4096 it has ONE ring slot per warp (two would need 246 KB, more than a block may opt in to).  Two CTAs per SM
+// (__launch_bounds__ allows it for V <= 8) while two blocks, each with the 1 KB the runtime reserves, fit in 227 KB.
+inline int sinkhorn_plan(bool backward, int B, int n, int m, SinkPlan* p) {
+  const char* who = backward ? "sinkhorn_bwd" : "sinkhorn";
+  if (m <= 512)                { p->V = 4;  p->W = 1; p->slots = 2; }
+  else if (m <= 1024)          { p->V = 4;  p->W = 2; p->slots = 2; }
+  else if (m <= 2048)          { p->V = 8;  p->W = 2; p->slots = 2; }
+  else if (m <= 4096)          { p->V = 16; p->W = 2; p->slots = backward ? 1 : 2; }
+  else if (m <= SINK_MAX_COLS) { p->V = 16; p->W = 4; p->slots = 1; }
+  else return fail(OG_EUNSUPPORTED, "%s: m = %d > %d columns not supported (swap the images)", who, m, SINK_MAX_COLS);
+  p->mpad = (int)align_up(m + 1, 4);
+  p->smem = sinkhorn_smem(backward, p->V, p->W, p->slots, p->mpad);
+  p->occ = (p->V <= 8 && 2 * (p->smem + 1024) <= OG_SMEM_OPTIN_MAX) ? 2 : 1;
+  // strips per pair / pairs per cooperative launch for p->occ co-resident CTAs per SM
   const int sms = device_info().ok ? device_info().sm_count : 132;
-  const int slots_total = sms * p->occ;                 // co-resident CTAs of the cooperative launch
-  p->pairs_per_launch = std::min(B < slots_total ? B : slots_total, (int)(SINK_BARRIER_BYTES / 128));
-  // experiment knobs: OG_SINK_PAIRS = pairs per launch (L2 blocking), OG_SINK_SP = max strips per pair
-  static const int env_pairs = [] { const char* e = getenv("OG_SINK_PAIRS"); return e ? atoi(e) : 0; }();
-  static const int env_sp = [] { const char* e = getenv("OG_SINK_SP"); return e ? atoi(e) : 32; }();
-  if (env_pairs > 0 && env_pairs < p->pairs_per_launch) p->pairs_per_launch = env_pairs;
-  int sp = slots_total / p->pairs_per_launch;
-  if (sp > env_sp) sp = env_sp;
+  const int ctas = sms * p->occ;                       // co-resident CTAs of the cooperative launch
+  p->pairs_per_launch = std::min(B < ctas ? B : ctas, (int)(SINK_BARRIER_BYTES / 128));
+  int sp = std::min(ctas / p->pairs_per_launch, SINK_MAX_STRIPS);
   const int max_sp = cdiv(n + 1, SINK_WARPS / p->W);
   if (sp > max_sp) sp = max_sp;
   if (sp < 1) sp = 1;
   p->SP = sp;
   p->rows_per_strip = cdiv(n + 1, sp);
-}
-
-inline int sinkhorn_plan(int B, int n, int m, SinkPlan* p) {
-  p->mpad = (int)align_up(m + 1, 4);
-  if (m <= 512)       { p->V = 4;  p->W = 1; p->slots = 2; p->occ = 2; p->smem = sinkhorn_smem<4, 1, 2>(p->mpad); }
-  else if (m <= 1024) { p->V = 4;  p->W = 2; p->slots = 2; p->occ = 2; p->smem = sinkhorn_smem<4, 2, 2>(p->mpad); }
-  else if (m <= 2048) { p->V = 8;  p->W = 2; p->slots = 2; p->occ = 2; p->smem = sinkhorn_smem<8, 2, 2>(p->mpad); }
-  else if (m <= 4096) { p->V = 16; p->W = 2; p->slots = 2; p->occ = 1; p->smem = sinkhorn_smem<16, 2, 2>(p->mpad); }
-  else if (m <= SINK_MAX_COLS) { p->V = 16; p->W = 4; p->slots = 1; p->occ = 1; p->smem = sinkhorn_smem<16, 4, 1>(p->mpad); }
-  else return fail(OG_EUNSUPPORTED, "sinkhorn: m = %d > %d columns not supported (swap the images)", m, SINK_MAX_COLS);
-  static const int env_occ = [] { const char* e = getenv("OG_SINK_OCC"); return e ? atoi(e) : 0; }();      // experiment: force 1 CTA / SM
-  // experiment: OG_SINK_CFG=VWS picks another instantiation for 1024 < m <= 2048 (824 = V 8, W 2, 4 slots; 1612; 444)
-  static const int env_cfg = [] { const char* e = getenv("OG_SINK_CFG"); return e ? atoi(e) : 0; }();
-  if (m > 1024 && m <= 2048) {
-    if (env_cfg == 824)  { p->V = 8;  p->W = 2; p->slots = 4; p->occ = 1; p->smem = sinkhorn_smem<8, 2, 4>(p->mpad); }
-    if (env_cfg == 1612) { p->V = 16; p->W = 1; p->slots = 2; p->occ = 1; p->smem = sinkhorn_smem<16, 1, 2>(p->mpad); }
-    if (env_cfg == 444)  { p->V = 4;  p->W = 4; p->slots = 4; p->occ = 2; p->smem = sinkhorn_smem<4, 4, 4>(p->mpad); }
-  }
-  if (env_occ == 1) p->occ = 1;
-  sinkhorn_decompose(p, B, n);
   return OG_OK;
 }
 
-inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
-  SinkPlan p;
-  if (sinkhorn_plan(B, n, m, &p) != OG_OK) return -1;
-  // sized for the largest strip count any occupancy setting may choose (the plan depends on the device only through the SM count)
-  const int64_t sp_max = std::max(p.SP, 32);
-  return SINK_BARRIER_BYTES + align_up((int64_t)B * (n + 1) * 4, 256) + align_up(2LL * B * sp_max * p.mpad * 4, 256);
+inline int sinkhorn_check_rows(const char* who, const float* S, int64_t lds, int64_t strideS, int m) {
+  if (lds % 4 != 0 || lds < m || (reinterpret_cast<uintptr_t>(S) & 15) || strideS % 4 != 0)
+    return fail(OG_EINVAL, "%s: S rows must be 16-byte aligned (lds %% 4 == 0, lds >= m)", who);
+  return OG_OK;
 }
 
-template <int V, int W, int SLOTS>
-inline int sinkhorn_launch_v(SinkArgs a, const SinkPlan& p, cudaStream_t stream) {
-  constexpr size_t smem_max = sinkhorn_smem<V, W, SLOTS>(128 * V * W + 4);     // largest request of this instantiation: m = 128 V W
-  static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "sinkhorn_kernel: shared memory beyond what one block may opt in to");
-  if (const int rc = smem_opt_in<sinkhorn_kernel<V, W, SLOTS>>((int)smem_max)) return rc;
+// host-side constants exactly as the reference builds them (float32 throughout)
+struct SinkConsts { float norm, log_a_last, log_b_last; };
+inline SinkConsts sinkhorn_consts(int n, int m) {
+  const float norm = -logf((float)(n + m));
+  return {norm, norm + (float)log((double)m),        // log_a[-1] += math.log(n_cols)
+          norm + (float)log((double)n)};             // log_b[-1] += math.log(n_rows)
+}
+
+// One cooperative launch of Kernel = <pass kernel><V, W, SLOTS> over a.B pairs.
+template <auto Kernel, int V, int W, int SLOTS, class Args>
+inline int sinkhorn_coop_launch(const Args& a, const SinkPlan& p, cudaStream_t stream) {
+  constexpr size_t smem_max = sinkhorn_smem(Args::kBackward, V, W, SLOTS, 128 * V * W + 4);   // largest request: m = 128 V W
+  static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "Sinkhorn kernel: shared memory beyond what one block may opt in to");
+  if (const int rc = smem_opt_in<Kernel>((int)smem_max)) return rc;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.B * a.SP);
   cfg.blockDim = dim3(SINK_WARPS * 32);
@@ -467,60 +468,58 @@ inline int sinkhorn_launch_v(SinkArgs a, const SinkPlan& p, cudaStream_t stream)
   attr[0].id = cudaLaunchAttributeCooperative;
   attr[0].val.cooperative = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  OG_CUDA(cudaLaunchKernelEx(&cfg, sinkhorn_kernel<V, W, SLOTS>, a));
+  OG_CUDA(cudaLaunchKernelEx(&cfg, Kernel, a));
   launch_counter()++;
   return OG_OK;
+}
+
+// Calls launch(b0, nb) for pairs [b0, b0 + nb): as many pairs per cooperative launch as the plan allows, each launch with the
+// barrier counters of its pairs zeroed.
+template <class Launch>
+inline int sinkhorn_for_each_launch(const SinkPlan& p, int B, unsigned int* barrier, cudaStream_t stream, Launch&& launch) {
+  for (int b0 = 0; b0 < B; b0 += p.pairs_per_launch) {
+    const int nb = std::min(p.pairs_per_launch, B - b0);
+    OG_CUDA(cudaMemsetAsync(barrier, 0, (size_t)nb * 128, stream));
+    if (const int rc = launch(b0, nb)) return rc;
+  }
+  return OG_OK;
+}
+
+inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
+  SinkPlan p;
+  if (sinkhorn_plan(false, B, n, m, &p) != OG_OK) return -1;
+  return SINK_BARRIER_BYTES + align_up((int64_t)B * (n + 1) * 4, 256) + align_up(2LL * B * SINK_MAX_STRIPS * p.mpad * 4, 256);
 }
 
 inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int B, int n, int m,
                            int iters, float reg, float* scores, void* ws, int64_t ws_bytes, cudaStream_t stream,
                            float* hist_u = nullptr, float* hist_v = nullptr) {
   SinkPlan p;
-  int rc = sinkhorn_plan(B, n, m, &p);
-  if (rc != OG_OK) return rc;
+  if (const int rc = sinkhorn_plan(false, B, n, m, &p)) return rc;
   if (ws_bytes < sinkhorn_workspace_bytes(B, n, m)) return fail(OG_EWORKSPACE, "sinkhorn: workspace too small");
-  if (lds % 4 != 0 || lds < m || (reinterpret_cast<uintptr_t>(S) & 15) || strideS % 4 != 0)
-    return fail(OG_EINVAL, "sinkhorn: S rows must be 16-byte aligned (lds %% 4 == 0, lds >= m)");
+  if (const int rc = sinkhorn_check_rows("sinkhorn", S, lds, strideS, m)) return rc;
   char* w = static_cast<char*>(ws);
   unsigned int* barrier = reinterpret_cast<unsigned int*>(w); w += SINK_BARRIER_BYTES;
   float* u = reinterpret_cast<float*>(w); w += align_up((int64_t)B * (n + 1) * 4, 256);
   float* partial = reinterpret_cast<float*>(w);
-  // host-side constants exactly as the reference builds them (float32 throughout)
-  const float norm = -logf((float)(n + m));
-  const float log_a_last = norm + (float)log((double)m);     // log_a[-1] += math.log(n_cols)
-  const float log_b_last = norm + (float)log((double)n);     // log_b[-1] += math.log(n_rows)
+  const SinkConsts k = sinkhorn_consts(n, m);
   if (hist_v) OG_CUDA(cudaMemsetAsync(hist_v, 0, (size_t)B * (iters + 1) * (m + 1) * sizeof(float), stream));   // row 0 of every pair = v_0 = 0
-  for (int b0 = 0; b0 < B; b0 += p.pairs_per_launch) {
-    const int nb = std::min(p.pairs_per_launch, B - b0);
+  return sinkhorn_for_each_launch(p, B, barrier, stream, [&](int b0, int nb) {
     SinkArgs a;
     a.S = S + (int64_t)b0 * strideS; a.lds = lds; a.strideS = strideS; a.dustbin = dustbin;
     a.B = nb; a.n = n; a.m = m; a.iters = iters; a.reg = reg;
-    a.norm = norm; a.log_a_last = log_a_last; a.log_b_last = log_b_last;
+    a.norm = k.norm; a.log_a_last = k.log_a_last; a.log_b_last = k.log_b_last;
     a.scores = scores + (int64_t)b0 * (n + 1) * (m + 1);
     a.u = u; a.partial = partial; a.barrier = barrier;
     a.SP = p.SP; a.rows_per_strip = p.rows_per_strip; a.mpad = p.mpad;
     a.hist_u = hist_u ? hist_u + (int64_t)b0 * iters * (n + 1) : nullptr;
     a.hist_v = hist_v ? hist_v + (int64_t)b0 * (iters + 1) * (m + 1) : nullptr;
-    {                                                  // L2-resident subset: ~res_mb MB of this launch's matrices (OG_SINK_L2_MB, 0 = off)
-      static const int res_mb = [] { const char* e = getenv("OG_SINK_L2_MB"); return e ? atoi(e) : SINK_L2_RESIDENT_MB; }();
-      const double total = (double)nb * n * (double)m * 4.0;
-      const double frac = total > 0 ? std::min(1.0, res_mb * 1048576.0 / total) : 0.0;
-      a.res_q16 = (int)(frac * 65536.0);
-      static const int pf = [] { const char* e = getenv("OG_SINK_PF"); return e ? atoi(e) : SINK_L2_PREFETCH_ROWS; }();
-      a.pf_rows = pf;
-    }
-    OG_CUDA(cudaMemsetAsync(barrier, 0, (size_t)nb * 128, stream));
-    if (p.V == 8 && p.slots == 4)   rc = sinkhorn_launch_v<8, 2, 4>(a, p, stream);
-    else if (p.V == 16 && p.W == 1) rc = sinkhorn_launch_v<16, 1, 2>(a, p, stream);
-    else if (p.V == 4 && p.W == 4)  rc = sinkhorn_launch_v<4, 4, 4>(a, p, stream);
-    else if (p.V == 4 && p.W == 1)  rc = sinkhorn_launch_v<4, 1, 2>(a, p, stream);
-    else if (p.V == 4)              rc = sinkhorn_launch_v<4, 2, 2>(a, p, stream);
-    else if (p.V == 8)              rc = sinkhorn_launch_v<8, 2, 2>(a, p, stream);
-    else if (p.W == 2)              rc = sinkhorn_launch_v<16, 2, 2>(a, p, stream);
-    else                            rc = sinkhorn_launch_v<16, 4, 1>(a, p, stream);
-    if (rc != OG_OK) return rc;
-  }
-  return OG_OK;
+    if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<sinkhorn_kernel<4, 1, 2>, 4, 1, 2>(a, p, stream);
+    if (p.V == 4)             return sinkhorn_coop_launch<sinkhorn_kernel<4, 2, 2>, 4, 2, 2>(a, p, stream);
+    if (p.V == 8)             return sinkhorn_coop_launch<sinkhorn_kernel<8, 2, 2>, 8, 2, 2>(a, p, stream);
+    if (p.W == 2)             return sinkhorn_coop_launch<sinkhorn_kernel<16, 2, 2>, 16, 2, 2>(a, p, stream);
+    return sinkhorn_coop_launch<sinkhorn_kernel<16, 4, 1>, 16, 4, 1>(a, p, stream);
+  });
 }
 
 }  // namespace og

@@ -8,9 +8,10 @@
 //     P2_ij = exp(Z_ij + u_t,i + v_t,j - log_b_j)   (column-normalised)     Zbar -= vbar_t,j P2_ij ;  ubar_t,i -= sum_j vbar_t,j P2_ij
 //     P1_ij = exp(Z_ij + u_t,i + v_{t-1},j - log_a_i) (row-normalised)      Zbar -= ubar_t,i P1_ij ;  vbar_{t-1},j = - sum_i ubar_t,i P1_ij
 // P1 = P2 * wq_j / a_i with wq_j = exp(v_{t-1},j - v_t,j + log_b_j), so one sweep over Z with ONE exponential per element
-// serves both reductions of an iteration - the forward kernel's structure (csrc/sinkhorn.cuh: strips of rows, W warps per
-// row, bulk-copy row ring, per-pair barrier, deterministic column reduction), with u_t / v_t read from the history the
-// forward pass recorded.  The matrix gradient is then one more pass with Z in registers:
+// serves both reductions of an iteration - the forward kernel's structure, built from the same pieces (csrc/sinkhorn.cuh:
+// strips of rows, W warps per row, bulk-copy row ring, per-pair barrier, deterministic column reduction, one plan and one
+// launcher), with u_t / v_t read from the history the forward pass recorded.  The matrix gradient is then one more pass with
+// Z in registers:
 //     Zbar_ij = G_ij - sum_t exp(Z_ij + u_t,i + cvec_t,j) (vbar_t,j + coef_t,i wq_t,j),   coef_t,i = ubar_t,i / a_i
 // (T exponentials per element from the MUFU pipe, no HBM traffic beyond Z, G and the result).
 // HBM-bound like the forward pass: T sweeps over Z.  d loss / d S = Zbar[:N, :M] / reg; d loss / d dustbin = the sum of
@@ -21,6 +22,7 @@
 namespace og {
 
 struct SinkBwdArgs {
+  static constexpr bool kBackward = true;
   const float* S; int64_t lds, strideS;
   const float* dustbin;
   int B, n, m, iters;
@@ -41,7 +43,8 @@ struct SinkBwdArgs {
 template <int V, int W, int SLOTS>
 __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bwd_kernel(SinkBwdArgs a) {
   extern __shared__ __align__(128) float og_sinkb_smem[];
-  constexpr int C = 128 * V, MC = W * C, G = SINK_WARPS / W;
+  using Strip = SinkStrip<V, W>;
+  constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G;
   float* cvec_s = og_sinkb_smem;                       // [MC + 4]  v_t,j - log_b_j  (-inf for the padding columns; [MC] = dustbin column)
   float* vbar_s = cvec_s + MC + 4;                     // [MC + 4]  vbar_t,j
   float* wq_s = vbar_s + MC + 4;                       // [MC + 4]
@@ -49,28 +52,12 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
   float* ring = red + G * a.mpad;                      // [SINK_WARPS][SLOTS][C]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);
   float* xr = reinterpret_cast<float*>(bars + SINK_WARPS * SLOTS);               // [2][G][W] partial row sums
-  const int b = blockIdx.x / a.SP, strip = blockIdx.x % a.SP;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int grp = warp / W, sub = warp % W;
-  const int c0 = sub * C;
-  const int n = a.n, m = a.m, T = a.iters;
-  const int r0 = strip * a.rows_per_strip;
-  const int r1 = min(r0 + a.rows_per_strip, n + 1);
-  const int r1_real = min(r1, n);
-  const float* __restrict__ Sb = a.S + (int64_t)b * a.strideS;
-  const bool unit_reg = (a.reg == 1.0f);
-  const float dz = unit_reg ? __ldg(a.dustbin) : __fdiv_rn(__ldg(a.dustbin), a.reg);
+  const Strip s(a);
+  const int n = a.n, m = a.m, T = a.iters, b = s.b, tid = s.tid;
   const float ia_reg = expf(-a.norm), ia_last = expf(-a.log_a_last);      // 1 / a_i
-  const int seg_cols = min(m, c0 + C) - c0;
-  const bool has_seg = seg_cols > 0;
-  const uint32_t seg_bytes = has_seg ? (uint32_t)(((seg_cols + 3) / 4) * 16) : 0u;
-  float* my_ring = ring + warp * SLOTS * C;
-  uint64_t* my_bars = bars + warp * SLOTS;
+  SinkRowRing<V, W, SLOTS, false, SinkBwdArgs> rows(a, s, ring, bars);
+  const float dz = rows.dz;
 
-  if (lane == 0) {
-    for (int sl = 0; sl < SLOTS; ++sl) sink_mbar_init(&my_bars[sl]);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   for (int j = tid; j <= MC; j += blockDim.x) {        // vbar_T = column sums of G
     float vb = 0.f;
     if (j < m) vb = __ldg(a.vbar_init + (int64_t)b * (m + 1) + j);
@@ -79,65 +66,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
   }
   __syncthreads();
 
-  uint32_t issued = 0, consumed = 0;
-  auto prefetch_first = [&]() {
-    if (lane == 0 && has_seg) {
-      for (int sl = 0; sl < SLOTS; ++sl) {
-        const int row = r0 + grp + sl * G;
-        if (row < r1_real) {
-          sink_row_copy(my_ring + (issued % SLOTS) * C, Sb + (int64_t)row * a.lds + c0, seg_bytes, &my_bars[issued % SLOTS]);
-          ++issued;
-        }
-      }
-    }
-  };
-  auto take_row = [&](int row, float4 (&z)[V]) {
-    if (row < n) {
-      if (has_seg) {
-        const uint32_t sl = consumed % SLOTS, ph = (consumed / SLOTS) & 1;
-        sink_mbar_wait(&my_bars[sl], ph);
-        const float4* src = reinterpret_cast<const float4*>(my_ring + sl * C);
-#pragma unroll
-        for (int k = 0; k < V; ++k) {
-          const int idx = lane + 32 * k;
-          z[k] = (c0 + 4 * idx < m) ? src[idx] : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-        if (m & 3) {
-#pragma unroll
-          for (int k = 0; k < V; ++k) {
-            const int c = c0 + 4 * (lane + 32 * k);
-            if (c < m && c + 3 >= m) {
-              if (c + 1 >= m) z[k].y = 0.f;
-              if (c + 2 >= m) z[k].z = 0.f;
-              z[k].w = 0.f;
-            }
-          }
-        }
-        ++consumed;
-        __syncwarp();
-        const int nxt = row + SLOTS * G;
-        if (lane == 0 && nxt < r1_real) {
-          sink_row_copy(my_ring + sl * C, Sb + (int64_t)nxt * a.lds + c0, seg_bytes, &my_bars[sl]);
-          ++issued;
-        }
-        if (!unit_reg) {
-#pragma unroll
-          for (int k = 0; k < V; ++k) {
-            z[k].x = __fdiv_rn(z[k].x, a.reg); z[k].y = __fdiv_rn(z[k].y, a.reg);
-            z[k].z = __fdiv_rn(z[k].z, a.reg); z[k].w = __fdiv_rn(z[k].w, a.reg);
-          }
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < V; ++k) z[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    } else {
-#pragma unroll
-      for (int k = 0; k < V; ++k) z[k] = make_float4(dz, dz, dz, dz);
-    }
-  };
-
-  prefetch_first();
+  rows.prime();
   uint32_t rowpar = 0;
   for (int it = T - 1; it >= 0; --it) {
     // column constants of iteration t = it + 1 (every CTA of the pair builds the same values)
@@ -154,7 +83,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
       cvec_s[j] = cv; wq_s[j] = wq;
     }
     __syncthreads();
-    if (strip == 0) {                                  // history for the matrix-gradient pass
+    if (s.strip == 0) {                                // history for the matrix-gradient pass
       const int64_t o = ((int64_t)b * T + it) * (m + 1);
       for (int j = tid; j <= m; j += blockDim.x) {
         const int js = (j < m) ? j : MC;
@@ -168,14 +97,14 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
     const float cv_m = cvec_s[MC], vb_m = vbar_s[MC];
     const float* ut = a.hist_u + ((int64_t)b * T + it) * (n + 1);
 
-    for (int row = r0 + grp; row < r1; row += G) {
+    for (int row = s.r0 + s.grp; row < s.r1; row += G) {
       float4 z[V];
-      take_row(row, z);
+      rows.take(row, z);
       const float u_i = __ldcg(ut + row);
       float rs = 0.f;
 #pragma unroll
       for (int k = 0; k < V; ++k) {
-        const int c = c0 + 4 * (lane + 32 * k);
+        const int c = s.c0 + 4 * (s.lane + 32 * k);
         const float4 cv = *reinterpret_cast<const float4*>(cvec_s + c);
         const float4 vb = *reinterpret_cast<const float4*>(vbar_s + c);
         z[k].x = ex2_approx(((z[k].x + cv.x) + u_i) * LOG2E_F);     // P2_ij <= 1: no shift needed; padding: 2^-inf = 0
@@ -184,20 +113,17 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
         z[k].w = ex2_approx(((z[k].w + cv.w) + u_i) * LOG2E_F);
         rs = fmaf(z[k].x, vb.x, rs); rs = fmaf(z[k].y, vb.y, rs); rs = fmaf(z[k].z, vb.z, rs); rs = fmaf(z[k].w, vb.w, rs);
       }
-      const float e_m = (sub == 0) ? ex2_approx(((dz + cv_m) + u_i) * LOG2E_F) : 0.f;
+      const float e_m = (s.sub == 0) ? ex2_approx(((dz + cv_m) + u_i) * LOG2E_F) : 0.f;
       float r_i = warp_sum(rs) + e_m * vb_m;
       if (W > 1) {
-        float* x = xr + (rowpar * G + grp) * W;
-        if (lane == 0) x[sub] = r_i;
-        asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "n"(W * 32) : "memory");
+        const float* x = sink_row_exchange(xr, r_i, s, rowpar);
         r_i = 0.f;
 #pragma unroll
         for (int w2 = 0; w2 < W; ++w2) r_i += x[w2];
-        rowpar ^= 1u;
       }
       const float ub0 = (it == T - 1) ? __ldg(a.ubar_init + (int64_t)b * (n + 1) + row) : 0.f;
       const float coef = (ub0 - r_i) * ((row < n) ? ia_reg : ia_last);      // ubar_t,i / a_i
-      if (sub == 0 && lane == 0) a.hist_coef[((int64_t)b * T + it) * (n + 1) + row] = coef;
+      if (s.sub == 0 && s.lane == 0) a.hist_coef[((int64_t)b * T + it) * (n + 1) + row] = coef;
 #pragma unroll
       for (int k = 0; k < V; ++k) {
         cacc[k].x = fmaf(z[k].x, coef, cacc[k].x); cacc[k].y = fmaf(z[k].y, coef, cacc[k].y);
@@ -205,42 +131,9 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
       }
       cacc_m = fmaf(e_m, coef, cacc_m);
     }
-    prefetch_first();
-    float* myred = red + grp * a.mpad;
-#pragma unroll
-    for (int k = 0; k < V; ++k) {
-      const int c = c0 + 4 * (lane + 32 * k);
-      if (c < m) *reinterpret_cast<float4*>(myred + c) = cacc[k];
-    }
-    __syncthreads();
-    if (sub == 0 && lane == 0) myred[m] = cacc_m;
-    __syncthreads();
-    const int pbuf = (T - 1 - it) & 1;
-    float* part = a.partial + ((int64_t)pbuf * a.B * a.SP + (int64_t)b * a.SP + strip) * a.mpad;
-    for (int j = tid; j <= m; j += blockDim.x) {
-      float s = 0.f;
-#pragma unroll
-      for (int w = 0; w < G; ++w) s += red[w * a.mpad + j];
-      part[j] = s;
-    }
-    grid_barrier(a.barrier + 32 * b, (unsigned int)(T - it) * (unsigned int)a.SP);
-    const float* pb = a.partial + ((int64_t)pbuf * a.B * a.SP + (int64_t)b * a.SP) * a.mpad;
-    for (int j4 = tid; 4 * j4 <= m; j4 += blockDim.x) {            // vbar_{t-1},j = - wq_j sum_i coef_i e_ij
-      float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 8
-      for (int s = 0; s < a.SP; ++s) {
-        const float4 q = __ldcg(reinterpret_cast<const float4*>(pb + (int64_t)s * a.mpad) + j4);
-        c.x += q.x; c.y += q.y; c.z += q.z; c.w += q.w;
-      }
-      const float cc[4] = {c.x, c.y, c.z, c.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int j = 4 * j4 + e;
-        if (j < m) vbar_s[j] = -wq_s[j] * cc[e];
-        else if (j == m) vbar_s[MC] = -wq_s[MC] * cc[e];
-      }
-    }
-    __syncthreads();
+    if (it > 0) rows.prime();                          // the next iteration's first rows fly during the reduction
+    // vbar_{t-1},j = - wq_j sum_i coef_i e_ij
+    sink_column_reduce(a, s, red, cacc, cacc_m, T - 1 - it, [&](int j, float c) { vbar_s[j] = -wq_s[j] * c; });
   }
 }
 
@@ -368,59 +261,16 @@ __global__ void __launch_bounds__(256) sinkb_dustbin_kernel(const float* __restr
 // history the forward pass records for the backward pass: u [B][T][n+1] then v [B][T+1][m+1]
 inline int64_t sinkhorn_hist_floats(int B, int n, int m, int T) { return (int64_t)B * T * (n + 1) + (int64_t)B * (T + 1) * (m + 1); }
 
-template <int V, int W, int SLOTS>
-constexpr size_t sinkhorn_bwd_smem(int mpad) {
-  constexpr int C = 128 * V, G = SINK_WARPS / W;
-  return ((size_t)3 * (W * C + 4) + (size_t)G * mpad + (size_t)SINK_WARPS * SLOTS * C) * sizeof(float) +
-         (size_t)SINK_WARPS * SLOTS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float) + 128;
-}
-
-// The backward sweep keeps three column vectors in shared memory where the forward keeps one, so it has its own instantiation per
-// column band: the same V and W as the forward, but ONE ring slot per warp for 2048 < m <= 4096 (two slots would need 246 KB, more
-// than a block may opt in to).  Two CTAs per SM only while two blocks (each with the 1 KB the runtime reserves) fit in 227 KB.
-// The instantiation, the occupancy (and with it the strip decomposition) and the workspace size all come from this plan.
-inline int sinkhorn_bwd_plan(int B, int n, int m, SinkPlan* p) {
-  p->mpad = (int)align_up(m + 1, 4);
-  if (m <= 512)       { p->V = 4;  p->W = 1; p->slots = 2; p->smem = sinkhorn_bwd_smem<4, 1, 2>(p->mpad); }
-  else if (m <= 1024) { p->V = 4;  p->W = 2; p->slots = 2; p->smem = sinkhorn_bwd_smem<4, 2, 2>(p->mpad); }
-  else if (m <= 2048) { p->V = 8;  p->W = 2; p->slots = 2; p->smem = sinkhorn_bwd_smem<8, 2, 2>(p->mpad); }
-  else if (m <= 4096) { p->V = 16; p->W = 2; p->slots = 1; p->smem = sinkhorn_bwd_smem<16, 2, 1>(p->mpad); }
-  else if (m <= SINK_MAX_COLS) { p->V = 16; p->W = 4; p->slots = 1; p->smem = sinkhorn_bwd_smem<16, 4, 1>(p->mpad); }
-  else return fail(OG_EUNSUPPORTED, "sinkhorn_bwd: m = %d > %d columns not supported (swap the images)", m, SINK_MAX_COLS);
-  p->occ = (p->V <= 8 && 2 * (p->smem + 1024) <= OG_SMEM_OPTIN_MAX) ? 2 : 1;     // (__launch_bounds__: 2 CTAs only for V <= 8)
-  sinkhorn_decompose(p, B, n);
-  return OG_OK;
-}
-
 inline int64_t sinkhorn_bwd_workspace_bytes(int B, int n, int m, int T) {
   SinkPlan p;
-  if (sinkhorn_bwd_plan(B, n, m, &p) != OG_OK) return -1;
-  const int64_t sp_max = std::max(p.SP, 32), nrs = cdiv(n + 1, SINKB_RS_ROWS);
+  if (sinkhorn_plan(true, B, n, m, &p) != OG_OK) return -1;
+  const int64_t nrs = cdiv(n + 1, SINKB_RS_ROWS);
   int64_t f = 0;
   f += align_up((int64_t)B * (n + 1), 64) + align_up((int64_t)B * (m + 1), 64);                 // ubar_init, vbar_init
   f += align_up((int64_t)B * nrs * (m + 1), 64);                                                // column-sum partials
   f += align_up((int64_t)B * T * (n + 1), 64) + 3 * align_up((int64_t)B * T * (m + 1), 64);     // coef, cvec, vbar, wq histories
-  f += align_up(2LL * B * sp_max * p.mpad, 64) + align_up((int64_t)B, 64);                      // strip partials, per-pair dustbin sums
+  f += align_up(2LL * B * SINK_MAX_STRIPS * p.mpad, 64) + align_up((int64_t)B, 64);             // strip partials, per-pair dustbin sums
   return SINK_BARRIER_BYTES + 256 + f * 4;
-}
-
-template <int V, int W, int SLOTS>
-inline int sinkhorn_bwd_launch_v(SinkBwdArgs a, const SinkPlan& p, cudaStream_t stream) {
-  constexpr size_t smem_max = sinkhorn_bwd_smem<V, W, SLOTS>(128 * V * W + 4);     // largest request of this instantiation: m = 128 V W
-  static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "sinkhorn_bwd_kernel: shared memory beyond what one block may opt in to");
-  if (const int rc = smem_opt_in<sinkhorn_bwd_kernel<V, W, SLOTS>>((int)smem_max)) return rc;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(a.B * a.SP);
-  cfg.blockDim = dim3(SINK_WARPS * 32);
-  cfg.dynamicSmemBytes = p.smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  OG_CUDA(cudaLaunchKernelEx(&cfg, sinkhorn_bwd_kernel<V, W, SLOTS>, a));
-  launch_counter()++;
-  return OG_OK;
 }
 
 // G = d loss / d scores [B, n+1, m+1] (dense) -> dZ = d loss / d S_aug [B, n+1, m+1], ddustbin [1]
@@ -428,13 +278,11 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
                                const float* hist, const float* G, float* dZ, float* ddustbin, void* ws, int64_t ws_bytes,
                                cudaStream_t stream) {
   SinkPlan p;
-  int rc = sinkhorn_bwd_plan(B, n, m, &p);
-  if (rc != OG_OK) return rc;
+  if (const int rc = sinkhorn_plan(true, B, n, m, &p)) return rc;
   if (ws_bytes < sinkhorn_bwd_workspace_bytes(B, n, m, iters)) return fail(OG_EWORKSPACE, "sinkhorn_bwd: workspace too small");
-  if (lds % 4 != 0 || lds < m || (reinterpret_cast<uintptr_t>(S) & 15) || strideS % 4 != 0)
-    return fail(OG_EINVAL, "sinkhorn_bwd: S rows must be 16-byte aligned (lds %% 4 == 0, lds >= m)");
+  if (const int rc = sinkhorn_check_rows("sinkhorn_bwd", S, lds, strideS, m)) return rc;
   const int T = iters;
-  const int64_t sp_max = std::max(p.SP, 32), nrs = cdiv(n + 1, SINKB_RS_ROWS);
+  const int64_t nrs = cdiv(n + 1, SINKB_RS_ROWS);
   char* w = static_cast<char*>(ws);
   unsigned int* barrier = reinterpret_cast<unsigned int*>(w); w += SINK_BARRIER_BYTES;
   unsigned int* counter = reinterpret_cast<unsigned int*>(w); w += 256;
@@ -447,11 +295,9 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   float* hist_cvec = take((int64_t)B * T * (m + 1));
   float* hist_vbar = take((int64_t)B * T * (m + 1));
   float* hist_wq = take((int64_t)B * T * (m + 1));
-  float* partial = take(2LL * B * sp_max * p.mpad);
+  float* partial = take(2LL * B * SINK_MAX_STRIPS * p.mpad);
   float* per_pair = take(B);
-  const float norm = -logf((float)(n + m));
-  const float log_a_last = norm + (float)log((double)m);
-  const float log_b_last = norm + (float)log((double)n);
+  const SinkConsts k = sinkhorn_consts(n, m);
   const int m1 = m + 1, n1 = n + 1;
   sinkb_rowsum_kernel<<<cdiv(B * n1, 8), 256, 0, stream>>>(G, B * n1, m1, ubar_init);
   OG_LAUNCH_CHECK("sinkb_rowsum_kernel");
@@ -462,14 +308,13 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   launch_counter() += 3;
   SinkBwdArgs a;
   a.S = S; a.lds = lds; a.strideS = strideS; a.dustbin = dustbin; a.B = B; a.n = n; a.m = m; a.iters = T; a.reg = reg;
-  a.norm = norm; a.log_a_last = log_a_last; a.log_b_last = log_b_last;
+  a.norm = k.norm; a.log_a_last = k.log_a_last; a.log_b_last = k.log_b_last;
   a.hist_u = hist; a.hist_v = hist + (int64_t)B * T * (n + 1);
   a.ubar_init = ubar_init; a.vbar_init = vbar_init;
   a.hist_coef = hist_coef; a.hist_cvec = hist_cvec; a.hist_vbar = hist_vbar; a.hist_wq = hist_wq;
   a.partial = partial; a.barrier = barrier; a.SP = p.SP; a.rows_per_strip = p.rows_per_strip; a.mpad = p.mpad;
   if (T > 0) {
-    for (int b0 = 0; b0 < B; b0 += p.pairs_per_launch) {
-      const int nb = std::min(p.pairs_per_launch, B - b0);
+    const int rc = sinkhorn_for_each_launch(p, B, barrier, stream, [&](int b0, int nb) {
       SinkBwdArgs g = a;
       g.B = nb;
       g.S = S + (int64_t)b0 * strideS;
@@ -477,14 +322,13 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
       g.ubar_init = ubar_init + (int64_t)b0 * n1; g.vbar_init = vbar_init + (int64_t)b0 * m1;
       g.hist_coef = hist_coef + (int64_t)b0 * T * n1; g.hist_cvec = hist_cvec + (int64_t)b0 * T * m1;
       g.hist_vbar = hist_vbar + (int64_t)b0 * T * m1; g.hist_wq = hist_wq + (int64_t)b0 * T * m1;
-      OG_CUDA(cudaMemsetAsync(barrier, 0, (size_t)nb * 128, stream));
-      if (p.V == 4 && p.W == 1)       rc = sinkhorn_bwd_launch_v<4, 1, 2>(g, p, stream);
-      else if (p.V == 4)              rc = sinkhorn_bwd_launch_v<4, 2, 2>(g, p, stream);
-      else if (p.V == 8)              rc = sinkhorn_bwd_launch_v<8, 2, 2>(g, p, stream);
-      else if (p.W == 2)              rc = sinkhorn_bwd_launch_v<16, 2, 1>(g, p, stream);
-      else                            rc = sinkhorn_bwd_launch_v<16, 4, 1>(g, p, stream);
-      if (rc != OG_OK) return rc;
-    }
+      if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<sinkhorn_bwd_kernel<4, 1, 2>, 4, 1, 2>(g, p, stream);
+      if (p.V == 4)             return sinkhorn_coop_launch<sinkhorn_bwd_kernel<4, 2, 2>, 4, 2, 2>(g, p, stream);
+      if (p.V == 8)             return sinkhorn_coop_launch<sinkhorn_bwd_kernel<8, 2, 2>, 8, 2, 2>(g, p, stream);
+      if (p.W == 2)             return sinkhorn_coop_launch<sinkhorn_bwd_kernel<16, 2, 1>, 16, 2, 1>(g, p, stream);
+      return sinkhorn_coop_launch<sinkhorn_bwd_kernel<16, 4, 1>, 16, 4, 1>(g, p, stream);
+    });
+    if (rc != OG_OK) return rc;
   }
   sinkb_dz_kernel<<<dim3(cdiv(m1, SINKB_TC), cdiv(n1, SINKB_TR), B), 256, 0, stream>>>(a, G, dZ, 1.f / reg);
   OG_LAUNCH_CHECK("sinkb_dz_kernel");

@@ -133,6 +133,41 @@ def test_tensor_core_kernels_are_hopper_native_and_address_shared_memory_directl
     assert len(attn) == 3 and all(c['MUFU'] >= 32 for c in attn)
 
 
+def test_sinkhorn_kernels_are_the_planned_instantiations_without_spills():
+    """Static check of the built library (cuobjdump, no GPU; OG_LIB names another build): it holds exactly the five forward and
+    five backward cooperative Sinkhorn instantiations sinkhorn_plan can select, and none touches local memory (STL / LDL:
+    spills) - the V = 16 forms sit within a few registers of the 255 limit."""
+    import re
+    import shutil
+    import subprocess
+    from openglue_b200 import _cabi
+    tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
+    if not os.path.exists(tool):
+        pytest.skip('cuobjdump not available')
+    path = os.environ.get('OG_LIB') or _cabi.LIB_PATH
+    assert os.path.exists(path), f'library not built: {path}'
+    res = subprocess.run([tool, '-sass', path], capture_output=True, text=True)
+    assert res.returncode == 0, res.stderr
+    funcs, cur = {}, None
+    for line in res.stdout.splitlines():
+        m = re.match(r'\s*Function : _ZN2og(?:15sinkhorn_kernel|19sinkhorn_bwd_kernel)ILi(\d+)ELi(\d+)ELi(\d+)EEEvNS_\d+([A-Za-z]\w*)E$', line)
+        if m:
+            cur = funcs.setdefault((m.group(4),) + tuple(int(g) for g in m.group(1, 2, 3)), [])
+            continue
+        if re.match(r'\s*Function : ', line):
+            cur = None
+            continue
+        m = re.match(r'\s*/\*[0-9a-f]+\*/\s+(?:@!?U?P(?:\d+|T)\s+)?([A-Z0-9_.]+)', line)
+        if m and cur is not None:
+            cur.append(m.group(1).split('.')[0])
+    bands = [(4, 1), (4, 2), (8, 2), (16, 2), (16, 4)]
+    fwd = {('SinkArgs', v, w, 1 if w == 4 else 2) for v, w in bands}
+    bwd = {('SinkBwdArgs', v, w, 1 if v == 16 else 2) for v, w in bands}
+    assert set(funcs) == fwd | bwd, sorted(funcs)
+    for name, ops in funcs.items():
+        assert 'STL' not in ops and 'LDL' not in ops, name
+
+
 def test_bench_work_accounting_reproduces_the_survey_table():
     """bench.py's algorithmic FLOP / byte formulas against the values SURVEY.md (section 8d, Appendix B) states for the BASELINE
     configurations - the numerators of `roofline.achieved` and of the judge's own check."""

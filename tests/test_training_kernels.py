@@ -1,7 +1,7 @@
 """The training kernels at training sizes, each against a float64 reference that shares none of its code.
 
 a. The Sinkhorn training forward (og_sinkhorn_train_fwd) and backward (og_sinkhorn_bwd) through the C ABI, at both edges of every
-   column band of the backward's instantiation table (csrc/sinkhorn_bwd.cuh: sinkhorn_bwd_plan), against the reverse-recurrence
+   column band of the instantiation table (csrc/sinkhorn.cuh: sinkhorn_plan), against the reverse-recurrence
    oracle (oracle/sinkhorn_grad_oracle.py, pinned to the reference's autograd by tests/test_sinkhorn_grad.py).
 b. The operators of csrc/train_ops.cuh (transpose / copy, column sums, BatchNorm forward and backward, row softmax and its backward,
    the split-K reduction, axpby, the residual mix, the keypoint-encoder input) against float64 torch, autograd where the operator is
