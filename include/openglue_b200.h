@@ -376,7 +376,8 @@ int og_kenc_input(const float* kpts, const float* side, int rows, int side_info_
  *   og_sp_compact       per image: surviving pixels in row-major order (torch.nonzero) -> cand_idx / cand_score [B, cap], count [B]
  *   og_sp_select        per image: n_out[b] keypoints, mode[b] = 0 in candidate order | 1 = the largest scores, descending (torch.topk,
  *                       equal scores: lower index first; top_k_keypoints utils.py:34-39, min_stack models/features/utils.py:28-56);
- *                       kpts [B,out_cap,2] as (x, y) floats, scores [B,out_cap];  max_count = the largest count (<= 16384)
+ *                       kpts [B,out_cap,2] as (x, y) floats, scores [B,out_cap];  max_count = the largest count (<= 16384);
+ *                       the caller guarantees n_out[b] <= min(count[b], cap, out_cap) (a larger n_out reads unwritten candidates)
  *   og_sp_sample_desc   sample_desc_from_points (utils.py:14-31): bilinear grid_sample (align_corners False) of the coarse descriptors
  *                       [B,Hc,Wc,D] at the keypoints + F.normalize -> desc [B,out_cap,D]                                        */
 int og_sp_im2col3x3(const float* x, int B, int H, int W, int C, float* out, void* stream);

@@ -135,6 +135,8 @@ __global__ void __launch_bounds__(1024) sp_compact_kernel(const float* __restric
 // selection of n_out[b] keypoints of image b from its candidate list: mode[b] = 0 keep the (row-major) order, 1 = the n_out largest
 // scores in descending order (torch.topk; equal scores: lower index first).  Outputs keypoints as (x, y) floats (model.py:108),
 // scores, both [B, out_cap, ...].  One CTA per image; the sort is a bitonic sort of (score, position) in shared memory.
+// Caller contract (not checked on the device): n_out[b] <= min(count[b], cap) and n_out[b] <= out_cap, and max_count >= every count[b]
+// (it sizes the shared memory); a larger n_out reads candidate slots that were never written.
 constexpr int SP_MAX_CAND = 16384;
 __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__ cand_idx, const float* __restrict__ cand_score,
                                                          const int* __restrict__ count, const int* __restrict__ n_out, const int* __restrict__ mode,

@@ -80,10 +80,20 @@ class SuperPointNet(nn.Module):
             raise RuntimeError('openglue_b200.SuperPointNet needs CUDA tensors (sm_90a); there is no CPU path')
         if image.dim() != 4 or image.shape[1] != 1 or image.shape[2] % 8 or image.shape[3] % 8:
             raise ValueError('image must be [B, 1, H, W] with H, W multiples of 8')
+        H, W = image.shape[2], image.shape[3]
+        probs, coarse = self._network(image)
+        return self._keypoints(probs, coarse, H, W)
+
+    def _ops(self, dev):
+        return _Ops(dev, _cabi.OG_PREC_FP32 if self.precision == 'fp32' else _cabi.OG_PREC_TF32X3)
+
+    def _network(self, image: torch.Tensor):
+        """The layers (model.py:61-78): image [B, 1, H, W] -> (probs [B hc wc, 65] after the cell softmax, coarse [B hc wc, D] with
+        unit rows), NHWC, hc = H / 8, wc = W / 8."""
+        dev = image.device
         B, _, H, W = image.shape
         x = image.detach().float().contiguous()                       # [B, 1, H, W] == NHWC with one channel
-        prec = _cabi.OG_PREC_FP32 if self.precision == 'fp32' else _cabi.OG_PREC_TF32X3
-        ops = _Ops(dev, prec)
+        ops = self._ops(dev)
         lib = ops.lib
         wts = self._weights()
         with torch.cuda.device(dev):
@@ -114,6 +124,18 @@ class SuperPointNet(nn.Module):
             probs = ops.linear(pa, *wts['convPb'])                       # [B hc wc, 65]
             _cabi.check(lib.og_softmax_rows(_p(probs), 65, probs.shape[0], 65, st), 'og_softmax_rows')
             self.last_probs = probs.view(B, hc, wc, 65)                  # kept for inspection / tests
+        return probs, coarse
+
+    def _keypoints(self, probs: torch.Tensor, coarse: torch.Tensor, H: int, W: int):
+        """The post-processing of forward (model.py:84-129) from the layers' outputs: probs [B hc wc, 65] and coarse [B hc wc, D]
+        (NHWC, hc = H / 8, wc = W / 8, CUDA float32) -> (lafs [B,N,2,3], scores [B,N], descriptors [B,N,D])."""
+        dev = probs.device
+        hc, wc = H // 8, W // 8
+        B = probs.shape[0] // (hc * wc)
+        ops = self._ops(dev)
+        lib = ops.lib
+        with torch.cuda.device(dev):
+            st = ops.st()
             heat = ops.empty(B, H, W)
             _cabi.check(lib.og_sp_heat_nms(_p(probs), B, hc, wc, int(self.nms_kernel), float(self.keypoint_threshold), int(self.remove_borders_size),
                                            _p(heat), st), 'og_sp_heat_nms')

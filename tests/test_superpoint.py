@@ -31,6 +31,21 @@ def _decisions(heat, nms, thr, border, margin):
     return keep & inb, decisive | ~inb
 
 
+def _disagreements(ours, ref, keep, decisive, heat, margin):
+    """Keypoints of one image, ours and the reference's (sets of (x, y)), against the per-pixel rule: a pixel whose NMS decision is
+    decisive (`_decisions`) must be in both outputs or in neither - unless the output is a top-k of fewer than all kept pixels and
+    the pixel's score is not above both outputs' lowest score by more than `margin` (then the cut decides, not the rule).
+    Returns the number of decisive pixels on which the outputs differ."""
+    H, W = heat.shape
+    mask = lambda pts: torch.zeros(H * W, dtype=torch.bool).index_fill_(0, torch.tensor([y * W + x for x, y in pts], dtype=torch.long), True).view(H, W)
+    m_ours, m_ref = mask(ours), mask(ref)
+    decided = decisive.clone()
+    if min(len(ours), len(ref)) < int(keep.sum()):
+        lowest = lambda m: float(heat[m].min()) if m.any() else float('inf')
+        decided &= heat > max(lowest(m_ours), lowest(m_ref)) + margin
+    return int(((m_ours != m_ref) & decided).sum())
+
+
 @pytest.mark.parametrize('name', CASES)
 def test_superpoint_fixture_is_self_consistent(name):
     """The fixture's keypoints follow from its own dense heat map by the restated rule (this is what pins the test helper)."""
@@ -127,21 +142,19 @@ def test_superpoint_matches_reference(name, precision):
     all_decisive = bool(decisive.all())
     if all_decisive:
         assert lafs.shape == ref_lafs.shape
-    matched = 0
+    margin = 10 * max(err, 1e-7)
     for b in range(batch):
         ours = {(int(x), int(y)): j for j, (x, y) in enumerate(lafs[b, :, :, 2].tolist())}
-        for j, (x, y) in enumerate(ref_lafs[b, :, :, 2].long().tolist()):
+        ref_pts = [tuple(p) for p in ref_lafs[b, :, :, 2].long().tolist()]
+        for j, (x, y) in enumerate(ref_pts):
             if (x, y) in ours:
                 i = ours[(x, y)]
-                matched += 1
                 assert abs(float(scores[b, i]) - float(ref_scores[b, j])) <= bound + ref_err    # the fixture's scores are the reference's fp32 run
                 assert (desc[b, i] - ref_desc[b, j]).abs().max() <= 1e-4
-            else:
-                assert not all_decisive, (b, x, y)
-    total = ref_lafs.shape[0] * ref_lafs.shape[1]
-    assert matched >= 0.99 * total, (matched, total)
-    if all_decisive and (maxk == -1 or name == 'superpoint_thr'):
-        pass
+        # every pixel whose decision is decisive - by the NMS rule and, for a top-k, by the cut - is decided the same way
+        bad = _disagreements(list(ours), ref_pts, keep[b], decisive[b], fx['heat_f64'][b].float(), margin)
+        print(f'  image {b}: {len(ours)} / {len(ref_pts)} keypoints, {int((~decisive[b]).sum())} non-decisive pixels, {bad} decisive disagreements')
+        assert bad == 0
     # ordering: where the reference's order is decided by score gaps larger than the error, ours is the same sequence
     if all_decisive:
         for b in range(batch):
