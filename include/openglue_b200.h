@@ -390,6 +390,38 @@ int og_sp_select(const int* cand_idx, const float* cand_score, const int* count,
 int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const float* kpts, const int* n_out, int out_cap, int max_n, int cell,
                       float* desc, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Local features -> matcher inputs, and matches -> the compact match list of stand-alone inference.
+ *   og_prepare_features  prepare_features_output (models/features/utils.py:54-65) with the LAF -> side-information converter
+ *                        superglue.laf_to_sideinfo_method names (models/laf_converter.py:108-128).  One thread per keypoint.
+ *                        lafs [R,2,3] = [[a00, a01, x], [a10, a11, y]];  s = sqrt(|(a00 a11 - a10 a01) + 1e-10|) (kornia get_laf_scale)
+ *                          kpts [R,2] = (x, y)  (may be NULL: not written)
+ *                          side [R, (responses ? 1 : 0) + dim]:  r, or log(r + 0.1) when log_response  (responses NULL: no column),
+ *                          then by method:  NONE  -                                              (dim 0)
+ *                                           SCALE  log s                                         (dim 1)
+ *                                           ROTATION  a01/s, a00/s                               (dim 2)
+ *                                           SCALE_ROTATION  log s, a01/s, a00/s                  (dim 3)
+ *                                           AFFINE  log s, a00/s, a01/s, a10/s, a11/s            (dim 5)
+ *                        Separately rounded IEEE operations in ATen's order (no FMA contraction): every column except the
+ *                        logarithms equals the reference's fp32 result bit for bit (where ATen's square root is correctly
+ *                        rounded: its vectorised CPU form is 1 ulp off on a few frames in a thousand).
+ *   og_match_compact     the boolean indexing of OpenGlueMatcher.forward (inference.py:192-209) on og_match_fwd's output: every
+ *                        (b, i) with matches0[b, i] >= 0, in pair-major then i order (deterministic) ->
+ *                          pair [B n] int64 (batch_indexes), ij [B n, 2] int64 (i, j = original_matching_idxs),
+ *                          confidence [B n] = mscores0[b, i], out_lafs0/1 [B n, 2, 3] = lafs0[b, i] / lafs1[b, j],
+ *                          out_kpts0/1 [B n, 2] = their centres;  total [1] int64 = the number of matches (rows past it are
+ *                          not written).  matches0 [B,n] int64, mscores0 [B,n], lafs0 [B,n,2,3], lafs1 [B,m,2,3].
+ *                        The predicate is matches0 >= 0, never the score: a mutual match whose exp underflowed to 0 is kept
+ *                        when the threshold is negative.                                                             */
+typedef enum og_laf_method {
+  OG_LAF_NONE = 0, OG_LAF_SCALE = 1, OG_LAF_ROTATION = 2, OG_LAF_SCALE_ROTATION = 3, OG_LAF_AFFINE = 4
+} og_laf_method;
+int og_prepare_features(const float* lafs, const float* responses, int64_t R, int method, int log_response, float* kpts, float* side,
+                        void* stream);
+int og_match_compact(const int64_t* matches0, const float* mscores0, const float* lafs0, const float* lafs1, int B, int n, int m,
+                     int64_t* pair, int64_t* ij, float* confidence, float* out_lafs0, float* out_lafs1, float* out_kpts0,
+                     float* out_kpts1, int64_t* total, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,9 +11,12 @@ and the steps either side of those:
     matching_log_probs(S, dustbin_score, num_iters, reg)      (differentiable Sinkhorn: forward + backward kernels)
     SuperGlue(config).train()(data)                           (training mode: batch-statistics BatchNorm, explicit backward pass)
     SuperPointNet(max_keypoints, ...)(image) -> (lafs, scores, descriptors)   (the detector / descriptor front-end; SuperPointNetBn: its BatchNorm variant)
+    prepare_features_output(lafs, responses, desc, get_laf_to_sideinfo_converter(method), ...)   (front-end output -> SuperGlue input)
+    OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
 """
 from .gt_matches import generate_gt_matches  # noqa: F401
 from .feature_cache import FeatureStore, collate_features  # noqa: F401
+from .features import OpenGlueMatcher, get_laf_to_sideinfo_converter, prepare_features_output  # noqa: F401
 from .losses import criterion  # noqa: F401
 from .sinkhorn import matching_log_probs  # noqa: F401
 from .superglue import MatchingCore, PendingMatches, SuperGlue  # noqa: F401

@@ -114,6 +114,9 @@ SYMBOLS = {
     'og_sp_compact': (_I, [_P, _I, _I, _I, _P, _P, _P, _P]),
     'og_sp_select': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P]),
     'og_sp_sample_desc': (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P]),
+    # local features -> matcher inputs, matches -> compact list
+    'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
+    'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

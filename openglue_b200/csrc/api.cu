@@ -13,6 +13,7 @@
 #include "collate.cuh"
 #include "train_ops.cuh"
 #include "superpoint.cuh"
+#include "features.cuh"
 #include <math.h>
 #include <string.h>
 #include <vector>
@@ -604,6 +605,32 @@ int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const f
   if (max_n <= 0) return OG_OK;
   sp_sample_desc_kernel<<<dim3(cdiv(max_n, 8), B), 256, 0, (cudaStream_t)stream>>>(coarse, Hc, Wc, D, kpts, n_out, out_cap, cell, desc);
   OG_LAUNCH_CHECK("sp_sample_desc_kernel");
+  launch_counter()++;
+  return OG_OK;
+}
+
+// ---- local features -> matcher inputs, matches -> compact list (csrc/features.cuh) ----
+int og_prepare_features(const float* lafs, const float* responses, int64_t R, int method, int log_response, float* kpts, float* side,
+                        void* stream) {
+  OG_CHECK_ARG(method >= OG_LAF_NONE && method <= OG_LAF_AFFINE, "prepare_features: unknown LAF method %d", method);
+  const int width = (responses ? 1 : 0) + laf_side_dim(method);
+  OG_CHECK_ARG(lafs && R >= 0 && (width == 0 || side), "prepare_features: bad arguments");
+  if (R == 0 || (width == 0 && !kpts)) return OG_OK;
+  prepare_features_kernel<<<(unsigned)((R + 255) / 256), 256, 0, (cudaStream_t)stream>>>(lafs, responses, R, method, log_response, kpts,
+                                                                                          side, width);
+  OG_LAUNCH_CHECK("prepare_features_kernel");
+  launch_counter()++;
+  return OG_OK;
+}
+int og_match_compact(const int64_t* matches0, const float* mscores0, const float* lafs0, const float* lafs1, int B, int n, int m,
+                     int64_t* pair, int64_t* ij, float* confidence, float* out_lafs0, float* out_lafs1, float* out_kpts0,
+                     float* out_kpts1, int64_t* total, void* stream) {
+  OG_CHECK_ARG(matches0 && mscores0 && lafs0 && lafs1 && pair && ij && confidence && out_lafs0 && out_lafs1 && out_kpts0 && out_kpts1 && total,
+               "match_compact: null pointer");
+  OG_CHECK_ARG(B > 0 && n > 0 && m > 0 && (int64_t)B * n <= INT32_MAX - 1024, "match_compact: bad sizes");
+  match_compact_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(matches0, mscores0, lafs0, lafs1, B * n, n, m, pair, ij, confidence, out_lafs0,
+                                                             out_lafs1, out_kpts0, out_kpts1, total);
+  OG_LAUNCH_CHECK("match_compact_kernel");
   launch_counter()++;
   return OG_OK;
 }

@@ -71,6 +71,24 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// One step of an ordered (stable) compaction by one CTA: every thread holds one element of a chunk, in thread order, flagged by
+// `on`.  Returns the element's output slot (meaningful where `on`): `base` + the number of flagged elements before it in the
+// chunk; then advances the shared running count `base` by the chunk's total.  Ballot per warp, a serial scan of the warp totals
+// (`warp_tot`: shared, one int per warp).  Called by every thread of the CTA.
+__device__ __forceinline__ int cta_ordered_slot(bool on, int* warp_tot, int& base) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned bal = __ballot_sync(0xffffffffu, on);
+  if (lane == 0) warp_tot[warp] = __popc(bal);
+  __syncthreads();
+  int before = 0;
+  for (int w = 0; w < warp; ++w) before += warp_tot[w];
+  const int pos = base + before + __popc(bal & ((1u << lane) - 1u));
+  __syncthreads();
+  if (threadIdx.x == blockDim.x - 1) base = pos + (on ? 1 : 0);
+  __syncthreads();
+  return pos;
+}
+
 __device__ __forceinline__ float ex2_approx(float x) {
   float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y;
 }

@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(1024) sp_compact_kernel(const float* __restric
                                                           float* __restrict__ cand_score, int* __restrict__ count) {
   __shared__ int warp_tot[32];
   __shared__ int base;
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = blockIdx.x, tid = threadIdx.x;
   const float* h = heat + (int64_t)b * HW;
   if (tid == 0) base = 0;
   __syncthreads();
@@ -118,16 +118,8 @@ __global__ void __launch_bounds__(1024) sp_compact_kernel(const float* __restric
     const int p = p0 + tid;
     const float v = p < HW ? h[p] : 0.f;
     const bool on = v != 0.f;
-    const unsigned bal = __ballot_sync(0xffffffffu, on);
-    if (lane == 0) warp_tot[warp] = __popc(bal);
-    __syncthreads();
-    int before = 0;
-    for (int w = 0; w < warp; ++w) before += warp_tot[w];
-    const int pos = base + before + __popc(bal & ((1u << lane) - 1u));
+    const int pos = cta_ordered_slot(on, warp_tot, base);
     if (on && pos < cap) { cand_idx[(int64_t)b * cap + pos] = p; cand_score[(int64_t)b * cap + pos] = v; }
-    __syncthreads();
-    if (tid == 1023) base = pos + (on ? 1 : 0);
-    __syncthreads();
   }
   if (tid == 0) count[b] = base;
 }

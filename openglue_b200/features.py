@@ -1,0 +1,194 @@
+"""Local features -> matcher inputs, and the stand-alone image-pair matcher.  Drop-ins for the reference's
+
+    models.laf_converter.get_laf_to_sideinfo_converter(method_name)       (models/laf_converter.py:108-128)
+    models.features.utils.prepare_features_output(lafs, responses, desc, laf_converter, permute_desc, log_response)   (utils.py:54-65)
+    inference.OpenGlueMatcher(local_feature, matcher, match_config)       (inference.py:81-211)
+
+The geometry of each keypoint's local affine frame (LAF) - log-scale, orientation or the full affine shape - becomes the side
+information the keypoint encoder of ``SuperGlue`` takes next to the response.  ``prepare_features_output`` is ONE launch of
+``og_prepare_features`` (csrc/features.cuh): keypoints and side information come out of the same pass over the LAFs, and every
+column except the logarithms equals the reference's fp32 result bit for bit (the square root is the correctly rounded one, which
+ATen's vectorised CPU form misses by an ulp on a few frames in a thousand).  ``OpenGlueMatcher`` runs an image pair (or
+pre-extracted features) through the front-end, this step, ``SuperGlue`` with ``MatchingCore``'s match extraction, and the ordered
+compaction ``og_match_compact`` to the reference's compact match list; reading the number of matches is its one host
+synchronisation, where the reference's boolean indexing synchronises too.
+
+CUDA tensors only, and no autograd: the reference never differentiates these outputs.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Dict
+
+import torch
+import torch.nn as nn
+
+from . import _cabi
+from .superglue import SuperGlue
+
+__all__ = ['LAFConverter', 'get_laf_to_sideinfo_converter', 'prepare_features_output', 'compact_matches', 'OpenGlueMatcher']
+
+# method name -> (og_laf_method, side-information columns after the response)
+_METHODS = {'none': (0, 0), 'scale': (1, 1), 'rotation': (2, 2), 'scale_rotation': (3, 3), 'affine': (4, 5)}
+
+
+def _p(t):
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def _st(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _device_f32(t: torch.Tensor, name: str) -> torch.Tensor:
+    if not torch.is_tensor(t) or t.device.type != 'cuda':
+        raise RuntimeError(f'openglue_b200: {name} must be a CUDA tensor (sm_90a); there is no CPU path')
+    t = t.detach()
+    return (t if t.dtype == torch.float32 else t.float()).contiguous()
+
+
+def _lafs(lafs: torch.Tensor) -> torch.Tensor:
+    lafs = _device_f32(lafs, 'lafs')
+    if lafs.dim() != 4 or lafs.shape[2:] != (2, 3):
+        raise ValueError(f'lafs must be [B, N, 2, 3], got {tuple(lafs.shape)}')
+    return lafs
+
+
+class LAFConverter:
+    """LAF -> side information for one method (the reference's ``LAFConverter`` with its conversion functions):
+    ``side_info_dim`` columns per keypoint, ``__call__(lafs [B,N,2,3]) -> [B,N,side_info_dim]``."""
+
+    def __init__(self, method: str):
+        self.method = method
+        self._code, self._dim = _METHODS[method]
+
+    @property
+    def side_info_dim(self) -> int:
+        return self._dim
+
+    def __call__(self, lafs: torch.Tensor) -> torch.Tensor:
+        lafs = _lafs(lafs)
+        B, N = lafs.shape[:2]
+        out = torch.empty(B, N, self._dim, dtype=torch.float32, device=lafs.device)
+        if self._dim and B * N:
+            with torch.cuda.device(lafs.device):
+                _cabi.check(_cabi.lib().og_prepare_features(_p(lafs), None, B * N, self._code, 0, None, _p(out), _st(lafs.device)),
+                            'og_prepare_features')
+        return out
+
+    def __repr__(self):
+        return f'LAFConverter({self.method!r})'
+
+
+def get_laf_to_sideinfo_converter(method_name: str = 'none') -> LAFConverter:
+    """The converter ``superglue.laf_to_sideinfo_method`` names: 'none' | 'scale' | 'rotation' | 'scale_rotation' | 'affine'
+    (case-insensitive; anything else raises the reference's ``NameError``)."""
+    name = method_name.lower()
+    if name not in _METHODS:
+        raise NameError('Unexpected name for the method: {}'.format(method_name))
+    return LAFConverter(name)
+
+
+def prepare_features_output(lafs, responses, desc, laf_converter: LAFConverter, permute_desc: bool = False,
+                            log_response: bool = False) -> Dict[str, torch.Tensor]:
+    """-> {'keypoints' [B,N,2], 'side_info' [B,N,1+dim], 'local_descriptors'}: the reference's dict, from one kernel launch.
+    side_info = [response (log(response + 0.1) when ``log_response``), laf_converter(lafs)]."""
+    if not isinstance(laf_converter, LAFConverter):
+        raise TypeError('laf_converter must come from openglue_b200.get_laf_to_sideinfo_converter')
+    lafs = _lafs(lafs)
+    B, N = lafs.shape[:2]
+    responses = _device_f32(responses, 'responses')
+    if tuple(responses.shape) != (B, N):
+        raise ValueError(f'responses must be [B, N] = {(B, N)}, got {tuple(responses.shape)}')
+    if not torch.is_tensor(desc) or desc.device.type != 'cuda':
+        raise RuntimeError('openglue_b200: desc must be a CUDA tensor (sm_90a); there is no CPU path')
+    dev = lafs.device
+    kpts = torch.empty(B, N, 2, dtype=torch.float32, device=dev)
+    side = torch.empty(B, N, 1 + laf_converter.side_info_dim, dtype=torch.float32, device=dev)
+    if B * N:
+        with torch.cuda.device(dev):
+            _cabi.check(_cabi.lib().og_prepare_features(_p(lafs), _p(responses), B * N, laf_converter._code, int(bool(log_response)),
+                                                        _p(kpts), _p(side), _st(dev)), 'og_prepare_features')
+    return {'keypoints': kpts, 'side_info': side, 'local_descriptors': desc.permute(0, 2, 1) if permute_desc else desc}
+
+
+def compact_matches(matches0: torch.Tensor, mscores0: torch.Tensor, lafs0: torch.Tensor, lafs1: torch.Tensor) -> Dict[str, torch.Tensor]:
+    """The compact match list of ``OpenGlueMatcher.forward`` (inference.py:192-209) from ``matches0`` [B,n] (-1: no match) and
+    ``matching_scores0`` [B,n]: every (b, i) with ``matches0[b, i] >= 0``, pair-major then by i, as the reference's boolean
+    indexing orders them.  One kernel launch, then one read of the count."""
+    dev = matches0.device
+    if dev.type != 'cuda':
+        raise RuntimeError('openglue_b200: matches0 must be a CUDA tensor (sm_90a); there is no CPU path')
+    matches0 = matches0.detach().long().contiguous()
+    mscores0 = _device_f32(mscores0, 'matching_scores0')
+    lafs0, lafs1 = _lafs(lafs0), _lafs(lafs1)
+    B, n = matches0.shape
+    m = lafs1.shape[1]
+    if tuple(mscores0.shape) != (B, n) or lafs0.shape[:2] != (B, n) or lafs1.shape[0] != B:
+        raise ValueError('inconsistent batch / keypoint counts')
+    cap = B * n
+    i64 = dict(dtype=torch.int64, device=dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    pair, ij, conf = torch.empty(cap, **i64), torch.empty(cap, 2, **i64), torch.empty(cap, **f32)
+    l0, l1 = torch.empty(cap, 2, 3, **f32), torch.empty(cap, 2, 3, **f32)
+    k0, k1 = torch.empty(cap, 2, **f32), torch.empty(cap, 2, **f32)
+    total = torch.empty(1, **i64)
+    if cap and m:
+        with torch.cuda.device(dev):
+            _cabi.check(_cabi.lib().og_match_compact(_p(matches0), _p(mscores0), _p(lafs0), _p(lafs1), B, n, m, _p(pair), _p(ij), _p(conf),
+                                                     _p(l0), _p(l1), _p(k0), _p(k1), _p(total), _st(dev)), 'og_match_compact')
+        nc = int(total.item())                  # the one host synchronisation (the reference's boolean indexing)
+    else:
+        nc = 0
+    return {'original_matching_idxs': ij[:nc], 'batch_indexes': pair[:nc], 'confidence': conf[:nc],
+            'lafs0': l0[:nc][None], 'lafs1': l1[:nc][None], 'keypoints0': k0[:nc], 'keypoints1': k1[:nc]}
+
+
+class OpenGlueMatcher(nn.Module):
+    """Drop-in for the reference's ``inference.OpenGlueMatcher`` (inference.py:81-211): correspondences between two images from
+    local features followed by SuperGlue.
+
+    ``local_feature``: the front-end, ``image [B,1,H,W] -> (lafs, responses, descriptors)`` (e.g. ``openglue_b200.SuperPointNet``);
+    ``matcher``: an ``openglue_b200.SuperGlue``; ``match_config``: the reference's config with ``superglue.laf_to_sideinfo_method``,
+    optional ``superglue.log_transform_response`` and ``inference.match_threshold``.
+
+    ``forward(data)`` takes ``image0`` / ``image1`` [B,1,H,W] and, optionally, pre-extracted ``lafs{0,1}``, ``descriptors{0,1}``,
+    ``responses{0,1}`` (the images then only give their sizes); it sets ``data['image{0,1}_size']`` as the reference does and
+    returns ``original_matching_idxs`` [NC,2], ``batch_indexes`` [NC], ``confidence`` [NC], ``lafs0`` / ``lafs1`` [1,NC,2,3],
+    ``keypoints0`` / ``keypoints1`` [NC,2]."""
+
+    def __init__(self, local_feature: nn.Module, matcher: SuperGlue, match_config: Dict = {}) -> None:
+        super().__init__()
+        if not isinstance(matcher, SuperGlue):
+            raise TypeError('openglue_b200.OpenGlueMatcher takes an openglue_b200.SuperGlue as its matcher')
+        self.local_feature = local_feature
+        self.laf_converter = get_laf_to_sideinfo_converter(match_config['superglue']['laf_to_sideinfo_method'])
+        self.matcher = matcher
+        self.match_config = match_config
+        self.eval()
+
+    def extract_features(self, image: torch.Tensor, mask=None) -> Dict[str, torch.Tensor]:
+        lafs, resps, descs = self.local_feature(image)
+        return {'lafs': lafs, 'responses': resps, 'descriptors': descs}
+
+    @torch.no_grad()
+    def forward(self, data: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        feats = []
+        for i in (0, 1):
+            if f'lafs{i}' not in data or f'descriptors{i}' not in data:
+                f = self.extract_features(data[f'image{i}'])
+                feats.append((f['lafs'], f['descriptors'], f['responses']))
+            else:
+                feats.append((data[f'lafs{i}'], data[f'descriptors{i}'], data[f'responses{i}']))
+        (lafs0, descs0, resps0), (lafs1, descs1, resps1) = feats
+        _, _, h0, w0 = data['image0'].shape
+        _, _, h1, w1 = data['image1'].shape
+        data['image0_size'], data['image1_size'] = [w0, h0], [w1, h1]
+        log_response = self.match_config['superglue'].get('log_transform_response', False)
+        f0 = prepare_features_output(lafs0, resps0, descs0, self.laf_converter, log_response=log_response)
+        f1 = prepare_features_output(lafs1, resps1, descs1, self.laf_converter, log_response=log_response)
+        inputs = {**data, **{k + '0': v for k, v in f0.items()}, **{k + '1': v for k, v in f1.items()}}
+        # MatchingCore's path: SuperGlue + mutual-argmax extraction in one call
+        res = self.matcher.run(inputs, want_matches=True, want_context=False,
+                               match_threshold=float(self.match_config['inference']['match_threshold']))
+        return compact_matches(res['matches0'], res['matching_scores0'], lafs0, lafs1)
