@@ -422,6 +422,20 @@ int og_match_compact(const int64_t* matches0, const float* mscores0, const float
                      int64_t* pair, int64_t* ij, float* confidence, float* out_lafs0, float* out_lafs1, float* out_kpts0,
                      float* out_kpts1, int64_t* total, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Homography-pretraining image pairs (OxfordParis1MDataset.__getitem__, data/oxford_paris_dataset.py:27-66, without the decode,
+ * the INTER_AREA resize and the colour augmentation).  One launch for B images:
+ *   rgb [B,H,W,3] uint8 (rows of 3 W bytes, no alignment required);  warp_offset [B,4,2] int32 device, (x, y) per corner in the
+ *   order (off, off), (off, H-off-1), (W-off-1, off), (W-off-1, H-off-1), each in [-offset, offset) (the caller checks the range)
+ *   -> image0 [B,h,w] fp32 = gray(crop) / 255,  image1 [B,h,w] = gray(crop(warpPerspective(rgb, H_warp))) / 255,
+ *      H_true [B,3,3] fp32 (the homography relating the crops),  h = H - 2 offset, w = W - 2 offset.
+ *   cv2's arithmetic throughout (getPerspectiveTransform by LU, warpPerspective's fixed-point INTER_LINEAR with a constant-0
+ *   border, cvtColor RGB2GRAY): equal to cv2 4.13 bit for bit wherever its LU solve succeeds.  A pivot below 100 DBL_EPSILON
+ *   gives H = [[0,0,0],[0,0,0],[0,0,1]] (OpenCV's LU rule; cv2 4.13 falls back to an SVD there instead); no error is reported.
+ *   OG_EINVAL without a launch: a null pointer, B outside [1, 65535], offset < 1 or 2 offset >= min(H, W).                   */
+int og_homography_pairs(const uint8_t* rgb, int B, int H, int W, int offset, const int32_t* warp_offset, float* image0, float* image1,
+                        float* H_true, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,8 +13,10 @@ and the steps either side of those:
     SuperPointNet(max_keypoints, ...)(image) -> (lafs, scores, descriptors)   (the detector / descriptor front-end; SuperPointNetBn: its BatchNorm variant)
     prepare_features_output(lafs, responses, desc, get_laf_to_sideinfo_converter(method), ...)   (front-end output -> SuperGlue input)
     OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
+    synthesize_homography_pairs(images_u8, offset, warp_offset, generator)   (the homography-pretraining dataset's pairs, batched)
 """
 from .gt_matches import generate_gt_matches  # noqa: F401
+from .homography import synthesize_homography_pairs  # noqa: F401
 from .feature_cache import FeatureStore, collate_features  # noqa: F401
 from .features import OpenGlueMatcher, get_laf_to_sideinfo_converter, prepare_features_output  # noqa: F401
 from .losses import criterion  # noqa: F401

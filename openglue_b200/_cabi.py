@@ -117,6 +117,8 @@ SYMBOLS = {
     # local features -> matcher inputs, matches -> compact list
     'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    # homography-pretraining pairs
+    'og_homography_pairs': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -14,6 +14,7 @@
 #include "train_ops.cuh"
 #include "superpoint.cuh"
 #include "features.cuh"
+#include "homography.cuh"
 #include <math.h>
 #include <string.h>
 #include <vector>
@@ -631,6 +632,22 @@ int og_match_compact(const int64_t* matches0, const float* mscores0, const float
   match_compact_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(matches0, mscores0, lafs0, lafs1, B * n, n, m, pair, ij, confidence, out_lafs0,
                                                              out_lafs1, out_kpts0, out_kpts1, total);
   OG_LAUNCH_CHECK("match_compact_kernel");
+  launch_counter()++;
+  return OG_OK;
+}
+
+// ---- homography-pretraining pairs (csrc/homography.cuh) ----
+int og_homography_pairs(const uint8_t* rgb, int B, int H, int W, int offset, const int32_t* warp_offset, float* image0, float* image1,
+                        float* H_true, void* stream) {
+  OG_CHECK_ARG(rgb && warp_offset && image0 && image1 && H_true, "homography_pairs: null pointer");
+  OG_CHECK_ARG(B >= 1 && B <= 65535, "homography_pairs: B = %d must be in [1, 65535]", B);
+  OG_CHECK_ARG(offset >= 1 && H > 0 && W > 0 && 2 * (int64_t)offset < (H < W ? H : W),
+               "homography_pairs: offset %d must be >= 1 with 2 offset < min(H, W) = min(%d, %d)", offset, H, W);
+  OG_CHECK_ARG((int64_t)HG_ROWS * W <= INT32_MAX, "homography_pairs: W = %d too large", W);
+  const int h = H - 2 * offset;
+  homography_pairs_kernel<<<dim3(cdiv(h, HG_ROWS), B), HG_THREADS, 0, (cudaStream_t)stream>>>(rgb, H, W, offset, hg_block_width(H, W),
+                                                                                               warp_offset, image0, image1, H_true);
+  OG_LAUNCH_CHECK("homography_pairs_kernel");
   launch_counter()++;
   return OG_OK;
 }
