@@ -141,7 +141,8 @@ int og_superglue_forward_f16(const og_config* cfg, const float* packed_weights,
                              int64_t* matches1, float* mscores1,
                              void* workspace, int64_t workspace_bytes, void* stream);
 
-/* Number of kernel launches the last og_superglue_forward on this thread enqueued. */
+/* Number of kernels this thread has enqueued since the last og_superglue_forward (or _f16) began, that forward's own
+ * launches included.  Every operator entry point adds the kernels it launches.                                      */
 int og_last_forward_launches(void);
 
 /* Kernel-variant switches kept for callers of earlier builds.  sm_90 has no CTA-pair MMA, so there is one GEMM and one

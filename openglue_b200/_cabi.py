@@ -10,6 +10,8 @@ import ctypes as C
 import os
 from typing import Optional
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libopenglue_b200.so')
 
@@ -149,6 +151,24 @@ def check(rc: int, what: str) -> None:
     if rc != OG_OK:
         msg = lib().og_last_error()
         raise OpenGlueB200Error(f'{what} failed with status {rc}: {msg.decode() if msg else "?"}')
+
+
+def check_size(n: int, what: str) -> int:
+    """The result of a ``*_workspace_bytes`` / ``*_floats`` query; a negative one (rejected arguments) raises."""
+    n = int(n)
+    if n < 0:
+        check(n, what)
+    return n
+
+
+def ptr(t: Optional[torch.Tensor], off: int = 0) -> Optional[C.c_void_p]:
+    """Device pointer to element ``off`` of ``t`` (None for None), as the C ABI takes it."""
+    return None if t is None else C.c_void_p(t.data_ptr() + off * t.element_size())
+
+
+def stream(dev=None) -> C.c_void_p:
+    """The current CUDA stream of ``dev`` (default: the current device), as the C ABI takes it."""
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def make_config(config: dict, match_threshold: float = 0.2, precision: int = OG_PREC_FP32) -> OgConfig:

@@ -9,10 +9,7 @@ from typing import Dict
 import torch
 
 from . import _cabi
-
-
-def _p(t, off: int = 0):
-    return None if t is None else C.c_void_p(t.data_ptr() + 4 * off)
+from ._cabi import ptr
 
 
 def _pad4(n: int) -> int:
@@ -28,7 +25,7 @@ class _Ops:
         self._ws: Dict[int, torch.Tensor] = {}
 
     def st(self):
-        return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        return _cabi.stream(self.dev)
 
     def empty(self, *shape):
         return torch.empty(*shape, dtype=torch.float32, device=self.dev)
@@ -39,7 +36,7 @@ class _Ops:
     def ws(self, cols: int) -> torch.Tensor:
         t = self._ws.get(cols)
         if t is None:
-            t = self._ws[cols] = self.empty(int(self.lib.og_train_workspace_floats(cols)))
+            t = self._ws[cols] = self.empty(_cabi.check_size(self.lib.og_train_workspace_floats(cols), 'og_train_workspace_floats'))
         return t
 
     # ---- Y[b] = alpha [A | A2][b] . W[b]^T + bias (+ relu) (+ R[b]);  pointers = (tensor, float offset) ----
@@ -47,21 +44,21 @@ class _Ops:
              relu=False, alpha=1.0, R=None, ldr=0, r_off=0, batch=1, strideA=0, strideA2=0, strideW=0, strideY=0, strideR=0,
              Yt=None, ldyt=0, strideYt=0, yt_off=0):
         a = _cabi.OgLinearArgs()
-        a.A, a.lda, a.strideA = _p(A, a_off), lda, strideA
-        a.A2, a.lda2, a.strideA2 = _p(A2, a2_off), lda2, strideA2
+        a.A, a.lda, a.strideA = ptr(A, a_off), lda, strideA
+        a.A2, a.lda2, a.strideA2 = ptr(A2, a2_off), lda2, strideA2
         a.k1, a.k2 = k1, k2
-        a.W, a.ldw, a.strideW = _p(W, w_off), ldw, strideW
-        a.bias = _p(bias)
+        a.W, a.ldw, a.strideW = ptr(W, w_off), ldw, strideW
+        a.bias = ptr(bias)
         a.rows, a.nout, a.batch = rows, nout, batch
         a.alpha, a.relu = float(alpha), int(relu)
-        a.R, a.ldr, a.strideR = _p(R, r_off), ldr, strideR
+        a.R, a.ldr, a.strideR = ptr(R, r_off), ldr, strideR
         a.rscale = None
-        a.Y, a.ldy, a.strideY = _p(Y, y_off), ldy, strideY
-        a.Yt, a.ldyt, a.strideYt = _p(Yt, yt_off), ldyt, strideYt
+        a.Y, a.ldy, a.strideY = ptr(Y, y_off), ldy, strideY
+        a.Yt, a.ldyt, a.strideYt = ptr(Yt, yt_off), ldyt, strideYt
         scratch = None
         if self.prec != _cabi.OG_PREC_FP32:
             scratch = self.empty(max(int(self.lib.og_linear_auto_scratch_floats(C.byref(a))), 4))
-        _cabi.check(self.lib.og_linear_auto_fwd(C.byref(a), self.prec, _p(scratch), self.st()), 'og_linear_auto_fwd')
+        _cabi.check(self.lib.og_linear_auto_fwd(C.byref(a), self.prec, ptr(scratch), self.st()), 'og_linear_auto_fwd')
 
     def linear(self, X, W, bias=None, *, relu=False, A2=None, R=None, out=None):
         """X [rows, k1] (| A2 [rows, k2]) . W[nout, k1 + k2]^T + bias (+ R) -> [rows, nout]"""
@@ -85,22 +82,22 @@ class _Ops:
     def colsum(self, X, Y=None, Z=None):
         rows, cols = X.shape
         out = self.empty(cols)
-        _cabi.check(self.lib.og_colsum(_p(X), X.stride(0), _p(Y), Y.stride(0) if Y is not None else 0, _p(Z), Z.stride(0) if Z is not None else 0,
-                                       rows, cols, _p(out), _p(self.ws(cols)), self.st()), 'og_colsum')
+        _cabi.check(self.lib.og_colsum(ptr(X), X.stride(0), ptr(Y), Y.stride(0) if Y is not None else 0, ptr(Z), Z.stride(0) if Z is not None else 0,
+                                       rows, cols, ptr(out), ptr(self.ws(cols)), self.st()), 'og_colsum')
         return out
 
     def axpby(self, x, y, a=1.0, b=1.0, out=None):
         out = out if out is not None else torch.empty_like(x)
-        _cabi.check(self.lib.og_axpby(_p(x), _p(y), float(a), float(b), _p(out), x.numel(), self.st()), 'og_axpby')
+        _cabi.check(self.lib.og_axpby(ptr(x), ptr(y), float(a), float(b), ptr(out), x.numel(), self.st()), 'og_axpby')
         return out
 
     def transpose_raw(self, X, x_off, ld_in, stride_in, out, ld_out, stride_out, batch, rows, cols, transpose):
-        _cabi.check(self.lib.og_transpose(_p(X, x_off), ld_in, stride_in, _p(out), ld_out, stride_out, batch, rows, cols, int(transpose), self.st()),
+        _cabi.check(self.lib.og_transpose(ptr(X, x_off), ld_in, stride_in, ptr(out), ld_out, stride_out, batch, rows, cols, int(transpose), self.st()),
                     'og_transpose')
 
     def kenc_input(self, kpts, side, rows, S, width, height):
         out = self.empty(rows, 2 + S)
-        _cabi.check(self.lib.og_kenc_input(_p(kpts), _p(side) if S else None, rows, S, float(width), float(height), _p(out), self.st()), 'og_kenc_input')
+        _cabi.check(self.lib.og_kenc_input(ptr(kpts), ptr(side) if S else None, rows, S, float(width), float(height), ptr(out), self.st()), 'og_kenc_input')
         return out
 
     def attention(self, q, k, v, B, nq, nk, H, dh):
@@ -110,80 +107,76 @@ class _Ops:
         o = self.empty(B * nq, d)
         if self.prec != _cabi.OG_PREC_FP32 and dh in (32, 64):
             khi, klo = torch.empty_like(k), torch.empty_like(k)
-            _cabi.check(self.lib.og_split_tf32(_p(k), _p(khi), _p(klo), k.numel(), self.st()), 'og_split_tf32')
+            _cabi.check(self.lib.og_split_tf32(ptr(k), ptr(khi), ptr(klo), k.numel(), self.st()), 'og_split_tf32')
             vt = self.transpose(v, batch=B, rows=nk, cols=d)            # [B, d, pad4(nk)], zero padded
             vthi, vtlo = torch.empty_like(vt), torch.empty_like(vt)
-            _cabi.check(self.lib.og_split_tf32(_p(vt), _p(vthi), _p(vtlo), vt.numel(), self.st()), 'og_split_tf32')
-            _cabi.check(self.lib.og_attention_tc_fwd(_p(q), d, nq * d, _p(khi), _p(klo), d, _p(vthi), _p(vtlo), vt.shape[2], _p(o), d, nq * d,
+            _cabi.check(self.lib.og_split_tf32(ptr(vt), ptr(vthi), ptr(vtlo), vt.numel(), self.st()), 'og_split_tf32')
+            _cabi.check(self.lib.og_attention_tc_fwd(ptr(q), d, nq * d, ptr(khi), ptr(klo), d, ptr(vthi), ptr(vtlo), vt.shape[2], ptr(o), d, nq * d,
                                                      B, nq, nk, H, dh, self.st()), 'og_attention_tc_fwd')
             return o
-        _cabi.check(self.lib.og_attention_fwd(_p(q), d, nq * d, _p(k), d, nk * d, _p(v), d, nk * d, _p(o), d, nq * d, B, nq, nk, H, dh,
+        _cabi.check(self.lib.og_attention_fwd(ptr(q), d, nq * d, ptr(k), d, nk * d, ptr(v), d, nk * d, ptr(o), d, nq * d, B, nq, nk, H, dh,
                                               _cabi.OG_PREC_FP32, self.st()), 'og_attention_fwd')
         return o
 
     def softmax_rows(self, P, ld, rows, cols):
-        _cabi.check(self.lib.og_softmax_rows(_p(P), ld, rows, cols, self.st()), 'og_softmax_rows')
+        _cabi.check(self.lib.og_softmax_rows(ptr(P), ld, rows, cols, self.st()), 'og_softmax_rows')
 
     def softmax_bwd_rows(self, P, dP, ld, rows, cols, scale):
-        _cabi.check(self.lib.og_softmax_bwd_rows(_p(P), _p(dP), ld, rows, cols, float(scale), self.st()), 'og_softmax_bwd_rows')
+        _cabi.check(self.lib.og_softmax_bwd_rows(ptr(P), ptr(dP), ld, rows, cols, float(scale), self.st()), 'og_softmax_bwd_rows')
 
     def mix_fwd(self, g, l, mix):
         rows, d = g.shape
         out = self.empty(rows, d)
-        _cabi.check(self.lib.og_mix_fwd(_p(g), _p(l), _p(mix), _p(out), rows, d, self.st()), 'og_mix_fwd')
+        _cabi.check(self.lib.og_mix_fwd(ptr(g), ptr(l), ptr(mix), ptr(out), rows, d, self.st()), 'og_mix_fwd')
         return out
 
     def mix_bwd(self, dm, mix):
         rows, d = dm.shape
         dg, dl = self.empty(rows, d), self.empty(rows, d)
-        _cabi.check(self.lib.og_mix_bwd(_p(dm), _p(mix), _p(dg), _p(dl), rows, d, self.st()), 'og_mix_bwd')
+        _cabi.check(self.lib.og_mix_bwd(ptr(dm), ptr(mix), ptr(dg), ptr(dl), rows, d, self.st()), 'og_mix_bwd')
         return dg, dl
 
     def mix_param_grad(self, csum, mix):
         d = mix.numel()
         out = self.empty(d)
-        _cabi.check(self.lib.og_mix_param_grad(_p(csum), _p(mix), _p(out), d, self.st()), 'og_mix_param_grad')
+        _cabi.check(self.lib.og_mix_param_grad(ptr(csum), ptr(mix), ptr(out), d, self.st()), 'og_mix_param_grad')
         return out
 
     def bn_fwd(self, a, gamma, beta, eps, momentum, running_mean, running_var):
         rows, cols = a.shape
         y, mean, invstd = self.empty(rows, cols), self.empty(cols), self.empty(cols)
-        _cabi.check(self.lib.og_bn_train_fwd(_p(a), a.stride(0), rows, cols, 1, _p(gamma), _p(beta), float(eps), float(momentum), _p(y), cols,
-                                             _p(mean), _p(invstd), _p(running_mean), _p(running_var), _p(self.ws(cols)), self.st()), 'og_bn_train_fwd')
+        _cabi.check(self.lib.og_bn_train_fwd(ptr(a), a.stride(0), rows, cols, 1, ptr(gamma), ptr(beta), float(eps), float(momentum), ptr(y), cols,
+                                             ptr(mean), ptr(invstd), ptr(running_mean), ptr(running_var), ptr(self.ws(cols)), self.st()), 'og_bn_train_fwd')
         return y, mean, invstd
 
     def bn_bwd(self, dy, a, gamma, mean, invstd):
         rows, cols = a.shape
         da, dgamma, dbeta = self.empty(rows, cols), self.empty(cols), self.empty(cols)
-        _cabi.check(self.lib.og_bn_train_bwd(_p(dy), dy.stride(0), _p(a), a.stride(0), rows, cols, 1, _p(gamma), _p(mean), _p(invstd), _p(da), cols,
-                                             _p(dgamma), _p(dbeta), _p(self.ws(cols)), self.st()), 'og_bn_train_bwd')
+        _cabi.check(self.lib.og_bn_train_bwd(ptr(dy), dy.stride(0), ptr(a), a.stride(0), rows, cols, 1, ptr(gamma), ptr(mean), ptr(invstd), ptr(da), cols,
+                                             ptr(dgamma), ptr(dbeta), ptr(self.ws(cols)), self.st()), 'og_bn_train_bwd')
         return da, dgamma, dbeta
 
     def sinkhorn_fwd(self, Sp, dust, B, n, m, iters, reg):
         lib, lds = self.lib, Sp.shape[2]
         scores = self.empty(B, n + 1, m + 1)
         hist = self.empty(max(int(lib.og_sinkhorn_hist_floats(B, n, m, iters)), 1))
-        wsb = lib.og_sinkhorn_workspace_bytes(B, n, m)
-        if wsb < 0:
-            _cabi.check(int(wsb), 'og_sinkhorn_workspace_bytes')
+        wsb = _cabi.check_size(lib.og_sinkhorn_workspace_bytes(B, n, m), 'og_sinkhorn_workspace_bytes')
         ws = torch.empty(wsb, dtype=torch.uint8, device=self.dev)
-        _cabi.check(lib.og_sinkhorn_train_fwd(_p(Sp), lds, n * lds, _p(dust), B, n, m, iters, reg, _p(scores), _p(hist), _p(ws), wsb, self.st()),
+        _cabi.check(lib.og_sinkhorn_train_fwd(ptr(Sp), lds, n * lds, ptr(dust), B, n, m, iters, reg, ptr(scores), ptr(hist), ptr(ws), wsb, self.st()),
                     'og_sinkhorn_train_fwd')
         return scores, hist
 
     def sinkhorn_bwd(self, Sp, dust, hist, G, B, n, m, iters, reg):
         lib, lds = self.lib, Sp.shape[2]
         dZ, dd = self.empty(B, n + 1, m + 1), self.empty(1)
-        wsb = lib.og_sinkhorn_bwd_workspace_bytes(B, n, m, iters)
-        if wsb < 0:
-            _cabi.check(int(wsb), 'og_sinkhorn_bwd_workspace_bytes')
+        wsb = _cabi.check_size(lib.og_sinkhorn_bwd_workspace_bytes(B, n, m, iters), 'og_sinkhorn_bwd_workspace_bytes')
         ws = torch.empty(wsb, dtype=torch.uint8, device=self.dev)
-        _cabi.check(lib.og_sinkhorn_bwd(_p(Sp), lds, n * lds, _p(dust), B, n, m, iters, reg, _p(hist), _p(G), _p(dZ), _p(dd), _p(ws), wsb, self.st()),
+        _cabi.check(lib.og_sinkhorn_bwd(ptr(Sp), lds, n * lds, ptr(dust), B, n, m, iters, reg, ptr(hist), ptr(G), ptr(dZ), ptr(dd), ptr(ws), wsb, self.st()),
                     'og_sinkhorn_bwd')
         return dZ, dd
 
     def sum_batches(self, part, S, rows, cols, out, out_off, ld, accumulate=True):
-        _cabi.check(self.lib.og_sum_batches(_p(part), S, rows, cols, _p(out, out_off), ld, int(accumulate), self.st()), 'og_sum_batches')
+        _cabi.check(self.lib.og_sum_batches(ptr(part), S, rows, cols, ptr(out, out_off), ld, int(accumulate), self.st()), 'og_sum_batches')
 
     def _transpose_chunks(self, X, S, Kc):
         """[rows, cols] -> zero-padded [S, cols, Kc]: chunk s holds rows [s Kc, (s + 1) Kc) transposed"""

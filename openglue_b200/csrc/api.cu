@@ -289,9 +289,7 @@ int og_linear_auto_fwd(const og_linear_args* a, int precision, float* split_scra
     const int64_t wf = weight_floats(*a);
     float* hi = split_scratch; float* lo = split_scratch + align_up(wf, 64);
     if (linear_sm90_eligible(gemm_args<TcLinearArgs>(*a), hi, lo, a->ldw) && (reinterpret_cast<uintptr_t>(a->W) & 15) == 0) {
-      split_tf32_kernel<<<(unsigned)((wf + 255) / 256), 256, 0, st>>>(a->W, hi, lo, wf);
-      OG_LAUNCH_CHECK("split_tf32_kernel");
-      launch_counter()++;
+      if (const int rc = OG_LAUNCH(split_tf32_kernel, (unsigned)((wf + 255) / 256), 256, 0, st, a->W, hi, lo, wf)) return rc;
       return linear_tc_run(*a, hi, lo, SplitOut(), st);
     }
   }
@@ -300,9 +298,7 @@ int og_linear_auto_fwd(const og_linear_args* a, int precision, float* split_scra
 
 int og_split_tf32(const float* src, float* hi, float* lo, int64_t n, void* stream) {
   OG_CHECK_ARG(src && hi && lo && n > 0, "split_tf32: bad arguments");
-  split_tf32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(src, hi, lo, n);
-  OG_LAUNCH_CHECK("split_tf32_kernel");
-  return OG_OK;
+  return OG_LAUNCH(split_tf32_kernel, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, src, hi, lo, n);
 }
 
 int og_attention_fwd(const float* q, int64_t ldq, int64_t strideq, const float* k, int64_t ldk, int64_t stridek,
@@ -454,12 +450,10 @@ int og_bn_train_fwd(const float* a_, int64_t lda, int rows, int cols, int relu, 
   if (rc != OG_OK) return rc;
   r.mu = save_mean; r.out0 = var;
   if ((rc = colreduce_launch<2>(r, st)) != OG_OK) return rc;
-  bn_finish_stats_kernel<<<cdiv(cols, 256), 256, 0, st>>>(save_mean, var, cols, rows, eps, momentum, save_invstd, running_mean, running_var);
-  OG_LAUNCH_CHECK("bn_finish_stats_kernel");
-  bn_apply_kernel<<<eltwise_grid((int64_t)rows * cols), 256, 0, st>>>(a_, lda, rows, cols, relu, save_mean, save_invstd, gamma, beta, y, ldy);
-  OG_LAUNCH_CHECK("bn_apply_kernel");
-  launch_counter() += 2;
-  return OG_OK;
+  if ((rc = OG_LAUNCH(bn_finish_stats_kernel, cdiv(cols, 256), 256, 0, st, save_mean, var, cols, rows, eps, momentum, save_invstd,
+                      running_mean, running_var)) != OG_OK) return rc;
+  return OG_LAUNCH(bn_apply_kernel, eltwise_grid((int64_t)rows * cols), 256, 0, st, a_, lda, rows, cols, relu, save_mean, save_invstd, gamma,
+                   beta, y, ldy);
 }
 
 int og_bn_train_bwd(const float* dy, int64_t lddy, const float* a_, int64_t lda, int rows, int cols, int relu,
@@ -473,118 +467,80 @@ int og_bn_train_bwd(const float* dy, int64_t lddy, const float* a_, int64_t lda,
   r.partial = workspace + 2 * (int64_t)cols; r.out0 = dbeta; r.out1 = dgamma;
   int rc = colreduce_launch<3>(r, st);
   if (rc != OG_OK) return rc;
-  bn_bwd_apply_kernel<<<eltwise_grid((int64_t)rows * cols), 256, 0, st>>>(dy, lddy, a_, lda, rows, cols, relu, save_mean, save_invstd, gamma,
-                                                                            dgamma, dbeta, da, ldda);
-  OG_LAUNCH_CHECK("bn_bwd_apply_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(bn_bwd_apply_kernel, eltwise_grid((int64_t)rows * cols), 256, 0, st, dy, lddy, a_, lda, rows, cols, relu, save_mean,
+                   save_invstd, gamma, dgamma, dbeta, da, ldda);
 }
 
 int og_softmax_rows(float* S, int64_t ld, int64_t rows, int cols, void* stream) {
   OG_CHECK_ARG(S && rows >= 0 && cols > 0 && ld >= cols, "softmax_rows: bad arguments");
   if (rows == 0) return OG_OK;
   OG_CHECK_ARG((rows + 7) / 8 <= 0x7fffffffLL, "softmax_rows: too many rows");
-  softmax_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(S, ld, rows, cols);
-  OG_LAUNCH_CHECK("softmax_rows_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, S, ld, rows, cols);
 }
 
 int og_softmax_bwd_rows(const float* P, float* dP, int64_t ld, int64_t rows, int cols, float scale, void* stream) {
   OG_CHECK_ARG(P && dP && rows >= 0 && cols > 0 && ld >= cols, "softmax_bwd_rows: bad arguments");
   if (rows == 0) return OG_OK;
   OG_CHECK_ARG((rows + 7) / 8 <= 0x7fffffffLL, "softmax_bwd_rows: too many rows");
-  softmax_bwd_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(P, dP, ld, rows, cols, scale);
-  OG_LAUNCH_CHECK("softmax_bwd_rows_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(softmax_bwd_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, P, dP, ld, rows, cols, scale);
 }
 
 int og_sum_batches(const float* part, int S, int rows, int cols, float* out, int64_t ld_out, int accumulate, void* stream) {
   OG_CHECK_ARG(part && out && S > 0 && rows > 0 && cols > 0 && ld_out >= cols, "sum_batches: bad arguments");
-  sum_batches_kernel<<<eltwise_grid((int64_t)rows * cols), 256, 0, (cudaStream_t)stream>>>(part, S, rows, cols, out, ld_out, accumulate);
-  OG_LAUNCH_CHECK("sum_batches_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(sum_batches_kernel, eltwise_grid((int64_t)rows * cols), 256, 0, (cudaStream_t)stream, part, S, rows, cols, out, ld_out,
+                   accumulate);
 }
 
 int og_axpby(const float* x, const float* y, float a_, float b, float* out, int64_t n, void* stream) {
   OG_CHECK_ARG(x && out && n >= 0, "axpby: bad arguments");
   if (n == 0) return OG_OK;
-  axpby_kernel<<<eltwise_grid(n), 256, 0, (cudaStream_t)stream>>>(x, y, a_, b, out, n);
-  OG_LAUNCH_CHECK("axpby_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(axpby_kernel, eltwise_grid(n), 256, 0, (cudaStream_t)stream, x, y, a_, b, out, n);
 }
 
 int og_mix_fwd(const float* g, const float* l, const float* mix, float* out, int64_t rows, int d, void* stream) {
   OG_CHECK_ARG(g && l && mix && out && rows > 0 && d > 0, "mix_fwd: bad arguments");
-  mix_fwd_kernel<<<eltwise_grid(rows * d), 256, 0, (cudaStream_t)stream>>>(g, l, mix, out, rows, d);
-  OG_LAUNCH_CHECK("mix_fwd_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(mix_fwd_kernel, eltwise_grid(rows * d), 256, 0, (cudaStream_t)stream, g, l, mix, out, rows, d);
 }
 
 int og_mix_bwd(const float* dm, const float* mix, float* dg, float* dl, int64_t rows, int d, void* stream) {
   OG_CHECK_ARG(dm && mix && (dg || dl) && rows > 0 && d > 0, "mix_bwd: bad arguments");
-  mix_bwd_kernel<<<eltwise_grid(rows * d), 256, 0, (cudaStream_t)stream>>>(dm, mix, dg, dl, rows, d);
-  OG_LAUNCH_CHECK("mix_bwd_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(mix_bwd_kernel, eltwise_grid(rows * d), 256, 0, (cudaStream_t)stream, dm, mix, dg, dl, rows, d);
 }
 
 int og_mix_param_grad(const float* colsum, const float* mix, float* dmix, int d, void* stream) {
   OG_CHECK_ARG(colsum && mix && dmix && d > 0, "mix_param_grad: bad arguments");
-  mix_param_grad_kernel<<<cdiv(d, 256), 256, 0, (cudaStream_t)stream>>>(colsum, mix, dmix, d);
-  OG_LAUNCH_CHECK("mix_param_grad_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(mix_param_grad_kernel, cdiv(d, 256), 256, 0, (cudaStream_t)stream, colsum, mix, dmix, d);
 }
 
 int og_kenc_input(const float* kpts, const float* side, int rows, int side_info_size, float width, float height, float* out, void* stream) {
   OG_CHECK_ARG(kpts && out && rows > 0 && side_info_size >= 0 && (side_info_size == 0 || side), "kenc_input: bad arguments");
-  kenc_input_kernel<<<cdiv(rows, 256), 256, 0, (cudaStream_t)stream>>>(kpts, side, rows, side_info_size, width - 1.f, height - 1.f, out);
-  OG_LAUNCH_CHECK("kenc_input_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(kenc_input_kernel, cdiv(rows, 256), 256, 0, (cudaStream_t)stream, kpts, side, rows, side_info_size, width - 1.f,
+                   height - 1.f, out);
 }
 
 // ---- SuperPoint front-end operators (row f4; csrc/superpoint.cuh) ----
 int og_sp_im2col3x3(const float* x, int B, int H, int W, int C, float* out, void* stream) {
   OG_CHECK_ARG(x && out && B > 0 && H > 0 && W > 0 && C > 0, "sp_im2col3x3: bad arguments");
-  im2col3x3_kernel<<<sp_grid((int64_t)B * H * W * 9 * ((C % 4 == 0) ? C / 4 : C)), 256, 0, (cudaStream_t)stream>>>(x, B, H, W, C, out);
-  OG_LAUNCH_CHECK("im2col3x3_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(im2col3x3_kernel, sp_grid((int64_t)B * H * W * 9 * ((C % 4 == 0) ? C / 4 : C)), 256, 0, (cudaStream_t)stream, x, B, H, W,
+                   C, out);
 }
 int og_sp_maxpool2x2(const float* x, int B, int H, int W, int C, float* out, void* stream) {
   OG_CHECK_ARG(x && out && B > 0 && H > 0 && W > 0 && C > 0 && H % 2 == 0 && W % 2 == 0, "sp_maxpool2x2: bad arguments");
-  maxpool2x2_kernel<<<sp_grid((int64_t)B * (H / 2) * (W / 2) * C), 256, 0, (cudaStream_t)stream>>>(x, B, H, W, C, out);
-  OG_LAUNCH_CHECK("maxpool2x2_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(maxpool2x2_kernel, sp_grid((int64_t)B * (H / 2) * (W / 2) * C), 256, 0, (cudaStream_t)stream, x, B, H, W, C, out);
 }
 int og_row_normalize(float* x, int64_t rows, int C, int mode, float eps, void* stream) {
   OG_CHECK_ARG(x && rows >= 0 && C > 0 && (mode == 0 || mode == 1), "row_normalize: bad arguments");
   if (rows == 0) return OG_OK;
-  row_normalize_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x, rows, C, mode, eps);
-  OG_LAUNCH_CHECK("row_normalize_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(row_normalize_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, x, rows, C, mode, eps);
 }
 int og_sp_heat_nms(const float* probs, int B, int Hc, int Wc, int nms_kernel, float threshold, int border, float* heat, void* stream) {
   OG_CHECK_ARG(probs && heat && B > 0 && Hc > 0 && Wc > 0 && nms_kernel > 0 && nms_kernel % 2 == 1 && border >= 0, "sp_heat_nms: bad arguments");
-  sp_heat_nms_kernel<<<sp_grid((int64_t)B * Hc * Wc * 64), 256, 0, (cudaStream_t)stream>>>(probs, B, Hc, Wc, nms_kernel, threshold, border, heat);
-  OG_LAUNCH_CHECK("sp_heat_nms_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(sp_heat_nms_kernel, sp_grid((int64_t)B * Hc * Wc * 64), 256, 0, (cudaStream_t)stream, probs, B, Hc, Wc, nms_kernel,
+                   threshold, border, heat);
 }
 int og_sp_compact(const float* heat, int B, int HW, int cap, int* cand_idx, float* cand_score, int* count, void* stream) {
   OG_CHECK_ARG(heat && cand_idx && cand_score && count && B > 0 && HW > 0 && cap > 0, "sp_compact: bad arguments");
-  sp_compact_kernel<<<B, 1024, 0, (cudaStream_t)stream>>>(heat, HW, cap, cand_idx, cand_score, count);
-  OG_LAUNCH_CHECK("sp_compact_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(sp_compact_kernel, B, 1024, 0, (cudaStream_t)stream, heat, HW, cap, cand_idx, cand_score, count);
 }
 int og_sp_select(const int* cand_idx, const float* cand_score, const int* count, const int* n_out, const int* mode, int B, int cap, int W,
                  int out_cap, int max_count, float* kpts, float* scores, void* stream) {
@@ -595,19 +551,15 @@ int og_sp_select(const int* cand_idx, const float* cand_score, const int* count,
   while (n2 < max_count) n2 <<= 1;
   const int smem = 2 * n2 * 4;
   if (const int rc = smem_opt_in<sp_select_kernel>(2 * SP_MAX_CAND * 4)) return rc;
-  sp_select_kernel<<<B, 1024, smem, (cudaStream_t)stream>>>(cand_idx, cand_score, count, n_out, mode, cap, W, out_cap, kpts, scores);
-  OG_LAUNCH_CHECK("sp_select_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(sp_select_kernel, B, 1024, smem, (cudaStream_t)stream, cand_idx, cand_score, count, n_out, mode, cap, W, out_cap, kpts,
+                   scores);
 }
 int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const float* kpts, const int* n_out, int out_cap, int max_n, int cell,
                       float* desc, void* stream) {
   OG_CHECK_ARG(coarse && kpts && n_out && desc && B > 0 && Hc > 0 && Wc > 0 && D > 0 && out_cap > 0 && cell > 0, "sp_sample_desc: bad arguments");
   if (max_n <= 0) return OG_OK;
-  sp_sample_desc_kernel<<<dim3(cdiv(max_n, 8), B), 256, 0, (cudaStream_t)stream>>>(coarse, Hc, Wc, D, kpts, n_out, out_cap, cell, desc);
-  OG_LAUNCH_CHECK("sp_sample_desc_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(sp_sample_desc_kernel, dim3(cdiv(max_n, 8), B), 256, 0, (cudaStream_t)stream, coarse, Hc, Wc, D, kpts, n_out, out_cap,
+                   cell, desc);
 }
 
 // ---- local features -> matcher inputs, matches -> compact list (csrc/features.cuh) ----
@@ -617,11 +569,8 @@ int og_prepare_features(const float* lafs, const float* responses, int64_t R, in
   const int width = (responses ? 1 : 0) + laf_side_dim(method);
   OG_CHECK_ARG(lafs && R >= 0 && (width == 0 || side), "prepare_features: bad arguments");
   if (R == 0 || (width == 0 && !kpts)) return OG_OK;
-  prepare_features_kernel<<<(unsigned)((R + 255) / 256), 256, 0, (cudaStream_t)stream>>>(lafs, responses, R, method, log_response, kpts,
-                                                                                          side, width);
-  OG_LAUNCH_CHECK("prepare_features_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(prepare_features_kernel, (unsigned)((R + 255) / 256), 256, 0, (cudaStream_t)stream, lafs, responses, R, method,
+                   log_response, kpts, side, width);
 }
 int og_match_compact(const int64_t* matches0, const float* mscores0, const float* lafs0, const float* lafs1, int B, int n, int m,
                      int64_t* pair, int64_t* ij, float* confidence, float* out_lafs0, float* out_lafs1, float* out_kpts0,
@@ -629,11 +578,8 @@ int og_match_compact(const int64_t* matches0, const float* mscores0, const float
   OG_CHECK_ARG(matches0 && mscores0 && lafs0 && lafs1 && pair && ij && confidence && out_lafs0 && out_lafs1 && out_kpts0 && out_kpts1 && total,
                "match_compact: null pointer");
   OG_CHECK_ARG(B > 0 && n > 0 && m > 0 && (int64_t)B * n <= INT32_MAX - 1024, "match_compact: bad sizes");
-  match_compact_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(matches0, mscores0, lafs0, lafs1, B * n, n, m, pair, ij, confidence, out_lafs0,
-                                                             out_lafs1, out_kpts0, out_kpts1, total);
-  OG_LAUNCH_CHECK("match_compact_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(match_compact_kernel, 1, 1024, 0, (cudaStream_t)stream, matches0, mscores0, lafs0, lafs1, B * n, n, m, pair, ij, confidence,
+                   out_lafs0, out_lafs1, out_kpts0, out_kpts1, total);
 }
 
 // ---- homography-pretraining pairs (csrc/homography.cuh) ----
@@ -645,11 +591,8 @@ int og_homography_pairs(const uint8_t* rgb, int B, int H, int W, int offset, con
                "homography_pairs: offset %d must be >= 1 with 2 offset < min(H, W) = min(%d, %d)", offset, H, W);
   OG_CHECK_ARG((int64_t)HG_ROWS * W <= INT32_MAX, "homography_pairs: W = %d too large", W);
   const int h = H - 2 * offset;
-  homography_pairs_kernel<<<dim3(cdiv(h, HG_ROWS), B), HG_THREADS, 0, (cudaStream_t)stream>>>(rgb, H, W, offset, hg_block_width(H, W),
-                                                                                               warp_offset, image0, image1, H_true);
-  OG_LAUNCH_CHECK("homography_pairs_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(homography_pairs_kernel, dim3(cdiv(h, HG_ROWS), B), HG_THREADS, 0, (cudaStream_t)stream, rgb, H, W, offset,
+                   hg_block_width(H, W), warp_offset, image0, image1, H_true);
 }
 
 static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi, const float* Wlo, const __half* W16h,
@@ -688,12 +631,11 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
   float* x0 = w.x; float* x1 = w.x + (int64_t)R0 * d;
 
   // ---- keypoint encoder (positional_encoding.py:16-19) + descriptors (superglue.py:52-55) ----
-  kenc_input_kernel<<<cdiv(R0, 256), 256, 0, st>>>(kpts0, side0, R0, S, img_wh[0] - 1.f, img_wh[1] - 1.f, w.in0);
-  OG_LAUNCH_CHECK("kenc_input_kernel");
-  kenc_input_kernel<<<cdiv(R1, 256), 256, 0, st>>>(kpts1, side1, R1, S, img_wh[2] - 1.f, img_wh[3] - 1.f,
-                                                    w.in0 + (int64_t)R0 * (2 + S));
-  OG_LAUNCH_CHECK("kenc_input_kernel");
-  launch_counter() += 2;
+  if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, S, img_wh[0] - 1.f, img_wh[1] - 1.f, w.in0)) != OG_OK)
+    return rc;
+  if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, S, img_wh[2] - 1.f, img_wh[3] - 1.f,
+                      w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
+    return rc;
   {
     const float* cur = w.in0;
     float* bufs[2] = {w.h0, w.h1};
@@ -750,9 +692,7 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
     OG_CUDA(cudaMemsetAsync(w.slots, 0, (size_t)w.nslots * 4, st));
     sx[0] = sx[1] = new_slot();
     const int64_t nx = (int64_t)R * d;
-    amax_kernel<<<(unsigned)std::min<int64_t>((nx + 2047) / 2048, 1184), 256, 0, st>>>(w.x, nx, sx[0]);
-    OG_LAUNCH_CHECK("amax_kernel");
-    launch_counter()++;
+    if ((rc = OG_LAUNCH(amax_kernel, (unsigned)std::min<int64_t>((nx + 2047) / 2048, 1184), 256, 0, st, w.x, nx, sx[0])) != OG_OK) return rc;
   }
   // the fp16 GEMM of `a`: operand amax slots am0 .. am2 (of A, A2) and the meta of weight t of layer l (og_pack_f16)
   auto args16 = [&](const og_linear_args& a, float* am0, float* am1, float* am2, int l, int t) {
@@ -953,14 +893,13 @@ int og_weight_split_f16(const float* w, const float* bias, int rows, int cols, v
   OG_CHECK_ARG(w && hi16 && lo16 && meta && rows > 0 && cols > 0, "weight_split_f16: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   OG_CUDA(cudaMemsetAsync(meta, 0, 4 * sizeof(float), st));
-  weight_meta_kernel<<<cdiv(rows, 8), 256, 0, st>>>(w, bias, rows, cols, meta);
-  OG_LAUNCH_CHECK("weight_meta_kernel");
+  int rc;
+  if ((rc = OG_LAUNCH(weight_meta_kernel, cdiv(rows, 8), 256, 0, st, w, bias, rows, cols, meta)) != OG_OK) return rc;
   const int64_t nel = (int64_t)rows * cols;
-  split_f16_kernel<<<(unsigned)((nel + 255) / 256), 256, 0, st>>>(w, static_cast<__half*>(hi16), static_cast<__half*>(lo16), nel, meta);
-  OG_LAUNCH_CHECK("split_f16_kernel");
-  finish_meta_kernel<<<1, 1, 0, st>>>(meta);
-  OG_LAUNCH_CHECK("finish_meta_kernel");
-  return OG_OK;
+  if ((rc = OG_LAUNCH(split_f16_kernel, (unsigned)((nel + 255) / 256), 256, 0, st, w, static_cast<__half*>(hi16), static_cast<__half*>(lo16),
+                      nel, meta)) != OG_OK)
+    return rc;
+  return OG_LAUNCH(finish_meta_kernel, 1, 1, 0, st, meta);
 }
 
 int og_pack_f16(const og_config* cfg, const float* Wp, void* hi16, void* lo16, float* meta, void* stream) {
@@ -986,9 +925,7 @@ int og_amax(const float* x, int64_t n, float* slot, void* stream) {
   OG_CHECK_ARG(x && slot && n > 0, "amax: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   OG_CUDA(cudaMemsetAsync(slot, 0, sizeof(float), st));
-  amax_kernel<<<(unsigned)std::min<int64_t>((n + 2047) / 2048, 1184), 256, 0, st>>>(x, n, slot);
-  OG_LAUNCH_CHECK("amax_kernel");
-  return OG_OK;
+  return OG_LAUNCH(amax_kernel, (unsigned)std::min<int64_t>((n + 2047) / 2048, 1184), 256, 0, st, x, n, slot);
 }
 
 int og_linear_f16_fwd(const og_linear_args* a, const void* Wh16, const void* Wl16, const float* w_meta, const float* a_amax,

@@ -138,16 +138,13 @@ inline int attention_simt_launch(const AttnArgs& a, int head_dim, cudaStream_t s
   case DH_: {                                                                                    \
     constexpr int smem = (DH_ * (ATQ + ATK) + ATK * DH_ + ATK * ATQ) * (int)sizeof(float);       \
     if (const int rc = smem_opt_in<attention_simt_kernel<DH_>>(smem)) return rc;                 \
-    attention_simt_kernel<DH_><<<grid, 256, smem, stream>>>(a);                                  \
-  } break;
+    return OG_LAUNCH(attention_simt_kernel<DH_>, grid, 256, smem, stream, a);                    \
+  }
   switch (head_dim) {
     OG_ATTN_CASE(8) OG_ATTN_CASE(16) OG_ATTN_CASE(32) OG_ATTN_CASE(64)
     default: return fail(OG_EUNSUPPORTED, "attention: head_dim %d not in {8,16,32,64}", head_dim);
   }
 #undef OG_ATTN_CASE
-  OG_LAUNCH_CHECK("attention_simt_kernel");
-  launch_counter()++;
-  return OG_OK;
 }
 
 }  // namespace og

@@ -472,8 +472,8 @@ inline int attention_sm90_launch(const TcAttnArgs& a, const F16AttnScales& sc, c
     if ((rc = tc::make_tmap_2d(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
   }
   if ((rc = smem_opt_in<attention_sm90_kernel<DH, F16>>(C::SMEM_BYTES)) != OG_OK) return rc;
-  return tc::pdl_launch(attention_sm90_kernel<DH, F16>, dim3(cdiv(a.nq, BM), a.num_heads, a.batch), dim3(C::THREADS), C::SMEM_BYTES,
-                        stream, mkh, mkl, mvh, mvl, a, sc);
+  return launch("attention_sm90_kernel", attention_sm90_kernel<DH, F16>, LaunchAttr::pdl, dim3(cdiv(a.nq, BM), a.num_heads, a.batch),
+                dim3(C::THREADS), C::SMEM_BYTES, stream, mkh, mkl, mvh, mvl, a, sc);
 }
 
 inline bool attention_tc_eligible(int head_dim, int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo) {

@@ -116,10 +116,7 @@ inline int collate_launch(CollateArgs a, int max_count, cudaStream_t stream) {
   a.sort_n = n2;
   const size_t smem = (size_t)n2 * 8;
   if (const int rc = smem_opt_in<collate_kernel>(COLLATE_MAX_KPTS * 8)) return rc;
-  collate_kernel<<<dim3(a.B, 2), COLLATE_THREADS, smem, stream>>>(a);
-  OG_LAUNCH_CHECK("collate_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(collate_kernel, dim3(a.B, 2), COLLATE_THREADS, smem, stream, a);
 }
 
 }  // namespace og

@@ -4,6 +4,8 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <stdlib.h>
+#include <utility>
 #include "../../include/openglue_b200.h"
 
 namespace og {
@@ -17,10 +19,49 @@ inline int fail(int code, const char* fmt, ...) {
 #define OG_CHECK_ARG(cond, ...) do { if (!(cond)) return og::fail(OG_EINVAL, __VA_ARGS__); } while (0)
 #define OG_CUDA(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) \
   return og::fail(OG_ECUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e_), __FILE__, __LINE__); } while (0)
-#define OG_LAUNCH_CHECK(name) do { cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) \
-  return og::fail(OG_ECUDA, "launch of %s failed: %s", name, cudaGetErrorString(e_)); } while (0)
 
+// Kernels this thread has enqueued through launch() (og_last_forward_launches); og_superglue_forward resets it when it starts.
 inline int& launch_counter() { static thread_local int c = 0; return c; }
+
+// OG_PDL=0 turns the programmatic dependent launches (LaunchAttr::pdl) into plain launches.
+inline int& pdl_mode() {
+  static int v = [] { const char* e = getenv("OG_PDL"); return e ? atoi(e) : 1; }();
+  return v;
+}
+
+enum class LaunchAttr { none, pdl, cooperative };
+
+// Enqueues kernel(args...) on `stream` over `grid` x `block` with `smem` bytes of dynamic shared memory and the launch attribute
+// `attr`, and counts it in launch_counter().  Every kernel of the library is launched here.  A failed launch is reported as
+// "launch of <name> failed" and its error is cleared, so that it does not surface later in an unrelated cudaGetLastError.
+template <class... Params, class... Args>
+inline int launch(const char* name, void (*kernel)(Params...), LaunchAttr attr, dim3 grid, dim3 block, size_t smem,
+                  cudaStream_t stream, Args&&... args) {
+  cudaLaunchAttribute at[1] = {};
+  if (attr == LaunchAttr::pdl) {
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+  } else if (attr == LaunchAttr::cooperative) {
+    at[0].id = cudaLaunchAttributeCooperative;
+    at[0].val.cooperative = 1;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = at;
+  cfg.numAttrs = (attr == LaunchAttr::cooperative || (attr == LaunchAttr::pdl && pdl_mode())) ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();
+    return fail(OG_ECUDA, "launch of %s failed: %s", name, cudaGetErrorString(e));
+  }
+  ++launch_counter();
+  return OG_OK;
+}
+// launch() without an attribute, named after the kernel expression
+#define OG_LAUNCH(kernel, ...) og::launch(#kernel, kernel, og::LaunchAttr::none, __VA_ARGS__)
 
 // Per-device state (a process may drive several GPUs: MatchingCore(device=...), .to(dev)): the capability cache and the
 // "function attribute already set" flags (smem_opt_in) are indexed by the CURRENT device, never process-global.

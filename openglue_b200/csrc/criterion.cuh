@@ -103,10 +103,7 @@ inline int criterion_launch(const float* scores, const int64_t* gt0, const int64
   a.per_pair = reinterpret_cast<float*>(static_cast<char*>(ws) + 256);
   a.loss = loss; a.dscores = dscores; a.grad_scale = grad_scale;
   OG_CUDA(cudaMemsetAsync(a.counter, 0, 4, stream));
-  criterion_kernel<<<B, CRIT_THREADS, 0, stream>>>(a);
-  OG_LAUNCH_CHECK("criterion_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(criterion_kernel, B, CRIT_THREADS, 0, stream, a);
 }
 
 }  // namespace og

@@ -155,22 +155,14 @@ inline int gt_matches_launch(const float* kpts0, const float* kpts1, int B, int 
   uint8_t* mask1 = reinterpret_cast<uint8_t*>(take((int64_t)B * m));
   int* nn0 = reinterpret_cast<int*>(take((int64_t)B * n * 4));
   int* nn1 = reinterpret_cast<int*>(take((int64_t)B * m * 4));
-  gt_prepare_kernel<<<cdiv(2 * B, 64), 64, 0, st>>>(tf, B, prep);
-  OG_LAUNCH_CHECK("gt_prepare_kernel");
-  gt_reproject_kernel<<<dim3(cdiv(n, 256), B), 256, 0, st>>>(kpts0, n, 0, tf, prep, k0t, mask0);
-  OG_LAUNCH_CHECK("gt_reproject_kernel");
-  gt_reproject_kernel<<<dim3(cdiv(m, 256), B), 256, 0, st>>>(kpts1, m, 1, tf, prep, k1t, mask1);
-  OG_LAUNCH_CHECK("gt_reproject_kernel");
-  gt_nearest_kernel<<<dim3(cdiv(n, 256), B), 256, 0, st>>>(k0t, n, kpts1, m, nn0);
-  OG_LAUNCH_CHECK("gt_nearest_kernel");
-  gt_nearest_kernel<<<dim3(cdiv(m, 256), B), 256, 0, st>>>(k1t, m, kpts0, n, nn1);
-  OG_LAUNCH_CHECK("gt_nearest_kernel");
-  gt_mutual_kernel<<<dim3(cdiv(n, 256), B), 256, 0, st>>>(nn0, nn1, mask0, n, m, gt0);
-  OG_LAUNCH_CHECK("gt_mutual_kernel");
-  gt_mutual_kernel<<<dim3(cdiv(m, 256), B), 256, 0, st>>>(nn1, nn0, mask1, m, n, gt1);
-  OG_LAUNCH_CHECK("gt_mutual_kernel");
-  launch_counter() += 7;
-  return OG_OK;
+  int rc;
+  if ((rc = OG_LAUNCH(gt_prepare_kernel, cdiv(2 * B, 64), 64, 0, st, tf, B, prep))) return rc;
+  if ((rc = OG_LAUNCH(gt_reproject_kernel, dim3(cdiv(n, 256), B), 256, 0, st, kpts0, n, 0, tf, prep, k0t, mask0))) return rc;
+  if ((rc = OG_LAUNCH(gt_reproject_kernel, dim3(cdiv(m, 256), B), 256, 0, st, kpts1, m, 1, tf, prep, k1t, mask1))) return rc;
+  if ((rc = OG_LAUNCH(gt_nearest_kernel, dim3(cdiv(n, 256), B), 256, 0, st, k0t, n, kpts1, m, nn0))) return rc;
+  if ((rc = OG_LAUNCH(gt_nearest_kernel, dim3(cdiv(m, 256), B), 256, 0, st, k1t, m, kpts0, n, nn1))) return rc;
+  if ((rc = OG_LAUNCH(gt_mutual_kernel, dim3(cdiv(n, 256), B), 256, 0, st, nn0, nn1, mask0, n, m, gt0))) return rc;
+  return OG_LAUNCH(gt_mutual_kernel, dim3(cdiv(m, 256), B), 256, 0, st, nn1, nn0, mask1, m, n, gt1);
 }
 
 }  // namespace og

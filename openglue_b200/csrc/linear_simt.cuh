@@ -149,10 +149,7 @@ inline int linear_simt_launch(const og_linear_args& a, cudaStream_t stream) {
   f.vecY = a.Y && (a.ldy % 4 == 0) && (a.strideY % 4 == 0) && aligned16(a.Y);
   f.vecYt = a.Yt && (a.ldyt % 4 == 0) && (a.strideYt % 4 == 0) && aligned16(a.Yt);
   dim3 grid(cdiv(a.nout, LBN), cdiv(a.rows, LBM), a.batch);
-  linear_simt_kernel<<<grid, 256, 0, stream>>>(a, f);
-  OG_LAUNCH_CHECK("linear_simt_kernel");
-  launch_counter()++;
-  return OG_OK;
+  return OG_LAUNCH(linear_simt_kernel, grid, 256, 0, stream, a, f);
 }
 
 }  // namespace og

@@ -485,7 +485,8 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
   const int tiles = cdiv(a.nout, BN) * cdiv(a.rows, BM) * a.batch;
   const int sms = device_info().ok ? device_info().sm_count : 132;
   // persistent: each CTA walks tiles blockIdx.x + i gridDim.x
-  return tc::pdl_launch(linear_sm90_kernel<Args>, dim3(std::min(tiles, sms)), dim3(THREADS), C::SMEM_BYTES, stream, ma, ma2, mh, ml, a);
+  return launch("linear_sm90_kernel", linear_sm90_kernel<Args>, LaunchAttr::pdl, dim3(std::min(tiles, sms)), dim3(THREADS), C::SMEM_BYTES,
+                stream, ma, ma2, mh, ml, a);
 }
 // The two operand forms, instantiated next to the template: where the kernels sit in the binary (and so a cuobjdump -sass
 // comparison of two builds) does not depend on where the host code first launches them.

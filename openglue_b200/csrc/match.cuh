@@ -105,17 +105,12 @@ inline int match_launch(const float* scores, int B, int n, int m, float thr, int
   int* colidx = reinterpret_cast<int*>(w); w += align_up((int64_t)B * m * 4, 256);
   float* pval = reinterpret_cast<float*>(w); w += align_up((int64_t)B * chunks * m * 4, 256);
   int* pidx = reinterpret_cast<int*>(w);
-  match_rowmax_kernel<<<dim3(cdiv(n, 8), B), 256, 0, stream>>>(scores, n, m, rowval, rowidx);
-  OG_LAUNCH_CHECK("match_rowmax_kernel");
-  match_colmax_kernel<<<dim3(cdiv(m, 256), chunks, B), 256, 0, stream>>>(scores, n, m, chunks, pval, pidx);
-  OG_LAUNCH_CHECK("match_colmax_kernel");
-  match_colreduce_kernel<<<dim3(cdiv(m, 256), B), 256, 0, stream>>>(n, m, chunks, pval, pidx, colidx);
-  OG_LAUNCH_CHECK("match_colreduce_kernel");
-  match_finalize_kernel<<<dim3(cdiv(std::max(n, m), 256), B), 256, 0, stream>>>(n, m, thr, rowval, rowidx, colidx,
-                                                                                matches0, mscores0, matches1, mscores1);
-  OG_LAUNCH_CHECK("match_finalize_kernel");
-  launch_counter() += 4;
-  return OG_OK;
+  int rc;
+  if ((rc = OG_LAUNCH(match_rowmax_kernel, dim3(cdiv(n, 8), B), 256, 0, stream, scores, n, m, rowval, rowidx))) return rc;
+  if ((rc = OG_LAUNCH(match_colmax_kernel, dim3(cdiv(m, 256), chunks, B), 256, 0, stream, scores, n, m, chunks, pval, pidx))) return rc;
+  if ((rc = OG_LAUNCH(match_colreduce_kernel, dim3(cdiv(m, 256), B), 256, 0, stream, n, m, chunks, pval, pidx, colidx))) return rc;
+  return OG_LAUNCH(match_finalize_kernel, dim3(cdiv(std::max(n, m), 256), B), 256, 0, stream, n, m, thr, rowval, rowidx, colidx,
+                   matches0, mscores0, matches1, mscores1);
 }
 
 }  // namespace og

@@ -459,18 +459,8 @@ inline int sinkhorn_coop_launch(const Args& a, const SinkPlan& p, cudaStream_t s
   constexpr size_t smem_max = sinkhorn_smem(Args::kBackward, V, W, SLOTS, 128 * V * W + 4);   // largest request: m = 128 V W
   static_assert(smem_max <= OG_SMEM_OPTIN_MAX, "Sinkhorn kernel: shared memory beyond what one block may opt in to");
   if (const int rc = smem_opt_in<Kernel>((int)smem_max)) return rc;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(a.B * a.SP);
-  cfg.blockDim = dim3(SINK_WARPS * 32);
-  cfg.dynamicSmemBytes = p.smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  OG_CUDA(cudaLaunchKernelEx(&cfg, Kernel, a));
-  launch_counter()++;
-  return OG_OK;
+  return launch(Args::kBackward ? "sinkhorn_bwd_kernel" : "sinkhorn_kernel", Kernel, LaunchAttr::cooperative, dim3(a.B * a.SP),
+                dim3(SINK_WARPS * 32), p.smem, stream, a);
 }
 
 // Calls launch(b0, nb) for pairs [b0, b0 + nb): as many pairs per cooperative launch as the plan allows, each launch with the

@@ -299,13 +299,10 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   float* per_pair = take(B);
   const SinkConsts k = sinkhorn_consts(n, m);
   const int m1 = m + 1, n1 = n + 1;
-  sinkb_rowsum_kernel<<<cdiv(B * n1, 8), 256, 0, stream>>>(G, B * n1, m1, ubar_init);
-  OG_LAUNCH_CHECK("sinkb_rowsum_kernel");
-  sinkb_colsum_kernel<<<dim3(cdiv(m1, 256), (unsigned)nrs, B), 256, 0, stream>>>(G, n1, m1, colpart);
-  OG_LAUNCH_CHECK("sinkb_colsum_kernel");
-  sinkb_colsum_finish_kernel<<<dim3(cdiv(m1, 256), B), 256, 0, stream>>>(colpart, (int)nrs, m1, vbar_init);
-  OG_LAUNCH_CHECK("sinkb_colsum_finish_kernel");
-  launch_counter() += 3;
+  int rc;
+  if ((rc = OG_LAUNCH(sinkb_rowsum_kernel, cdiv(B * n1, 8), 256, 0, stream, G, B * n1, m1, ubar_init))) return rc;
+  if ((rc = OG_LAUNCH(sinkb_colsum_kernel, dim3(cdiv(m1, 256), (unsigned)nrs, B), 256, 0, stream, G, n1, m1, colpart))) return rc;
+  if ((rc = OG_LAUNCH(sinkb_colsum_finish_kernel, dim3(cdiv(m1, 256), B), 256, 0, stream, colpart, (int)nrs, m1, vbar_init))) return rc;
   SinkBwdArgs a;
   a.S = S; a.lds = lds; a.strideS = strideS; a.dustbin = dustbin; a.B = B; a.n = n; a.m = m; a.iters = T; a.reg = reg;
   a.norm = k.norm; a.log_a_last = k.log_a_last; a.log_b_last = k.log_b_last;
@@ -314,7 +311,7 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   a.hist_coef = hist_coef; a.hist_cvec = hist_cvec; a.hist_vbar = hist_vbar; a.hist_wq = hist_wq;
   a.partial = partial; a.barrier = barrier; a.SP = p.SP; a.rows_per_strip = p.rows_per_strip; a.mpad = p.mpad;
   if (T > 0) {
-    const int rc = sinkhorn_for_each_launch(p, B, barrier, stream, [&](int b0, int nb) {
+    rc = sinkhorn_for_each_launch(p, B, barrier, stream, [&](int b0, int nb) {
       SinkBwdArgs g = a;
       g.B = nb;
       g.S = S + (int64_t)b0 * strideS;
@@ -330,13 +327,9 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
     });
     if (rc != OG_OK) return rc;
   }
-  sinkb_dz_kernel<<<dim3(cdiv(m1, SINKB_TC), cdiv(n1, SINKB_TR), B), 256, 0, stream>>>(a, G, dZ, 1.f / reg);
-  OG_LAUNCH_CHECK("sinkb_dz_kernel");
+  if ((rc = OG_LAUNCH(sinkb_dz_kernel, dim3(cdiv(m1, SINKB_TC), cdiv(n1, SINKB_TR), B), 256, 0, stream, a, G, dZ, 1.f / reg))) return rc;
   OG_CUDA(cudaMemsetAsync(counter, 0, 4, stream));
-  sinkb_dustbin_kernel<<<B, 256, 0, stream>>>(dZ, B, n, m, per_pair, counter, ddustbin);
-  OG_LAUNCH_CHECK("sinkb_dustbin_kernel");
-  launch_counter() += 2;
-  return OG_OK;
+  return OG_LAUNCH(sinkb_dustbin_kernel, B, 256, 0, stream, dZ, B, n, m, per_pair, counter, ddustbin);
 }
 
 }  // namespace og

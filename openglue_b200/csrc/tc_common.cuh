@@ -2,7 +2,6 @@
 // A operand in registers and B in shared memory), wgmma shared-memory descriptors, tf32 / fp16 hi/lo splits.
 // Descriptor bit layouts follow the PTX ISA (wgmma matrix descriptor).
 #pragma once
-#include <stdlib.h>
 #include <string.h>
 #include "common.cuh"
 #include <cuda.h>
@@ -88,32 +87,12 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 }
 
 // ----------------------------------------------------------------------------- programmatic dependent launch
-// Kernels launched with cudaLaunchAttributeProgrammaticStreamSerialization may become resident while the previous kernel
-// of the stream is still draining: launch_dependents (issued at the very top) lets the NEXT kernel's CTAs take an SM as soon
-// as this kernel's CTA leaves it, and grid_dependency_wait blocks until the PREVIOUS kernel has completed and flushed its
-// writes.  Everything before the wait (barrier init, tensor-map prefetch) overlaps the previous kernel's tail.
+// Kernels launched with LaunchAttr::pdl (cudaLaunchAttributeProgrammaticStreamSerialization) may become resident while the
+// previous kernel of the stream is still draining: launch_dependents (issued at the very top) lets the NEXT kernel's CTAs take
+// an SM as soon as this kernel's CTA leaves it, and grid_dependency_wait blocks until the PREVIOUS kernel has completed and
+// flushed its writes.  Everything before the wait (barrier init, tensor-map prefetch) overlaps the previous kernel's tail.
 __device__ __forceinline__ void launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-inline int& pdl_mode() {
-  static int v = [] { const char* e = getenv("OG_PDL"); return e ? atoi(e) : 1; }();
-  return v;
-}
-// kernel<<<grid, block, smem, stream>>>(args...), as a programmatic dependent launch unless pdl_mode() is 0
-template <class... Params, class... Args>
-inline int pdl_launch(void (*kernel)(Params...), dim3 grid, dim3 block, int smem, cudaStream_t stream, const Args&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_mode() ? 1 : 0;
-  OG_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
-  launch_counter()++;
-  return OG_OK;
-}
 
 // ----------------------------------------------------------------------------- warp specialization
 // setmaxnreg moves registers between the warpgroups of a CTA (every warp of the warpgroup executes it; N a multiple of 8 in

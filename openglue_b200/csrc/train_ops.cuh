@@ -48,15 +48,11 @@ inline int transpose_launch(const float* in, int64_t ld_in, int64_t stride_in, f
   if (transpose) {
     dim3 grid(cdiv(cols, 32), cdiv(rows, 32), batch);
     if (grid.y > 65535 || grid.z > 65535) return fail(OG_EUNSUPPORTED, "transpose: %d rows x %d batches exceed the grid limits", rows, batch);
-    transpose_kernel<<<grid, 256, 0, st>>>(in, ld_in, stride_in, out, ld_out, stride_out, rows, cols);
-  } else {
-    dim3 grid(std::min(cdiv(cols, 256), 64), std::min(rows, 4096), batch);
-    if (grid.z > 65535) return fail(OG_EUNSUPPORTED, "copy2d: %d batches exceed the grid limits", batch);
-    copy2d_kernel<<<grid, 256, 0, st>>>(in, ld_in, stride_in, out, ld_out, stride_out, rows, cols);
+    return OG_LAUNCH(transpose_kernel, grid, 256, 0, st, in, ld_in, stride_in, out, ld_out, stride_out, rows, cols);
   }
-  OG_LAUNCH_CHECK("transpose_kernel");
-  launch_counter()++;
-  return OG_OK;
+  dim3 grid(std::min(cdiv(cols, 256), 64), std::min(rows, 4096), batch);
+  if (grid.z > 65535) return fail(OG_EUNSUPPORTED, "copy2d: %d batches exceed the grid limits", batch);
+  return OG_LAUNCH(copy2d_kernel, grid, 256, 0, st, in, ld_in, stride_in, out, ld_out, stride_out, rows, cols);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -138,12 +134,8 @@ inline int colreduce_launch(ColReduceArgs a, cudaStream_t st) {
   a.chunks = std::max(1, std::min(COLRED_MAX_CHUNKS, cdiv(a.rows, 64)));
   a.rows_per_chunk = cdiv(std::max(a.rows, 1), a.chunks);
   a.chunks = std::max(1, cdiv(a.rows, a.rows_per_chunk));
-  colreduce_stage1<MODE><<<dim3(cdiv(a.cols, 64), a.chunks), 256, 0, st>>>(a);
-  OG_LAUNCH_CHECK("colreduce_stage1");
-  colreduce_stage2<MODE><<<cdiv(a.cols, 256), 256, 0, st>>>(a);
-  OG_LAUNCH_CHECK("colreduce_stage2");
-  launch_counter() += 2;
-  return OG_OK;
+  if (const int rc = OG_LAUNCH(colreduce_stage1<MODE>, dim3(cdiv(a.cols, 64), a.chunks), 256, 0, st, a)) return rc;
+  return OG_LAUNCH(colreduce_stage2<MODE>, cdiv(a.cols, 256), 256, 0, st, a);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -17,7 +17,6 @@ dict, but the selection / gather / depth lookup run in ``og_collate_fwd`` on the
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
@@ -25,6 +24,7 @@ import numpy as np
 import torch
 
 from . import _cabi
+from ._cabi import ptr, stream
 
 __all__ = ['FeatureStore', 'collate_features', 'convert_h5_to_npz', 'save_features_npz']
 
@@ -139,7 +139,6 @@ def collate_features(batch: Sequence[Dict[str, Any]], target_num_keypoints: int,
     if 'depth0' in tf:
         depth = [torch.stack([x['transformation'][f'depth{img}'] for x in batch]).float().contiguous() for img in (0, 1)]
     lib = _cabi.lib()
-    p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
     with torch.cuda.device(dev):
         d_lafs, d_scores, d_desc = (stage[k].to(dev, non_blocking=True) for k in ('lafs', 'scores', 'desc'))
         d_off = torch.from_numpy(offsets).to(dev, non_blocking=True)
@@ -149,12 +148,12 @@ def collate_features(batch: Sequence[Dict[str, Any]], target_num_keypoints: int,
         out.update({f'scores{i}': torch.empty(B, K, device=dev) for i in (0, 1)})
         out.update({f'descriptors{i}': torch.empty(B, K, D, device=dev) for i in (0, 1)})
         kdepth = [torch.empty(B, K, device=dev) if d is not None else None for d in d_depth]
-        rc = lib.og_collate_fwd(p(d_lafs), p(d_scores), p(d_desc), p(d_off), p(d_sel), max(counts),
-                                p(d_depth[0]), 0 if d_depth[0] is None else d_depth[0].shape[-2], 0 if d_depth[0] is None else d_depth[0].shape[-1],
-                                p(d_depth[1]), 0 if d_depth[1] is None else d_depth[1].shape[-2], 0 if d_depth[1] is None else d_depth[1].shape[-1],
-                                B, K, D, p(out['lafs0']), p(out['lafs1']), p(out['scores0']), p(out['scores1']),
-                                p(out['descriptors0']), p(out['descriptors1']), p(kdepth[0]), p(kdepth[1]),
-                                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        rc = lib.og_collate_fwd(ptr(d_lafs), ptr(d_scores), ptr(d_desc), ptr(d_off), ptr(d_sel), max(counts),
+                                ptr(d_depth[0]), 0 if d_depth[0] is None else d_depth[0].shape[-2], 0 if d_depth[0] is None else d_depth[0].shape[-1],
+                                ptr(d_depth[1]), 0 if d_depth[1] is None else d_depth[1].shape[-2], 0 if d_depth[1] is None else d_depth[1].shape[-1],
+                                B, K, D, ptr(out['lafs0']), ptr(out['lafs1']), ptr(out['scores0']), ptr(out['scores1']),
+                                ptr(out['descriptors0']), ptr(out['descriptors1']), ptr(kdepth[0]), ptr(kdepth[1]),
+                                stream(dev))
         _cabi.check(rc, 'og_collate_fwd')
         for t in (d_lafs, d_scores, d_desc, d_off, d_sel, *d_depth):
             if t is not None:

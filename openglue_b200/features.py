@@ -17,27 +17,19 @@ CUDA tensors only, and no autograd: the reference never differentiates these out
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict
 
 import torch
 import torch.nn as nn
 
 from . import _cabi
+from ._cabi import ptr, stream
 from .superglue import SuperGlue
 
 __all__ = ['LAFConverter', 'get_laf_to_sideinfo_converter', 'prepare_features_output', 'compact_matches', 'OpenGlueMatcher']
 
 # method name -> (og_laf_method, side-information columns after the response)
 _METHODS = {'none': (0, 0), 'scale': (1, 1), 'rotation': (2, 2), 'scale_rotation': (3, 3), 'affine': (4, 5)}
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _st(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _device_f32(t: torch.Tensor, name: str) -> torch.Tensor:
@@ -72,7 +64,7 @@ class LAFConverter:
         out = torch.empty(B, N, self._dim, dtype=torch.float32, device=lafs.device)
         if self._dim and B * N:
             with torch.cuda.device(lafs.device):
-                _cabi.check(_cabi.lib().og_prepare_features(_p(lafs), None, B * N, self._code, 0, None, _p(out), _st(lafs.device)),
+                _cabi.check(_cabi.lib().og_prepare_features(ptr(lafs), None, B * N, self._code, 0, None, ptr(out), stream(lafs.device)),
                             'og_prepare_features')
         return out
 
@@ -107,8 +99,8 @@ def prepare_features_output(lafs, responses, desc, laf_converter: LAFConverter, 
     side = torch.empty(B, N, 1 + laf_converter.side_info_dim, dtype=torch.float32, device=dev)
     if B * N:
         with torch.cuda.device(dev):
-            _cabi.check(_cabi.lib().og_prepare_features(_p(lafs), _p(responses), B * N, laf_converter._code, int(bool(log_response)),
-                                                        _p(kpts), _p(side), _st(dev)), 'og_prepare_features')
+            _cabi.check(_cabi.lib().og_prepare_features(ptr(lafs), ptr(responses), B * N, laf_converter._code, int(bool(log_response)),
+                                                        ptr(kpts), ptr(side), stream(dev)), 'og_prepare_features')
     return {'keypoints': kpts, 'side_info': side, 'local_descriptors': desc.permute(0, 2, 1) if permute_desc else desc}
 
 
@@ -135,8 +127,8 @@ def compact_matches(matches0: torch.Tensor, mscores0: torch.Tensor, lafs0: torch
     total = torch.empty(1, **i64)
     if cap and m:
         with torch.cuda.device(dev):
-            _cabi.check(_cabi.lib().og_match_compact(_p(matches0), _p(mscores0), _p(lafs0), _p(lafs1), B, n, m, _p(pair), _p(ij), _p(conf),
-                                                     _p(l0), _p(l1), _p(k0), _p(k1), _p(total), _st(dev)), 'og_match_compact')
+            _cabi.check(_cabi.lib().og_match_compact(ptr(matches0), ptr(mscores0), ptr(lafs0), ptr(lafs1), B, n, m, ptr(pair), ptr(ij), ptr(conf),
+                                                     ptr(l0), ptr(l1), ptr(k0), ptr(k1), ptr(total), stream(dev)), 'og_match_compact')
         nc = int(total.item())                  # the one host synchronisation (the reference's boolean indexing)
     else:
         nc = 0

@@ -66,13 +66,12 @@ def gt_matches(kpts0: torch.Tensor, kpts1: torch.Tensor, transformation: Dict[st
     k0, k1 = _f32(kpts0, dev), _f32(kpts1, dev)
     lib = _cabi.lib()
     with torch.cuda.device(dev):
-        ws_bytes = lib.og_gt_matches_workspace_bytes(B, n, m)
+        ws_bytes = _cabi.check_size(lib.og_gt_matches_workspace_bytes(B, n, m), 'og_gt_matches_workspace_bytes')
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         gt0 = torch.empty(B, n, dtype=torch.int64, device=dev)
         gt1 = torch.empty(B, m, dtype=torch.int64, device=dev)
-        rc = lib.og_gt_matches_fwd(C.c_void_p(k0.data_ptr()), C.c_void_p(k1.data_ptr()), B, n, m, C.byref(tf),
-                                   C.c_void_p(gt0.data_ptr()), C.c_void_p(gt1.data_ptr()), C.c_void_p(ws.data_ptr()), ws_bytes,
-                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        rc = lib.og_gt_matches_fwd(_cabi.ptr(k0), _cabi.ptr(k1), B, n, m, C.byref(tf), _cabi.ptr(gt0), _cabi.ptr(gt1), _cabi.ptr(ws), ws_bytes,
+                                   _cabi.stream(dev))
         _cabi.check(rc, 'og_gt_matches_fwd')
         for t in keep + [k0, k1, ws]:                      # the kernels are only enqueued: keep their inputs alive on this stream
             t.record_stream(torch.cuda.current_stream(dev))

@@ -17,18 +17,14 @@ CUDA tensors only, and no autograd.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional
 
 import torch
 
 from . import _cabi
+from ._cabi import ptr, stream
 
 __all__ = ['synthesize_homography_pairs']
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr())
 
 
 def synthesize_homography_pairs(images_u8: torch.Tensor, offset: int, warp_offset: Optional[torch.Tensor] = None,
@@ -73,7 +69,6 @@ def synthesize_homography_pairs(images_u8: torch.Tensor, offset: int, warp_offse
     image1 = torch.empty(B, 1, h, w, dtype=torch.float32, device=dev)
     H_true = torch.empty(B, 3, 3, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        _cabi.check(_cabi.lib().og_homography_pairs(_p(images_u8), B, H, W, offset, _p(warp_offset), _p(image0), _p(image1),
-                                                    _p(H_true), stream), 'og_homography_pairs')
+        _cabi.check(_cabi.lib().og_homography_pairs(ptr(images_u8), B, H, W, offset, ptr(warp_offset), ptr(image0), ptr(image1),
+                                                    ptr(H_true), stream(dev)), 'og_homography_pairs')
     return {'image0': image0, 'image1': image1, 'transformation': {'type': ['perspective'] * B, 'H': H_true}}

@@ -9,12 +9,12 @@ d loss / d scores - the sparse scatter that starts the backward pass.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional, Tuple
 
 import torch
 
 from . import _cabi
+from ._cabi import ptr, stream
 
 __all__ = ['criterion', 'criterion_with_grad']
 
@@ -32,13 +32,12 @@ def _run(y_true: Dict[str, torch.Tensor], y_pred: Dict[str, torch.Tensor], want_
         raise ValueError(f'gt_matches shapes {tuple(gt0.shape)}, {tuple(gt1.shape)} do not fit scores {tuple(scores.shape)}')
     lib = _cabi.lib()
     with torch.cuda.device(dev):
-        wsb = lib.og_criterion_workspace_bytes(B)
+        wsb = _cabi.check_size(lib.og_criterion_workspace_bytes(B), 'og_criterion_workspace_bytes')
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         loss = torch.empty(2, dtype=torch.float32, device=dev)
         dscores = torch.zeros_like(scores) if want_grad else None
-        p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
-        rc = lib.og_criterion_fwd(p(scores), p(gt0), p(gt1), B, n1 - 1, m1 - 1, p(loss), p(dscores), float(grad_scale), p(ws), wsb,
-                                  C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        rc = lib.og_criterion_fwd(ptr(scores), ptr(gt0), ptr(gt1), B, n1 - 1, m1 - 1, ptr(loss), ptr(dscores), float(grad_scale), ptr(ws), wsb,
+                                  stream(dev))
         _cabi.check(rc, 'og_criterion_fwd')
     return loss, dscores
 

@@ -36,9 +36,7 @@ def pack_weights(state_dict: Dict[str, torch.Tensor], config: dict, ogcfg: _cabi
     keeps the folds unrounded (used by the tests to check the algebra alone)."""
     lib = _cabi.lib()
     sd = {k: v.detach().cpu() for k, v in state_dict.items()}
-    total = lib.og_packed_weight_floats(ogcfg)
-    if total < 0:
-        _cabi.check(int(total), 'og_packed_weight_floats')
+    total = _cabi.check_size(lib.og_packed_weight_floats(ogcfg), 'og_packed_weight_floats')
     out = torch.zeros(total, dtype=dtype)
     d = int(config['descriptor_dim'])
     use_offset = bool(config['attention_gnn'].get('use_offset', False))

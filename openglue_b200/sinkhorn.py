@@ -9,17 +9,12 @@ the T x (N+1)(M+1) tape).  There is no CPU path.
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
 from . import _cabi
+from ._ops import _Ops
 
 __all__ = ['matching_log_probs']
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
 
 
 class _Sinkhorn(torch.autograd.Function):
@@ -33,17 +28,8 @@ class _Sinkhorn(torch.autograd.Function):
         Sp = torch.zeros(B, n, lds, dtype=torch.float32, device=dev)       # 16-byte aligned rows (the kernels' layout)
         Sp[:, :, :m] = S.detach().float()
         dust = dustbin.detach().float().reshape(1).contiguous()
-        lib = _cabi.lib()
         with torch.cuda.device(dev):
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            scores = torch.empty(B, n + 1, m + 1, dtype=torch.float32, device=dev)
-            hist = torch.empty(max(int(lib.og_sinkhorn_hist_floats(B, n, m, num_iters)), 1), dtype=torch.float32, device=dev)
-            wsb = lib.og_sinkhorn_workspace_bytes(B, n, m)
-            if wsb < 0:
-                _cabi.check(int(wsb), 'og_sinkhorn_workspace_bytes')
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            _cabi.check(lib.og_sinkhorn_train_fwd(_p(Sp), lds, n * lds, _p(dust), B, n, m, int(num_iters), float(reg), _p(scores), _p(hist),
-                                                  _p(ws), wsb, st), 'og_sinkhorn_train_fwd')
+            scores, hist = _Ops(dev, _cabi.OG_PREC_FP32).sinkhorn_fwd(Sp, dust, B, n, m, int(num_iters), float(reg))
         ctx.save_for_backward(Sp, dust, hist)
         ctx.meta = (B, n, m, lds, int(num_iters), float(reg), dustbin.shape, S.dtype, dustbin.dtype)
         return scores
@@ -54,17 +40,8 @@ class _Sinkhorn(torch.autograd.Function):
         B, n, m, lds, T, reg, dshape, sdt, ddt = ctx.meta
         dev = Sp.device
         G = G.detach().float().contiguous()
-        lib = _cabi.lib()
         with torch.cuda.device(dev):
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            dZ = torch.empty(B, n + 1, m + 1, dtype=torch.float32, device=dev)
-            dd = torch.empty(1, dtype=torch.float32, device=dev)
-            wsb = lib.og_sinkhorn_bwd_workspace_bytes(B, n, m, T)
-            if wsb < 0:
-                _cabi.check(int(wsb), 'og_sinkhorn_bwd_workspace_bytes')
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            _cabi.check(lib.og_sinkhorn_bwd(_p(Sp), lds, n * lds, _p(dust), B, n, m, T, reg, _p(hist), _p(G), _p(dZ), _p(dd), _p(ws), wsb, st),
-                        'og_sinkhorn_bwd')
+            dZ, dd = _Ops(dev, _cabi.OG_PREC_FP32).sinkhorn_bwd(Sp, dust, hist, G, B, n, m, T, reg)
         return dZ[:, :n, :m].to(sdt), dd.reshape(dshape).to(ddt), None, None
 
 

@@ -18,6 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
+from ._cabi import ptr, stream
 from .packing import pack_weights
 
 __all__ = ['SuperGlue', 'MatchingCore', 'PendingMatches']
@@ -155,19 +156,16 @@ class SuperGlue(nn.Module):
             if self._precision() != _cabi.OG_PREC_FP32:        # operand split for the tensor-core kernels
                 self._packed_hi, self._packed_lo = torch.empty_like(self._packed), torch.empty_like(self._packed)
                 with torch.cuda.device(device):
-                    _cabi.check(_cabi.lib().og_split_tf32(
-                        C.c_void_p(self._packed.data_ptr()), C.c_void_p(self._packed_hi.data_ptr()),
-                        C.c_void_p(self._packed_lo.data_ptr()), self._packed.numel(),
-                        C.c_void_p(torch.cuda.current_stream(device).cuda_stream)), 'og_split_tf32')
+                    _cabi.check(_cabi.lib().og_split_tf32(ptr(self._packed), ptr(self._packed_hi), ptr(self._packed_lo), self._packed.numel(),
+                                                          stream(device)), 'og_split_tf32')
             if self._precision() == _cabi.OG_PREC_FP16X3:      # fp16 hi/lo split of the GNN weights + per-tensor scales / norms
                 lib = _cabi.lib()
                 self._packed_h16 = torch.zeros(self._packed.numel(), dtype=torch.float16, device=device)
                 self._packed_l16 = torch.zeros_like(self._packed_h16)
                 self._meta16 = torch.zeros(max(int(lib.og_f16_meta_floats(self._ogcfg)), 4), dtype=torch.float32, device=device)
                 with torch.cuda.device(device):
-                    _cabi.check(lib.og_pack_f16(self._ogcfg, C.c_void_p(self._packed.data_ptr()), C.c_void_p(self._packed_h16.data_ptr()),
-                                                C.c_void_p(self._packed_l16.data_ptr()), C.c_void_p(self._meta16.data_ptr()),
-                                                C.c_void_p(torch.cuda.current_stream(device).cuda_stream)), 'og_pack_f16')
+                    _cabi.check(lib.og_pack_f16(self._ogcfg, ptr(self._packed), ptr(self._packed_h16), ptr(self._packed_l16), ptr(self._meta16),
+                                                stream(device)), 'og_pack_f16')
             self._packed_key = key
         return self._packed
 
@@ -220,9 +218,7 @@ class SuperGlue(nn.Module):
             if match_threshold is not None and float(match_threshold) != cfg.match_threshold:
                 cfg = _cabi.OgConfig.from_buffer_copy(cfg)             # per call: never written back into the shared config
                 cfg.match_threshold = float(match_threshold)
-            ws_bytes = lib.og_workspace_bytes(cfg, B, n, m)
-            if ws_bytes < 0:
-                _cabi.check(int(ws_bytes), 'og_workspace_bytes')
+            ws_bytes = _cabi.check_size(lib.og_workspace_bytes(cfg, B, n, m), 'og_workspace_bytes')
             if self._workspace is None or self._workspace.numel() < ws_bytes or self._workspace.device != dev:
                 self._workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
                 self._bump_alloc()
@@ -241,9 +237,8 @@ class SuperGlue(nn.Module):
                 ms1 = torch.empty(B, m, dtype=torch.float32, device=dev)
                 out.update(matches0=m0, matching_scores0=ms0, matches1=m1, matching_scores1=ms1)
             wh = (C.c_float * 4)(w0, h0, w1, h1)
-            ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())
             tail = (B, n, m, ptr(k0), ptr(k1), ptr(s0), ptr(s1), ptr(d0), ptr(d1), wh, ptr(ctx0), ptr(ctx1), ptr(scores), ptr(m0), ptr(ms0),
-                    ptr(m1), ptr(ms1), ptr(self._workspace), ws_bytes, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+                    ptr(m1), ptr(ms1), ptr(self._workspace), ws_bytes, stream(dev))
             if cfg.precision == _cabi.OG_PREC_FP16X3:
                 rc = lib.og_superglue_forward_f16(cfg, ptr(packed), ptr(self._packed_hi), ptr(self._packed_lo), ptr(self._packed_h16),
                                                   ptr(self._packed_l16), ptr(self._meta16), *tail)

@@ -14,7 +14,6 @@ folded once in float64 on the host.  There is no CPU path.
 """
 from __future__ import annotations
 
-import ctypes as C
 import pathlib
 from typing import Optional, Union
 
@@ -22,7 +21,8 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
-from ._ops import _Ops, _p
+from ._cabi import ptr
+from ._ops import _Ops
 
 __all__ = ['SuperPointNet', 'SuperPointNetBn']
 
@@ -103,7 +103,7 @@ class SuperPointNet(nn.Module):
             def conv3(t, h, w, cin, name, relu=True):
                 wp, bias = wts[name]
                 a = col[:B * h * w * 9 * cin].view(B * h * w, 9 * cin)
-                _cabi.check(lib.og_sp_im2col3x3(_p(t), B, h, w, cin, _p(a), st), 'og_sp_im2col3x3')
+                _cabi.check(lib.og_sp_im2col3x3(ptr(t), B, h, w, cin, ptr(a), st), 'og_sp_im2col3x3')
                 return ops.linear(a, wp, bias, relu=relu)               # [B h w, cout] = NHWC
 
             h, w, cin = H, W, 1
@@ -112,17 +112,17 @@ class SuperPointNet(nn.Module):
                 x = conv3(x, h, w, cin, f'conv{i + 1}b'); cin = ch[3]
                 if i != 3:
                     y = ops.empty(B * (h // 2) * (w // 2), cin)
-                    _cabi.check(lib.og_sp_maxpool2x2(_p(x), B, h, w, cin, _p(y), st), 'og_sp_maxpool2x2')
+                    _cabi.check(lib.og_sp_maxpool2x2(ptr(x), B, h, w, cin, ptr(y), st), 'og_sp_maxpool2x2')
                     x, h, w = y, h // 2, w // 2
             hc, wc = h, w
             # descriptor head (model.py:68-71)
             da = conv3(x, hc, wc, 128, 'convDa')
             coarse = ops.linear(da, *wts['convDb'])
-            _cabi.check(lib.og_row_normalize(_p(coarse), coarse.shape[0], self.descriptor_dim, 0, 0.0, st), 'og_row_normalize')
+            _cabi.check(lib.og_row_normalize(ptr(coarse), coarse.shape[0], self.descriptor_dim, 0, 0.0, st), 'og_row_normalize')
             # detector head (model.py:73-75) + heat map, NMS, threshold, borders (model.py:82-99)
             pa = conv3(x, hc, wc, 128, 'convPa')
             probs = ops.linear(pa, *wts['convPb'])                       # [B hc wc, 65]
-            _cabi.check(lib.og_softmax_rows(_p(probs), 65, probs.shape[0], 65, st), 'og_softmax_rows')
+            _cabi.check(lib.og_softmax_rows(ptr(probs), 65, probs.shape[0], 65, st), 'og_softmax_rows')
             self.last_probs = probs.view(B, hc, wc, 65)                  # kept for inspection / tests
         return probs, coarse
 
@@ -137,13 +137,13 @@ class SuperPointNet(nn.Module):
         with torch.cuda.device(dev):
             st = ops.st()
             heat = ops.empty(B, H, W)
-            _cabi.check(lib.og_sp_heat_nms(_p(probs), B, hc, wc, int(self.nms_kernel), float(self.keypoint_threshold), int(self.remove_borders_size),
-                                           _p(heat), st), 'og_sp_heat_nms')
+            _cabi.check(lib.og_sp_heat_nms(ptr(probs), B, hc, wc, int(self.nms_kernel), float(self.keypoint_threshold), int(self.remove_borders_size),
+                                           ptr(heat), st), 'og_sp_heat_nms')
             cap = min(H * W, _MAX_CAND)
             cand_idx = torch.empty(B, cap, dtype=torch.int32, device=dev)
             cand_score = ops.empty(B, cap)
             count = torch.empty(B, dtype=torch.int32, device=dev)
-            _cabi.check(lib.og_sp_compact(_p(heat), B, H * W, cap, C.c_void_p(cand_idx.data_ptr()), _p(cand_score), C.c_void_p(count.data_ptr()), st),
+            _cabi.check(lib.og_sp_compact(ptr(heat), B, H * W, cap, ptr(cand_idx), ptr(cand_score), ptr(count), st),
                         'og_sp_compact')
             counts = count.tolist()                                      # the one host synchronisation (the reference's nonzero)
             if max(counts) > cap:
@@ -161,11 +161,10 @@ class SuperPointNet(nn.Module):
             n_out = torch.tensor(keep, dtype=torch.int32, device=dev)
             modes = torch.tensor(mode, dtype=torch.int32, device=dev)
             kpts, scores = ops.empty(B, n, 2), ops.empty(B, n)
-            ip = lambda t: C.c_void_p(t.data_ptr())
-            _cabi.check(lib.og_sp_select(ip(cand_idx), _p(cand_score), ip(count), ip(n_out), ip(modes), B, cap, W, n, max(counts), _p(kpts), _p(scores), st),
+            _cabi.check(lib.og_sp_select(ptr(cand_idx), ptr(cand_score), ptr(count), ptr(n_out), ptr(modes), B, cap, W, n, max(counts), ptr(kpts), ptr(scores), st),
                         'og_sp_select')
             desc = ops.empty(B, n, d)
-            _cabi.check(lib.og_sp_sample_desc(_p(coarse), B, hc, wc, d, _p(kpts), ip(n_out), n, n, 8, _p(desc), st), 'og_sp_sample_desc')
+            _cabi.check(lib.og_sp_sample_desc(ptr(coarse), B, hc, wc, d, ptr(kpts), ptr(n_out), n, n, 8, ptr(desc), st), 'og_sp_sample_desc')
             lafs = torch.zeros(B, n, 2, 3, dtype=torch.float32, device=dev)  # identity frame + position (model.py:119-127)
             lafs[:, :, 0, 0] = 1.0
             lafs[:, :, 1, 1] = 1.0

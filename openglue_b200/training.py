@@ -20,7 +20,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import _cabi
-from ._ops import _Ops, _p, _pad4  # noqa: F401  (tests build their torch double of the kernels on _Ops' composite helpers)
+from ._ops import _Ops, _pad4  # noqa: F401  (tests build their torch double of the kernels on _Ops' composite helpers)
 
 __all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep']
 

@@ -12,7 +12,6 @@ prepare_features_output, the ordered compaction of the matches, and OpenGlueMatc
 4. GPU, OpenGlueMatcher on the two reference-minted matcher fixtures in every precision, and on a SuperPointNet image pair against
    a by-hand composition of the same public pieces.
 """
-import ctypes as C
 import os
 import sys
 
@@ -27,6 +26,7 @@ from gen_golden_features import (MATCH_CASES, METHODS, get_laf_center, get_laf_s
 
 import openglue_b200  # noqa: E402
 from openglue_b200 import features as FT  # noqa: E402
+from openglue_b200._cabi import ptr as _p, stream as _st  # noqa: E402
 
 GOLDEN = os.path.join(HERE, 'golden')
 DEV = 'cuda:0'
@@ -198,14 +198,6 @@ def _lib():
 def _check(rc, what):
     from openglue_b200 import _cabi
     _cabi.check(rc, what)
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _poisoned(n, dtype=torch.float32):

@@ -12,17 +12,10 @@ import pytest
 import torch
 
 from openglue_b200 import _cabi
+from openglue_b200._cabi import ptr as _p, stream as _st
 
 DEV = 'cuda:0'
 F16_BOUND, TF32_BOUND = 2e-6, 1.5e-6
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _sms():

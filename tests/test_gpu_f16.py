@@ -7,18 +7,11 @@ import pytest
 import torch
 
 from openglue_b200 import _cabi
+from openglue_b200._cabi import ptr as _p, stream as _st
 from oracle import superglue_oracle as O
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def split16(x2d, bias=None):

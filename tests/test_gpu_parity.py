@@ -15,6 +15,7 @@ import torch
 
 from conftest import GOLDEN_BIG, GOLDEN_FULL, GOLDEN_SAMPLED
 from openglue_b200 import _cabi
+from openglue_b200._cabi import ptr as _ptr, stream as _stream
 from openglue_b200.superglue import MatchingCore, SuperGlue
 from openglue_b200.synthetic import default_config, synthetic_pairs, synthetic_state_dict
 from oracle import superglue_oracle as O
@@ -34,14 +35,6 @@ def _model(cfg, sd, precision='fp32'):
     model = SuperGlue(cfg).eval()
     model.load_state_dict(sd, strict=True)
     return model.to(DEV)
-
-
-def _ptr(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def decisive_rows(scores_ref, margin):

@@ -7,14 +7,11 @@ import torch
 
 from conftest import GOLDEN_FULL
 from openglue_b200 import _cabi
+from openglue_b200._cabi import ptr as _p
 from openglue_b200.superglue import MatchingCore, SuperGlue
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
 
 
 @pytest.mark.parametrize('mode', [2, 0, 1])
@@ -31,7 +28,7 @@ def test_linear_tc_operator(mode, rows, k1, k2, nout, batch, per_batch_b):
     X = torch.cat([A, A2], -1) if k2 else A
     ref = (0.5 * (X.double() @ W.double().transpose(1, 2)) + bias.double()).relu() + R.double()
     lib = _cabi.lib()
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    st = _cabi.stream()
     dA, dW, db, dR = A.to(DEV), W.to(DEV), bias.to(DEV), R.to(DEV)
     dA2 = A2.to(DEV) if k2 else None
     Whi, Wlo = torch.empty_like(dW), torch.empty_like(dW)
@@ -70,7 +67,7 @@ def test_attention_tc_operator(B, H, dh, nq, nk):
     to_ref = lambda t: t.transpose(1, 2).reshape(B, H, dh, -1)
     ref = O.softmax_attention(to_ref(q).double(), to_ref(k).double(), to_ref(v).double()).reshape(B, d, nq).transpose(1, 2)
     lib = _cabi.lib()
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    st = _cabi.stream()
     dq, dk = q.to(DEV), k.to(DEV)
     ldv = (nk + 3) // 4 * 4
     dvt = torch.zeros(B, d, ldv, device=DEV)

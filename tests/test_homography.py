@@ -296,9 +296,8 @@ def _run_cabi(images_dev, offsets_dev, off):
     h, w = H - 2 * off, W - 2 * off
     bufs = [torch.full((B * h * w + GUARD,), float('nan'), device=DEV) for _ in range(2)]
     hbuf = torch.full((B * 9 + GUARD,), float('nan'), device=DEV)
-    rc = _lib().og_homography_pairs(C.c_void_p(images_dev.data_ptr()), B, H, W, off, C.c_void_p(offsets_dev.data_ptr()),
-                                    C.c_void_p(bufs[0].data_ptr()), C.c_void_p(bufs[1].data_ptr()), C.c_void_p(hbuf.data_ptr()),
-                                    C.c_void_p(torch.cuda.current_stream().cuda_stream))
+    from openglue_b200._cabi import ptr, stream
+    rc = _lib().og_homography_pairs(ptr(images_dev), B, H, W, off, ptr(offsets_dev), ptr(bufs[0]), ptr(bufs[1]), ptr(hbuf), stream())
     assert rc == 0, _lib().og_last_error()
     torch.cuda.synchronize()
     for t in (*bufs, hbuf):

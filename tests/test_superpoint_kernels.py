@@ -10,7 +10,6 @@
 
 Every GPU case prints what it measured next to its bound (run with -s).
 """
-import ctypes as C
 import math
 import os
 import sys
@@ -23,6 +22,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(os.path.dirname(HERE), 'oracle'))
 from gen_golden_superpoint_post import CASES as POST_CASES, inputs_sha256, post_inputs  # noqa: E402
 from test_superpoint import _decisions, _disagreements  # noqa: E402
+from openglue_b200._cabi import ptr as _p, stream as _st  # noqa: E402
 
 DEV = 'cuda:0'
 U = 2.0 ** -24                  # unit roundoff of float32
@@ -40,14 +40,6 @@ def _lib():
 def _check(rc, what):
     from openglue_b200 import _cabi
     _cabi.check(rc, what)
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _poisoned(n, dtype=torch.float32):

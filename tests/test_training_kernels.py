@@ -17,6 +17,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from openglue_b200._cabi import ptr as _p, stream as _st
 from oracle import loss_oracle as L
 from oracle import sinkhorn_grad_oracle as SG
 
@@ -32,14 +33,6 @@ def _lib():
 def _check(rc, what):
     from openglue_b200 import _cabi
     _cabi.check(rc, what)
-
-
-def _p(t, off=0):
-    return None if t is None else C.c_void_p(t.data_ptr() + t.element_size() * off)
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _sm_count():
