@@ -52,9 +52,9 @@ template <int DH, bool F16> struct Cfg {
   static constexpr int STAGE = 2 * K_TILE + 2 * V_TILE;
   static constexpr int STAGES = 3;
   static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE + 128;
-  // Fits the 196 KB shared-memory configuration of the GEMM kernels (193 KB + the 1 KB an SM reserves per block): a kernel that
-  // needs the 228 KB configuration leaves the SMs in it, and the GEMMs that follow in a step measured 5 % slower there.
-  static_assert(SMEM_BYTES + 1024 <= 196 * 1024, "shared-memory configuration of the GEMM kernels");
+  // Runs in the 228 KB shared-memory configuration, as the GEMM kernels do (preferred carveout set at launch): a kernel in
+  // another configuration makes the SMs switch between neighbours, which measured 5 % on the GEMMs of a step.
+  static_assert(SMEM_BYTES <= OG_SMEM_OPTIN_MAX, "dynamic shared memory of one block");
 };
 }  // namespace tca
 
@@ -471,7 +471,7 @@ inline int attention_sm90_launch(const TcAttnArgs& a, const F16AttnScales& sc, c
     if ((rc = tc::make_tmap_2d(&mvh, vthi, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
     if ((rc = tc::make_tmap_2d(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
   }
-  if ((rc = smem_opt_in<attention_sm90_kernel<DH, F16>>(C::SMEM_BYTES)) != OG_OK) return rc;
+  if ((rc = smem_opt_in<attention_sm90_kernel<DH, F16>>(C::SMEM_BYTES, true)) != OG_OK) return rc;   // the GEMMs' configuration
   return launch("attention_sm90_kernel", attention_sm90_kernel<DH, F16>, LaunchAttr::pdl, dim3(cdiv(a.nq, BM), a.num_heads, a.batch),
                 dim3(C::THREADS), C::SMEM_BYTES, stream, mkh, mkl, mvh, mvl, a, sc);
 }

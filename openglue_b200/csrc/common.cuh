@@ -88,12 +88,15 @@ inline const DeviceInfo& device_info() {
 constexpr size_t OG_SMEM_OPTIN_MAX = 227 * 1024;
 // Opts Kernel in to `bytes` of dynamic shared memory, once per device.  The flag is keyed on the kernel itself (every template
 // instantiation has its own) and set only after the call succeeded, so a failed opt-in is retried on the next launch.
+// max_carveout: the kernel prefers the largest shared-memory configuration of the SM (228 KB on sm_90) even where it needs less,
+// so that it does not switch the SMs' configuration against neighbours that need it.
 template <auto Kernel>
-inline int smem_opt_in(int bytes) {
+inline int smem_opt_in(int bytes, bool max_carveout = false) {
   static bool done[OG_MAX_DEVICES] = {};
   bool& d = done[current_device()];
   if (!d) {
     OG_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    if (max_carveout) OG_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     d = true;
   }
   return OG_OK;

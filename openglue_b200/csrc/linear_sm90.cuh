@@ -74,11 +74,14 @@ template <bool F16> struct Cfg {
   static constexpr int STAGE = A_BYTES + 2 * B_TILE;
   static constexpr int STAGES = F16 ? 3 : 4;              // 192 KB
   static constexpr int CHUNK = 2;                         // K blocks per wgmma accumulator chunk
-  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE + 128;
-  // The attention kernel and the GEMMs share the 196 KB shared-memory configuration (193 KB + the 1 KB an SM reserves per
-  // block): a kernel that needs the 228 KB configuration moves the SMs there, and the kernels around it run slower.
-  static_assert(SMEM_BYTES + 1024 <= 196 * 1024, "shared-memory configuration of the attention and GEMM kernels");
+  // fp16 form: an output staging buffer per consumer, one 64-row x 64-column half of its tile (fp32, or fp16 hi + lo)
+  static constexpr int STAGING = F16 ? 64 * 64 * 4 : 0;
+  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE + 2 * STAGING + 128;
+  // The GEMMs and the attention kernel run in the 228 KB shared-memory configuration (cudaFuncAttributePreferredSharedMemory-
+  // Carveout, set at launch): a neighbour in another configuration would make the SMs switch between kernels.
+  static_assert(SMEM_BYTES <= OG_SMEM_OPTIN_MAX, "dynamic shared memory of one block");
 };
+constexpr int EPI = 3;                                    // named barriers EPI + consumer: one consumer's epilogue (ids 1, 2: TURN)
 // output tile `tile` of the static schedule: column tile fastest, then row tile, then batch item
 __host__ __device__ __forceinline__ void tile_origin(int tile, int tiles_n, int tiles_m, int& n0, int& m0, int& bz) {
   const int rt = tile / tiles_n;
@@ -95,38 +98,39 @@ __device__ __forceinline__ const float* sw128_f32(const uint8_t* tile, int r, in
   return reinterpret_cast<const float*>(tile + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4);
 }
 
-__device__ __forceinline__ void store_half_pair(__half* p, uint32_t v, bool both) {
-  if (both) *reinterpret_cast<uint32_t*>(p) = v;
-  else *p = __ushort_as_half((unsigned short)(v & 0xffffu));
-}
-// the first n (< 8) 16-bit elements of v, element 0 at p
-__device__ __forceinline__ void store_b16_run(__half* p, uint4 v, int n) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    if (i < n) p[i] = __ushort_as_half((unsigned short)(i & 1 ? w[i >> 1] >> 16 : w[i >> 1] & 0xffffu));
-}
+// Output tensor maps of the fp16 form, one per output (box: 32 fp32 or 64 fp16 elements x 64 rows x 1, 128-byte swizzle):
+// y = Y [batch, rows, cols], hi / lo = Yh / Yl [batch, rows, cols], thi / tlo = Yth / Ytl [batch, cols, rows] (cols: nout, or
+// kind_cols with nkinds > 1).  tma = 0: the base, a stride or the row length of some output is not a multiple of 16 bytes, and
+// the staged boxes are stored by the consumer's threads (out_copy_box).
+struct OutMaps {
+  CUtensorMap y, hi, lo, thi, tlo;
+  int tma;
+};
 
-// Lane t of a quad holds w[j] = 16-bit elements (8j + 2t, 8j + 2t + 1) of one row (element 0 in the low half), j = 0..15.  Returns
-// the elements 8 (4q + t) .. 8 (4q + t) + 7 of that row: two rounds of exchanges within the quad (whole quads must take part).
-__device__ __forceinline__ uint4 quad_gather_b16(const uint32_t (&w)[16], int q, int t) {
-  const uint32_t x0 = w[4 * q], x1 = w[4 * q + 1], x2 = w[4 * q + 2], x3 = w[4 * q + 3];
-  const bool odd = t & 1, upper = t & 2;
-  // lanes t, t ^ 1: the even lane collects blocks 4q / 4q + 2, the odd lane blocks 4q + 1 / 4q + 3, four elements each
-  const uint32_t r0 = __shfl_xor_sync(0xffffffffu, odd ? x0 : x1, 1), r1 = __shfl_xor_sync(0xffffffffu, odd ? x2 : x3, 1);
-  const uint2 p0 = odd ? make_uint2(r0, x1) : make_uint2(x0, r0);  // block 4q + (t & 1), elements 4 (t >> 1) .. + 3
-  const uint2 p1 = odd ? make_uint2(r1, x3) : make_uint2(x2, r1);  // block 4q + 2 + (t & 1)
-  // lanes t, t ^ 2: the lower pair completes block 4q + t from p0, the upper pair from p1
-  const uint2 sd = upper ? p0 : p1;
-  const uint32_t s0 = __shfl_xor_sync(0xffffffffu, sd.x, 2), s1 = __shfl_xor_sync(0xffffffffu, sd.y, 2);
-  return upper ? make_uint4(s0, s1, p1.x, p1.y) : make_uint4(p0.x, p0.y, s0, s1);
+// byte offset of 16-byte chunk `chunk` of row `r` in a box of 128-byte rows written with the 128-byte swizzle
+__device__ __forceinline__ int sw128_chunk(int r, int chunk) { return r * 128 + ((chunk ^ (r & 7)) << 4); }
+
+// The box at `box` ([64 rows x 128 bytes], 128-byte swizzle) to T elements base[bz * bstride + (o0 + o) * ld + i0 + i] with
+// o0 + o < olim and i0 + i < ilim, by the 128 threads of one consumer (tid).
+template <class T>
+__device__ __forceinline__ void out_copy_box(const uint8_t* box, T* base, int64_t ld, int64_t bstride, int bz, int i0, int o0, int ilim,
+                                             int olim, int tid) {
+  constexpr int NI = 128 / sizeof(T);
+  for (int idx = tid; idx < 64 * NI; idx += 128) {
+    const int o = idx / NI, i = idx - o * NI;
+    if (o0 + o >= olim || i0 + i >= ilim) continue;
+    const int b = i * (int)sizeof(T);
+    base[(int64_t)bz * bstride + (int64_t)(o0 + o) * ld + i0 + i] =
+        *reinterpret_cast<const T*>(box + sw128_chunk(o, b >> 4) + (b & 15));
+  }
 }
 
 template <class Args>
 __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                       const __grid_constant__ CUtensorMap map_a2,
                                                                       const __grid_constant__ CUtensorMap map_bhi,
-                                                                      const __grid_constant__ CUtensorMap map_blo, Args a) {
+                                                                      const __grid_constant__ CUtensorMap map_blo,
+                                                                      const __grid_constant__ OutMaps om, Args a) {
   using namespace tcf;
   using namespace tc;
   constexpr bool F16 = std::is_same<Args, F16LinearArgs>::value;
@@ -136,7 +140,7 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
   launch_dependents();
   extern __shared__ uint8_t og_lin_smem_raw[];
   uint8_t* smem = align_smem_1024(og_lin_smem_raw);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * C::STAGE);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * C::STAGE + 2 * C::STAGING);
   uint64_t* empty = full + S;
   volatile uint32_t* timeout_flag = reinterpret_cast<uint32_t*>(empty + S);   // a consumer's wait on `full` timed out
 
@@ -150,6 +154,13 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
     fence_barrier_init();
     prefetch_tensormap(&map_a); prefetch_tensormap(&map_a2);
     prefetch_tensormap(&map_bhi); prefetch_tensormap(&map_blo);
+    if constexpr (F16) {
+      if (om.tma) {
+        if (a.Y) prefetch_tensormap(&om.y);
+        if (a.Yh) { prefetch_tensormap(&om.hi); prefetch_tensormap(&om.lo); }
+        if (a.Yth) { prefetch_tensormap(&om.thi); prefetch_tensormap(&om.tlo); }
+      }
+    }
   }
   __syncthreads();
   grid_dependency_wait();                                    // A, the amax slots and the residual come from previous kernels
@@ -290,7 +301,10 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
       if (kb + 1 < nkb) mma_block(kb + 1, ahi1, alo1, ahi0, alo0);
     }
 
-    // ---- epilogue: thread holds rows r0 / r0 + 8, columns n0 + 8j + 2t (+1), j = 0..15
+    // ---- epilogue: thread holds rows r0 / r0 + 8, columns n0 + 8j + 2t (+1), j = 0..15.  fp16 form: each 64-column half of
+    // the consumer's 64 x 128 outputs is computed into its staging buffer and stored from there by TMA, so the consumer goes on
+    // to the next tile's MMAs while the copy engine writes the tile; before it writes the buffer again, it waits for the reads of
+    // the previous stores.
     if constexpr (F16) {
       const float s_w = __ldg(a.w_meta);
       int okind = a.Y ? 1 : (a.Yh ? 2 : 3), kidx = 0, ocols = a.nout;
@@ -303,18 +317,28 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
       }
       if (okind != 1) sos = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(wm + 1), __ldg(wm + 2)));
       float tmax = 0.f;
-      if (okind == 1) {
-        // Every load of the epilogue is issued before its first store: the compiler may not move a load across a store to a
-        // pointer that could alias it, and loads interleaved with the stores expose one memory latency per 8-column block.
+      uint8_t* stg = smem + S * C::STAGE + c * C::STAGING;   // two boxes of 64 rows x 128 bytes
+      const int rl = warp * 16 + g;                          // rows r0 / r0 + 8 within the consumer's 64
+      const int orow = m0 + 64 * c, bzy = a.strideY ? bz : 0, bzt = a.strideYt ? bz : 0;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int grow = m0 + r0 + 8 * h;
-          if (grow >= a.rows) continue;
-          const float* rrow = a.R ? a.R + (int64_t)bz * a.strideR + (int64_t)grow * a.ldr : nullptr;
+      for (int hf = 0; hf < 2; ++hf) {
+        const int oc = n0 - kidx * ocols + 64 * hf;          // first column of this half in its output
+        // the half's values are computed in registers first, so that the wait for the previous stores' reads overlaps them
+        auto buffer_free = [&] {
+          if (tid == 0) bulk_wait_read<0>();
+          named_bar_sync(EPI + c, 128);
+        };
+        if (okind == 1) {
+          float2 yv[2][8];
+          // Every load of the half is issued before its first store: the compiler may not move a load across a store to a
+          // pointer that could alias it, and loads interleaved with the stores expose one memory latency per 8-column block.
+          // R may be Y: the half's residual is read before any of it is stored.
 #pragma unroll
-          for (int jh = 0; jh < 16; jh += 8) {
-            // bias and residual of columns n0 + 8 (jh + i / 2) + 2t + (i % 2), loaded before the stores (R may be Y: each
-            // element is read and written by this thread only)
+          for (int h = 0; h < 2; ++h) {
+            const int grow = m0 + r0 + 8 * h;
+            const float* rrow = a.R && grow < a.rows ? a.R + (int64_t)bz * a.strideR + (int64_t)grow * a.ldr : nullptr;
+            const int jh = 8 * hf;
+            // bias and residual of columns n0 + 8 (jh + i / 2) + 2t + (i % 2)
             float bv[16], rv[16];
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
@@ -327,90 +351,78 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
             for (int jj = 0; jj < 8; ++jj) {
               const int j = jh + jj;
               const int col = n0 + 8 * j + 2 * t;
-              if (col >= a.nout) continue;
               const bool two = col + 1 < a.nout;
               float y0 = fmaf(racc[4 * j + 2 * h], alpha_t, bv[2 * jj]);
               float y1 = two ? fmaf(racc[4 * j + 2 * h + 1], alpha_t, bv[2 * jj + 1]) : 0.f;
               if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
-              const int64_t o = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy + col;
               if (a.R) {
                 y0 += rv[2 * jj];
                 if (two) y1 += rv[2 * jj + 1];
               }
-              if (two) *reinterpret_cast<float2*>(a.Y + o) = make_float2(y0, y1);
-              else a.Y[o] = y0;
-              tmax = fmaxf(tmax, fmaxf(fabsf(y0), fabsf(y1)));
+              if (grow < a.rows && col < a.nout) tmax = fmaxf(tmax, fmaxf(fabsf(y0), fabsf(y1)));
+              yv[h][jj] = make_float2(y0, y1);
             }
           }
-        }
-      } else {
-        // fp16 hi / lo operands: every element is computed first (also rows / columns past the tensor, which are not stored), so
-        // that whole warps take part in the shuffles that regroup them into 16-byte runs
-        uint32_t hv[2][16], lv[2][16];                       // [row r0 | r0 + 8][j]: columns n0 + 8j + 2t, +1 (element 0 low)
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int col = n0 + 8 * j + 2 * t;
-          const bool two = col + 1 < a.nout;
-          const float b0 = a.bias && col < a.nout ? __ldg(a.bias + col) : 0.f;
-          const float b1 = a.bias && two ? __ldg(a.bias + col + 1) : 0.f;
+          buffer_free();
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float y0 = fmaf(racc[4 * j + 2 * h], alpha_t, b0);
-            float y1 = two ? fmaf(racc[4 * j + 2 * h + 1], alpha_t, b1) : 0.f;
-            if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
-            split_f16x2(y0 * sos, y1 * sos, hv[h][j], lv[h][j]);
-          }
-        }
-        if (okind == 2) {
-          const bool wide = a.ldy % 8 == 0 && a.strideY % 8 == 0 && al16(a.Yh) && al16(a.Yl);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int grow = m0 + r0 + 8 * h;
-            const int64_t orow = (int64_t)bz * a.strideY + (int64_t)grow * a.ldy - kidx * ocols;
-            if (wide) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {                  // this thread stores columns n0 + 8 (4q + t) .. + 7
-                const uint4 vh = quad_gather_b16(hv[h], q, t), vl = quad_gather_b16(lv[h], q, t);
-                const int col = n0 + 8 * (4 * q + t);
-                if (grow >= a.rows || col >= a.nout) continue;
-                if (col + 8 <= a.nout) {
-                  *reinterpret_cast<uint4*>(a.Yh + orow + col) = vh;
-                  *reinterpret_cast<uint4*>(a.Yl + orow + col) = vl;
-                } else {
-                  store_b16_run(a.Yh + orow + col, vh, a.nout - col);
-                  store_b16_run(a.Yl + orow + col, vl, a.nout - col);
-                }
-              }
-            } else if (grow < a.rows) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const int col = n0 + 8 * j + 2 * t;
-                if (col >= a.nout) continue;
-                store_half_pair(a.Yh + orow + col, hv[h][j], col + 1 < a.nout);
-                store_half_pair(a.Yl + orow + col, lv[h][j], col + 1 < a.nout);
-              }
-            }
+            for (int jj = 0; jj < 8; ++jj)                     // box jj / 4 holds columns 32 (jj / 4) .. + 31 of the half
+              *reinterpret_cast<float2*>(stg + (jj >> 2) * 8192 + sw128_chunk(rl + 8 * h, 2 * (jj & 3) + (t >> 1)) + (t & 1) * 8) = yv[h][jj];
           }
         } else {
-          // V^T: the lanes of a warp hold 16 rows of a column, two 16-byte runs.  Gathering such runs in one lane (an 8 x 8 exchange)
-          // made each store touch 32 columns, 32 rows of V^T that lie ldyt apart, and measured 3x slower than these stores.
+          // fp16 hi / lo operands (box 0: hi, box 1: lo): every element is computed (also rows / columns past the tensor, which
+          // are not stored), then written as 8 x 8 matrices (h, jj) by stmatrix, four per instruction
+          uint32_t hv[2][8], lv[2][8];                         // [row r0 | r0 + 8][jj]: columns n0 + 8 (8 hf + jj) + 2t, +1
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int grow = m0 + r0 + 8 * h;
-            if (grow < a.rows) {
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * hf + jj;
+            const int col = n0 + 8 * j + 2 * t;
+            const bool two = col + 1 < a.nout;
+            const float b0 = a.bias && col < a.nout ? __ldg(a.bias + col) : 0.f;
+            const float b1 = a.bias && two ? __ldg(a.bias + col + 1) : 0.f;
 #pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const int col = n0 + 8 * j + 2 * t;
-                if (col >= a.nout) continue;
-                const int64_t o = (int64_t)bz * a.strideYt + grow + (int64_t)(col - kidx * ocols) * a.ldyt;
-                a.Yth[o] = __ushort_as_half((unsigned short)(hv[h][j] & 0xffffu)); a.Ytl[o] = __ushort_as_half((unsigned short)(lv[h][j] & 0xffffu));
-                if (col + 1 < a.nout) {
-                  a.Yth[o + a.ldyt] = __ushort_as_half((unsigned short)(hv[h][j] >> 16));
-                  a.Ytl[o + a.ldyt] = __ushort_as_half((unsigned short)(lv[h][j] >> 16));
-                }
-              }
+            for (int h = 0; h < 2; ++h) {
+              float y0 = fmaf(racc[4 * j + 2 * h], alpha_t, b0);
+              float y1 = two ? fmaf(racc[4 * j + 2 * h + 1], alpha_t, b1) : 0.f;
+              if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+              split_f16x2(y0 * sos, y1 * sos, hv[h][jj], lv[h][jj]);
             }
           }
+          buffer_free();
+          const int m = lane >> 3, k = lane & 7;               // this lane addresses row k of matrix m: h = m % 2, jj = 2q + m / 2
+          const uint32_t stg_u = smem_u32(stg);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const uint32_t rh[4] = {hv[0][2 * q], hv[1][2 * q], hv[0][2 * q + 1], hv[1][2 * q + 1]};
+            const uint32_t rlo[4] = {lv[0][2 * q], lv[1][2 * q], lv[0][2 * q + 1], lv[1][2 * q + 1]};
+            if (okind == 2) {                                  // row: keypoint; 16-byte chunk: 8 columns
+              const uint32_t ad = stg_u + sw128_chunk(warp * 16 + 8 * (m & 1) + k, 2 * q + (m >> 1));
+              stmatrix_x4(ad, rh); stmatrix_x4(ad + 8192, rlo);
+            } else {                                           // V^T, row: column (channel); 16-byte chunk: 8 keypoints
+              const uint32_t ad = stg_u + sw128_chunk(8 * (2 * q + (m >> 1)) + k, 2 * warp + (m & 1));
+              stmatrix_x4_trans(ad, rh); stmatrix_x4_trans(ad + 8192, rlo);
+            }
+          }
+        }
+        fence_proxy_async();
+        named_bar_sync(EPI + c, 128);
+        if (om.tma) {
+          if (tid == 0) {
+            if (okind == 1) { tma_store_3d(&om.y, stg, oc, orow, bzy); tma_store_3d(&om.y, stg + 8192, oc + 32, orow, bzy); }
+            else if (okind == 2) { tma_store_3d(&om.hi, stg, oc, orow, bzy); tma_store_3d(&om.lo, stg + 8192, oc, orow, bzy); }
+            else { tma_store_3d(&om.thi, stg, orow, oc, bzt); tma_store_3d(&om.tlo, stg + 8192, orow, oc, bzt); }
+            bulk_commit();
+          }
+        } else if (okind == 1) {
+          out_copy_box(stg, a.Y, a.ldy, a.strideY, bz, oc, orow, ocols, a.rows, tid);
+          out_copy_box(stg + 8192, a.Y, a.ldy, a.strideY, bz, oc + 32, orow, ocols, a.rows, tid);
+        } else if (okind == 2) {
+          out_copy_box(stg, a.Yh, a.ldy, a.strideY, bz, oc, orow, ocols, a.rows, tid);
+          out_copy_box(stg + 8192, a.Yl, a.ldy, a.strideY, bz, oc, orow, ocols, a.rows, tid);
+        } else {
+          out_copy_box(stg, a.Yth, a.ldyt, a.strideYt, bz, orow, oc, a.rows, ocols, tid);
+          out_copy_box(stg + 8192, a.Ytl, a.ldyt, a.strideYt, bz, orow, oc, a.rows, ocols, tid);
         }
       }
       if (okind == 1 && a.amax_out) {
@@ -461,6 +473,8 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
       }
     }
   }
+  // the outputs' stores have read the staging buffers (which live as long as the CTA) and are complete before the CTA exits
+  if constexpr (F16) { if (tid == 0) bulk_wait<0>(); }
 }
 
 template <class Args, class BT>
@@ -481,12 +495,33 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
     if ((rc = tc::make_tmap_2d(&mh, Bhi, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
     if ((rc = tc::make_tmap_2d(&ml, Blo, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
   }
-  if ((rc = smem_opt_in<linear_sm90_kernel<Args>>(C::SMEM_BYTES)) != OG_OK) return rc;
+  OutMaps om;
+  memset(&om, 0, sizeof(om));
+  if constexpr (F16) {
+    // TMA stores need 16-byte aligned outputs with strides in multiples of 16 bytes, and they clip a box at the end of a row only
+    // to a multiple of 16 bytes (measured on H100: a row of 334 fp32 had two more elements written).  Any other layout is
+    // stored by the threads.
+    const int ocols = a.nkinds > 1 ? a.kind_cols : a.nout;
+    const auto ok16 = [&](const void* p, int64_t ld, int64_t stride, int64_t inner, int esz) {
+      return al16(p) && ld * esz % 16 == 0 && (a.batch == 1 || stride * esz % 16 == 0) && inner * esz % 16 == 0;
+    };
+    om.tma = (!a.Y || ok16(a.Y, a.ldy, a.strideY, ocols, 4)) &&
+             (!a.Yh || (ok16(a.Yh, a.ldy, a.strideY, ocols, 2) && ok16(a.Yl, a.ldy, a.strideY, ocols, 2))) &&
+             (!a.Yth || (ok16(a.Yth, a.ldyt, a.strideYt, a.rows, 2) && ok16(a.Ytl, a.ldyt, a.strideYt, a.rows, 2)));
+    if (om.tma && a.Y) om.tma = tc::make_tmap_3d(&om.y, a.Y, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
+    if (om.tma && a.Yh)
+      om.tma = tc::make_tmap_3d_f16(&om.hi, a.Yh, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK &&
+               tc::make_tmap_3d_f16(&om.lo, a.Yl, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
+    if (om.tma && a.Yth)
+      om.tma = tc::make_tmap_3d_f16(&om.thi, a.Yth, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK &&
+               tc::make_tmap_3d_f16(&om.tlo, a.Ytl, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK;
+  }
+  if ((rc = smem_opt_in<linear_sm90_kernel<Args>>(C::SMEM_BYTES, true)) != OG_OK) return rc;
   const int tiles = cdiv(a.nout, BN) * cdiv(a.rows, BM) * a.batch;
   const int sms = device_info().ok ? device_info().sm_count : 132;
   // persistent: each CTA walks tiles blockIdx.x + i gridDim.x
   return launch("linear_sm90_kernel", linear_sm90_kernel<Args>, LaunchAttr::pdl, dim3(std::min(tiles, sms)), dim3(THREADS), C::SMEM_BYTES,
-                stream, ma, ma2, mh, ml, a);
+                stream, ma, ma2, mh, ml, om, a);
 }
 // The two operand forms, instantiated next to the template: where the kernels sit in the binary (and so a cuobjdump -sass
 // comparison of two builds) does not depend on where the host code first launches them.

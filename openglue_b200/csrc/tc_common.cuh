@@ -85,6 +85,30 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// Stores of a shared-memory box to global memory through a tensor map (the parts of the box outside the tensor are not
+// written).  The writes to the box must be made visible to the async proxy first (fence_proxy_async, then a barrier among the
+// writing threads).  The stores of one thread are grouped by bulk_commit: bulk_wait_read<N> returns once at most N groups still
+// read shared memory (the box may then be written again), bulk_wait<N> once at most N groups are still incomplete.
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Four 8 x 8 matrices of 16-bit elements from the mma fragment layout (lane l holds row l / 4, elements 2 (l % 4), +1 of matrix
+// i in r[i]) to shared memory: lane l gives the address of row l % 8 of matrix l / 8 (16 bytes).  trans: the rows written are the
+// matrices' columns.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
 
 // ----------------------------------------------------------------------------- programmatic dependent launch
 // Kernels launched with LaunchAttr::pdl (cudaLaunchAttributeProgrammaticStreamSerialization) may become resident while the
@@ -271,6 +295,24 @@ inline int make_tmap_2d_f16(CUtensorMap* map, const __half* base, uint64_t rows,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled (f16) failed (%d): rows=%llu cols=%llu ld=%llu", (int)r,
                                      (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld);
+  return OG_OK;
+}
+
+// 3-D fp16 tensor [batch, rows, cols] (row stride ld, batch stride bstride, in elements); box = 64 halves (128 bytes) x box_rows x 1,
+// 128B swizzle.
+inline int make_tmap_3d_f16(CUtensorMap* map, const __half* base, uint64_t batch, uint64_t rows, uint64_t cols, uint64_t ld,
+                            uint64_t bstride, uint32_t box_rows) {
+  PFN_encodeTiled fn = get_encode_fn();
+  if (!fn) return fail(OG_ECUDA, "cuTensorMapEncodeTiled entry point not available");
+  if (batch <= 1 || bstride == 0) { batch = 1; bstride = rows * ld; }
+  cuuint64_t dims[3] = {cols, rows, batch};
+  cuuint64_t strides[2] = {ld * sizeof(__half), bstride * sizeof(__half)};
+  cuuint32_t box[3] = {64, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled (3d f16) failed (%d)", (int)r);
   return OG_OK;
 }
 
