@@ -148,35 +148,48 @@ template <class T> static T gemm_args(const og_linear_args& a) {
   return t;
 }
 
-// Launches the tensor-core GEMM t = gemm_args(a) + the caller's fields on the weight split Bhi / Blo (a.W's layout); an
-// untileable shape fails with "who: why".
+// Whether the tensor-core GEMM can run t = gemm_args(a) + the caller's fields on the weight split Bhi / Blo (a.W's layout): every
+// batch item starts at a whole row of B, and linear_sm90_eligible holds.
 template <class T, class BT>
-static int linear_sm90_run(const og_linear_args& a, const T& t, const BT* Bhi, const BT* Blo, const char* who, const char* why,
-                           cudaStream_t s) {
-  if (a.strideW && a.strideW % a.ldw != 0) return fail(OG_EUNSUPPORTED, "%s: strideW must be a multiple of ldw", who);
-  if (!linear_sm90_eligible(t, Bhi, Blo, a.ldw)) return fail(OG_EUNSUPPORTED, "%s: %s", who, why);
+static bool gemm_tileable(const og_linear_args& a, const T& t, const BT* Bhi, const BT* Blo) {
+  return (!a.strideW || a.strideW % a.ldw == 0) && linear_sm90_eligible(t, Bhi, Blo, a.ldw);
+}
+
+// Launches the tensor-core GEMM t on a shape gemm_tileable accepted.
+template <class T, class BT>
+static int gemm_launch(const og_linear_args& a, const T& t, const BT* Bhi, const BT* Blo, cudaStream_t s) {
   // rows the B tensor map may touch: the LAST batch item only owns nout rows (a map declared over b_rows_per_batch * batch rows
   // would let a 128-row TMA box read past the end of a head-sliced or exactly-sized operand; rows beyond the map are zero-filled)
   const int64_t brows = a.strideW ? (int64_t)t.b_rows_per_batch * (a.batch - 1) + a.nout : a.nout;
   return linear_sm90_launch(t, Bhi, Blo, a.ldw, brows, s);
 }
 
+// gemm_launch, where an untileable shape fails with "who: why"
+template <class T, class BT>
+static int linear_sm90_run(const og_linear_args& a, const T& t, const BT* Bhi, const BT* Blo, const char* who, const char* why,
+                           cudaStream_t s) {
+  if (!gemm_tileable(a, t, Bhi, Blo))
+    return fail(OG_EUNSUPPORTED, "%s: %s", who, a.strideW && a.strideW % a.ldw != 0 ? "strideW must be a multiple of ldw" : why);
+  return gemm_launch(a, t, Bhi, Blo, s);
+}
+
 // Split-output request for the tensor-core path (the fp32 CUDA-core path ignores it).
 struct SplitOut { float *Yhi = nullptr, *Ylo = nullptr, *Ythi = nullptr, *Ytlo = nullptr; };
 
-static int linear_tc_run(const og_linear_args& a, const float* Whi, const float* Wlo, const SplitOut& so, cudaStream_t s) {
+static TcLinearArgs tc_args(const og_linear_args& a, const SplitOut& so) {
   TcLinearArgs t = gemm_args<TcLinearArgs>(a);
   t.Yhi = so.Yhi; t.Ylo = so.Ylo; t.Ythi = so.Ythi; t.Ytlo = so.Ytlo;
-  return linear_sm90_run(a, t, Whi, Wlo, "linear_tc",
-                         "needs K >= 32, K % 4 == 0, k1 % 32 == 0 with a second operand and 16-byte aligned rows", s);
+  return t;
 }
 
 // Kernel selection for one linear layer: the wgmma 3xTF32 GEMM when asked for and the shape is tileable,
 // otherwise the fp32 CUDA-core kernel (tiny K such as the 3-channel keypoint-encoder input).
 static int linear_dispatch(const og_linear_args& a, int precision, cudaStream_t s, const float* Whi = nullptr,
                            const float* Wlo = nullptr, const SplitOut& so = SplitOut()) {
-  if (precision == OG_PREC_TF32X3 && Whi && Wlo && linear_sm90_eligible(gemm_args<TcLinearArgs>(a), Whi, Wlo, a.ldw))
-    return linear_tc_run(a, Whi, Wlo, so, s);
+  if (precision == OG_PREC_TF32X3 && Whi && Wlo) {
+    const TcLinearArgs t = tc_args(a, so);
+    if (gemm_tileable(a, t, Whi, Wlo)) return gemm_launch(a, t, Whi, Wlo, s);
+  }
   if (so.Yhi || so.Ythi) return fail(OG_EUNSUPPORTED, "split outputs need the tensor-core path");
   return linear_simt_launch(a, s);
 }
@@ -262,7 +275,7 @@ int og_linear_fwd(const og_linear_args* a, int precision, void* stream) {
   OG_CHECK_ARG(precision == OG_PREC_FP32, "linear: the tensor-core form takes pre-split weights (og_linear_tc_fwd)");
   OG_CHECK_ARG(a->rows > 0 && a->nout > 0 && a->batch > 0 && a->k1 > 0 && a->k2 >= 0, "linear: bad sizes");
   OG_CHECK_ARG(a->k2 == 0 || a->A2, "linear: k2 > 0 needs A2");
-  return linear_dispatch(*a, precision, (cudaStream_t)stream);
+  return linear_simt_launch(*a, (cudaStream_t)stream);
 }
 
 int og_linear_tc_fwd(const og_linear_args* a, const float* Whi, const float* Wlo, float* Yhi, float* Ylo, float* Ythi,
@@ -272,7 +285,8 @@ int og_linear_tc_fwd(const og_linear_args* a, const float* Whi, const float* Wlo
   OG_CHECK_ARG((Yhi == nullptr) == (Ylo == nullptr) && (Ythi == nullptr) == (Ytlo == nullptr), "linear_tc: hi/lo come in pairs");
   (void)mode;                                      // every mode runs the one sm_90 kernel (see the header)
   SplitOut so; so.Yhi = Yhi; so.Ylo = Ylo; so.Ythi = Ythi; so.Ytlo = Ytlo;
-  return linear_tc_run(*a, Whi, Wlo, so, (cudaStream_t)stream);
+  return linear_sm90_run(*a, tc_args(*a, so), Whi, Wlo, "linear_tc",
+                         "needs K >= 32, K % 4 == 0, k1 % 32 == 0 with a second operand and 16-byte aligned rows", (cudaStream_t)stream);
 }
 
 // one GEMM of the training step: wgmma 3xTF32 when the shape is tileable (W is split on the fly into split_scratch, 2 x the
@@ -285,12 +299,13 @@ int og_linear_auto_fwd(const og_linear_args* a, int precision, float* split_scra
   OG_CHECK_ARG(a && a->A && a->W && (a->Y || a->Yt), "linear_auto: null pointer");
   OG_CHECK_ARG(a->rows > 0 && a->nout > 0 && a->batch > 0 && a->k1 > 0 && a->k2 >= 0, "linear_auto: bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision != OG_PREC_FP32 && split_scratch && (!a->strideW || a->strideW % a->ldw == 0)) {
+  if (precision != OG_PREC_FP32 && split_scratch && aligned16(a->W)) {
     const int64_t wf = weight_floats(*a);
     float* hi = split_scratch; float* lo = split_scratch + align_up(wf, 64);
-    if (linear_sm90_eligible(gemm_args<TcLinearArgs>(*a), hi, lo, a->ldw) && (reinterpret_cast<uintptr_t>(a->W) & 15) == 0) {
+    const TcLinearArgs t = gemm_args<TcLinearArgs>(*a);
+    if (gemm_tileable(*a, t, hi, lo)) {
       if (const int rc = OG_LAUNCH(split_tf32_kernel, (unsigned)((wf + 255) / 256), 256, 0, st, a->W, hi, lo, wf)) return rc;
-      return linear_tc_run(*a, hi, lo, SplitOut(), st);
+      return gemm_launch(*a, t, hi, lo, st);
     }
   }
   return linear_simt_launch(*a, st);

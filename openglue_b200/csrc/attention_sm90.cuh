@@ -460,17 +460,10 @@ inline int attention_sm90_launch(const TcAttnArgs& a, const F16AttnScales& sc, c
   using C = Cfg<DH, F16>;
   CUtensorMap mkh, mkl, mvh, mvl;
   int rc;
-  if constexpr (F16) {
-    if ((rc = tc::make_tmap_2d_f16(&mkh, khi, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d_f16(&mkl, klo, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d_f16(&mvh, vthi, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d_f16(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
-  } else {
-    if ((rc = tc::make_tmap_2d(&mkh, khi, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d(&mkl, klo, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d(&mvh, vthi, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
-  }
+  if ((rc = tc::make_tmap_2d(&mkh, khi, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
+  if ((rc = tc::make_tmap_2d(&mkl, klo, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
+  if ((rc = tc::make_tmap_2d(&mvh, vthi, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
+  if ((rc = tc::make_tmap_2d(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
   if ((rc = smem_opt_in<attention_sm90_kernel<DH, F16>>(C::SMEM_BYTES, true)) != OG_OK) return rc;   // the GEMMs' configuration
   return launch("attention_sm90_kernel", attention_sm90_kernel<DH, F16>, LaunchAttr::pdl, dim3(cdiv(a.nq, BM), a.num_heads, a.batch),
                 dim3(C::THREADS), C::SMEM_BYTES, stream, mkh, mkl, mvh, mvl, a, sc);

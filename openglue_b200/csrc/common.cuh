@@ -104,6 +104,7 @@ inline int smem_opt_in(int bytes, bool max_carveout = false) {
 
 __host__ __device__ inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+__host__ __device__ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll

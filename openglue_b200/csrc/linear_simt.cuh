@@ -139,8 +139,6 @@ __global__ void __launch_bounds__(256, 2) linear_simt_kernel(og_linear_args a, L
   }
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 inline int linear_simt_launch(const og_linear_args& a, cudaStream_t stream) {
   LinearFlags f;
   f.vecA = (a.k1 % 4 == 0) && (a.k2 % 4 == 0) && (a.lda % 4 == 0) && (a.strideA % 4 == 0) && aligned16(a.A) &&

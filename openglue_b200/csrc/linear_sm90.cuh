@@ -91,8 +91,6 @@ __host__ __device__ __forceinline__ void tile_origin(int tile, int tiles_n, int 
 }
 }  // namespace tcf
 
-__host__ __device__ inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 // fp32 element (r, c) of a [rows x 32] fp32 tile written by TMA with the 128-byte swizzle
 __device__ __forceinline__ const float* sw128_f32(const uint8_t* tile, int r, int c) {
   return reinterpret_cast<const float*>(tile + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4);
@@ -488,13 +486,8 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
   if ((rc = tc::make_tmap_3d(&ma, a.A, a.strideA ? a.batch : 1, a.rows, a.k1, a.lda, a.strideA, BM)) != OG_OK) return rc;
   if (a.A2) { if ((rc = tc::make_tmap_3d(&ma2, a.A2, a.strideA2 ? a.batch : 1, a.rows, a.k2, a.lda2, a.strideA2, BM)) != OG_OK) return rc; }
   else ma2 = ma;
-  if constexpr (F16) {
-    if ((rc = tc::make_tmap_2d_f16(&mh, Bhi, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d_f16(&ml, Blo, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
-  } else {
-    if ((rc = tc::make_tmap_2d(&mh, Bhi, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
-    if ((rc = tc::make_tmap_2d(&ml, Blo, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
-  }
+  if ((rc = tc::make_tmap_2d(&mh, Bhi, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
+  if ((rc = tc::make_tmap_2d(&ml, Blo, (uint64_t)b_total_rows, (uint64_t)K, (uint64_t)ldb, BN)) != OG_OK) return rc;
   OutMaps om;
   memset(&om, 0, sizeof(om));
   if constexpr (F16) {
@@ -503,18 +496,18 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
     // stored by the threads.
     const int ocols = a.nkinds > 1 ? a.kind_cols : a.nout;
     const auto ok16 = [&](const void* p, int64_t ld, int64_t stride, int64_t inner, int esz) {
-      return al16(p) && ld * esz % 16 == 0 && (a.batch == 1 || stride * esz % 16 == 0) && inner * esz % 16 == 0;
+      return aligned16(p) && ld * esz % 16 == 0 && (a.batch == 1 || stride * esz % 16 == 0) && inner * esz % 16 == 0;
     };
     om.tma = (!a.Y || ok16(a.Y, a.ldy, a.strideY, ocols, 4)) &&
              (!a.Yh || (ok16(a.Yh, a.ldy, a.strideY, ocols, 2) && ok16(a.Yl, a.ldy, a.strideY, ocols, 2))) &&
              (!a.Yth || (ok16(a.Yth, a.ldyt, a.strideYt, a.rows, 2) && ok16(a.Ytl, a.ldyt, a.strideYt, a.rows, 2)));
     if (om.tma && a.Y) om.tma = tc::make_tmap_3d(&om.y, a.Y, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
     if (om.tma && a.Yh)
-      om.tma = tc::make_tmap_3d_f16(&om.hi, a.Yh, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK &&
-               tc::make_tmap_3d_f16(&om.lo, a.Yl, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
+      om.tma = tc::make_tmap_3d(&om.hi, a.Yh, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK &&
+               tc::make_tmap_3d(&om.lo, a.Yl, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
     if (om.tma && a.Yth)
-      om.tma = tc::make_tmap_3d_f16(&om.thi, a.Yth, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK &&
-               tc::make_tmap_3d_f16(&om.tlo, a.Ytl, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK;
+      om.tma = tc::make_tmap_3d(&om.thi, a.Yth, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK &&
+               tc::make_tmap_3d(&om.tlo, a.Ytl, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK;
   }
   if ((rc = smem_opt_in<linear_sm90_kernel<Args>>(C::SMEM_BYTES, true)) != OG_OK) return rc;
   const int tiles = cdiv(a.nout, BN) * cdiv(a.rows, BM) * a.batch;
@@ -532,14 +525,14 @@ template int linear_sm90_launch(const F16LinearArgs&, const __half*, const __hal
 // (a K block comes from one of the two tensors).
 inline bool linear_sm90_eligible(const TcLinearArgs& a, const float* Bhi, const float* Blo, int64_t ldb) {
   const int K = a.k1 + a.k2;
-  return K >= 32 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && al16(a.A) &&
-         (!a.A2 || (a.k1 % 32 == 0 && a.lda2 % 4 == 0 && a.strideA2 % 4 == 0 && al16(a.A2))) && ldb % 4 == 0 && al16(Bhi) && al16(Blo);
+  return K >= 32 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && aligned16(a.A) &&
+         (!a.A2 || (a.k1 % 32 == 0 && a.lda2 % 4 == 0 && a.strideA2 % 4 == 0 && aligned16(a.A2))) && ldb % 4 == 0 && aligned16(Bhi) && aligned16(Blo);
 }
 
 inline bool linear_sm90_eligible(const F16LinearArgs& a, const __half* Bh, const __half* Bl, int64_t ldb) {
   const int K = a.k1 + a.k2;
-  if (!(K >= 64 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && al16(a.A) && ldb % 8 == 0 && al16(Bh) && al16(Bl))) return false;
-  if (a.A2 && (a.k1 % 32 != 0 || a.lda2 % 4 != 0 || a.strideA2 % 4 != 0 || !al16(a.A2))) return false;
+  if (!(K >= 64 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && aligned16(a.A) && ldb % 8 == 0 && aligned16(Bh) && aligned16(Bl))) return false;
+  if (a.A2 && (a.k1 % 32 != 0 || a.lda2 % 4 != 0 || a.strideA2 % 4 != 0 || !aligned16(a.A2))) return false;
   if (!a.w_meta || !(a.amax_in[0] || a.amax_in[1] || a.amax_in[2])) return false;
   const int kinds = (a.Y ? 1 : 0) + (a.Yh ? 1 : 0) + (a.Yth ? 1 : 0);
   if (a.nkinds > 1) {                                       // stacked projections: kinds kind0 .. kind0 + nkinds - 1, one output each
@@ -547,8 +540,8 @@ inline bool linear_sm90_eligible(const F16LinearArgs& a, const __half* Bh, const
     if ((a.kind0 == 0) != (a.Y != nullptr) || !a.Yh || (a.kind0 + a.nkinds == 3) != (a.Yth != nullptr) || a.R || a.relu) return false;
     if (a.Yth && !a.scale_out_v) return false;
   } else if (kinds != 1) return false;
-  if (a.Y && !(a.ldy % 2 == 0 && a.strideY % 2 == 0 && al16(a.Y))) return false;
-  if (a.Yh && !(a.Yl && a.ldy % 2 == 0 && a.strideY % 2 == 0 && al16(a.Yh) && al16(a.Yl) && !a.R && a.scale_out)) return false;
+  if (a.Y && !(a.ldy % 2 == 0 && a.strideY % 2 == 0 && aligned16(a.Y))) return false;
+  if (a.Yh && !(a.Yl && a.ldy % 2 == 0 && a.strideY % 2 == 0 && aligned16(a.Yh) && aligned16(a.Yl) && !a.R && a.scale_out)) return false;
   if (a.Yth && !(a.Ytl && !a.R && (a.scale_out || a.scale_out_v))) return false;
   return true;
 }

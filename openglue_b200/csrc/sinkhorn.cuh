@@ -440,7 +440,7 @@ inline int sinkhorn_plan(bool backward, int B, int n, int m, SinkPlan* p) {
 }
 
 inline int sinkhorn_check_rows(const char* who, const float* S, int64_t lds, int64_t strideS, int m) {
-  if (lds % 4 != 0 || lds < m || (reinterpret_cast<uintptr_t>(S) & 15) || strideS % 4 != 0)
+  if (lds % 4 != 0 || lds < m || !aligned16(S) || strideS % 4 != 0)
     return fail(OG_EINVAL, "%s: S rows must be 16-byte aligned (lds %% 4 == 0, lds >= m)", who);
   return OG_OK;
 }

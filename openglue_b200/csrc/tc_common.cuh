@@ -6,6 +6,7 @@
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <type_traits>
 
 namespace og {
 namespace tc {
@@ -249,71 +250,38 @@ inline PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// 2-D fp32 row-major tensor [rows, cols] with row stride ld (floats); box = 32 floats x box_rows, 128B swizzle.
-inline int make_tmap_2d(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  PFN_encodeTiled fn = get_encode_fn();
-  if (!fn) return fail(OG_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * sizeof(float)};
-  cuuint32_t box[2] = {32, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu", (int)r,
-                                     (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld);
-  return OG_OK;
-}
-
-// 3-D fp32 tensor [batch, rows, cols] (row stride ld, batch stride bstride, in floats); box = 32 cols x box_rows x 1.
-inline int make_tmap_3d(CUtensorMap* map, const float* base, uint64_t batch, uint64_t rows, uint64_t cols, uint64_t ld,
-                        uint64_t bstride, uint32_t box_rows) {
+// Tensor map of a T tensor (float or __half) [batch, rows, cols] with row stride ld and batch stride bstride (in elements),
+// in boxes of one 128-byte row (32 fp32 or 64 fp16 elements) x box_rows x 1, 128-byte swizzle; box parts outside the tensor load
+// as zeros and are not stored.  rank 2 describes [rows, cols] alone; rank 3 with batch <= 1 or bstride == 0 has one batch item.
+template <class T>
+inline int make_tmap(CUtensorMap* map, int rank, const T* base, uint64_t batch, uint64_t rows, uint64_t cols, uint64_t ld,
+                     uint64_t bstride, uint32_t box_rows) {
+  static_assert(std::is_same<T, float>::value || std::is_same<T, __half>::value, "fp32 or fp16 tensor");
+  constexpr bool F32 = std::is_same<T, float>::value;
   PFN_encodeTiled fn = get_encode_fn();
   if (!fn) return fail(OG_ECUDA, "cuTensorMapEncodeTiled entry point not available");
   if (batch <= 1 || bstride == 0) { batch = 1; bstride = rows * ld; }
   cuuint64_t dims[3] = {cols, rows, batch};
-  cuuint64_t strides[2] = {ld * sizeof(float), bstride * sizeof(float)};
-  cuuint32_t box[3] = {32, box_rows, 1};
+  cuuint64_t strides[2] = {ld * sizeof(T), bstride * sizeof(T)};
+  cuuint32_t box[3] = {128 / sizeof(T), box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  CUresult r = fn(map, F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<T*>(base), dims,
+                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled (3d) failed (%d)", (int)r);
+  if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled (%dd %s) failed (%d): rows=%llu cols=%llu ld=%llu", rank,
+                                     F32 ? "fp32" : "fp16", (int)r, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld);
   return OG_OK;
 }
-
-// fp16 row-major tensor [rows, cols] with row stride ld (ELEMENTS); box = 64 halves (128 bytes) x box_rows, 128B swizzle.
-inline int make_tmap_2d_f16(CUtensorMap* map, const __half* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  PFN_encodeTiled fn = get_encode_fn();
-  if (!fn) return fail(OG_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * sizeof(__half)};
-  cuuint32_t box[2] = {64, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled (f16) failed (%d): rows=%llu cols=%llu ld=%llu", (int)r,
-                                     (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld);
-  return OG_OK;
+// [rows, cols], loaded with tma_load_2d
+template <class T>
+inline int make_tmap_2d(CUtensorMap* map, const T* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
+  return make_tmap(map, 2, base, 1, rows, cols, ld, 0, box_rows);
 }
-
-// 3-D fp16 tensor [batch, rows, cols] (row stride ld, batch stride bstride, in elements); box = 64 halves (128 bytes) x box_rows x 1,
-// 128B swizzle.
-inline int make_tmap_3d_f16(CUtensorMap* map, const __half* base, uint64_t batch, uint64_t rows, uint64_t cols, uint64_t ld,
-                            uint64_t bstride, uint32_t box_rows) {
-  PFN_encodeTiled fn = get_encode_fn();
-  if (!fn) return fail(OG_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-  if (batch <= 1 || bstride == 0) { batch = 1; bstride = rows * ld; }
-  cuuint64_t dims[3] = {cols, rows, batch};
-  cuuint64_t strides[2] = {ld * sizeof(__half), bstride * sizeof(__half)};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(OG_ECUDA, "cuTensorMapEncodeTiled (3d f16) failed (%d)", (int)r);
-  return OG_OK;
+// [batch, rows, cols], loaded with tma_load_3d or stored with tma_store_3d
+template <class T>
+inline int make_tmap_3d(CUtensorMap* map, const T* base, uint64_t batch, uint64_t rows, uint64_t cols, uint64_t ld, uint64_t bstride,
+                        uint32_t box_rows) {
+  return make_tmap(map, 3, base, batch, rows, cols, ld, bstride, box_rows);
 }
 
 }  // namespace tc
