@@ -219,7 +219,7 @@ int og_attention_tc_fwd(const float* q, int64_t ldq, int64_t strideq,
  *   og_amax: slot = max |x|.
  *   og_linear_f16_fwd: args as og_linear_fwd (W, rscale, Yt ignored / must be NULL); exactly ONE output kind:
  *       args->Y (fp32, + optional R residual, amax_out) | Yh,Yl (fp16 [rows, nout], ldy) | Yth,Ytl (fp16 [nout, rows], ldyt);
- *       fp16 outputs are written with *scale_out (derived from a bound: a_amax * meta[1] + meta[2]).
+ *       fp16 outputs are written with *scale_out (derived from a bound: |alpha| * a_amax * meta[1] + meta[2]).
  *   og_attention_f16_fwd: q fp32 with its amax; khi/klo fp16 [batch*nk, ldk] with k_scale; vthi/vtlo fp16 [batch*d, ldvt]
  *       with v_scale; head_dim 64.  swap_halves is a layout probe and must be 0.                                      */
 int og_weight_split_f16(const float* w, const float* bias, int rows, int cols, void* hi16, void* lo16, float* meta, void* stream);

@@ -209,12 +209,12 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
       if (a.nkinds > 1) {
         for (int kk = 0; kk < a.nkinds; ++kk) {
           const float* w2 = a.w_meta + 4 * kk;
-          const float so = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(w2 + 1), __ldg(w2 + 2)));
+          const float so = f16_out_scale_for(a.alpha, amax_a, __ldg(w2 + 1), __ldg(w2 + 2));
           if (a.kind0 + kk == 1 && a.scale_out) *a.scale_out = so;
           if (a.kind0 + kk == 2 && a.scale_out_v) *a.scale_out_v = so;
         }
       } else if (!a.Y && a.scale_out) {
-        *a.scale_out = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(a.w_meta + 1), __ldg(a.w_meta + 2)));
+        *a.scale_out = f16_out_scale_for(a.alpha, amax_a, __ldg(a.w_meta + 1), __ldg(a.w_meta + 2));
       }
     }
   }
@@ -313,7 +313,7 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
         wm = a.w_meta + 4 * kidx;
         alpha_t = a.alpha / (s_a * __ldg(wm));
       }
-      if (okind != 1) sos = f16_scale_for(fabsf(a.alpha) * fmaf(amax_a, __ldg(wm + 1), __ldg(wm + 2)));
+      if (okind != 1) sos = f16_out_scale_for(a.alpha, amax_a, __ldg(wm + 1), __ldg(wm + 2));
       float tmax = 0.f;
       uint8_t* stg = smem + S * C::STAGE + c * C::STAGING;   // two boxes of 64 rows x 128 bytes
       const int rl = warp * 16 + g;                          // rows r0 / r0 + 8 within the consumer's 64

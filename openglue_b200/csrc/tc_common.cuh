@@ -224,6 +224,11 @@ __host__ __device__ __forceinline__ float f16_scale_for(float bound) {
   float r; memcpy(&r, &sb, 4); return r;
 #endif
 }
+// scale of a GEMM's fp16 output y = alpha (A . W_n) + b_n, written before its maximum is known: from the bound
+// |y| <= |alpha| amax(A) max_n ||W_n||_1 + max |b| (the bias is added after alpha, so it is not scaled by it)
+__host__ __device__ __forceinline__ float f16_out_scale_for(float alpha, float a_amax, float w_l1, float b_max) {
+  return f16_scale_for(fmaf(fabsf(alpha) * a_amax, w_l1, b_max));
+}
 // two already-scaled values -> packed hi halves and packed lo halves (element 0 in the low 16 bits)
 __device__ __forceinline__ void split_f16x2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const __half2 h = __floats2half2_rn(x0, x1);
