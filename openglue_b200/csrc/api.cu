@@ -134,7 +134,7 @@ static og_linear_args lin(const float* A, int64_t lda, int k, const float* W, co
 }
 
 // The fields of the tensor-core GEMM arguments (TcLinearArgs or F16LinearArgs) that come from og_linear_args; the split and
-// fp16 outputs and the fp16 operand scales are the caller's.  The fp16 form has no rscale or fp32 transposed output.
+// fp16 outputs and the fp16 operand scales are the caller's.  The fp16 form has no rscale or fp32 transposed output (a.Y: run F16_Y).
 template <class T> static T gemm_args(const og_linear_args& a) {
   T t;
   memset(&t, 0, sizeof(t));
@@ -143,8 +143,11 @@ template <class T> static T gemm_args(const og_linear_args& a) {
   t.b_rows_per_batch = a.strideW ? (int)(a.strideW / a.ldw) : 0;
   t.bias = a.bias; t.rows = a.rows; t.nout = a.nout; t.batch = a.batch; t.alpha = a.alpha; t.relu = a.relu;
   t.R = a.R; t.ldr = a.ldr; t.strideR = a.strideR;
-  t.Y = a.Y; t.ldy = a.ldy; t.strideY = a.strideY; t.ldyt = a.ldyt; t.strideYt = a.strideYt;
-  if constexpr (std::is_same<T, TcLinearArgs>::value) { t.rscale = a.rscale; t.Yt = a.Yt; }
+  if constexpr (std::is_same<T, TcLinearArgs>::value) {
+    t.Y = a.Y; t.ldy = a.ldy; t.strideY = a.strideY; t.Yt = a.Yt; t.ldyt = a.ldyt; t.strideYt = a.strideYt; t.rscale = a.rscale;
+  } else {
+    t.out[F16_Y] = {a.Y, nullptr, nullptr, a.ldy, a.strideY, nullptr}; t.kind0 = F16_Y; t.nkinds = 1; t.kind_cols = a.nout;
+  }
   return t;
 }
 
@@ -719,7 +722,7 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
     return linear_sm90_run(a, g, W16h + woff, W16l + woff, "forward", "a layer is not tileable by the fp16 GEMM", st);
   };
   // F16 with d % 128 == 0 (every shipped config): the projections that share their input run as ONE launch over the stacked
-  // weights (F16LinearArgs::nkinds): Q | K | V in a self layer (same keypoints), K | V in a cross layer (+ Q on its own).
+  // weights (one run of kinds): Q | K | V in a self layer (same keypoints), K | V in a cross layer (+ Q on its own).
   const bool fuse_qkv = fuse_qkv_mode() && d % tcf::BN == 0;
 
   // Q of the rows q, K and V of the rows kv (q itself in a self layer)
@@ -739,11 +742,11 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
       return (r = part(q, 0, d)) != OG_OK ? r : part(kv, d, 2 * d);
     }
     const int64_t ldv = vt_ld(kv), voff = vt_off(kv);
-    og_linear_args aq = lin(xq, d, d, Wp + wq, Wp + bq, q.rows(), d, w.q + (int64_t)q.row0 * d, d);
-    og_linear_args ak = lin(xkv, d, d, Wp + wq + dd, Wp + bq + d, kv.rows(), d, nullptr, d);
-    og_linear_args av = lin(xkv, d, d, Wp + wq + 2 * dd, Wp + bq + 2 * d, kv.len, d, nullptr, d);   // V^T batched per sequence
-    av.batch = kv.count; av.strideA = (int64_t)kv.len * d; av.ldyt = ldv; av.strideYt = (int64_t)d * ldv;
     if (att == Att::TF32) {
+      og_linear_args aq = lin(xq, d, d, Wp + wq, Wp + bq, q.rows(), d, w.q + (int64_t)q.row0 * d, d);
+      og_linear_args ak = lin(xkv, d, d, Wp + wq + dd, Wp + bq + d, kv.rows(), d, nullptr, d);
+      og_linear_args av = lin(xkv, d, d, Wp + wq + 2 * dd, Wp + bq + 2 * d, kv.len, d, nullptr, d);   // V^T batched per sequence
+      av.batch = kv.count; av.strideA = (int64_t)kv.len * d; av.ldyt = ldv; av.strideYt = (int64_t)d * ldv;
       SplitOut sk, sv;
       sk.Yhi = w.khi + (int64_t)kv.row0 * d; sk.Ylo = w.klo + (int64_t)kv.row0 * d;
       sv.Ythi = w.vthi + voff; sv.Ytlo = w.vtlo + voff;
@@ -753,28 +756,27 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
     }
     SeqSlots& s = ss[q.img == 1];
     s = {new_slot(), new_slot(), new_slot(), new_slot()};
-    if (!(fuse_qkv && self)) {
-      F16LinearArgs gq = args16(aq, xslot(q, 0), xslot(q, 1), nullptr, l, 0);
-      gq.amax_out = s.q;
-      if ((r = run16(aq, gq, wq)) != OG_OK) return r;
-    }
-    if (fuse_qkv) {
-      const int k0 = self ? 0 : 1, nk = 3 - k0;
-      og_linear_args a = lin(xkv, d, d, Wp + wq + k0 * dd, Wp + bq + k0 * d, kv.len, nk * d, k0 == 0 ? w.q + (int64_t)kv.row0 * d : nullptr, d);
-      a.batch = kv.count; a.strideA = a.strideY = (int64_t)kv.len * d; a.ldyt = ldv; a.strideYt = (int64_t)d * ldv;
-      F16LinearArgs g = args16(a, xslot(kv, 0), xslot(kv, 1), nullptr, l, k0);
-      g.nkinds = nk; g.kind0 = k0; g.kind_cols = d;
-      if (k0 == 0) g.amax_out = s.q;
-      g.Yh = kh16 + (int64_t)kv.row0 * d; g.Yl = kl16 + (int64_t)kv.row0 * d; g.scale_out = s.k;
-      g.Yth = vth16 + voff; g.Ytl = vtl16 + voff; g.scale_out_v = s.v;
-      return run16(a, g, wq + k0 * dd);
-    }
-    F16LinearArgs gk = args16(ak, xslot(kv, 0), xslot(kv, 1), nullptr, l, 1);
-    gk.Yh = kh16 + (int64_t)kv.row0 * d; gk.Yl = kl16 + (int64_t)kv.row0 * d; gk.scale_out = s.k;
-    if ((r = run16(ak, gk, wq + dd)) != OG_OK) return r;
-    F16LinearArgs gv = args16(av, xslot(kv, 0), xslot(kv, 1), nullptr, l, 2);
-    gv.Yth = vth16 + voff; gv.Ytl = vtl16 + voff; gv.scale_out = s.v;
-    return run16(av, gv, wq + 2 * dd);
+    // Q of the rows q, K and V^T of the rows kv, each with its batch stride per sequence
+    const F16Out out[F16_KINDS] = {
+        {w.q + (int64_t)q.row0 * d, nullptr, nullptr, d, (int64_t)q.len * d, nullptr},
+        {nullptr, kh16 + (int64_t)kv.row0 * d, kl16 + (int64_t)kv.row0 * d, d, (int64_t)kv.len * d, s.k},
+        {nullptr, vth16 + voff, vtl16 + voff, ldv, (int64_t)d * ldv, s.v}};
+    // The kinds k0 .. k0 + nk - 1 of the rows g in one launch over their stacked weights.  A run that writes V^T is batched per
+    // sequence, as V^T's layout is; Q or K alone is one batch item of all rows of g.
+    auto run = [&](const Seqs& g, int k0, int nk) {
+      const bool per_seq = k0 + nk == F16_KINDS;
+      og_linear_args a = lin(w.x + (int64_t)g.row0 * d, d, d, Wp + wq + k0 * dd, Wp + bq + k0 * d, per_seq ? g.len : g.rows(), nk * d, nullptr, d);
+      if (per_seq) { a.batch = g.count; a.strideA = (int64_t)g.len * d; }
+      F16LinearArgs ga = args16(a, xslot(g, 0), xslot(g, 1), nullptr, l, k0);
+      std::copy(out, out + F16_KINDS, ga.out);
+      ga.kind0 = k0; ga.nkinds = nk; ga.kind_cols = d; ga.amax_out = s.q;
+      return run16(a, ga, wq + k0 * dd);
+    };
+    if (fuse_qkv && self) return run(q, F16_Y, 3);
+    if (fuse_qkv) return (r = run(q, F16_Y, 1)) != OG_OK ? r : run(kv, F16_K, 2);
+    for (int k = F16_Y; k < F16_KINDS; ++k)
+      if ((r = run(k == F16_Y ? q : kv, k, 1)) != OG_OK) return r;
+    return OG_OK;
   };
 
   // o[q] = attention of the queries q over the keys / values kv
@@ -949,9 +951,11 @@ int og_linear_f16_fwd(const og_linear_args* a, const void* Wh16, const void* Wl1
   OG_CHECK_ARG(a->rows > 0 && a->nout > 0 && a->batch > 0 && a->k1 > 0 && a->k2 >= 0, "linear_f16: bad sizes");
   OG_CHECK_ARG(!a->rscale && !a->Yt, "linear_f16: rscale / fp32 transposed outputs are not part of the fp16 form");
   F16LinearArgs g = gemm_args<F16LinearArgs>(*a);
-  g.Yh = static_cast<__half*>(Yh); g.Yl = static_cast<__half*>(Yl);
-  g.Yth = static_cast<__half*>(Yth); g.Ytl = static_cast<__half*>(Ytl);
-  g.amax_in[0] = a_amax; g.w_meta = w_meta; g.amax_out = amax_out; g.scale_out = scale_out; g.swap_halves = swap_halves;
+  g.out[F16_K] = {nullptr, static_cast<__half*>(Yh), static_cast<__half*>(Yl), a->ldy, a->strideY, scale_out};
+  g.out[F16_VT] = {nullptr, static_cast<__half*>(Yth), static_cast<__half*>(Ytl), a->ldyt, a->strideYt, scale_out};
+  g.kind0 = a->Y ? F16_Y : Yh ? F16_K : F16_VT;
+  g.nkinds = (a->Y != nullptr) + (Yh != nullptr) + (Yth != nullptr) == 1;   // no output or several: an empty run, not tileable
+  g.amax_in[0] = a_amax; g.w_meta = w_meta; g.amax_out = amax_out; g.swap_halves = swap_halves;
   return linear_sm90_run(*a, g, static_cast<const __half*>(Wh16), static_cast<const __half*>(Wl16), "linear_f16",
                          "needs K >= 64, 16-byte aligned rows, exactly one output kind (Y | Yh,Yl | Yth,Ytl)", (cudaStream_t)stream);
 }

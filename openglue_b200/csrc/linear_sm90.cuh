@@ -38,10 +38,16 @@ struct TcLinearArgs {
   float* Yt;  float* Ythi; float* Ytlo; int64_t ldyt; int64_t strideYt;    // transposed outputs [nout, rows]
 };
 
-// Output kinds of the fp16 form: 1 = fp32 Y (bias / ReLU / residual, amax tracking), 2 = row-major fp16 hi / lo (K operand of the
-// attention kernel), 3 = transposed fp16 hi / lo (V^T operand).  nkinds > 1: SEVERAL projections of the same A in one launch
-// (Q | K | V or K | V, B = the stacked weights): the kind of a tile follows from its column block (kind0 + n0 / kind_cols), every
-// kind with its own weight scale / norm bound (w_meta + 4 per kind).
+// Output kinds of the fp16 form: F16_Y = fp32 Y [batch, rows, cols] (bias / ReLU / residual, amax tracking; Q in the forward
+// pass), F16_K = row-major fp16 hi / lo [batch, rows, cols] (K operand of the attention kernel), F16_VT = transposed fp16 hi / lo
+// [batch, cols, rows] (V^T operand).  The fp16 kinds' halves are written with a scale that the kernel publishes in their slot.
+enum F16Kind { F16_Y, F16_K, F16_VT, F16_KINDS };
+struct F16Out { float* y; __half *hi, *lo; int64_t ld, stride; float* scale; };   // y: F16_Y; hi, lo, scale: fp16 kinds
+
+// A launch writes the run of kinds kind0 .. kind0 + nkinds - 1 from ONE product of A with B (with nkinds > 1: the stacked
+// weights of several projections of the same A, Q | K | V or K | V).  The i-th kind of the run is output columns
+// [i kind_cols, (i + 1) kind_cols), with its own weight scale / norm bound at w_meta + 4 i; the kind of a tile is
+// kind0 + n0 / kind_cols.  A single output is nkinds = 1 with kind_cols = nout.
 struct F16LinearArgs {
   const float* A;  int64_t lda;  int64_t strideA;
   const float* A2; int64_t lda2; int64_t strideA2;
@@ -51,17 +57,13 @@ struct F16LinearArgs {
   int rows, nout, batch;
   float alpha;
   int relu;
-  const float* R; int64_t ldr; int64_t strideR;          // fp32 residual (kind 1)
-  float* Y; int64_t ldy; int64_t strideY;                // kind 1
-  __half* Yh; __half* Yl;                                // kind 2 (same ldy / strideY, in elements)
-  __half* Yth; __half* Ytl; int64_t ldyt; int64_t strideYt;   // kind 3: [nout, rows] per batch item
+  const float* R; int64_t ldr; int64_t strideR;          // fp32 residual (F16_Y)
+  F16Out out[F16_KINDS];                // indexed by kind; only the run's entries are read
+  int kind0, nkinds, kind_cols;
   const float* amax_in[3];              // device scalars bounding |A| and |A2| (null entries ignored; at least one required)
   const float* w_meta;                  // device {scale of the pre-split B, max_n ||B_n||_1, max |bias|}
   float* amax_out;                      // optional: max |Y| (atomicMax; zeroed by the caller)
-  float* scale_out;                     // kinds 2 / 3: receives the scale the fp16 outputs were written with
   int swap_halves;                      // debug: pack A with element 2c in the HIGH half (probe of the register operand layout)
-  int nkinds, kind0, kind_cols;         // nkinds > 1: output kinds kind0 .. kind0 + nkinds - 1, kind_cols columns each (multiple of 128)
-  float* scale_out_v;                   // nkinds > 1: scale of the transposed (kind 2) output; scale_out is the row-major (kind 1) one
 };
 
 namespace tcf {
@@ -96,12 +98,12 @@ __device__ __forceinline__ const float* sw128_f32(const uint8_t* tile, int r, in
   return reinterpret_cast<const float*>(tile + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4);
 }
 
-// Output tensor maps of the fp16 form, one per output (box: 32 fp32 or 64 fp16 elements x 64 rows x 1, 128-byte swizzle):
-// y = Y [batch, rows, cols], hi / lo = Yh / Yl [batch, rows, cols], thi / tlo = Yth / Ytl [batch, cols, rows] (cols: nout, or
-// kind_cols with nkinds > 1).  tma = 0: the base, a stride or the row length of some output is not a multiple of 16 bytes, and
-// the staged boxes are stored by the consumer's threads (out_copy_box).
+// Output tensor maps of the fp16 form, one per output tensor of the run's kinds (box: 32 fp32 or 64 fp16 elements x 64 rows x 1,
+// 128-byte swizzle; cols = kind_cols): hi[k] stores kind k's Y or hi halves, lo[k - 1] the lo halves of the fp16 kind k.
+// tma = 0: the base, a stride or the row length of some output is not a multiple of 16 bytes, and the staged boxes are stored
+// by the consumer's threads (out_copy_box).
 struct OutMaps {
-  CUtensorMap y, hi, lo, thi, tlo;
+  CUtensorMap hi[F16_KINDS], lo[F16_KINDS - 1];
   int tma;
 };
 
@@ -153,11 +155,9 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
     prefetch_tensormap(&map_a); prefetch_tensormap(&map_a2);
     prefetch_tensormap(&map_bhi); prefetch_tensormap(&map_blo);
     if constexpr (F16) {
-      if (om.tma) {
-        if (a.Y) prefetch_tensormap(&om.y);
-        if (a.Yh) { prefetch_tensormap(&om.hi); prefetch_tensormap(&om.lo); }
-        if (a.Yth) { prefetch_tensormap(&om.thi); prefetch_tensormap(&om.tlo); }
-      }
+#pragma unroll
+      for (int k = 0; k < F16_KINDS; ++k)                   // the run's maps
+        if (om.tma && k >= a.kind0 && k < a.kind0 + a.nkinds) { prefetch_tensormap(&om.hi[k]); if (k) prefetch_tensormap(&om.lo[k - 1]); }
     }
   }
   __syncthreads();
@@ -205,16 +205,12 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
 #pragma unroll
     for (int i = 0; i < 3; ++i) if (a.amax_in[i]) amax_a = fmaxf(amax_a, __ldcg(a.amax_in[i]));
     s_a = f16_scale_for(amax_a);
-    if (blockIdx.x == 0 && threadIdx.x == 128) {             // one thread of the grid publishes the output scales
-      if (a.nkinds > 1) {
-        for (int kk = 0; kk < a.nkinds; ++kk) {
-          const float* w2 = a.w_meta + 4 * kk;
-          const float so = f16_out_scale_for(a.alpha, amax_a, __ldg(w2 + 1), __ldg(w2 + 2));
-          if (a.kind0 + kk == 1 && a.scale_out) *a.scale_out = so;
-          if (a.kind0 + kk == 2 && a.scale_out_v) *a.scale_out_v = so;
-        }
-      } else if (!a.Y && a.scale_out) {
-        *a.scale_out = f16_out_scale_for(a.alpha, amax_a, __ldg(a.w_meta + 1), __ldg(a.w_meta + 2));
+    if (blockIdx.x == 0 && threadIdx.x == 128) {             // one thread of the grid publishes the fp16 kinds' output scales
+#pragma unroll
+      for (int k = F16_K; k < F16_KINDS; ++k) {
+        if (k < a.kind0 || k >= a.kind0 + a.nkinds) continue;
+        const float* wm = a.w_meta + 4 * (k - a.kind0);
+        *a.out[k].scale = f16_out_scale_for(a.alpha, amax_a, __ldg(wm + 1), __ldg(wm + 2));
       }
     }
   }
@@ -304,29 +300,26 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
     // to the next tile's MMAs while the copy engine writes the tile; before it writes the buffer again, it waits for the reads of
     // the previous stores.
     if constexpr (F16) {
-      const float s_w = __ldg(a.w_meta);
-      int okind = a.Y ? 1 : (a.Yh ? 2 : 3), kidx = 0, ocols = a.nout;
-      float alpha_t = a.alpha / (s_a * s_w), sos = 1.f;
-      const float* wm = a.w_meta;
-      if (a.nkinds > 1) {
-        kidx = n0 / a.kind_cols; okind = a.kind0 + kidx + 1; ocols = a.kind_cols;
-        wm = a.w_meta + 4 * kidx;
-        alpha_t = a.alpha / (s_a * __ldg(wm));
-      }
-      if (okind != 1) sos = f16_out_scale_for(a.alpha, amax_a, __ldg(wm + 1), __ldg(wm + 2));
+      // the tile's place in the run (n0 / kind_cols without a division: n0 < nout <= 3 kind_cols), and its kind
+      const int kidx = (n0 >= a.kind_cols) + (n0 >= 2 * a.kind_cols), kind = a.kind0 + kidx;
+      const float* wm = a.w_meta + 4 * kidx;
+      const float alpha_t = a.alpha / (s_a * __ldg(wm));
+      const float sos = kind != F16_Y ? f16_out_scale_for(a.alpha, amax_a, __ldg(wm + 1), __ldg(wm + 2)) : 1.f;
       float tmax = 0.f;
       uint8_t* stg = smem + S * C::STAGE + c * C::STAGING;   // two boxes of 64 rows x 128 bytes
       const int rl = warp * 16 + g;                          // rows r0 / r0 + 8 within the consumer's 64
-      const int orow = m0 + 64 * c, bzy = a.strideY ? bz : 0, bzt = a.strideYt ? bz : 0;
+      // the outputs by constant indices: a run-time index into the parameters would copy them to local memory
+      const F16Out &oy = a.out[F16_Y], &ok = a.out[F16_K], &ovt = a.out[F16_VT];
+      const int orow = m0 + 64 * c, bzy = oy.stride ? bz : 0, bzk = ok.stride ? bz : 0, bzt = ovt.stride ? bz : 0, cols = a.kind_cols;
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
-        const int oc = n0 - kidx * ocols + 64 * hf;          // first column of this half in its output
+        const int oc = n0 - kidx * cols + 64 * hf;           // first column of this half in its output
         // the half's values are computed in registers first, so that the wait for the previous stores' reads overlaps them
         auto buffer_free = [&] {
           if (tid == 0) bulk_wait_read<0>();
           named_bar_sync(EPI + c, 128);
         };
-        if (okind == 1) {
+        if (kind == F16_Y) {
           float2 yv[2][8];
           // Every load of the half is issued before its first store: the compiler may not move a load across a store to a
           // pointer that could alias it, and loads interleaved with the stores expose one memory latency per 8-column block.
@@ -394,7 +387,7 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
           for (int q = 0; q < 4; ++q) {
             const uint32_t rh[4] = {hv[0][2 * q], hv[1][2 * q], hv[0][2 * q + 1], hv[1][2 * q + 1]};
             const uint32_t rlo[4] = {lv[0][2 * q], lv[1][2 * q], lv[0][2 * q + 1], lv[1][2 * q + 1]};
-            if (okind == 2) {                                  // row: keypoint; 16-byte chunk: 8 columns
+            if (kind == F16_K) {                               // row: keypoint; 16-byte chunk: 8 columns
               const uint32_t ad = stg_u + sw128_chunk(warp * 16 + 8 * (m & 1) + k, 2 * q + (m >> 1));
               stmatrix_x4(ad, rh); stmatrix_x4(ad + 8192, rlo);
             } else {                                           // V^T, row: column (channel); 16-byte chunk: 8 keypoints
@@ -407,23 +400,23 @@ __global__ void __launch_bounds__(tcf::THREADS, 1) linear_sm90_kernel(const __gr
         named_bar_sync(EPI + c, 128);
         if (om.tma) {
           if (tid == 0) {
-            if (okind == 1) { tma_store_3d(&om.y, stg, oc, orow, bzy); tma_store_3d(&om.y, stg + 8192, oc + 32, orow, bzy); }
-            else if (okind == 2) { tma_store_3d(&om.hi, stg, oc, orow, bzy); tma_store_3d(&om.lo, stg + 8192, oc, orow, bzy); }
-            else { tma_store_3d(&om.thi, stg, orow, oc, bzt); tma_store_3d(&om.tlo, stg + 8192, orow, oc, bzt); }
+            if (kind == F16_Y) { tma_store_3d(&om.hi[F16_Y], stg, oc, orow, bzy); tma_store_3d(&om.hi[F16_Y], stg + 8192, oc + 32, orow, bzy); }
+            else if (kind == F16_K) { tma_store_3d(&om.hi[F16_K], stg, oc, orow, bzk); tma_store_3d(&om.lo[0], stg + 8192, oc, orow, bzk); }
+            else { tma_store_3d(&om.hi[F16_VT], stg, orow, oc, bzt); tma_store_3d(&om.lo[1], stg + 8192, orow, oc, bzt); }
             bulk_commit();
           }
-        } else if (okind == 1) {
-          out_copy_box(stg, a.Y, a.ldy, a.strideY, bz, oc, orow, ocols, a.rows, tid);
-          out_copy_box(stg + 8192, a.Y, a.ldy, a.strideY, bz, oc + 32, orow, ocols, a.rows, tid);
-        } else if (okind == 2) {
-          out_copy_box(stg, a.Yh, a.ldy, a.strideY, bz, oc, orow, ocols, a.rows, tid);
-          out_copy_box(stg + 8192, a.Yl, a.ldy, a.strideY, bz, oc, orow, ocols, a.rows, tid);
+        } else if (kind == F16_Y) {
+          out_copy_box(stg, oy.y, oy.ld, oy.stride, bz, oc, orow, cols, a.rows, tid);
+          out_copy_box(stg + 8192, oy.y, oy.ld, oy.stride, bz, oc + 32, orow, cols, a.rows, tid);
+        } else if (kind == F16_K) {
+          out_copy_box(stg, ok.hi, ok.ld, ok.stride, bz, oc, orow, cols, a.rows, tid);
+          out_copy_box(stg + 8192, ok.lo, ok.ld, ok.stride, bz, oc, orow, cols, a.rows, tid);
         } else {
-          out_copy_box(stg, a.Yth, a.ldyt, a.strideYt, bz, orow, oc, a.rows, ocols, tid);
-          out_copy_box(stg + 8192, a.Ytl, a.ldyt, a.strideYt, bz, orow, oc, a.rows, ocols, tid);
+          out_copy_box(stg, ovt.hi, ovt.ld, ovt.stride, bz, orow, oc, a.rows, cols, tid);
+          out_copy_box(stg + 8192, ovt.lo, ovt.ld, ovt.stride, bz, orow, oc, a.rows, cols, tid);
         }
       }
-      if (okind == 1 && a.amax_out) {
+      if (kind == F16_Y && a.amax_out) {
         tmax = warp_max(tmax);
         if (lane == 0 && tmax > 0.f) atomic_amax(a.amax_out, tmax);
       }
@@ -494,20 +487,17 @@ inline int linear_sm90_launch(const Args& a, const BT* Bhi, const BT* Blo, int64
     // TMA stores need 16-byte aligned outputs with strides in multiples of 16 bytes, and they clip a box at the end of a row only
     // to a multiple of 16 bytes (measured on H100: a row of 334 fp32 had two more elements written).  Any other layout is
     // stored by the threads.
-    const int ocols = a.nkinds > 1 ? a.kind_cols : a.nout;
-    const auto ok16 = [&](const void* p, int64_t ld, int64_t stride, int64_t inner, int esz) {
-      return aligned16(p) && ld * esz % 16 == 0 && (a.batch == 1 || stride * esz % 16 == 0) && inner * esz % 16 == 0;
-    };
-    om.tma = (!a.Y || ok16(a.Y, a.ldy, a.strideY, ocols, 4)) &&
-             (!a.Yh || (ok16(a.Yh, a.ldy, a.strideY, ocols, 2) && ok16(a.Yl, a.ldy, a.strideY, ocols, 2))) &&
-             (!a.Yth || (ok16(a.Yth, a.ldyt, a.strideYt, a.rows, 2) && ok16(a.Ytl, a.ldyt, a.strideYt, a.rows, 2)));
-    if (om.tma && a.Y) om.tma = tc::make_tmap_3d(&om.y, a.Y, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
-    if (om.tma && a.Yh)
-      om.tma = tc::make_tmap_3d(&om.hi, a.Yh, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK &&
-               tc::make_tmap_3d(&om.lo, a.Yl, a.batch, a.rows, ocols, a.ldy, a.strideY, 64) == OG_OK;
-    if (om.tma && a.Yth)
-      om.tma = tc::make_tmap_3d(&om.thi, a.Yth, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK &&
-               tc::make_tmap_3d(&om.tlo, a.Ytl, a.batch, ocols, a.rows, a.ldyt, a.strideYt, 64) == OG_OK;
+    om.tma = 1;
+    for (int k = a.kind0; k < a.kind0 + a.nkinds && om.tma; ++k) {
+      const F16Out& o = a.out[k];
+      const int rows = k == F16_VT ? a.kind_cols : a.rows, cols = k == F16_VT ? a.rows : a.kind_cols;
+      const auto map = [&](CUtensorMap* m, const auto* p) {
+        const int64_t esz = sizeof(*p);
+        return aligned16(p) && o.ld * esz % 16 == 0 && (a.batch == 1 || o.stride * esz % 16 == 0) && cols * esz % 16 == 0 &&
+               tc::make_tmap_3d(m, p, a.batch, rows, cols, o.ld, o.stride, 64) == OG_OK;
+      };
+      om.tma = k == F16_Y ? map(&om.hi[k], o.y) : map(&om.hi[k], o.hi) && map(&om.lo[k - 1], o.lo);
+    }
   }
   if ((rc = smem_opt_in<linear_sm90_kernel<Args>>(C::SMEM_BYTES, true)) != OG_OK) return rc;
   const int tiles = cdiv(a.nout, BN) * cdiv(a.rows, BM) * a.batch;
@@ -534,15 +524,15 @@ inline bool linear_sm90_eligible(const F16LinearArgs& a, const __half* Bh, const
   if (!(K >= 64 && a.k1 % 4 == 0 && a.k2 % 4 == 0 && a.lda % 4 == 0 && a.strideA % 4 == 0 && aligned16(a.A) && ldb % 8 == 0 && aligned16(Bh) && aligned16(Bl))) return false;
   if (a.A2 && (a.k1 % 32 != 0 || a.lda2 % 4 != 0 || a.strideA2 % 4 != 0 || !aligned16(a.A2))) return false;
   if (!a.w_meta || !(a.amax_in[0] || a.amax_in[1] || a.amax_in[2])) return false;
-  const int kinds = (a.Y ? 1 : 0) + (a.Yh ? 1 : 0) + (a.Yth ? 1 : 0);
-  if (a.nkinds > 1) {                                       // stacked projections: kinds kind0 .. kind0 + nkinds - 1, one output each
-    if (a.kind0 < 0 || a.kind0 + a.nkinds > 3 || kinds != a.nkinds || a.kind_cols % tcf::BN != 0 || a.nout != a.nkinds * a.kind_cols) return false;
-    if ((a.kind0 == 0) != (a.Y != nullptr) || !a.Yh || (a.kind0 + a.nkinds == 3) != (a.Yth != nullptr) || a.R || a.relu) return false;
-    if (a.Yth && !a.scale_out_v) return false;
-  } else if (kinds != 1) return false;
-  if (a.Y && !(a.ldy % 2 == 0 && a.strideY % 2 == 0 && aligned16(a.Y))) return false;
-  if (a.Yh && !(a.Yl && a.ldy % 2 == 0 && a.strideY % 2 == 0 && aligned16(a.Yh) && aligned16(a.Yl) && !a.R && a.scale_out)) return false;
-  if (a.Yth && !(a.Ytl && !a.R && (a.scale_out || a.scale_out_v))) return false;
+  if (a.nkinds < 1 || a.kind0 < 0 || a.kind0 + a.nkinds > F16_KINDS || a.nout != a.nkinds * a.kind_cols) return false;
+  if (a.nkinds > 1 && (a.kind_cols % tcf::BN != 0 || a.relu)) return false;
+  if (a.R && (a.kind0 != F16_Y || a.nkinds > 1)) return false;    // the residual belongs to Y
+  for (int k = a.kind0; k < a.kind0 + a.nkinds; ++k) {
+    const F16Out& o = a.out[k];
+    if (k == F16_Y && !(o.y && o.ld % 2 == 0 && o.stride % 2 == 0 && aligned16(o.y))) return false;
+    if (k == F16_K && !(o.hi && o.lo && o.ld % 2 == 0 && o.stride % 2 == 0 && aligned16(o.hi) && aligned16(o.lo))) return false;
+    if (k != F16_Y && !(o.hi && o.lo && o.scale)) return false;
+  }
   return true;
 }
 
