@@ -23,6 +23,21 @@ from .packing import pack_weights
 
 __all__ = ['SuperGlue', 'MatchingCore', 'PendingMatches']
 
+# Counts (re)registrations of parameters, buffers and submodules on any module: ``conv.weight = nn.Parameter(...)`` or
+# ``bn.running_mean = t`` replaces a tensor object, which a cached list of a SuperGlue's tensors would not see.
+_registrations = 0
+
+
+def _count_registration(*_):
+    global _registrations
+    _registrations += 1
+
+
+for _register in (torch.nn.modules.module.register_module_parameter_registration_hook,
+                  torch.nn.modules.module.register_module_buffer_registration_hook,
+                  torch.nn.modules.module.register_module_module_registration_hook):
+    _register(_count_registration)
+
 
 def _feed_forward_params(*sizes: int) -> nn.Sequential:
     """Parameter container with the reference FeedForwardNet's key layout (models/utils.py:48-58):
@@ -134,10 +149,12 @@ class SuperGlue(nn.Module):
     def _weights_version(self):
         """Cheap fingerprint of the 333 parameter / buffer tensors (runs on every forward, ~50 us): in-place updates bump a
         tensor's ``_version`` (monotonic, so the sum changes), moves go through ``_apply`` / ``load_state_dict``, and the
-        storage addresses of ALL tensors catch ``p.data = new`` / ``vector_to_parameters`` / EMA swaps on any of them."""
+        storage addresses of ALL tensors catch ``p.data = new`` / ``vector_to_parameters`` / EMA swaps on any of them.  The
+        tensor list is collected again after any module registers a parameter, buffer or submodule (a replaced tensor)."""
         ts = getattr(self, '_tensors', None)
-        if ts is None:
+        if ts is None or self._tensors_at != _registrations:
             ts = self._tensors = list(self.parameters()) + list(self.buffers())
+            self._tensors_at = _registrations
         ver = ptr = 0
         for i, t in enumerate(ts):
             ver += t._version
@@ -296,7 +313,9 @@ class MatchingCore(nn.Module):
         """Replay (capturing on first use) the CUDA graph for this shape; inputs are copied into its static buffers."""
         shapes = tuple(tuple(data[k].shape) for k in self._TENSOR_KEYS)
         sizes = (SuperGlue._image_wh(data, 0), SuperGlue._image_wh(data, 1))       # plain floats (collated sizes are tensors)
-        key = (shapes, sizes, str(dev), self.superglue._weights_version(), self.match_threshold)
+        # the precision picks the captured kernels and packed-weight forms: a switch in config['precision'] repacks only at the
+        # next run, so the alloc-gen check below cannot see it yet
+        key = (shapes, sizes, str(dev), self.superglue._weights_version(), self.superglue._precision(), self.match_threshold)
         entry = self._graphs.get(key)
         if entry is not None and entry[3] != getattr(self.superglue, '_alloc_gen', 0):
             # the SuperGlue's workspace / packed weights were reallocated since this graph was captured (a bigger call

@@ -76,6 +76,36 @@ def test_unsupported_options_raise():
         model(data)
 
 
+def test_weights_version_sees_every_kind_of_weight_change():
+    """The fingerprint that keys the packed weights and the captured graphs changes with each way a weight can change,
+    including tensors replaced by assignment (a new Parameter, buffer or submodule object), and only then."""
+    cfg = default_config(descriptor_dim=64, num_stages=1, num_iters=5)
+    model = SuperGlue(cfg).eval()
+    model.load_state_dict(synthetic_state_dict(cfg))
+    layer = model.attention_gnn.layers[0].module
+
+    def scale_in_place():
+        with torch.no_grad():
+            model.linear_proj.weight.mul_(1.01)
+
+    changes = [
+        scale_in_place,
+        lambda: model.load_state_dict(synthetic_state_dict(cfg, seed=1)),
+        lambda: setattr(model.dustbin_score, 'data', model.dustbin_score.data + 1),
+        lambda: setattr(model.linear_proj, 'weight', torch.nn.Parameter(model.linear_proj.weight.detach() * 2)),
+        lambda: setattr(layer.fc[2], 'running_mean', layer.fc[2].running_mean + 1),
+        lambda: setattr(layer.mha, 'in_proj_q', torch.nn.Conv1d(64, 64, kernel_size=1)),
+    ]
+    seen = [model._weights_version()]
+    assert model._weights_version() == seen[0]
+    for change in changes:
+        change()
+        v = model._weights_version()
+        assert v not in seen
+        assert model._weights_version() == v
+        seen.append(v)
+
+
 @pytest.mark.parametrize('name', GOLDEN_FULL)
 def test_weight_folding_and_packing(golden, name):
     """packed weights + the kernel schedule (torch emulation, fp64) == oracle fp64."""
