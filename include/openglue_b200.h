@@ -437,6 +437,49 @@ int og_match_compact(const int64_t* matches0, const float* mscores0, const float
 int og_homography_pairs(const uint8_t* rgb, int B, int H, int W, int offset, const int32_t* warp_offset, float* image0, float* image1,
                         float* H_true, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Optimiser step of the reference's training loop (train.py, train_cached.py, pretrain_homography.py under Lightning):
+ *   torch.nn.utils.clip_grad_norm_(params, max_norm) -> torch.optim.Adam.step() -> StepLR(step_size=1, gamma).step()
+ * (models/matching_module.py:133-147; Lightning's gradient_clip_val), in one call of two kernels and with no host
+ * synchronisation, so that it can be captured in a CUDA graph.
+ *   segments  device table of nseg og_optim_segment: every fp32 parameter with a gradient, its Adam moments and its step
+ *             count (torch's per-parameter state['step']).  Segment s covers tiles tile0 .. tile0 + ceil(numel / OG_OPTIM_TILE) - 1
+ *             of the step; tile0 starts at 0 and runs on without gaps; ntiles = the total.  Pointers need 4-byte alignment;
+ *             a segment whose four arrays are 16-byte aligned runs the vector path.
+ *   state     og_optim_state: lr (read, then multiplied by lr_gamma), grad_norm / clip_coef (written), sched_steps
+ *             (incremented).  Zero-fill it once and set lr before the first call; the CTA counter is reset by the kernel.
+ *   workspace >= og_optim_workspace_bytes(nseg), 8-byte aligned.
+ * Per element, torch's foreach arithmetic, bit for bit (same rounding points and FMA contractions):
+ *   g *= clip_coef (written back);  m = lerp(m, g, 1 - beta1);  v = v beta2 + (1 - beta2) g g;
+ *   p += step_size (m / (sqrt(v) / bc2_sqrt + eps))
+ * with clip_coef = min(max_norm / (norm + 1e-6), 1) in fp32 (NaN norm -> NaN), the norm a deterministic fp64 reduction
+ * rounded once to fp32, and per segment step += 1, bc1 = 1 - beta1^step, bc2_sqrt = (1 - beta2^step)^0.5,
+ * step_size = -lr / bc1 in fp64, rounded once to fp32.
+ * OG_EINVAL without touching the GPU: null pointers, nseg or ntiles <= 0, max_norm <= 0, beta outside [0, 1), eps < 0,
+ * lr_gamma <= 0, a small workspace (OG_EWORKSPACE).
+ * og_adam_schedule (tests): the same device-derived scalars for steps 1 .. nsteps from an initial lr:
+ * lr_out[k] = the lr of step k + 1, step_size[k] / bc2_sqrt[k] its fp32 scalars.                        */
+#define OG_OPTIM_TILE 2048
+typedef struct og_optim_segment {
+  float* param; float* grad; float* exp_avg; float* exp_avg_sq;
+  float* step;                  /* one fp32 step count                                               */
+  int64_t numel;
+  int64_t tile0;
+} og_optim_segment;
+typedef struct og_optim_state {
+  double   lr;
+  float    grad_norm;           /* what clip_grad_norm_ returns                                      */
+  float    clip_coef;
+  uint32_t counter;             /* CTA counter of the norm kernel: zero between calls               */
+  uint32_t sched_steps;         /* scheduler steps taken (StepLR's last_epoch): +1 per call          */
+} og_optim_state;
+int64_t og_optim_state_bytes(void);
+int64_t og_optim_workspace_bytes(int nseg);
+int og_clip_adam_step(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
+                      double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes, void* stream);
+int og_adam_schedule(int64_t nsteps, double lr, double lr_gamma, double beta1, double beta2, double* lr_out, float* step_size,
+                     float* bc2_sqrt, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,6 +10,7 @@ and the steps either side of those:
     criterion(y_true, y_pred, margin=None) -> {'loss', 'metric_loss'}
     matching_log_probs(S, dustbin_score, num_iters, reg)      (differentiable Sinkhorn: forward + backward kernels)
     SuperGlue(config).train()(data)                           (training mode: batch-statistics BatchNorm, explicit backward pass)
+    ClippedAdam.from_config(superglue, config['train'])       (clip_grad_norm_ -> Adam -> StepLR, one device call, graph-capturable)
     SuperPointNet(max_keypoints, ...)(image) -> (lafs, scores, descriptors)   (the detector / descriptor front-end; SuperPointNetBn: its BatchNorm variant)
     prepare_features_output(lafs, responses, desc, get_laf_to_sideinfo_converter(method), ...)   (front-end output -> SuperGlue input)
     OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
@@ -20,6 +21,7 @@ from .homography import synthesize_homography_pairs  # noqa: F401
 from .feature_cache import FeatureStore, collate_features  # noqa: F401
 from .features import OpenGlueMatcher, get_laf_to_sideinfo_converter, prepare_features_output  # noqa: F401
 from .losses import criterion  # noqa: F401
+from .optim import ClippedAdam  # noqa: F401
 from .sinkhorn import matching_log_probs  # noqa: F401
 from .superglue import MatchingCore, PendingMatches, SuperGlue  # noqa: F401
 from .superpoint import SuperPointNet, SuperPointNetBn  # noqa: F401

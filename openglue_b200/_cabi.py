@@ -44,7 +44,7 @@ class OgLinearArgs(C.Structure):
 
 
 # every symbol include/openglue_b200.h declares: (restype, argtypes)
-_P, _I, _L, _F = C.c_void_p, C.c_int, C.c_int64, C.c_float
+_P, _I, _L, _F, _D = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
 _CFG = C.POINTER(OgConfig)
 class OgGtTransform(C.Structure):       # include/openglue_b200.h: og_gt_transform
     _fields_ = [('type', C.c_int32), ('H', C.c_void_p), ('K0', C.c_void_p), ('K1', C.c_void_p), ('R', C.c_void_p),
@@ -121,6 +121,11 @@ SYMBOLS = {
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     # homography-pretraining pairs
     'og_homography_pairs': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
+    # optimiser step: clip_grad_norm_ -> Adam -> StepLR
+    'og_optim_state_bytes': (_L, []),
+    'og_optim_workspace_bytes': (_L, [_I]),
+    'og_clip_adam_step': (_I, [_P, _I, _L, _D, _D, _D, _D, _D, _P, _P, _L, _P]),
+    'og_adam_schedule': (_I, [_L, _D, _D, _D, _D, _P, _P, _P, _P]),
 }
 
 _lib: Optional[C.CDLL] = None

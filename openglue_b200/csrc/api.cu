@@ -15,6 +15,7 @@
 #include "superpoint.cuh"
 #include "features.cuh"
 #include "homography.cuh"
+#include "optim.cuh"
 #include <math.h>
 #include <string.h>
 #include <vector>
@@ -611,6 +612,36 @@ int og_homography_pairs(const uint8_t* rgb, int B, int H, int W, int offset, con
   const int h = H - 2 * offset;
   return OG_LAUNCH(homography_pairs_kernel, dim3(cdiv(h, HG_ROWS), B), HG_THREADS, 0, (cudaStream_t)stream, rgb, H, W, offset,
                    hg_block_width(H, W), warp_offset, image0, image1, H_true);
+}
+
+// ---- optimiser step (csrc/optim.cuh) ----
+int64_t og_optim_state_bytes(void) { return (int64_t)sizeof(og_optim_state); }
+int64_t og_optim_workspace_bytes(int nseg) { return nseg > 0 ? optim_workspace_bytes(nseg) : -1; }
+
+static bool unit_beta(double b) { return b >= 0.0 && b < 1.0; }
+
+int og_clip_adam_step(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
+                      double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes, void* stream) {
+  OG_CHECK_ARG(segments && state && workspace, "clip_adam_step: null pointer");
+  OG_CHECK_ARG(nseg > 0 && ntiles > 0, "clip_adam_step: nseg = %d and ntiles = %lld must be positive", nseg, (long long)ntiles);
+  OG_CHECK_ARG(max_norm > 0.0, "clip_adam_step: max_norm = %g must be positive", max_norm);
+  OG_CHECK_ARG(unit_beta(beta1) && unit_beta(beta2), "clip_adam_step: betas (%g, %g) must lie in [0, 1)", beta1, beta2);
+  OG_CHECK_ARG(eps >= 0.0, "clip_adam_step: eps = %g must be >= 0", eps);
+  OG_CHECK_ARG(lr_gamma > 0.0, "clip_adam_step: lr_gamma = %g must be positive", lr_gamma);
+  if (workspace_bytes < optim_workspace_bytes(nseg)) return fail(OG_EWORKSPACE, "clip_adam_step: workspace too small");
+  const OptHyper h = {beta1, beta2, eps, max_norm, lr_gamma};
+  return optim_step_launch(segments, nseg, ntiles, h, state, workspace, (cudaStream_t)stream);
+}
+
+int og_adam_schedule(int64_t nsteps, double lr, double lr_gamma, double beta1, double beta2, double* lr_out, float* step_size,
+                     float* bc2_sqrt, void* stream) {
+  OG_CHECK_ARG(lr_out && step_size && bc2_sqrt, "adam_schedule: null pointer");
+  OG_CHECK_ARG(nsteps > 0 && nsteps < (1 << 24), "adam_schedule: nsteps = %lld must lie in [1, 2^24)", (long long)nsteps);
+  OG_CHECK_ARG(unit_beta(beta1) && unit_beta(beta2) && lr_gamma > 0.0, "adam_schedule: bad hyper-parameters");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (const int rc = OG_LAUNCH(adam_lr_chain_kernel, 1, 1, 0, st, nsteps, lr, lr_gamma, lr_out)) return rc;
+  return OG_LAUNCH(adam_scalars_kernel, (unsigned)std::min<int64_t>((nsteps + 255) / 256, 4096), 256, 0, st, nsteps, (const double*)lr_out,
+                   beta1, beta2, step_size, bc2_sqrt);
 }
 
 static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi, const float* Wlo, const __half* W16h,

@@ -362,14 +362,19 @@ def train_forward(model, data: dict) -> Dict[str, torch.Tensor]:
 
 
 class GraphedTrainStep:
-    """The whole training step of one batch shape - train-mode forward, ``criterion``, backward, gradients into ``param.grad`` -
-    captured ONCE into a CUDA graph and replayed: the eager step issues ~5000 kernel launches from Python and is launch-rate-bound,
-    the replay costs the kernels' own time.  Labels (``generate_gt_matches``) and the optimiser stay outside::
+    """The whole training step of one batch shape - train-mode forward, ``criterion``, backward, gradients into ``param.grad`` and,
+    with ``optimizer`` (a :class:`~openglue_b200.optim.ClippedAdam`), the optimiser step - captured ONCE into a CUDA graph and
+    replayed: the eager step issues ~5000 kernel launches from Python and is launch-rate-bound, the replay costs the kernels' own
+    time.  Labels (``generate_gt_matches``) stay outside::
 
-        step = GraphedTrainStep(model, data, y_true)          # model.train(); captures on the first batch
+        opt = ClippedAdam.from_config(model, config['train'])  # clip_grad_norm_ -> Adam -> StepLR, on the device
+        step = GraphedTrainStep(model, data, y_true, optimizer=opt)   # model.train(); captures on the first batch
         for data, y_true in loader:                           # same shapes
-            loss = step(data, y_true)                         # {'loss', 'metric_loss'}; gradients are in p.grad
-            optimizer.step()                                  # in-place updates keep the captured parameter addresses valid
+            loss = step(data, y_true)                         # {'loss', 'metric_loss'}: one replay is the whole iteration
+
+    Without ``optimizer`` the graph ends with the gradients in ``p.grad`` and any optimiser runs after the replay (in-place
+    updates keep the captured parameter addresses valid).  The capture's warm-up run is not a training step: the BatchNorm
+    buffers, and with ``optimizer`` the parameters and its state, are restored after it, so the first replay is step 1.
 
     The graph reads the parameters and BatchNorm buffers in place (so optimiser steps and running statistics carry over) and the
     inputs from static copies.  Re-create the object when shapes change or parameters are re-allocated (``.to()``, ``load_state_dict``
@@ -377,14 +382,18 @@ class GraphedTrainStep:
 
     _KEYS = ('keypoints0', 'keypoints1', 'side_info0', 'side_info1', 'local_descriptors0', 'local_descriptors1')
 
-    def __init__(self, model, data: dict, y_true: dict, nll_weight: float = 1.0):
+    def __init__(self, model, data: dict, y_true: dict, nll_weight: float = 1.0, optimizer=None):
         from .losses import _run as criterion_run
+        from .optim import ClippedAdam
         if not model.training:
             raise RuntimeError('GraphedTrainStep captures the training-mode step: call model.train() first')
         dev = data['keypoints0'].device
         if dev.type != 'cuda':
             raise RuntimeError('openglue_b200 training needs CUDA tensors (sm_90a); there is no CPU path')
-        self.model, self.dev = model, dev
+        if optimizer is not None and not isinstance(optimizer, ClippedAdam):
+            raise TypeError('GraphedTrainStep captures the optimiser step of openglue_b200.ClippedAdam only '
+                            f'(got {type(optimizer).__name__}): run other optimisers after the replay')
+        self.model, self.dev, self.optimizer = model, dev, optimizer
         self.static = dict(data)
         for k in self._KEYS:
             self.static[k] = data[k].detach().float().contiguous().clone()
@@ -401,10 +410,13 @@ class GraphedTrainStep:
             grads = step.backward(dscores)
             for name, p in self.params:
                 p.grad.copy_(grads[name].reshape(p.shape))
+            if optimizer is not None:
+                optimizer.step()
             return loss, scores
 
         with torch.cuda.device(dev):
             saved = [b.clone() for b in model.buffers()]                # the warm-up run must not count as a training step
+            saved_opt = None if optimizer is None else optimizer._snapshot()
             cur = torch.cuda.current_stream(dev)
             side = torch.cuda.Stream(dev)
             side.wait_stream(cur)
@@ -414,9 +426,14 @@ class GraphedTrainStep:
             torch.cuda.synchronize(dev)
             for b, s in zip(model.buffers(), saved):
                 b.copy_(s)
+            if optimizer is not None:
+                optimizer._restore(saved_opt)
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
                 self.loss, self.scores = run()
+            if optimizer is not None:                                    # the capture ran nothing: no parameter has state yet
+                self._opt_idx = optimizer._last_idx
+                optimizer._stepped = list(saved_opt[-1])
 
     def __call__(self, data: dict, y_true: dict) -> Dict[str, torch.Tensor]:
         for k in self._KEYS:
@@ -426,4 +443,6 @@ class GraphedTrainStep:
         for k in self.gt:
             self.gt[k].copy_(y_true[k], non_blocking=True)
         self.graph.replay()
+        if self.optimizer is not None:                                   # the kernels wrote the parameters through raw pointers
+            self.optimizer._stepped_now(self._opt_idx)
         return {'loss': self.loss[0], 'metric_loss': self.loss[1]}
