@@ -187,6 +187,17 @@ class SuperGlue(nn.Module):
         return self._packed
 
     # ------------------------------------------------------------------ forward
+    _HEAD_DIMS = (8, 16, 32, 64)                         # the head sizes the attention kernels are built for
+
+    def _check_head_dim(self) -> None:
+        """Raise before any kernel runs (and before train mode moves a BatchNorm buffer) when descriptor_dim / num_heads is not a
+        head size the attention kernels are built for.  Construction and load_state_dict accept such configs, so checkpoints can
+        still be loaded and converted."""
+        d, H = self.config['descriptor_dim'], self.config['attention_gnn']['num_heads']
+        if d % H or d // H not in self._HEAD_DIMS:
+            raise ValueError(f'head_dim = descriptor_dim / num_heads = {d} / {H} is not supported: openglue_b200 builds attention '
+                             f'for head_dim in {self._HEAD_DIMS}')
+
     @staticmethod
     def _image_wh(data: dict, idx: int):
         """reference superglue.py:35-38: image tensor [..., H, W] or image{idx}_size = (W, H)."""
@@ -201,6 +212,7 @@ class SuperGlue(nn.Module):
         if self.training:
             raise RuntimeError('openglue_b200.SuperGlue.run is the fused eval-mode path; in train() mode call forward() '
                                '(openglue_b200.training: batch-statistics BatchNorm + the explicit backward pass)')
+        self._check_head_dim()
         k0, k1 = data['keypoints0'], data['keypoints1']
         dev = k0.device
         if dev.type != 'cuda':

@@ -53,6 +53,7 @@ class TrainStep:
     ``{parameter name: gradient}`` (+ ``'local_descriptors0/1'``)."""
 
     def __init__(self, model, data: dict, ops=None):
+        model._check_head_dim()                         # before the forward pass moves any BatchNorm running buffer
         self.model = model
         cfg = model.config
         self.d = cfg['descriptor_dim']

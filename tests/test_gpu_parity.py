@@ -172,13 +172,25 @@ def test_forward_matches_reference_big(golden, name, precision, pair):
     (1, 1, 5, dict(descriptor_dim=256, num_stages=1, num_iters=5), 'flat'),            # head_dim 64: a single keypoint / single key block tail
     (3, 64, 1, dict(descriptor_dim=256, num_stages=2, num_iters=0), 'flat'),           # head_dim 64: one key, zero Sinkhorn iterations
     (2, 129, 257, dict(descriptor_dim=128, num_heads=2, num_stages=2, num_iters=10, residual=False), 'planted'),   # head_dim 64 with d = 128
+    (2, 150, 97, dict(descriptor_dim=192, num_heads=3, num_stages=2, num_iters=20), 'planted'),     # fp16 GNN with d % 128 != 0: unfused runs
+    (2, 70, 83, dict(descriptor_dim=64, num_heads=1, num_stages=2, num_iters=20), 'planted'),       # fp16 GNN narrower than one 128-wide tile
+    (2, 90, 61, dict(descriptor_dim=96, num_heads=3, num_stages=2, num_iters=20), 'planted'),       # tf32 attention, head_dim 32, d not 2^k
+    (2, 45, 50, dict(descriptor_dim=32, num_heads=4, num_stages=2, num_iters=20), 'planted'),       # head_dim 8: CUDA-core attention everywhere
+    (2, 60, 71, dict(descriptor_dim=64, num_stages=2, num_iters=20, hidden_layers_sizes=()), 'planted'),        # encoder without hidden layer
+    (2, 60, 71, dict(descriptor_dim=64, num_stages=2, num_iters=20, hidden_layers_sizes=(30, 50)), 'planted'),  # widths not multiples of 4
+    (2, 60, 71, dict(descriptor_dim=64, num_stages=2, num_iters=20, side_info_size=0), 'planted'),   # no side info
+    (2, 60, 71, dict(descriptor_dim=64, num_stages=2, num_iters=20), 'planted+images'),              # sizes from image tensors
 ])
 @pytest.mark.parametrize('precision', ['fp32', 'tf32x3', 'fp16x3'])
 def test_forward_matches_oracle(batch, n, m, kw, family, precision):
     cfg = default_config(**kw)
     sd = synthetic_state_dict(cfg, seed=3)
+    family, _, images = family.partition('+')
     data = synthetic_pairs(batch, n, m, cfg['descriptor_dim'], cfg['positional_encoding']['side_info_size'],
                            family=family, seed=77)
+    if images:                        # image tensors [B, 1, H, W] take precedence over image*_size (set wrong here on purpose)
+        data['image0'], data['image1'] = torch.zeros(batch, 1, 500, 700), torch.zeros(batch, 1, 640, 480)
+        data['image0_size'] = data['image1_size'] = (2000, 1000)
     ref = O.run(sd, cfg, data, 0.2)
     ref64 = O.run(sd, cfg, data, 0.2, dtype=torch.float64)
     bound = max(TOL, 2 * float((ref['scores'].double() - ref64['scores']).abs().max()))
@@ -186,9 +198,7 @@ def test_forward_matches_oracle(batch, n, m, kw, family, precision):
     res = MatchingCore(model, 0.2)(_to_dev(data), want_scores=True)
     assert (res['scores'].cpu().double() - ref64['scores']).abs().max() <= bound
     check_matches(res, ref, ref64['scores'], bound)
-    # context descriptors (superglue.py:66-69), written into POISONED buffers (an output the kernels skip must not pass by luck)
-    poison = [torch.full((batch, cfg['descriptor_dim'], k), float('nan'), device=DEV) for k in (n, m)]
-    del poison
+    # context descriptors (superglue.py:66-69)
     out = model(_to_dev(data))
     for i in (0, 1):
         c = out[f'context_descriptors{i}'].cpu().double()
@@ -220,6 +230,27 @@ def test_no_descriptors_option(precision):
     res = MatchingCore(_model(cfg, sd, precision), 0.2)(_to_dev(data), want_scores=True)
     assert (res['scores'].cpu().double() - ref64['scores']).abs().max() <= bound
     check_matches(res, ref, ref64['scores'], bound)
+
+
+@pytest.mark.parametrize('mode', ['eval', 'train'])
+def test_unsupported_head_dim_is_rejected_before_any_kernel(mode):
+    """d = 256 with 2 heads (head_dim 128, which the reference accepts) loads, then fails with a ValueError naming head_dim
+    before any kernel runs: in train mode no BatchNorm running buffer has moved."""
+    cfg = default_config(descriptor_dim=256, num_heads=2, num_stages=1, num_iters=5)
+    model = SuperGlue(dict(cfg, precision='tf32x3'))
+    model.load_state_dict(synthetic_state_dict(cfg, seed=1), strict=True)
+    model = model.to(DEV).train(mode == 'train')
+    before = {k: v.clone() for k, v in model.named_buffers()}
+    data = _to_dev(synthetic_pairs(2, 40, 30, 256, 1, family='flat', seed=2))
+    err = None
+    try:
+        model(data)
+    except Exception as e:                   # (checked below, after the buffers)
+        err = e
+    torch.cuda.synchronize()
+    moved = [k for k, v in model.named_buffers() if not torch.equal(v, before[k])]
+    assert not moved, f'buffers moved before the error: {moved}'
+    assert isinstance(err, ValueError) and 'head_dim' in str(err), repr(err)
 
 
 def test_host_buffers_roundtrip(golden):

@@ -106,18 +106,32 @@ def test_oracle_equals_staged_reference():
         pytest.skip('oracle/_ref is not staged (run `python oracle/build_ref.py` where /root/reference exists)')
     from openglue_b200.synthetic import default_config, synthetic_pairs, synthetic_state_dict
     SuperGlueRef = ref[0]
-    for seed, kw, (n, m) in [(11, dict(descriptor_dim=64, num_stages=2, num_iters=15), (97, 61)),
-                             (12, dict(descriptor_dim=128, num_stages=2, num_iters=7, side_info_size=6, use_offset=True, reg=0.7), (50, 75))]:
+    # the option rows of tests/test_gpu_parity.py::test_forward_matches_oracle; `images`: sizes from image tensors, which take
+    # precedence over image*_size (set wrong on purpose)
+    for seed, kw, (n, m), images in [
+            (11, dict(descriptor_dim=64, num_stages=2, num_iters=15), (97, 61), False),
+            (12, dict(descriptor_dim=128, num_stages=2, num_iters=7, side_info_size=6, use_offset=True, reg=0.7), (50, 75), False),
+            (13, dict(descriptor_dim=192, num_heads=3, num_stages=2, num_iters=10), (40, 33), False),
+            (14, dict(descriptor_dim=64, num_heads=1, num_stages=2, num_iters=10), (40, 33), False),
+            (15, dict(descriptor_dim=96, num_heads=3, num_stages=2, num_iters=10), (40, 33), False),
+            (16, dict(descriptor_dim=32, num_heads=4, num_stages=2, num_iters=10), (40, 33), False),
+            (17, dict(descriptor_dim=64, num_stages=2, num_iters=10, hidden_layers_sizes=()), (40, 33), False),
+            (18, dict(descriptor_dim=64, num_stages=2, num_iters=10, hidden_layers_sizes=(30, 50)), (40, 33), False),
+            (19, dict(descriptor_dim=64, num_stages=2, num_iters=10, side_info_size=0), (40, 33), False),
+            (20, dict(descriptor_dim=64, num_stages=2, num_iters=10), (40, 33), True)]:
         cfg = default_config(**kw)
         sd = synthetic_state_dict(cfg, seed=seed)
         data = synthetic_pairs(2, n, m, cfg['descriptor_dim'], cfg['positional_encoding']['side_info_size'], family='planted', seed=seed)
+        if images:
+            data['image0'], data['image1'] = torch.zeros(2, 1, 500, 700), torch.zeros(2, 1, 640, 480)
+            data['image0_size'] = data['image1_size'] = (2000, 1000)
         model = SuperGlueRef(dict(cfg)).eval()
         model.load_state_dict(sd, strict=True)
         with torch.no_grad():
             want = model(data)
         got = O.run(sd, cfg, data, 0.2)
         for key in ('scores', 'context_descriptors0', 'context_descriptors1'):
-            assert torch.equal(got[key], want[key]), key
+            assert torch.equal(got[key], want[key]), (kw, key)
 
 
 def test_label_and_loss_oracles_equal_staged_reference():
