@@ -198,9 +198,11 @@ static int linear_dispatch(const og_linear_args& a, int precision, cudaStream_t 
   return linear_simt_launch(a, s);
 }
 
-// floats of W a GEMM reads: batch weight blocks strideW apart, the last of them nout rows of ldw
+// floats of W a GEMM reads: batch weight blocks strideW apart, the last of them nout rows of ldw of which the last ends after
+// K elements (a head-sliced W, such as a column block of K, ends there; a whole last row of ldw would run past it)
 static int64_t weight_floats(const og_linear_args& a) {
-  return (a.batch > 1 && a.strideW) ? (int64_t)(a.batch - 1) * a.strideW + (int64_t)a.nout * a.ldw : (int64_t)a.nout * a.ldw;
+  const int64_t last = (int64_t)(a.nout - 1) * a.ldw + a.k1 + a.k2;
+  return (a.batch > 1 && a.strideW) ? (int64_t)(a.batch - 1) * a.strideW + last : last;
 }
 
 }  // namespace og

@@ -5,6 +5,7 @@
 // models/utils.py:53-57, superglue.py:58) and the score matmul (superglue.py:80-86).
 #pragma once
 #include "common.cuh"
+#include <algorithm>
 
 namespace og {
 
@@ -139,15 +140,32 @@ __global__ void __launch_bounds__(256, 2) linear_simt_kernel(og_linear_args a, L
   }
 }
 
+// grid.y counts 128-row tiles and stops at 65535: taller operands run as consecutive launches over row ranges of at most
+// LINEAR_MAX_ROWS rows, each with A, A2, R and Y advanced by its first row and Yt by its first column.  The ranges start at
+// multiples of 128 rows, so a row's tile, and with it its result, is the same as in one launch.
+constexpr int64_t LINEAR_MAX_ROWS = 65535 * (int64_t)LBM;
+
 inline int linear_simt_launch(const og_linear_args& a, cudaStream_t stream) {
+  if (a.batch > 65535) return fail(OG_EUNSUPPORTED, "linear: %d batches exceed the grid limit 65535", a.batch);
   LinearFlags f;
   f.vecA = (a.k1 % 4 == 0) && (a.k2 % 4 == 0) && (a.lda % 4 == 0) && (a.strideA % 4 == 0) && aligned16(a.A) &&
            (!a.A2 || ((a.lda2 % 4 == 0) && (a.strideA2 % 4 == 0) && aligned16(a.A2)));
   f.vecW = ((a.k1 + a.k2) % 4 == 0) && (a.ldw % 4 == 0) && (a.strideW % 4 == 0) && aligned16(a.W);
   f.vecY = a.Y && (a.ldy % 4 == 0) && (a.strideY % 4 == 0) && aligned16(a.Y);
   f.vecYt = a.Yt && (a.ldyt % 4 == 0) && (a.strideYt % 4 == 0) && aligned16(a.Yt);
-  dim3 grid(cdiv(a.nout, LBN), cdiv(a.rows, LBM), a.batch);
-  return OG_LAUNCH(linear_simt_kernel, grid, 256, 0, stream, a, f);
+  // the flags hold for every range: r0 is a multiple of 4, so an advanced pointer stays 16-byte aligned where its flag needs it
+  for (int64_t r0 = 0; r0 < a.rows; r0 += LINEAR_MAX_ROWS) {
+    og_linear_args p = a;
+    p.rows = (int)std::min<int64_t>(a.rows - r0, LINEAR_MAX_ROWS);
+    p.A += r0 * a.lda;
+    if (p.A2) p.A2 += r0 * a.lda2;
+    if (p.R) p.R += r0 * a.ldr;
+    if (p.Y) p.Y += r0 * a.ldy;
+    if (p.Yt) p.Yt += r0;
+    dim3 grid(cdiv(p.nout, LBN), cdiv(p.rows, LBM), p.batch);
+    if (const int rc = OG_LAUNCH(linear_simt_kernel, grid, 256, 0, stream, p, f)) return rc;
+  }
+  return OG_OK;
 }
 
 }  // namespace og
