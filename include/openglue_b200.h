@@ -238,6 +238,15 @@ int og_attention_f16_fwd(const float* q, int64_t ldq, int64_t strideq, const flo
  *   dustbin device scalar;   scores [B, n+1, m+1]
  *   workspace >= og_sinkhorn_workspace_bytes(B, n, m)                                          */
 int64_t og_sinkhorn_workspace_bytes(int batch, int n, int m);
+/* resident = 1 (default; env OG_SINK_RESIDENT): the forward Sinkhorn (og_sinkhorn_fwd, og_superglue_forward*) keeps each pair's
+ * score rows on chip for all its iterations wherever that plan fits (og_sinkhorn_plan); 0: the streaming kernel, which reads the
+ * score matrix from HBM in every iteration.  The column sums are added in another order, so scores agree to the last bits; both
+ * forms are deterministic.  The training form always streams.  Returns the previous setting; a negative argument only queries. */
+int og_set_sinkhorn_resident(int resident);
+/* How og_sinkhorn_fwd runs (batch, n, m) on the current device under the current setting: plan[0..9] = resident (1) or streaming
+ * (0), float4s per lane, warps per row, strips per pair, rows per strip, pairs per launch, rows per warp held in registers, rows
+ * per warp held in shared memory, dynamic shared memory per CTA (bytes), CTAs per SM. */
+int og_sinkhorn_plan(int batch, int n, int m, int64_t* plan);
 int og_sinkhorn_fwd(const float* S, int64_t lds, int64_t strideS, const float* dustbin,
                     int batch, int n, int m, int iters, float reg,
                     float* scores, void* workspace, int64_t workspace_bytes, void* stream);

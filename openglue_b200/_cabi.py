@@ -80,6 +80,8 @@ SYMBOLS = {
     'og_attention_fwd': (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _L, _I, _I, _I, _I, _I, _I, _P]),
     'og_attention_tc_fwd': (_I, [_P, _L, _L, _P, _P, _L, _P, _P, _L, _P, _L, _L, _I, _I, _I, _I, _I, _P]),
     'og_sinkhorn_workspace_bytes': (_L, [_I, _I, _I]),
+    'og_set_sinkhorn_resident': (_I, [_I]),
+    'og_sinkhorn_plan': (_I, [_I, _I, _I, _P]),
     'og_sinkhorn_fwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _L, _P]),
     'og_sinkhorn_hist_floats': (_L, [_I, _I, _I, _I]),
     'og_sinkhorn_train_fwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _P, _L, _P]),

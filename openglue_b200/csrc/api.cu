@@ -347,6 +347,27 @@ int og_attention_tc_fwd(const float* q, int64_t ldq, int64_t strideq, const floa
 
 int64_t og_sinkhorn_workspace_bytes(int batch, int n, int m) { return sinkhorn_workspace_bytes(batch, n, m); }
 
+int og_set_sinkhorn_resident(int resident) {
+  const int prev = sink_resident_mode();
+  if (resident >= 0) sink_resident_mode() = resident ? 1 : 0;
+  return prev;
+}
+
+int og_sinkhorn_plan(int batch, int n, int m, int64_t* plan) {
+  OG_CHECK_ARG(plan, "sinkhorn_plan: null pointer");
+  OG_CHECK_ARG(batch > 0 && n > 0 && m > 0, "sinkhorn_plan: bad sizes");
+  SinkPlan p;
+  const bool resident = sink_resident_mode() && sinkhorn_resident_plan(batch, n, m, &p);
+  if (!resident) {
+    if (const int rc = sinkhorn_plan(false, batch, n, m, &p)) return rc;
+    p.rows_reg = p.rows_smem = 0;
+  }
+  const int64_t v[10] = {resident, p.V, p.W, p.SP, p.rows_per_strip, p.pairs_per_launch, p.rows_reg, p.rows_smem,
+                         (int64_t)p.smem, p.occ};
+  for (int i = 0; i < 10; ++i) plan[i] = v[i];
+  return OG_OK;
+}
+
 int og_sinkhorn_fwd(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int batch, int n, int m,
                     int iters, float reg, float* scores, void* workspace, int64_t workspace_bytes, void* stream) {
   OG_CHECK_ARG(S && dustbin && scores && workspace, "sinkhorn: null pointer");

@@ -42,6 +42,8 @@ struct SinkArgs {
   float* partial;                        // [2, B, SP, mpad] workspace
   unsigned int* barrier;                 // [B] counters, one per pair, 128 bytes apart; zeroed before launch
   int SP, rows_per_strip, mpad;
+  int rows_smem;                         // resident kernel: rows per warp held in shared memory
+  float* vglob;                          // resident kernel: [B, mpad] 64-bit words, v as each strip publishes its columns
   float* hist_u;                         // optional [B][iters][n+1]: u_t of every iteration  (kept for the backward pass,
   float* hist_v;                         // optional [B][iters+1][m+1]: v_t, row 0 = v_0 = 0   csrc/sinkhorn_bwd.cuh)
 };
@@ -230,9 +232,10 @@ __device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkS
 // segment 0) -> CTA (red [G][mpad]: the row groups' warps own disjoint columns of their row) -> this strip's partial in global
 // memory (buffer k & 1 of two) -> barrier among the SP CTAs of the pair -> every CTA of the pair rebuilds the sums in the same
 // fixed order (bitwise identical across CTAs) and calls update(j, sum) for j < m and update(MC, sum) for the dustbin column.
-template <int V, int W, class Args, class Update>
-__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
-                                                   float cacc_m, int k, Update update) {
+// sink_strip_sums is its first part: the strip's column sums, passed to store(j, sum) for j <= m.
+template <int V, int W, class Args, class Store>
+__device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
+                                                float cacc_m, Store store) {
   const int m = a.m;
   float* myred = red + s.grp * a.mpad;
 #pragma unroll
@@ -243,14 +246,21 @@ __device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStri
   __syncthreads();                                    // (a) all float4 column sums are in `red`
   if (s.sub == 0 && s.lane == 0) myred[m] = cacc_m;   // column m = dustbin column (may overlap a float4 tail)
   __syncthreads();
-  const int64_t buf = (int64_t)(k & 1) * a.B * a.SP + (int64_t)s.b * a.SP;
-  float* part = a.partial + (buf + s.strip) * a.mpad;
   for (int j = s.tid; j <= m; j += blockDim.x) {
     float sum = 0.f;
 #pragma unroll
     for (int w = 0; w < SinkStrip<V, W>::G; ++w) sum += red[w * a.mpad + j];
-    part[j] = sum;
+    store(j, sum);
   }
+}
+
+template <int V, int W, class Args, class Update>
+__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
+                                                   float cacc_m, int k, Update update) {
+  const int m = a.m;
+  const int64_t buf = (int64_t)(k & 1) * a.B * a.SP + (int64_t)s.b * a.SP;
+  float* part = a.partial + (buf + s.strip) * a.mpad;
+  sink_strip_sums(a, s, red, cacc, cacc_m, [&](int j, float sum) { part[j] = sum; });
   // only the SP CTAs of this pair exchange data: a per-pair barrier (own 128-byte line) lets the pairs drift apart,
   // so HBM keeps streaming for the other pairs while one pair sits in its reduction / barrier phase
   grid_barrier(a.barrier + 32 * s.b, (unsigned int)(k + 1) * (unsigned int)a.SP);
@@ -274,6 +284,89 @@ __device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStri
   __syncthreads();
 }
 
+// One row of a forward sweep (iteration `it`) from this warp's segment q of it: t = z + v, the row's (max, sum) over the W warps of
+// its group, u_i (stored in the last iteration and in hist_u when recorded) and the row's share e_ij a_i / S_i of the column
+// sums, added to cacc (cacc_m: the dustbin column, counted by segment 0).  v_s: v of the pair in shared memory, v_m = v_s[MC].
+template <int V, int W>
+__device__ __forceinline__ void sink_fwd_row(const SinkArgs& a, const SinkStrip<V, W>& s, const float4 (&q)[V], const float* v_s,
+                                             float v_m, float dz, float a_reg, float a_last, float2* xr, uint32_t& rowpar, int row,
+                                             int it, f32x2 (&cacc)[2 * V], float& cacc_m) {
+  const int n = a.n, c0 = s.c0, lane = s.lane, sub = s.sub;
+  const f32x2 log2e2 = pk2(LOG2E_F, LOG2E_F);
+  f32x2 z[2 * V];
+#pragma unroll
+  for (int k = 0; k < V; ++k) { z[2 * k] = pk2(q[k].x, q[k].y); z[2 * k + 1] = pk2(q[k].z, q[k].w); }
+  // t = z + v, masked; maximum over this warp's segment (the dustbin column entry belongs to segment 0)
+  const float t_m = dz + v_m;
+  float mx = (sub == 0) ? t_m : -CUDART_INF_F;
+#pragma unroll
+  for (int k = 0; k < V; ++k) {
+    const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(v_s + c0 + 4 * (lane + 32 * k));   // columns >= m: finite z + (-inf) = -inf, e = 0
+    z[2 * k] = add2(z[2 * k], vv.x); z[2 * k + 1] = add2(z[2 * k + 1], vv.y);
+    float x0, x1, x2, x3; upk2(z[2 * k], x0, x1); upk2(z[2 * k + 1], x2, x3);
+    mx = fmaxf(mx, fmaxf(fmaxf(x0, x1), fmaxf(x2, x3)));
+  }
+  mx = warp_max(mx);
+  const float mxs = (mx == -CUDART_INF_F) ? 0.f : mx;               // an all-padding segment: e = 2^-inf = 0, not NaN
+  const f32x2 mxs2 = pk2(mxs, mxs);
+  f32x2 sum2a = 0ull, sum2b = 0ull;
+#pragma unroll
+  for (int k = 0; k < 2 * V; ++k) {
+    float x, y; upk2(mul2(sub2(z[k], mxs2), log2e2), x, y);
+    z[k] = pk2(ex2_approx(x), ex2_approx(y));
+    if (k & 1) sum2b = add2(sum2b, z[k]); else sum2a = add2(sum2a, z[k]);
+  }
+  float sa, sb; upk2(add2(sum2a, sum2b), sa, sb);
+  const float e_m = (sub == 0) ? ex2_approx((t_m - mxs) * LOG2E_F) : 0.f;
+  float s_i = warp_sum(sa + sb) + e_m;
+  float mxg = mx, f_w = 1.f;
+  if (W > 1) {                                     // combine the segments of the row: S = sum_w S_w 2^(mx_w - mx)
+    const float2* x = sink_row_exchange(xr, make_float2(mx, s_i), s, rowpar);
+    float2 p[W];
+#pragma unroll
+    for (int w2 = 0; w2 < W; ++w2) { p[w2] = x[w2]; mxg = fmaxf(mxg, p[w2].x); }
+    s_i = 0.f;
+#pragma unroll
+    for (int w2 = 0; w2 < W; ++w2) s_i = fmaf(p[w2].y, ex2_approx((p[w2].x - mxg) * LOG2E_F), s_i);   // fixed order: identical in every warp
+    f_w = ex2_approx((mx - mxg) * LOG2E_F);
+  }
+  const float w_i = __fdiv_rn((row < n) ? a_reg : a_last, s_i) * f_w;
+  if ((it == a.iters - 1 || a.hist_u) && sub == 0 && lane == 0) {
+    const float u_i = ((row < n) ? a.norm : a.log_a_last) - (mxg + logf(s_i));
+    if (it == a.iters - 1) a.u[(int64_t)s.b * (n + 1) + row] = u_i;
+    if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (n + 1) + row] = u_i;
+  }
+  const f32x2 w2 = pk2(w_i, w_i);
+#pragma unroll
+  for (int k = 0; k < 2 * V; ++k) cacc[k] = fma2(z[k], w2, cacc[k]);
+  cacc_m = fmaf(e_m, w_i, cacc_m);
+}
+
+// The final pass over one row: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111)
+template <int V, int W>
+__device__ __forceinline__ void sink_fwd_score_row(const SinkArgs& a, const SinkStrip<V, W>& s, const float4 (&z)[V], const float* v_s,
+                                                   float v_m, float dz, int row) {
+  const int n = a.n, m = a.m, c0 = s.c0, lane = s.lane;
+  float u_i = 0.f;
+  if (a.iters > 0) {
+    if (lane == 0) u_i = __ldcg(a.u + (int64_t)s.b * (n + 1) + row);
+    u_i = __shfl_sync(0xffffffffu, u_i, 0);
+  }
+  float* out = a.scores + ((int64_t)s.b * (n + 1) + row) * (m + 1);
+#pragma unroll
+  for (int k = 0; k < V; ++k) {
+    const int c = c0 + 4 * (lane + 32 * k);
+    if (c < m) {
+      const float4 vv = *reinterpret_cast<const float4*>(v_s + c);
+      if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - a.norm;
+      if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - a.norm;
+      if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - a.norm;
+      if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - a.norm;
+    }
+  }
+  if (s.sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - a.norm;
+}
+
 // SLOTS: ring depth per warp.  Configurations with V <= 8 need <= 128 registers and <= 106 KB of shared memory: two CTAs per
 // SM, so one CTA streams while the other sits in its per-iteration reduction / barrier phase.
 template <int V, int W, int SLOTS>
@@ -288,7 +381,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);   // [SINK_WARPS][SLOTS]
   float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS * SLOTS);             // [2][G][W] (max, sum) of a segment
   const Strip s(a);
-  const int n = a.n, m = a.m, c0 = s.c0, lane = s.lane, sub = s.sub;
+  const int m = a.m;
   const float a_reg = expf(a.norm), a_last = expf(a.log_a_last);
   SinkRowRing<V, W, SLOTS, true, SinkArgs> rows(a, s, ring, bars);
   const float dz = rows.dz;
@@ -299,7 +392,6 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
 
   rows.prime();
   uint32_t rowpar = 0;                                 // parity of the exchange buffer (alternates per row of the group)
-  const f32x2 log2e2 = pk2(LOG2E_F, LOG2E_F);
   for (int it = 0; it < a.iters; ++it) {
     f32x2 cacc[2 * V];
 #pragma unroll
@@ -310,53 +402,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
     for (int row = s.r0 + s.grp; row < s.r1; row += G) {
       float4 q[V];
       rows.take(row, q);
-      f32x2 z[2 * V];
-#pragma unroll
-      for (int k = 0; k < V; ++k) { z[2 * k] = pk2(q[k].x, q[k].y); z[2 * k + 1] = pk2(q[k].z, q[k].w); }
-      // t = z + v, masked; maximum over this warp's segment (the dustbin column entry belongs to segment 0)
-      const float t_m = dz + v_m;
-      float mx = (sub == 0) ? t_m : -CUDART_INF_F;
-#pragma unroll
-      for (int k = 0; k < V; ++k) {
-        const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(v_s + c0 + 4 * (lane + 32 * k));   // columns >= m: finite z + (-inf) = -inf, e = 0
-        z[2 * k] = add2(z[2 * k], vv.x); z[2 * k + 1] = add2(z[2 * k + 1], vv.y);
-        float x0, x1, x2, x3; upk2(z[2 * k], x0, x1); upk2(z[2 * k + 1], x2, x3);
-        mx = fmaxf(mx, fmaxf(fmaxf(x0, x1), fmaxf(x2, x3)));
-      }
-      mx = warp_max(mx);
-      const float mxs = (mx == -CUDART_INF_F) ? 0.f : mx;               // an all-padding segment: e = 2^-inf = 0, not NaN
-      const f32x2 mxs2 = pk2(mxs, mxs);
-      f32x2 sum2a = 0ull, sum2b = 0ull;
-#pragma unroll
-      for (int k = 0; k < 2 * V; ++k) {
-        float x, y; upk2(mul2(sub2(z[k], mxs2), log2e2), x, y);
-        z[k] = pk2(ex2_approx(x), ex2_approx(y));
-        if (k & 1) sum2b = add2(sum2b, z[k]); else sum2a = add2(sum2a, z[k]);
-      }
-      float sa, sb; upk2(add2(sum2a, sum2b), sa, sb);
-      const float e_m = (sub == 0) ? ex2_approx((t_m - mxs) * LOG2E_F) : 0.f;
-      float s_i = warp_sum(sa + sb) + e_m;
-      float mxg = mx, f_w = 1.f;
-      if (W > 1) {                                     // combine the segments of the row: S = sum_w S_w 2^(mx_w - mx)
-        const float2* x = sink_row_exchange(xr, make_float2(mx, s_i), s, rowpar);
-        float2 p[W];
-#pragma unroll
-        for (int w2 = 0; w2 < W; ++w2) { p[w2] = x[w2]; mxg = fmaxf(mxg, p[w2].x); }
-        s_i = 0.f;
-#pragma unroll
-        for (int w2 = 0; w2 < W; ++w2) s_i = fmaf(p[w2].y, ex2_approx((p[w2].x - mxg) * LOG2E_F), s_i);   // fixed order: identical in every warp
-        f_w = ex2_approx((mx - mxg) * LOG2E_F);
-      }
-      const float w_i = __fdiv_rn((row < n) ? a_reg : a_last, s_i) * f_w;
-      if ((it == a.iters - 1 || a.hist_u) && sub == 0 && lane == 0) {
-        const float u_i = ((row < n) ? a.norm : a.log_a_last) - (mxg + logf(s_i));
-        if (it == a.iters - 1) a.u[(int64_t)s.b * (n + 1) + row] = u_i;
-        if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (n + 1) + row] = u_i;
-      }
-      const f32x2 w2 = pk2(w_i, w_i);
-#pragma unroll
-      for (int k = 0; k < 2 * V; ++k) cacc[k] = fma2(z[k], w2, cacc[k]);
-      cacc_m = fmaf(e_m, w_i, cacc_m);
+      sink_fwd_row(a, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
     }
     rows.prime();                                      // next sweep's (or the final pass's) first rows fly during the reduction
     float4 c4[V];
@@ -371,35 +417,168 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
     }
   }
 
-  // final pass: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111)
-  {
-    const float v_m = v_s[MC];
-    for (int row = s.r0 + s.grp; row < s.r1; row += G) {
-      float4 z[V];
-      rows.take(row, z);
-      float u_i = 0.f;
-      if (a.iters > 0) {
-        if (lane == 0) u_i = __ldcg(a.u + (int64_t)s.b * (n + 1) + row);
-        u_i = __shfl_sync(0xffffffffu, u_i, 0);
-      }
-      float* out = a.scores + ((int64_t)s.b * (n + 1) + row) * (m + 1);
-#pragma unroll
-      for (int k = 0; k < V; ++k) {
-        const int c = c0 + 4 * (lane + 32 * k);
-        if (c < m) {
-          const float4 vv = *reinterpret_cast<const float4*>(v_s + c);
-          if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - a.norm;
-          if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - a.norm;
-          if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - a.norm;
-          if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - a.norm;
-        }
-      }
-      if (sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - a.norm;
-    }
+  const float v_m = v_s[MC];
+  for (int row = s.r0 + s.grp; row < s.r1; row += G) {
+    float4 z[V];
+    rows.take(row, z);
+    sink_fwd_score_row(a, s, z, v_s, v_m, dz, row);
   }
 }
 
-struct SinkPlan { int V, W, slots, occ, SP, rows_per_strip, mpad, pairs_per_launch; size_t smem; };
+// A value and the iteration (from 1) it belongs to, as one 64-bit word: a single-copy-atomic store and load carry both, so a reader
+// that sees the tag it waits for also sees the value, with no fence.
+__device__ __forceinline__ void sink_put(uint64_t* p, float x, uint32_t tag) {
+  asm volatile("st.relaxed.gpu.global.b64 [%0], %1;" ::"l"(p), "l"(((uint64_t)tag << 32) | __float_as_uint(x)) : "memory");
+}
+__device__ __forceinline__ uint64_t sink_get(const uint64_t* p) {
+  uint64_t w;
+  asm volatile("ld.relaxed.gpu.global.b64 %0, [%1];" : "=l"(w) : "l"(p) : "memory");
+  return w;
+}
+// x[u] = the value at at(u) once its tag is `tag` (0 where at(u) is null).  The N loads are in flight together, and so are the
+// reloads of the words that were not ready: a wait costs one memory round trip, not one per word.  SINK_POLL covers the
+// (m + 1) / 256 <= 9 words of v a thread reads for m <= 2048, and the strips a thread sums at the plan's strip counts.
+constexpr int SINK_POLL = 16;
+template <int N, class At>
+__device__ __forceinline__ void sink_take(float (&x)[N], At at, uint32_t tag) {
+  uint64_t w[N];
+#pragma unroll
+  for (int u = 0; u < N; ++u) { const uint64_t* p = at(u); w[u] = p ? sink_get(p) : (uint64_t)tag << 32; }
+  for (;;) {
+    bool ready = true;
+#pragma unroll
+    for (int u = 0; u < N; ++u) ready &= (uint32_t)(w[u] >> 32) == tag;
+    if (ready) break;
+#pragma unroll
+    for (int u = 0; u < N; ++u)
+      if ((uint32_t)(w[u] >> 32) != tag) w[u] = sink_get(at(u));
+  }
+#pragma unroll
+  for (int u = 0; u < N; ++u) x[u] = __uint_as_float((uint32_t)w[u]);
+}
+
+// The resident kernel: the streaming kernel's sweep over score rows held on chip.  Its CTAs (one per SM) load their strip's rows
+// once, in the first sweep, through a one-slot ring (in the space of the column sums, which the first sweep does not use before
+// its rows are in): a warp keeps its first RR rows in registers (RR V float4s per lane, fully unrolled, so only compile-time
+// indices) and the rest in shared memory (`held`), so each score matrix is read from HBM once per launch instead of once per
+// sweep.  The iterations are sink_fwd_row as in the streaming kernel.  The strips number up to the SM count, so instead of every
+// CTA summing every strip's partial (SP partials of the pair per CTA and iteration from L2) each strip sums the partials of its
+// own 1/SP of the columns in a fixed order and publishes v there (vglob), and every CTA of the pair reads v back.  Partials and v
+// travel as (value, iteration + 1) words (sink_put / sink_take), so a reader waits for exactly the words it needs and the pair
+// needs no barrier: a strip writes its next partials only after it has read all of v, which every owner publishes only after it
+// has read all partials of its columns, so one buffer of each suffices.  Both are zeroed before each launch.
+template <int V, int W, int RR>
+__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(SinkArgs a) {
+  extern __shared__ __align__(128) float og_sink_smem[];
+  using Strip = SinkStrip<V, W>;
+  constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G, NT = SINK_WARPS * 32;
+  float* v_s = og_sink_smem;                                              // [MC + 4]  as in sinkhorn_kernel
+  float* red = v_s + MC + 4;                                              // [G][mpad], or the ring [SINK_WARPS][1][C] in sweep 0
+  float* ring = red;
+  float* gsum = red + max(G * a.mpad, SINK_WARPS * C);                   // [NT]  per-group sums of a strip's columns
+  float4* held = reinterpret_cast<float4*>(gsum + NT);                    // [SINK_WARPS][rows_smem][C / 4]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(held + (size_t)SINK_WARPS * a.rows_smem * (C / 4));   // [SINK_WARPS]
+  float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS);             // [2][G][W]
+  const Strip s(a);
+  const int m = a.m, lane = s.lane;
+  const float a_reg = expf(a.norm), a_last = expf(a.log_a_last);
+  SinkRowRing<V, W, 1, true, SinkArgs> rows(a, s, ring, bars);
+  const float dz = rows.dz;
+  float4* mine = held + (size_t)(s.grp * W + s.sub) * a.rows_smem * (C / 4);
+  uint64_t* vg = reinterpret_cast<uint64_t*>(a.vglob) + (int64_t)s.b * a.mpad;
+
+  for (int j = s.tid; j < MC; j += blockDim.x) v_s[j] = (j < m) ? 0.f : -CUDART_INF_F;
+  if (s.tid == 0) v_s[MC] = 0.f;
+  __syncthreads();
+
+  rows.prime();
+  uint32_t rowpar = 0;
+  float4 zr[RR][V];                                    // the warp's rows r0 + grp + k G, k < RR
+  for (int it = 0; it <= a.iters; ++it) {             // it == iters: the final pass
+    const bool last = it == a.iters;
+    f32x2 cacc[2 * V];
+#pragma unroll
+    for (int k = 0; k < 2 * V; ++k) cacc[k] = 0ull;
+    float cacc_m = 0.f;
+    const float v_m = v_s[MC];
+    auto visit = [&](int row, const float4 (&q)[V]) {
+      if (last) sink_fwd_score_row(a, s, q, v_s, v_m, dz, row);
+      else sink_fwd_row(a, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
+    };
+#pragma unroll
+    for (int k = 0; k < RR; ++k) {
+      const int row = s.r0 + s.grp + k * G;
+      if (row < s.r1) {
+        if (it == 0) rows.take(row, zr[k]);
+        visit(row, zr[k]);
+      }
+    }
+    float4* h = mine;
+    for (int row = s.r0 + s.grp + RR * G; row < s.r1; row += G, h += C / 4) {
+      float4 q[V];
+      if (it == 0) {
+        rows.take(row, q);
+#pragma unroll
+        for (int k = 0; k < V; ++k) h[lane + 32 * k] = q[k];
+      } else {
+#pragma unroll
+        for (int k = 0; k < V; ++k) q[k] = h[lane + 32 * k];
+      }
+      visit(row, q);
+    }
+    if (last) break;
+
+    float4 c4[V];
+#pragma unroll
+    for (int k = 0; k < V; ++k) { upk2(cacc[2 * k], c4[k].x, c4[k].y); upk2(cacc[2 * k + 1], c4[k].z, c4[k].w); }
+    if (it == 0) __syncthreads();                      // every warp has taken its last row from the ring: `red` is free
+    const uint32_t tag = it + 1;
+    uint64_t* pt = reinterpret_cast<uint64_t*>(a.partial) + (int64_t)s.b * a.SP * a.mpad;
+    sink_strip_sums(a, s, red, c4, cacc_m, [&](int j, float sum) { sink_put(pt + (int64_t)s.strip * a.mpad + j, sum, tag); });
+    // this strip's columns [lo, lo + S): NG thread groups sum strips g, g + NG, ... of a column, then the groups are added in
+    // order (a fixed order: the same bits in every run)
+    const int S = cdiv(m + 1, a.SP), lo = s.strip * S, NG = S >= NT ? 1 : NT / S;
+    auto publish = [&](int j, float c) {
+      sink_put(vg + j, ((j < m) ? a.norm + v_s[j] : a.log_b_last + v_s[MC]) - logf(c), tag);
+    };
+    for (int i = s.tid; i < S * NG; i += NT) {
+      const int j = lo + i % S;
+      float sum = 0.f;
+      if (j <= m) {
+        for (int sp0 = i / S; sp0 < a.SP; sp0 += SINK_POLL * NG) {
+          float x[SINK_POLL];
+          sink_take<SINK_POLL>(x, [&](int u) { const int sp = sp0 + u * NG; return sp < a.SP ? pt + (int64_t)sp * a.mpad + j : nullptr; }, tag);
+#pragma unroll
+          for (int u = 0; u < SINK_POLL; ++u) sum += x[u];
+        }
+      }
+      if (NG > 1) gsum[i] = sum;
+      else if (j <= m) publish(j, sum);
+    }
+    if (NG > 1) {
+      __syncthreads();
+      for (int i = s.tid; i < S && lo + i <= m; i += NT) {
+        float sum = gsum[i];
+        for (int g = 1; g < NG; ++g) sum += gsum[g * S + i];
+        publish(lo + i, sum);
+      }
+    }
+    for (int j0 = s.tid; j0 <= m; j0 += SINK_POLL * NT) {
+      float x[SINK_POLL];
+      sink_take<SINK_POLL>(x, [&](int u) { const int j = j0 + u * NT; return j <= m ? vg + j : nullptr; }, tag);
+#pragma unroll
+      for (int u = 0; u < SINK_POLL; ++u) {
+        const int j = j0 + u * NT;
+        if (j <= m) v_s[(j < m) ? j : MC] = x[u];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// resident: the plan is for sinkhorn_resident_kernel (slots = 1, occ = 1); rows_reg / rows_smem: rows per warp in registers /
+// in shared memory
+struct SinkPlan { int V, W, slots, occ, SP, rows_per_strip, mpad, pairs_per_launch; size_t smem; bool resident; int rows_reg, rows_smem; };
 
 // Dynamic shared memory of one CTA: the column vectors of MC + 4 floats (forward: v; backward: cvec, vbar, wq), the row groups'
 // column sums [G][mpad], the row ring [SINK_WARPS][slots][C] and its mbarriers, the row exchange [2][G][W] (forward: (max, sum);
@@ -439,6 +618,54 @@ inline int sinkhorn_plan(bool backward, int B, int n, int m, SinkPlan* p) {
   return OG_OK;
 }
 
+// Dynamic shared memory of a resident CTA: v [MC + 4], the row groups' column sums [G][mpad] sharing their space with the one-slot
+// row ring [SINK_WARPS][C], the column groups' sums [256] float4, the held rows [SINK_WARPS][rows_smem][C], the mbarriers, the row
+// exchange and 128 bytes.
+constexpr size_t sinkhorn_resident_smem(int V, int W, int mpad, int rows_smem) {
+  const int C = 128 * V, G = SINK_WARPS / W;
+  return ((size_t)(W * C + 4) + (size_t)std::max(G * mpad, SINK_WARPS * C) + 4 * SINK_WARPS * 32 +
+          (size_t)SINK_WARPS * rows_smem * C) * sizeof(float) +
+         SINK_WARPS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float2) + 128;
+}
+
+// The resident plan, where it fits and pays: the bands up to 2048 columns (V <= 8; RR = 24 / V rows per warp in registers, 96
+// registers per thread: 32 / V spill), as many rows per warp in shared memory as the opt-in limit leaves, at most one CTA per SM,
+// a pair on at most half the SMs.  The pairs are spread evenly over the launches and each pair of a launch over as many SMs as
+// the launch leaves it.  One launch always pays: the streaming kernel leaves most SMs idle there.  Over several launches the
+// resident kernel is taken only where its modelled sweep time, over all launches, beats the streaming kernel's 2.7 TB/s.  Both
+// rates were measured on an H100 80GB HBM3 (700 W) with og_sinkhorn_fwd: a resident sweep takes about 3.8 us (exchanges) +
+// R (0.4 + 0.0625 V) us for R rows per warp (8 rows of 2048 columns: 11.0 us; 17 rows of 1024: 14.0 us), so 16 pairs of
+// 2048 x 2048 (eight launches) run resident in 8.9 ms against 9.9 ms streaming, while 32 pairs of 1024 x 1024 (four launches,
+// 5.6 ms against 5.0 ms) stream.  Returns false where the streaming kernel runs instead.
+inline bool sinkhorn_resident_plan(int B, int n, int m, SinkPlan* p) {
+  if (m > 2048 || sinkhorn_plan(false, B, n, m, p) != OG_OK) return false;
+  const int G = SINK_WARPS / p->W, rr = 24 / p->V, C = 128 * p->V;
+  const int sms = device_info().ok ? device_info().sm_count : 132;
+  const int rs_max = (int)((OG_SMEM_OPTIN_MAX - sinkhorn_resident_smem(p->V, p->W, p->mpad, 0)) / (SINK_WARPS * C * sizeof(float)));
+  const int sp_min = cdiv(n + 1, G * (rr + rs_max));  // strips a pair needs
+  if (2 * sp_min > sms) return false;
+  const int rounds = cdiv(B, std::min(B, sms / sp_min));
+  p->pairs_per_launch = cdiv(B, rounds);
+  const int sp = std::min(sms / p->pairs_per_launch, cdiv(n + 1, G));
+  p->rows_per_strip = cdiv(n + 1, sp);
+  p->SP = cdiv(n + 1, p->rows_per_strip);
+  const int rows_per_warp = cdiv(p->rows_per_strip, G);
+  const double resident_us = rounds * (3.8 + rows_per_warp * (0.4 + 0.0625 * p->V));
+  const double streaming_us = 4.0 * B * (n + 1) * (m + 1) / 2.7e6;
+  if (rounds > 1 && resident_us >= streaming_us) return false;
+  p->rows_reg = rr;
+  p->rows_smem = std::max(0, rows_per_warp - rr);
+  p->smem = sinkhorn_resident_smem(p->V, p->W, p->mpad, p->rows_smem);
+  p->slots = 1; p->occ = 1; p->resident = true;
+  return true;
+}
+
+// OG_SINK_RESIDENT=0 runs every forward Sinkhorn on the streaming kernel; 1 (default): the resident kernel where its plan fits.
+inline int& sink_resident_mode() {
+  static int v = [] { const char* e = getenv("OG_SINK_RESIDENT"); return e ? (atoi(e) != 0) : 1; }();
+  return v;
+}
+
 inline int sinkhorn_check_rows(const char* who, const float* S, int64_t lds, int64_t strideS, int m) {
   if (lds % 4 != 0 || lds < m || !aligned16(S) || strideS % 4 != 0)
     return fail(OG_EINVAL, "%s: S rows must be 16-byte aligned (lds %% 4 == 0, lds >= m)", who);
@@ -475,17 +702,34 @@ inline int sinkhorn_for_each_launch(const SinkPlan& p, int B, unsigned int* barr
   return OG_OK;
 }
 
+// The larger of the two kernels' needs, whichever the switch selects: rows of mpad floats after the barriers and u are the strip
+// partials [2][B][SINK_MAX_STRIPS] (streaming) or, as 64-bit words, [pairs_per_launch][SP] and then vglob [pairs_per_launch]
+// (resident).
 inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
-  SinkPlan p;
+  SinkPlan p, r;
   if (sinkhorn_plan(false, B, n, m, &p) != OG_OK) return -1;
-  return SINK_BARRIER_BYTES + align_up((int64_t)B * (n + 1) * 4, 256) + align_up(2LL * B * SINK_MAX_STRIPS * p.mpad * 4, 256);
+  int64_t rows = 2LL * B * SINK_MAX_STRIPS;
+  if (sinkhorn_resident_plan(B, n, m, &r)) rows = std::max<int64_t>(rows, 2LL * (r.SP + 1) * r.pairs_per_launch);
+  return SINK_BARRIER_BYTES + align_up((int64_t)B * (n + 1) * 4, 256) + align_up(rows * p.mpad * 4, 256);
+}
+
+template <int V, int W>
+inline int sinkhorn_resident_launch(const SinkArgs& a, const SinkPlan& p, cudaStream_t stream) {
+  constexpr auto kernel = sinkhorn_resident_kernel<V, W, 24 / V>;
+  if (const int rc = smem_opt_in<kernel>((int)OG_SMEM_OPTIN_MAX)) return rc;
+  return launch("sinkhorn_resident_kernel", kernel, LaunchAttr::cooperative, dim3(a.B * a.SP), dim3(SINK_WARPS * 32), p.smem,
+                stream, a);
 }
 
 inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int B, int n, int m,
                            int iters, float reg, float* scores, void* ws, int64_t ws_bytes, cudaStream_t stream,
                            float* hist_u = nullptr, float* hist_v = nullptr) {
   SinkPlan p;
-  if (const int rc = sinkhorn_plan(false, B, n, m, &p)) return rc;
+  const bool resident = !hist_u && !hist_v && sink_resident_mode() && sinkhorn_resident_plan(B, n, m, &p);
+  if (!resident) {
+    if (const int rc = sinkhorn_plan(false, B, n, m, &p)) return rc;
+    p.resident = false;
+  }
   if (ws_bytes < sinkhorn_workspace_bytes(B, n, m)) return fail(OG_EWORKSPACE, "sinkhorn: workspace too small");
   if (const int rc = sinkhorn_check_rows("sinkhorn", S, lds, strideS, m)) return rc;
   char* w = static_cast<char*>(ws);
@@ -502,8 +746,15 @@ inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const f
     a.scores = scores + (int64_t)b0 * (n + 1) * (m + 1);
     a.u = u; a.partial = partial; a.barrier = barrier;
     a.SP = p.SP; a.rows_per_strip = p.rows_per_strip; a.mpad = p.mpad;
+    a.rows_smem = p.resident ? p.rows_smem : 0;
+    a.vglob = partial + 2LL * p.pairs_per_launch * p.SP * p.mpad;
+    if (p.resident) OG_CUDA(cudaMemsetAsync(partial, 0, 8LL * (p.SP + 1) * p.pairs_per_launch * p.mpad, stream));
     a.hist_u = hist_u ? hist_u + (int64_t)b0 * iters * (n + 1) : nullptr;
     a.hist_v = hist_v ? hist_v + (int64_t)b0 * (iters + 1) * (m + 1) : nullptr;
+    if (p.resident) {
+      if (p.W == 1) return sinkhorn_resident_launch<4, 1>(a, p, stream);
+      return p.V == 4 ? sinkhorn_resident_launch<4, 2>(a, p, stream) : sinkhorn_resident_launch<8, 2>(a, p, stream);
+    }
     if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<sinkhorn_kernel<4, 1, 2>, 4, 1, 2>(a, p, stream);
     if (p.V == 4)             return sinkhorn_coop_launch<sinkhorn_kernel<4, 2, 2>, 4, 2, 2>(a, p, stream);
     if (p.V == 8)             return sinkhorn_coop_launch<sinkhorn_kernel<8, 2, 2>, 8, 2, 2>(a, p, stream);

@@ -1,0 +1,102 @@
+"""Time og_sinkhorn_fwd with the resident kernel against the streaming kernel, the two alternating in one process.
+
+    python tools/sinkhorn_timing.py [--launches 20] [--rounds 3] [--out DIR]
+
+For each shape (the BASELINE workloads' Sinkhorn, and one pair at the headline size) it prints the plan of each form, the median
+over `rounds` rounds of the mean CUDA-event time of `launches` back-to-back launches, the largest score difference between the
+two forms and whether two resident launches gave identical bits.  Needs a CUDA device."""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import os
+import statistics
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from openglue_b200 import _cabi  # noqa: E402
+from openglue_b200._cabi import ptr, stream  # noqa: E402
+
+# (label, pairs, n, m, iterations)
+SHAPES = [('C3', 16, 2048, 2048, 100), ('C2', 32, 1024, 1024, 100), ('C5', 1, 4096, 1024, 50), ('C1', 1, 512, 512, 20),
+          ('1 pair 2048', 1, 2048, 2048, 100)]
+
+
+def plan(lib, B, n, m):
+    out = (C.c_int64 * 10)()
+    _cabi.check(lib.og_sinkhorn_plan(B, n, m, out), 'og_sinkhorn_plan')
+    keys = ['resident', 'V', 'W', 'strips', 'rows_per_strip', 'pairs_per_launch', 'rows_reg', 'rows_smem', 'smem', 'occ']
+    return dict(zip(keys, list(out)))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--launches', type=int, default=20)
+    ap.add_argument('--rounds', type=int, default=3)
+    ap.add_argument('--out', default=None)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), 'needs a CUDA device'
+    smi = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                         capture_output=True, text=True).stdout.strip()
+    print('device:', smi)
+    lib = _cabi.lib()
+    dev = 'cuda:0'
+    results = []
+    for label, B, n, m, T in SHAPES:
+        g = torch.Generator(device=dev).manual_seed(7)
+        lds = (m + 3) // 4 * 4
+        S = torch.randn(B, n, lds, device=dev, generator=g) * 4
+        dust = torch.ones(1, device=dev)
+        wsb = lib.og_sinkhorn_workspace_bytes(B, n, m)
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        outs = {1: torch.empty(B, n + 1, m + 1, device=dev), 0: torch.empty(B, n + 1, m + 1, device=dev)}
+
+        def run(mode, out):
+            lib.og_set_sinkhorn_resident(mode)
+            _cabi.check(lib.og_sinkhorn_fwd(ptr(S), lds, n * lds, ptr(dust), B, n, m, T, 1.0, ptr(out), ptr(ws), wsb, stream()),
+                        'og_sinkhorn_fwd')
+
+        plans = {}
+        for mode in (1, 0):
+            lib.og_set_sinkhorn_resident(mode)
+            plans[mode] = plan(lib, B, n, m)
+            run(mode, outs[mode])
+        again = torch.empty_like(outs[1])
+        run(1, again)
+        torch.cuda.synchronize()
+        times = {1: [], 0: []}
+        for _ in range(args.rounds):
+            for mode in (1, 0):
+                lib.og_set_sinkhorn_resident(mode)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(args.launches):
+                    run(mode, outs[mode])
+                e1.record()
+                e1.synchronize()
+                times[mode].append(e0.elapsed_time(e1) / args.launches)
+        lib.og_set_sinkhorn_resident(1)
+        r = {'shape': label, 'pairs': B, 'n': n, 'm': m, 'iters': T,
+             'ms_resident': statistics.median(times[1]), 'ms_streaming': statistics.median(times[0]),
+             'ms_resident_rounds': times[1], 'ms_streaming_rounds': times[0],
+             'max_abs_diff': float((outs[1] - outs[0]).abs().max()), 'resident_bit_identical': bool(torch.equal(outs[1], again)),
+             'plan_resident': plans[1], 'plan_streaming': plans[0]}
+        r['hbm_gbs_streaming'] = (T + 1) * 4 * (n + 1) * (m + 1) * B / (r['ms_streaming'] * 1e-3) / 1e9
+        print(f"{label:12s} B={B:3d} {n}x{m} T={T:3d}: resident {r['ms_resident']:.3f} ms, streaming {r['ms_streaming']:.3f} ms "
+              f"({r['ms_streaming'] / r['ms_resident']:.2f}x), max|d| {r['max_abs_diff']:.2e}, "
+              f"deterministic {r['resident_bit_identical']}, plan {plans[1]}")
+        results.append(r)
+        del S, ws, outs, again
+        torch.cuda.empty_cache()
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, 'sinkhorn_timing.json'), 'w') as f:
+            json.dump({'device': smi, 'launches': args.launches, 'rounds': args.rounds, 'results': results}, f, indent=1)
+
+
+if __name__ == '__main__':
+    main()
