@@ -27,6 +27,7 @@
 #include "tc_common.cuh"
 #include <math_constants.h>
 #include <algorithm>
+#include <type_traits>
 
 namespace og {
 
@@ -284,62 +285,105 @@ __device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStri
   __syncthreads();
 }
 
-// One row of a forward sweep (iteration `it`) from this warp's segment q of it: t = z + v, the row's (max, sum) over the W warps of
-// its group, u_i (stored in the last iteration and in hist_u when recorded) and the row's share e_ij a_i / S_i of the column
-// sums, added to cacc (cacc_m: the dustbin column, counted by segment 0).  v_s: v of the pair in shared memory, v_m = v_s[MC].
-template <int V, int W>
-__device__ __forceinline__ void sink_fwd_row(const SinkArgs& a, const SinkStrip<V, W>& s, const float4 (&q)[V], const float* v_s,
-                                             float v_m, float dz, float a_reg, float a_last, float2* xr, uint32_t& rowpar, int row,
-                                             int it, f32x2 (&cacc)[2 * V], float& cacc_m) {
+// What a warp publishes in the row exchange of NR rows: (max, sum) of its segment of each row.
+template <int NR> using SinkRowStat = std::conditional_t<NR == 1, float2, float4>;
+
+// NR (1 or 2) rows of a forward sweep (iteration `it`), rows row0 and row0 + G, from this warp's segments q[r] of them: t = z + v,
+// each row's (max, sum) over the W warps of its group, u_i (stored in the last iteration and in hist_u when recorded) and the row's
+// share e_ij a_i / S_i of the column sums, added to cacc (cacc_m: the dustbin column, counted by segment 0) row by row in order.
+// v_s: v of the pair in shared memory, v_m = v_s[MC].  Two rows share one read of v and one exchange, and their reduction chains
+// are independent, so one row's shuffles run under the other's exponentials; each row's arithmetic is the same for NR = 1 and 2.
+template <int V, int W, int NR>
+__device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkStrip<V, W>& s, const float4 (*q)[V], const float* v_s,
+                                              float v_m, float dz, float a_reg, float a_last, SinkRowStat<NR>* xr, uint32_t& rowpar,
+                                              int row0, int it, f32x2 (&cacc)[2 * V], float& cacc_m) {
+  static_assert(NR == 1 || NR == 2, "one or two rows at a time");
   const int n = a.n, c0 = s.c0, lane = s.lane, sub = s.sub;
   const f32x2 log2e2 = pk2(LOG2E_F, LOG2E_F);
-  f32x2 z[2 * V];
+  f32x2 z[NR][2 * V];
 #pragma unroll
-  for (int k = 0; k < V; ++k) { z[2 * k] = pk2(q[k].x, q[k].y); z[2 * k + 1] = pk2(q[k].z, q[k].w); }
+  for (int r = 0; r < NR; ++r)
+#pragma unroll
+    for (int k = 0; k < V; ++k) { z[r][2 * k] = pk2(q[r][k].x, q[r][k].y); z[r][2 * k + 1] = pk2(q[r][k].z, q[r][k].w); }
   // t = z + v, masked; maximum over this warp's segment (the dustbin column entry belongs to segment 0)
   const float t_m = dz + v_m;
-  float mx = (sub == 0) ? t_m : -CUDART_INF_F;
+  float mx[NR];
+#pragma unroll
+  for (int r = 0; r < NR; ++r) mx[r] = (sub == 0) ? t_m : -CUDART_INF_F;
 #pragma unroll
   for (int k = 0; k < V; ++k) {
     const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(v_s + c0 + 4 * (lane + 32 * k));   // columns >= m: finite z + (-inf) = -inf, e = 0
-    z[2 * k] = add2(z[2 * k], vv.x); z[2 * k + 1] = add2(z[2 * k + 1], vv.y);
-    float x0, x1, x2, x3; upk2(z[2 * k], x0, x1); upk2(z[2 * k + 1], x2, x3);
-    mx = fmaxf(mx, fmaxf(fmaxf(x0, x1), fmaxf(x2, x3)));
-  }
-  mx = warp_max(mx);
-  const float mxs = (mx == -CUDART_INF_F) ? 0.f : mx;               // an all-padding segment: e = 2^-inf = 0, not NaN
-  const f32x2 mxs2 = pk2(mxs, mxs);
-  f32x2 sum2a = 0ull, sum2b = 0ull;
 #pragma unroll
-  for (int k = 0; k < 2 * V; ++k) {
-    float x, y; upk2(mul2(sub2(z[k], mxs2), log2e2), x, y);
-    z[k] = pk2(ex2_approx(x), ex2_approx(y));
-    if (k & 1) sum2b = add2(sum2b, z[k]); else sum2a = add2(sum2a, z[k]);
+    for (int r = 0; r < NR; ++r) {
+      z[r][2 * k] = add2(z[r][2 * k], vv.x); z[r][2 * k + 1] = add2(z[r][2 * k + 1], vv.y);
+      float x0, x1, x2, x3; upk2(z[r][2 * k], x0, x1); upk2(z[r][2 * k + 1], x2, x3);
+      mx[r] = fmaxf(mx[r], fmaxf(fmaxf(x0, x1), fmaxf(x2, x3)));
+    }
   }
-  float sa, sb; upk2(add2(sum2a, sum2b), sa, sb);
-  const float e_m = (sub == 0) ? ex2_approx((t_m - mxs) * LOG2E_F) : 0.f;
-  float s_i = warp_sum(sa + sb) + e_m;
-  float mxg = mx, f_w = 1.f;
-  if (W > 1) {                                     // combine the segments of the row: S = sum_w S_w 2^(mx_w - mx)
-    const float2* x = sink_row_exchange(xr, make_float2(mx, s_i), s, rowpar);
-    float2 p[W];
 #pragma unroll
-    for (int w2 = 0; w2 < W; ++w2) { p[w2] = x[w2]; mxg = fmaxf(mxg, p[w2].x); }
-    s_i = 0.f;
+  for (int r = 0; r < NR; ++r) mx[r] = warp_max(mx[r]);
+  float s_i[NR], e_m[NR];
 #pragma unroll
-    for (int w2 = 0; w2 < W; ++w2) s_i = fmaf(p[w2].y, ex2_approx((p[w2].x - mxg) * LOG2E_F), s_i);   // fixed order: identical in every warp
-    f_w = ex2_approx((mx - mxg) * LOG2E_F);
+  for (int r = 0; r < NR; ++r) {
+    const float mxs = (mx[r] == -CUDART_INF_F) ? 0.f : mx[r];      // an all-padding segment: e = 2^-inf = 0, not NaN
+    const f32x2 mxs2 = pk2(mxs, mxs);
+    f32x2 sum2a = 0ull, sum2b = 0ull;
+#pragma unroll
+    for (int k = 0; k < 2 * V; ++k) {
+      float x, y; upk2(mul2(sub2(z[r][k], mxs2), log2e2), x, y);
+      z[r][k] = pk2(ex2_approx(x), ex2_approx(y));
+      if (k & 1) sum2b = add2(sum2b, z[r][k]); else sum2a = add2(sum2a, z[r][k]);
+    }
+    float sa, sb; upk2(add2(sum2a, sum2b), sa, sb);
+    s_i[r] = sa + sb;
+    e_m[r] = (sub == 0) ? ex2_approx((t_m - mxs) * LOG2E_F) : 0.f;
   }
-  const float w_i = __fdiv_rn((row < n) ? a_reg : a_last, s_i) * f_w;
+#pragma unroll
+  for (int r = 0; r < NR; ++r) s_i[r] = warp_sum(s_i[r]) + e_m[r];
+  float mxg[NR], f_w[NR];
+#pragma unroll
+  for (int r = 0; r < NR; ++r) { mxg[r] = mx[r]; f_w[r] = 1.f; }
+  if (W > 1) {                                     // combine the segments of each row: S = sum_w S_w 2^(mx_w - mx)
+    SinkRowStat<NR> mine;
+    if constexpr (NR == 1) mine = make_float2(mx[0], s_i[0]);
+    else mine = make_float4(mx[0], s_i[0], mx[1], s_i[1]);
+    const SinkRowStat<NR>* x = sink_row_exchange(xr, mine, s, rowpar);
+    float pm[NR][W], ps[NR][W];
+#pragma unroll
+    for (int w2 = 0; w2 < W; ++w2) {
+      const SinkRowStat<NR> p = x[w2];
+      pm[0][w2] = p.x; ps[0][w2] = p.y;
+      if constexpr (NR == 2) { pm[1][w2] = p.z; ps[1][w2] = p.w; }
+    }
+#pragma unroll
+    for (int r = 0; r < NR; ++r) {
+#pragma unroll
+      for (int w2 = 0; w2 < W; ++w2) mxg[r] = fmaxf(mxg[r], pm[r][w2]);
+      s_i[r] = 0.f;
+#pragma unroll
+      for (int w2 = 0; w2 < W; ++w2) s_i[r] = fmaf(ps[r][w2], ex2_approx((pm[r][w2] - mxg[r]) * LOG2E_F), s_i[r]);   // fixed order: identical in every warp
+      f_w[r] = ex2_approx((mx[r] - mxg[r]) * LOG2E_F);
+    }
+  }
+  float w_i[NR];
+#pragma unroll
+  for (int r = 0; r < NR; ++r) w_i[r] = __fdiv_rn((row0 + r * SinkStrip<V, W>::G < n) ? a_reg : a_last, s_i[r]) * f_w[r];
   if ((it == a.iters - 1 || a.hist_u) && sub == 0 && lane == 0) {
-    const float u_i = ((row < n) ? a.norm : a.log_a_last) - (mxg + logf(s_i));
-    if (it == a.iters - 1) a.u[(int64_t)s.b * (n + 1) + row] = u_i;
-    if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (n + 1) + row] = u_i;
-  }
-  const f32x2 w2 = pk2(w_i, w_i);
 #pragma unroll
-  for (int k = 0; k < 2 * V; ++k) cacc[k] = fma2(z[k], w2, cacc[k]);
-  cacc_m = fmaf(e_m, w_i, cacc_m);
+    for (int r = 0; r < NR; ++r) {
+      const int row = row0 + r * SinkStrip<V, W>::G;
+      const float u_i = ((row < n) ? a.norm : a.log_a_last) - (mxg[r] + logf(s_i[r]));
+      if (it == a.iters - 1) a.u[(int64_t)s.b * (n + 1) + row] = u_i;
+      if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (n + 1) + row] = u_i;
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < NR; ++r) {
+    const f32x2 w2 = pk2(w_i[r], w_i[r]);
+#pragma unroll
+    for (int k = 0; k < 2 * V; ++k) cacc[k] = fma2(z[r][k], w2, cacc[k]);
+    cacc_m = fmaf(e_m[r], w_i[r], cacc_m);
+  }
 }
 
 // The final pass over one row: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111)
@@ -402,7 +446,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
     for (int row = s.r0 + s.grp; row < s.r1; row += G) {
       float4 q[V];
       rows.take(row, q);
-      sink_fwd_row(a, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
+      sink_fwd_rows<V, W, 1>(a, s, &q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
     }
     rows.prime();                                      // next sweep's (or the final pass's) first rows fly during the reduction
     float4 c4[V];
@@ -457,34 +501,77 @@ __device__ __forceinline__ void sink_take(float (&x)[N], At at, uint32_t tag) {
   for (int u = 0; u < N; ++u) x[u] = __uint_as_float((uint32_t)w[u]);
 }
 
+// The resident kernel's form of sink_strip_sums, in half the shared memory: the upper half of the row groups parks its column sums
+// in red [G/2][mpad] (the dustbin column in redm [G]), the lower half adds its own to them, and store(j, sum) gets the G/2 folded
+// sums added in order (a fixed order: the same bits in every run).
+template <int V, int W, class Args, class Store>
+__device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const SinkStrip<V, W>& s, float* red, float* redm,
+                                                       const float4 (&cacc)[V], float cacc_m, Store store) {
+  constexpr int H = SinkStrip<V, W>::G / 2;
+  const int m = a.m;
+  float4* fold = reinterpret_cast<float4*>(red + (s.grp % H) * a.mpad);
+  if (s.grp >= H) {
+#pragma unroll
+    for (int q = 0; q < V; ++q) {
+      const int c = s.c0 + 4 * (s.lane + 32 * q);
+      if (c < m) fold[c / 4] = cacc[q];                // entries >= m are zero
+    }
+  }
+  if (s.sub == 0 && s.lane == 0) redm[s.grp] = cacc_m;
+  __syncthreads();
+  if (s.grp < H) {
+#pragma unroll
+    for (int q = 0; q < V; ++q) {
+      const int c = s.c0 + 4 * (s.lane + 32 * q);
+      if (c < m) {
+        const float4 o = fold[c / 4];
+        fold[c / 4] = make_float4(cacc[q].x + o.x, cacc[q].y + o.y, cacc[q].z + o.z, cacc[q].w + o.w);
+      }
+    }
+  }
+  __syncthreads();
+  for (int j = s.tid; j <= m; j += blockDim.x) {
+    float sum = 0.f;
+#pragma unroll
+    for (int h = 0; h < H; ++h) sum += (j < m) ? red[h * a.mpad + j] : redm[h] + redm[h + H];
+    store(j, sum);
+  }
+}
+
 // The resident kernel: the streaming kernel's sweep over score rows held on chip.  Its CTAs (one per SM) load their strip's rows
-// once, in the first sweep, through a one-slot ring (in the space of the column sums, which the first sweep does not use before
-// its rows are in): a warp keeps its first RR rows in registers (RR V float4s per lane, fully unrolled, so only compile-time
-// indices) and the rest in shared memory (`held`), so each score matrix is read from HBM once per launch instead of once per
-// sweep.  The iterations are sink_fwd_row as in the streaming kernel.  The strips number up to the SM count, so instead of every
-// CTA summing every strip's partial (SP partials of the pair per CTA and iteration from L2) each strip sums the partials of its
-// own 1/SP of the columns in a fixed order and publishes v there (vglob), and every CTA of the pair reads v back.  Partials and v
-// travel as (value, iteration + 1) words (sink_put / sink_take), so a reader waits for exactly the words it needs and the pair
-// needs no barrier: a strip writes its next partials only after it has read all of v, which every owner publishes only after it
-// has read all partials of its columns, so one buffer of each suffices.  Both are zeroed before each launch.
+// once, in the first sweep, through a one-slot ring: a warp keeps its first RR rows in registers (RR V float4s per lane, fully
+// unrolled, so only compile-time indices) and the rest in shared memory (`held`, [slots][SINK_WARPS][C]), so each score matrix is
+// read from HBM once per launch instead of once per sweep.  The ring is the warp's last held slot, which its last row fills (a
+// dedicated slot where no row is held in shared memory).  After the first sweep a warp works on its rows two at a time
+// (sink_fwd_rows<2>: rows k and k + 1 of the warp, one read of v, one exchange, the two rows' reduction chains interleaved), an odd
+// last row alone; the first sweep and the final score pass go one row at a time.  The rows are added into the column sums in the
+// same order either way.  RR is even, so a pair never straddles registers and shared memory.  The strips number up to the SM
+// count, so instead of every CTA summing every strip's partial (SP partials of the pair per CTA and iteration from L2) each strip
+// sums the partials of its own 1/SP of the columns in a fixed order and publishes v there (vglob), and every CTA of the pair reads
+// v back.  Partials and v travel as (value, iteration + 1) words (sink_put / sink_take), so a reader waits for exactly the words it
+// needs and the pair needs no barrier: a strip writes its next partials only after it has read all of v, which every owner
+// publishes only after it has read all partials of its columns, so one buffer of each suffices.  Both are zeroed before each launch.
 template <int V, int W, int RR>
 __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(SinkArgs a) {
+  static_assert(RR % 2 == 0, "the register rows go two at a time");
   extern __shared__ __align__(128) float og_sink_smem[];
   using Strip = SinkStrip<V, W>;
-  constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G, NT = SINK_WARPS * 32;
+  constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G, NT = SINK_WARPS * 32, HS = SINK_WARPS * (C / 4);
+  const int slots = max(a.rows_smem, 1);
   float* v_s = og_sink_smem;                                              // [MC + 4]  as in sinkhorn_kernel
-  float* red = v_s + MC + 4;                                              // [G][mpad], or the ring [SINK_WARPS][1][C] in sweep 0
-  float* ring = red;
-  float* gsum = red + max(G * a.mpad, SINK_WARPS * C);                   // [NT]  per-group sums of a strip's columns
-  float4* held = reinterpret_cast<float4*>(gsum + NT);                    // [SINK_WARPS][rows_smem][C / 4]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(held + (size_t)SINK_WARPS * a.rows_smem * (C / 4));   // [SINK_WARPS]
-  float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS);             // [2][G][W]
+  float* red = v_s + MC + 4;                                              // [G / 2][mpad]
+  float* gsum = red + G / 2 * a.mpad;                                     // [NT]  per-group sums of a strip's columns
+  float4* held = reinterpret_cast<float4*>(gsum + NT);                    // [slots][SINK_WARPS][C / 4]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(held + (size_t)slots * HS);   // [SINK_WARPS]
+  float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS);             // [2][G][W]  one row's (max, sum)
+  float4* xr2 = reinterpret_cast<float4*>(xr + 2 * G * W);               // [2][G][W]  two rows'
+  float* redm = reinterpret_cast<float*>(xr2 + 2 * G * W);               // [G]
   const Strip s(a);
-  const int m = a.m, lane = s.lane;
+  const int m = a.m, lane = s.lane, row0 = s.r0 + s.grp;
   const float a_reg = expf(a.norm), a_last = expf(a.log_a_last);
-  SinkRowRing<V, W, 1, true, SinkArgs> rows(a, s, ring, bars);
+  float4* mine = held + (s.grp * W + s.sub) * (C / 4);
+  SinkRowRing<V, W, 1, true, SinkArgs> rows(a, s, reinterpret_cast<float*>(held + (size_t)(slots - 1) * HS), bars);
   const float dz = rows.dz;
-  float4* mine = held + (size_t)(s.grp * W + s.sub) * a.rows_smem * (C / 4);
   uint64_t* vg = reinterpret_cast<uint64_t*>(a.vglob) + (int64_t)s.b * a.mpad;
 
   for (int j = s.tid; j < MC; j += blockDim.x) v_s[j] = (j < m) ? 0.f : -CUDART_INF_F;
@@ -493,7 +580,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
 
   rows.prime();
   uint32_t rowpar = 0;
-  float4 zr[RR][V];                                    // the warp's rows r0 + grp + k G, k < RR
+  float4 zr[RR / 2][2][V];                             // the warp's rows row0 + k G, k < RR
   for (int it = 0; it <= a.iters; ++it) {             // it == iters: the final pass
     const bool last = it == a.iters;
     f32x2 cacc[2 * V];
@@ -501,40 +588,70 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
     for (int k = 0; k < 2 * V; ++k) cacc[k] = 0ull;
     float cacc_m = 0.f;
     const float v_m = v_s[MC];
-    auto visit = [&](int row, const float4 (&q)[V]) {
-      if (last) sink_fwd_score_row(a, s, q, v_s, v_m, dz, row);
-      else sink_fwd_row(a, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
+    auto one = [&](int row, const float4 (*q)[V]) {
+      sink_fwd_rows<V, W, 1>(a, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
     };
+    if (it == 0 || last) {
+      auto visit = [&](int row, const float4 (&q)[V]) {
+        if (last) sink_fwd_score_row(a, s, q, v_s, v_m, dz, row);
+        else one(row, &q);
+      };
 #pragma unroll
-    for (int k = 0; k < RR; ++k) {
-      const int row = s.r0 + s.grp + k * G;
+      for (int k = 0; k < RR; ++k) {
+        const int row = row0 + k * G;
+        if (row < s.r1) {
+          if (it == 0) rows.take(row, zr[k / 2][k % 2]);
+          visit(row, zr[k / 2][k % 2]);
+        }
+      }
+      float4* h = mine;
+      for (int row = row0 + RR * G; row < s.r1; row += G, h += HS) {
+        float4 q[V];
+        if (it == 0) {
+          rows.take(row, q);
+#pragma unroll
+          for (int k = 0; k < V; ++k) h[lane + 32 * k] = q[k];
+        } else {
+#pragma unroll
+          for (int k = 0; k < V; ++k) q[k] = h[lane + 32 * k];
+        }
+        visit(row, q);
+      }
+      if (last) break;
+    } else {
+      auto two = [&](int row, const float4 (*q)[V]) {
+        sink_fwd_rows<V, W, 2>(a, s, q, v_s, v_m, dz, a_reg, a_last, xr2, rowpar, row, it, cacc, cacc_m);
+      };
+#pragma unroll
+      for (int k = 0; k < RR; k += 2) {
+        const int row = row0 + k * G;
+        if (row + G < s.r1) two(row, zr[k / 2]);
+        else if (row < s.r1) one(row, zr[k / 2]);
+      }
+      const float4* h = mine;
+      int row = row0 + RR * G;
+      for (; row + G < s.r1; row += 2 * G, h += 2 * HS) {
+        float4 q[2][V];
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+          for (int k = 0; k < V; ++k) q[r][k] = h[r * HS + lane + 32 * k];
+        two(row, q);
+      }
       if (row < s.r1) {
-        if (it == 0) rows.take(row, zr[k]);
-        visit(row, zr[k]);
+        float4 q[1][V];
+#pragma unroll
+        for (int k = 0; k < V; ++k) q[0][k] = h[lane + 32 * k];
+        one(row, q);
       }
     }
-    float4* h = mine;
-    for (int row = s.r0 + s.grp + RR * G; row < s.r1; row += G, h += C / 4) {
-      float4 q[V];
-      if (it == 0) {
-        rows.take(row, q);
-#pragma unroll
-        for (int k = 0; k < V; ++k) h[lane + 32 * k] = q[k];
-      } else {
-#pragma unroll
-        for (int k = 0; k < V; ++k) q[k] = h[lane + 32 * k];
-      }
-      visit(row, q);
-    }
-    if (last) break;
 
     float4 c4[V];
 #pragma unroll
     for (int k = 0; k < V; ++k) { upk2(cacc[2 * k], c4[k].x, c4[k].y); upk2(cacc[2 * k + 1], c4[k].z, c4[k].w); }
-    if (it == 0) __syncthreads();                      // every warp has taken its last row from the ring: `red` is free
     const uint32_t tag = it + 1;
     uint64_t* pt = reinterpret_cast<uint64_t*>(a.partial) + (int64_t)s.b * a.SP * a.mpad;
-    sink_strip_sums(a, s, red, c4, cacc_m, [&](int j, float sum) { sink_put(pt + (int64_t)s.strip * a.mpad + j, sum, tag); });
+    sink_strip_sums_folded(a, s, red, redm, c4, cacc_m, [&](int j, float sum) { sink_put(pt + (int64_t)s.strip * a.mpad + j, sum, tag); });
     // this strip's columns [lo, lo + S): NG thread groups sum strips g, g + NG, ... of a column, then the groups are added in
     // order (a fixed order: the same bits in every run)
     const int S = cdiv(m + 1, a.SP), lo = s.strip * S, NG = S >= NT ? 1 : NT / S;
@@ -618,30 +735,32 @@ inline int sinkhorn_plan(bool backward, int B, int n, int m, SinkPlan* p) {
   return OG_OK;
 }
 
-// Dynamic shared memory of a resident CTA: v [MC + 4], the row groups' column sums [G][mpad] sharing their space with the one-slot
-// row ring [SINK_WARPS][C], the column groups' sums [256] float4, the held rows [SINK_WARPS][rows_smem][C], the mbarriers, the row
-// exchange and 128 bytes.
+// Dynamic shared memory of a resident CTA: v [MC + 4], the folded column sums [G/2][mpad], the column groups' sums [256] float4,
+// the held rows [max(rows_smem, 1)][SINK_WARPS][C] (the last slot is the first sweep's row ring), the mbarriers, the row exchanges
+// of one and of two rows, the dustbin column's sums [G] and 128 bytes.
 constexpr size_t sinkhorn_resident_smem(int V, int W, int mpad, int rows_smem) {
   const int C = 128 * V, G = SINK_WARPS / W;
-  return ((size_t)(W * C + 4) + (size_t)std::max(G * mpad, SINK_WARPS * C) + 4 * SINK_WARPS * 32 +
-          (size_t)SINK_WARPS * rows_smem * C) * sizeof(float) +
-         SINK_WARPS * sizeof(uint64_t) + (size_t)2 * G * W * sizeof(float2) + 128;
+  return ((size_t)(W * C + 4) + (size_t)G / 2 * mpad + 4 * SINK_WARPS * 32 + (size_t)SINK_WARPS * std::max(rows_smem, 1) * C) *
+             sizeof(float) +
+         SINK_WARPS * sizeof(uint64_t) + (size_t)2 * G * W * (sizeof(float2) + sizeof(float4)) + G * sizeof(float) + 128;
 }
 
-// The resident plan, where it fits and pays: the bands up to 2048 columns (V <= 8; RR = 24 / V rows per warp in registers, 96
-// registers per thread: 32 / V spill), as many rows per warp in shared memory as the opt-in limit leaves, at most one CTA per SM,
-// a pair on at most half the SMs.  The pairs are spread evenly over the launches and each pair of a launch over as many SMs as
-// the launch leaves it.  One launch always pays: the streaming kernel leaves most SMs idle there.  Over several launches the
-// resident kernel is taken only where its modelled sweep time, over all launches, beats the streaming kernel's 2.7 TB/s.  Both
-// rates were measured on an H100 80GB HBM3 (700 W) with og_sinkhorn_fwd: a resident sweep takes about 3.8 us (exchanges) +
-// R (0.4 + 0.0625 V) us for R rows per warp (8 rows of 2048 columns: 11.0 us; 17 rows of 1024: 14.0 us), so 16 pairs of
-// 2048 x 2048 (eight launches) run resident in 8.9 ms against 9.9 ms streaming, while 32 pairs of 1024 x 1024 (four launches,
-// 5.6 ms against 5.0 ms) stream.  Returns false where the streaming kernel runs instead.
+// The resident plan, where it fits and pays: the bands up to 2048 columns (V <= 8; RR = 16 / V rows per warp in registers, 64
+// registers per thread, which leaves room for the second row a warp works on; even, so that rows pair up within registers), as
+// many rows per warp in shared memory as the opt-in limit leaves, at most one CTA per SM, a pair on at most half the SMs.  The
+// pairs are spread evenly over the launches and each pair of a launch over as many SMs as the launch leaves it.  One launch
+// always pays: the streaming kernel leaves most SMs idle there.  Over several launches the resident kernel is taken only where
+// its modelled sweep time, over all launches, beats the streaming kernel's 2.7 TB/s.  Both rates were measured on an H100 80GB
+// HBM3 (700 W) with og_sinkhorn_fwd, the sweep model with the kernel sweeping one row at a time: about 3.8 us (exchanges) +
+// R (0.4 + 0.0625 V) us for R rows per warp (8 rows of 2048 columns: 11.0 us; 17 rows of 1024: 14.0 us).  Two rows at a time
+// the sweep takes less (8 rows of 2048 columns: 9.6 us), so the model errs towards streaming: 16 pairs of 2048 x 2048 (eight
+// launches) run resident, 7.8 ms against 9.9 ms streaming, while 32 pairs of 1024 x 1024 (four launches) stream.  Returns false
+// where the streaming kernel runs instead.
 inline bool sinkhorn_resident_plan(int B, int n, int m, SinkPlan* p) {
   if (m > 2048 || sinkhorn_plan(false, B, n, m, p) != OG_OK) return false;
-  const int G = SINK_WARPS / p->W, rr = 24 / p->V, C = 128 * p->V;
+  const int G = SINK_WARPS / p->W, rr = 16 / p->V, C = 128 * p->V;
   const int sms = device_info().ok ? device_info().sm_count : 132;
-  const int rs_max = (int)((OG_SMEM_OPTIN_MAX - sinkhorn_resident_smem(p->V, p->W, p->mpad, 0)) / (SINK_WARPS * C * sizeof(float)));
+  const int rs_max = 1 + (int)((OG_SMEM_OPTIN_MAX - sinkhorn_resident_smem(p->V, p->W, p->mpad, 1)) / (SINK_WARPS * C * sizeof(float)));
   const int sp_min = cdiv(n + 1, G * (rr + rs_max));  // strips a pair needs
   if (2 * sp_min > sms) return false;
   const int rounds = cdiv(B, std::min(B, sms / sp_min));
@@ -715,7 +834,7 @@ inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
 
 template <int V, int W>
 inline int sinkhorn_resident_launch(const SinkArgs& a, const SinkPlan& p, cudaStream_t stream) {
-  constexpr auto kernel = sinkhorn_resident_kernel<V, W, 24 / V>;
+  constexpr auto kernel = sinkhorn_resident_kernel<V, W, 16 / V>;
   if (const int rc = smem_opt_in<kernel>((int)OG_SMEM_OPTIN_MAX)) return rc;
   return launch("sinkhorn_resident_kernel", kernel, LaunchAttr::cooperative, dim3(a.B * a.SP), dim3(SINK_WARPS * 32), p.smem,
                 stream, a);
