@@ -328,6 +328,25 @@ int64_t og_criterion_workspace_bytes(int batch);
 int og_criterion_fwd(const float* scores, const int64_t* gt_matches0, const int64_t* gt_matches1, int batch, int n, int m,
                      float* loss, float* dscores, float grad_scale, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Metric terms of the same loss for a margin mu: criterion(..., margin=mu)['metric_loss'] (utils/losses.py:56-99 on the
+ * half cosine distance of utils/misc.py:106-113, dist = 0.25 |normalize(c0_i) - normalize(c1_j)|^2).
+ *   c0 [B, d, n], c1 [B, d, m]: the context descriptors (SuperGlue.forward's context_descriptors0/1);
+ *   gt_matches0/1 as og_criterion_fwd;  metric_loss [1] receives the value;
+ *   n0, u0 [B, n] and n1, u1 [B, m] (int64) receive the hard negatives: n0 / n1 = argmin over the row / column of dist with
+ *   every (i, gt0[i]) of a matched row masked, u0 / u1 the unmasked argmins (ties: the lowest index, as torch.argmin);
+ *   dc0 [B, d, n], dc1 [B, d, m] (both or neither) receive grad_scale * d metric_loss / d c0, c1 (overwritten).
+ * precision OG_PREC_FP32 or OG_PREC_TF32X3 selects the GEMMs behind the Gram X Y^T and the gradient.  Launches:
+ * 9 (16 with dc0/dc1) with OG_PREC_FP32; OG_PREC_TF32X3 adds one operand-split launch per GEMM that runs on the tensor cores:
+ * the Gram when d % 4 == 0 and d >= 32, with dc0/dc1 also dX when m rounded up to 4 is >= 32 and dY when n rounded up to 4 is
+ * >= 32 (other shapes run the exact fp32 kernel).  Deterministic, no host synchronisation.  OG_EINVAL without a
+ * launch: a null pointer, dc0 without dc1 (or the reverse), B outside [1, 65535], n, m or d < 1, another precision.
+ * og_metric_loss_workspace_bytes: -1 for such sizes.                                                          */
+int64_t og_metric_loss_workspace_bytes(int batch, int d, int n, int m, int want_grad, int precision);
+int og_metric_loss_fwd(const float* c0, const float* c1, const int64_t* gt_matches0, const int64_t* gt_matches1, int batch, int d,
+                       int n, int m, float margin, int precision, float* metric_loss, int64_t* n0, int64_t* u0, int64_t* n1,
+                       int64_t* u1, float* dc0, float* dc1, float grad_scale, void* workspace, int64_t workspace_bytes,
+                       void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Training-step operators (SURVEY.md section 8, row f1): what nn.BatchNorm1d in training mode and torch autograd do for the
  * reference around the contractions of SuperGlue.forward in MatchingTrainingModule.training_step

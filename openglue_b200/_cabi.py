@@ -93,6 +93,8 @@ SYMBOLS = {
     'og_collate_fwd': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'og_criterion_workspace_bytes': (_L, [_I]),
     'og_criterion_fwd': (_I, [_P, _P, _P, _I, _I, _I, _P, _P, _F, _P, _L, _P]),
+    'og_metric_loss_workspace_bytes': (_L, [_I, _I, _I, _I, _I, _I]),
+    'og_metric_loss_fwd': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P, _P, _P, _P, _P, _P, _P, _F, _P, _L, _P]),
     'og_gt_matches_fwd': (_I, [_P, _P, _I, _I, _I, C.POINTER(OgGtTransform), _P, _P, _P, _L, _P]),
     # training-step operators (row f1)
     'og_train_workspace_floats': (_L, [_I]),

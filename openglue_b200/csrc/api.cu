@@ -10,6 +10,7 @@
 #include "match.cuh"
 #include "gt_matches.cuh"
 #include "criterion.cuh"
+#include "metric_loss.cuh"
 #include "collate.cuh"
 #include "train_ops.cuh"
 #include "superpoint.cuh"
@@ -458,6 +459,23 @@ int og_criterion_fwd(const float* scores, const int64_t* gt_matches0, const int6
   OG_CHECK_ARG(batch > 0 && n > 0 && m > 0, "criterion: bad sizes");
   return criterion_launch(scores, gt_matches0, gt_matches1, batch, n, m, loss, dscores, grad_scale, workspace, workspace_bytes,
                           (cudaStream_t)stream);
+}
+
+static bool metric_sizes_ok(int batch, int d, int n, int m, int precision) {
+  return batch >= 1 && batch <= 65535 && d >= 1 && n >= 1 && m >= 1 && (precision == OG_PREC_FP32 || precision == OG_PREC_TF32X3);
+}
+int64_t og_metric_loss_workspace_bytes(int batch, int d, int n, int m, int want_grad, int precision) {
+  return metric_sizes_ok(batch, d, n, m, precision) ? metric_workspace_bytes(batch, n, m, d, want_grad, precision) : -1;
+}
+int og_metric_loss_fwd(const float* c0, const float* c1, const int64_t* gt_matches0, const int64_t* gt_matches1, int batch, int d,
+                       int n, int m, float margin, int precision, float* metric_loss, int64_t* n0, int64_t* u0, int64_t* n1,
+                       int64_t* u1, float* dc0, float* dc1, float grad_scale, void* workspace, int64_t workspace_bytes,
+                       void* stream) {
+  OG_CHECK_ARG(c0 && c1 && gt_matches0 && gt_matches1 && metric_loss && n0 && u0 && n1 && u1 && workspace, "metric_loss: null pointer");
+  OG_CHECK_ARG((dc0 == nullptr) == (dc1 == nullptr), "metric_loss: dc0 and dc1 come together");
+  OG_CHECK_ARG(metric_sizes_ok(batch, d, n, m, precision), "metric_loss: bad sizes or precision");
+  return metric_loss_launch(c0, c1, gt_matches0, gt_matches1, batch, d, n, m, margin, precision, metric_loss, n0, u0, n1, u1, dc0, dc1,
+                            grad_scale, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 // ---- training-step operators (row f1; csrc/train_ops.cuh) ----

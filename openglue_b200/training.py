@@ -379,11 +379,18 @@ class GraphedTrainStep:
 
     The graph reads the parameters and BatchNorm buffers in place (so optimiser steps and running statistics carry over) and the
     inputs from static copies.  Re-create the object when shapes change or parameters are re-allocated (``.to()``, ``load_state_dict``
-    keeps storage and is fine).  Results are bit-identical to the eager step (same kernels, same order)."""
+    keeps storage and is fine).  Results are bit-identical to the eager step (same kernels, same order).
+
+    ``margin`` / ``metric_weight`` (the reference's ``train.margin`` / ``train.metric_weight``, matching_module.py:101-105): with a
+    margin the graph also computes ``metric_loss`` on the context descriptors (``og_metric_loss_fwd``) and backpropagates
+    ``nll_weight * loss + metric_weight * metric_loss``, as ``criterion(..., margin=)`` does in the eager step; ``margin=None``
+    captures the margin-free step exactly as before."""
 
     _KEYS = ('keypoints0', 'keypoints1', 'side_info0', 'side_info1', 'local_descriptors0', 'local_descriptors1')
 
-    def __init__(self, model, data: dict, y_true: dict, nll_weight: float = 1.0, optimizer=None):
+    def __init__(self, model, data: dict, y_true: dict, nll_weight: float = 1.0, optimizer=None, margin: Optional[float] = None,
+                 metric_weight: float = 0.0):
+        from .losses import _metric_run
         from .losses import _run as criterion_run
         from .optim import ClippedAdam
         if not model.training:
@@ -406,9 +413,16 @@ class GraphedTrainStep:
 
         def run():
             step = TrainStep(model, self.static)
-            scores, _, _ = step.forward()
+            scores, c0, c1 = step.forward()
             loss, dscores = criterion_run(self.gt, {'scores': scores}, True, float(nll_weight))
-            grads = step.backward(dscores)
+            if margin is None:
+                grads = step.backward(dscores)
+            else:                                                        # metric_loss into loss[1]; its gradient scaled as autograd
+                _, _, dc0, dc1 = _metric_run(self.gt['gt_matches0'], self.gt['gt_matches1'], c0, c1, float(margin), True, 1.0,
+                                             out=loss[1:])
+                for dc in (dc0, dc1):                                    # scales the eager step's unit gradients (one rounding)
+                    step.ops.axpby(dc, None, float(metric_weight), 0.0, out=dc)
+                grads = step.backward(dscores, dc0, dc1)
             for name, p in self.params:
                 p.grad.copy_(grads[name].reshape(p.shape))
             if optimizer is not None:
