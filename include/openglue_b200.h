@@ -420,6 +420,42 @@ int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const f
                       float* desc, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * OpenCV SIFT front-end (OPENCV_SIFT: cv2.SIFT_create(contrastThreshold=-10000, edgeThreshold=-10000) + the reference's radius NMS,
+ * top-k, RootSIFT and LAFs; models/features/opencv/_features.py:10-18, base.py:14-182).  B same-size images per call.
+ * Keypoints are kp [B, cap, 5] = (x, y, size, angle, response) floats and octave [B, cap] (cv2's packed octave word), per image in
+ * cv2's order (x, y, size desc, angle, response desc, octave desc) without exact duplicates.
+ *   og_sift_workspace_bytes  the workspace of og_sift_detect / og_sift_describe (Gaussian and DoG pyramids, candidate lists);
+ *                            < 0 (OG_EUNSUPPORTED) when the image has no octave or more than 16
+ *   og_sift_detect           image [B, H, W] (dtype 0: uint8; 1: float32, quantised as the torch wrapper does: uint8(255 * x))
+ *                            -> kp, octave, count [B]; count[b] > cap means cap was too small and the outputs are incomplete.
+ *                            The pyramid stays in ws for og_sift_describe.
+ *   og_sift_select_workspace_bytes / og_sift_select
+ *                            greedy radius NMS (visit by response desc, equal responses by index asc; a kept point removes every
+ *                            point within nms_radius, inclusive; none when nms_radius <= 0) then the max_keypoints largest
+ *                            responses (all when <= 0): sel [B, cap] indices into kp by response desc, index asc; n_sel [B].
+ *                            Takes any keypoints, e.g. cv2's own; count[b] is clamped to [0, cap].
+ *   og_sift_describe         cv2's descriptors of kp[b, sel[b, j]], j < n_sel[b] (and < out_cap), from og_sift_detect's pyramid in ws
+ *                            (same B, H, W, cap), then normalize_descriptors (rootsift: L1 + sqrt, else L2) and lafs_from_opencv_kpts
+ *                            (mr_size 6): lafs [B, out_cap, 2, 3], scores [B, out_cap], desc [B, out_cap, 128], raw_desc (optional)
+ *                            [B, out_cap, 128] cv2's integer-valued descriptor.  max_n >= every n_sel[b] sizes the grid.
+ *   og_sift_rootsift_laf     normalize_descriptors + lafs_from_opencv_kpts of supplied kp [N, 5] and raw descriptors [N, 128]
+ *   og_sift_fast_atan2       out[i] = cv2's fastAtan2(y[i], x[i]) in degrees: fused = cv::hal::fastAtan2's vector form, 0 = the
+ *                            scalar one (cv2.fastAtan2)
+ *   og_sift_gaussian_taps    host only: cv2's float Gaussian kernel for sigma (taps computed in double, rounded to float); returns the
+ *                            number of taps, or OG_EUNSUPPORTED when it exceeds cap                                                  */
+int64_t og_sift_workspace_bytes(int B, int H, int W, int cap);
+int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
+                   int* count, void* stream);
+int64_t og_sift_select_workspace_bytes(int B, int cap);
+int og_sift_select(const float* kp, const int* count, int B, int cap, float nms_radius, int max_keypoints, void* work, int64_t work_bytes,
+                   int* sel, int* n_sel, void* stream);
+int og_sift_describe(const void* ws, int B, int H, int W, int cap, const float* kp, const int* octave, const int* sel, const int* n_sel,
+                     int out_cap, int max_n, int rootsift, float* lafs, float* scores, float* desc, float* raw_desc, void* stream);
+int og_sift_rootsift_laf(const float* kp, const float* raw_desc, int64_t N, int rootsift, float* lafs, float* scores, float* desc, void* stream);
+int og_sift_fast_atan2(const float* y, const float* x, int64_t n, int fused, float* out, void* stream);
+int og_sift_gaussian_taps(double sigma, float* taps, int cap);
+
+/* ---------------------------------------------------------------------------------------------
  * Local features -> matcher inputs, and matches -> the compact match list of stand-alone inference.
  *   og_prepare_features  prepare_features_output (models/features/utils.py:54-65) with the LAF -> side-information converter
  *                        superglue.laf_to_sideinfo_method names (models/laf_converter.py:108-128).  One thread per keypoint.

@@ -12,6 +12,7 @@ and the steps either side of those:
     SuperGlue(config).train()(data)                           (training mode: batch-statistics BatchNorm, explicit backward pass)
     ClippedAdam.from_config(superglue, config['train'])       (clip_grad_norm_ -> Adam -> StepLR, one device call, graph-capturable)
     SuperPointNet(max_keypoints, ...)(image) -> (lafs, scores, descriptors)   (the detector / descriptor front-end; SuperPointNetBn: its BatchNorm variant)
+    OpenCVSIFT(max_keypoints, nms_diameter, rootsift)(image) -> (lafs, scores, descriptors)   (OPENCV_SIFT: cv2's SIFT + radius NMS + RootSIFT)
     prepare_features_output(lafs, responses, desc, get_laf_to_sideinfo_converter(method), ...)   (front-end output -> SuperGlue input)
     OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
     synthesize_homography_pairs(images_u8, offset, warp_offset, generator)   (the homography-pretraining dataset's pairs, batched)
@@ -24,6 +25,7 @@ from .losses import criterion  # noqa: F401
 from .optim import ClippedAdam  # noqa: F401
 from .sinkhorn import matching_log_probs  # noqa: F401
 from .superglue import MatchingCore, PendingMatches, SuperGlue  # noqa: F401
+from .sift import OpenCVSIFT, sift_create_torch  # noqa: F401
 from .superpoint import SuperPointNet, SuperPointNetBn  # noqa: F401
 
 __version__ = '0.1.0'

@@ -120,6 +120,15 @@ SYMBOLS = {
     'og_sp_compact': (_I, [_P, _I, _I, _I, _P, _P, _P, _P]),
     'og_sp_select': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P]),
     'og_sp_sample_desc': (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P]),
+    # OpenCV SIFT front-end (row f7)
+    'og_sift_workspace_bytes': (_L, [_I, _I, _I, _I]),
+    'og_sift_detect': (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P, _P]),
+    'og_sift_select_workspace_bytes': (_L, [_I, _I]),
+    'og_sift_select': (_I, [_P, _P, _I, _I, _F, _I, _P, _L, _P, _P, _P]),
+    'og_sift_describe': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
+    'og_sift_rootsift_laf': (_I, [_P, _P, _L, _I, _P, _P, _P, _P]),
+    'og_sift_fast_atan2': (_I, [_P, _P, _L, _I, _P, _P]),
+    'og_sift_gaussian_taps': (_I, [_D, _P, _I]),
     # local features -> matcher inputs, matches -> compact list
     'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

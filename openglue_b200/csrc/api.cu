@@ -14,6 +14,7 @@
 #include "collate.cuh"
 #include "train_ops.cuh"
 #include "superpoint.cuh"
+#include "sift.cuh"
 #include "features.cuh"
 #include "homography.cuh"
 #include "optim.cuh"
@@ -620,6 +621,132 @@ int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const f
   if (max_n <= 0) return OG_OK;
   return OG_LAUNCH(sp_sample_desc_kernel, dim3(cdiv(max_n, 8), B), 256, 0, (cudaStream_t)stream, coarse, Hc, Wc, D, kpts, n_out, out_cap,
                    cell, desc);
+}
+
+// ---- OpenCV SIFT front-end (csrc/sift.cuh) ----
+int64_t og_sift_workspace_bytes(int B, int H, int W, int cap) {
+  SiftLayout L;
+  if (B <= 0 || B > 65535 || H <= 0 || W <= 0 || cap <= 0 || cap > (1 << 24)) return fail(OG_EINVAL, "sift_workspace_bytes: bad sizes");
+  if (!sift_layout(B, H, W, cap, L)) return fail(OG_EUNSUPPORTED, "sift: a %d x %d image has no octave or more than %d", H, W, SIFT_MAX_OCTAVES);
+  return L.total;
+}
+int og_sift_gaussian_taps(double sigma, float* taps, int cap) {
+  OG_CHECK_ARG(taps && sigma > 0 && cap > 0, "sift_gaussian_taps: bad arguments");
+  const int n = sift_gaussian_taps(sigma, taps, cap);
+  if (n < 0) return fail(OG_EUNSUPPORTED, "sift_gaussian_taps: sigma %g needs more than %d taps", sigma, cap);
+  return n;
+}
+static int sift_blur(const float* src, int B, int h, int w, double sigma, float* tmp, float* dst, float* dog, cudaStream_t st) {
+  SiftTaps t;
+  t.n = sift_gaussian_taps(sigma, t.k, SIFT_MAX_TAPS);
+  if (t.n < 0) return fail(OG_EUNSUPPORTED, "sift: sigma %g needs more than %d taps", sigma, SIFT_MAX_TAPS);
+  const int64_t n = (int64_t)B * h * w;
+  if (const int rc = OG_LAUNCH(sift_blur_rows_kernel, sift_grid(n), 256, 0, st, src, B, h, w, t, tmp)) return rc;
+  return OG_LAUNCH(sift_blur_cols_kernel, sift_grid(n), 256, 0, st, tmp, B, h, w, t, dst, src, dog);
+}
+int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
+                   int* count, void* stream) {
+  OG_CHECK_ARG(image && ws && kp && octave && count, "sift_detect: null pointer");
+  OG_CHECK_ARG(dtype == 0 || dtype == 1, "sift_detect: dtype must be 0 (uint8) or 1 (float32)");
+  const int64_t need = og_sift_workspace_bytes(B, H, W, cap);
+  if (need < 0) return (int)need;
+  OG_CHECK_ARG(ws_bytes >= need, "sift_detect: workspace of %lld bytes, %lld needed", (long long)ws_bytes, (long long)need);
+  SiftLayout L;
+  sift_layout(B, H, W, cap, L);
+  unsigned char* w8 = static_cast<unsigned char*>(ws);
+  cudaStream_t st = (cudaStream_t)stream;
+  const SiftPyramid P = sift_pyramid(w8, L, B);
+  float* tmp = reinterpret_cast<float*>(w8 + L.tmp_off);
+  int* loc_count = reinterpret_cast<int*>(w8 + L.cnt_off);
+  int* kp_count = loc_count + B;
+  SiftLoc* loc = reinterpret_cast<SiftLoc*>(w8 + L.loc_off);
+  float* kp_raw = reinterpret_cast<float*>(w8 + L.kp_off);
+  int* oct_raw = reinterpret_cast<int*>(w8 + L.oct_off);
+  int* work = reinterpret_cast<int*>(w8 + L.work_off);
+  const uint8_t* u8 = static_cast<const uint8_t*>(image);
+  if (dtype == 1) {
+    uint8_t* q = w8 + L.u8_off;
+    const int64_t n = (int64_t)B * H * W;
+    if (const int rc = OG_LAUNCH(sift_quantize_kernel, sift_grid(n), 256, 0, st, static_cast<const float*>(image), n, q)) return rc;
+    u8 = q;
+  }
+  OG_CUDA(cudaMemsetAsync(loc_count, 0, 2 * B * sizeof(int), st));
+  // createInitialImage: x2 INTER_LINEAR, then the blur from the assumed 0.5 (x2: 1.0) to sigma
+  float* up = P.oct[0].dog;                            // scratch until the first DoG level is written
+  if (const int rc = OG_LAUNCH(sift_upsample_kernel, sift_grid((int64_t)B * L.h[0] * L.w[0]), 256, 0, st, u8, B, H, W, up)) return rc;
+  const float sig_diff = sqrtf(std::max(SIFT_SIGMA * SIFT_SIGMA - 0.5f * 0.5f * 4, 0.01f));
+  if (const int rc = sift_blur(up, B, L.h[0], L.w[0], (double)sig_diff, tmp, P.oct[0].gauss, nullptr, st)) return rc;
+  // buildGaussianPyramid / buildDoGPyramid
+  double sig[SIFT_GAUSS];
+  sig[0] = SIFT_SIGMA_D;
+  const double k = pow(2., 1. / SIFT_LAYERS);
+  for (int i = 1; i < SIFT_GAUSS; ++i) {
+    const double prev = pow(k, (double)(i - 1)) * SIFT_SIGMA_D, total = prev * k;
+    sig[i] = sqrt(total * total - prev * prev);
+  }
+  for (int o = 0; o < L.nO; ++o) {
+    const SiftOctave& oc = P.oct[o];
+    const int64_t plane = (int64_t)B * oc.h * oc.w;
+    if (o > 0) {
+      const SiftOctave& pv = P.oct[o - 1];
+      if (const int rc = OG_LAUNCH(sift_downsample_kernel, sift_grid(plane), 256, 0, st, pv.gauss + (int64_t)SIFT_LAYERS * B * pv.h * pv.w,
+                                   B, pv.h, pv.w, oc.gauss)) return rc;
+    }
+    for (int i = 1; i < SIFT_GAUSS; ++i)
+      if (const int rc = sift_blur(oc.gauss + (i - 1) * plane, B, oc.h, oc.w, sig[i], tmp, oc.gauss + i * plane, oc.dog + (i - 1) * plane, st)) return rc;
+  }
+  // findScaleSpaceExtrema: extrema + interpolation, orientations
+  for (int o = 0; o < L.nO; ++o) {
+    const SiftOctave& oc = P.oct[o];
+    const int64_t n = (int64_t)B * SIFT_LAYERS * std::max(oc.h - 2 * SIFT_BORDER, 0) * std::max(oc.w - 2 * SIFT_BORDER, 0);
+    if (n == 0) continue;
+    if (const int rc = OG_LAUNCH(sift_extrema_kernel, sift_grid(n), 256, 0, st, oc, B, o, loc, L.loc_cap, loc_count)) return rc;
+  }
+  if (const int rc = OG_LAUNCH(sift_orientation_kernel, dim3(cdiv(L.loc_cap, 8), B), 256, 0, st, P, (const SiftLoc*)loc, L.loc_cap,
+                               (const int*)loc_count, kp_raw, oct_raw, cap, kp_count)) return rc;
+  // KeyPointsFilter::removeDuplicatedSorted
+  return OG_LAUNCH(sift_sort_unique_kernel, B, 1024, 0, st, (const float*)kp_raw, (const int*)oct_raw, (const int*)kp_count,
+                   (const int*)loc_count, L.loc_cap, cap, L.n2max, work, kp, octave, count);
+}
+int64_t og_sift_select_workspace_bytes(int B, int cap) {
+  if (B <= 0 || B > 65535 || cap <= 0 || cap > (1 << 24)) return fail(OG_EINVAL, "sift_select_workspace_bytes: bad sizes");
+  int n2 = 1;
+  while (n2 < cap) n2 <<= 1;
+  return (int64_t)B * 4 * n2 * 4;
+}
+int og_sift_select(const float* kp, const int* count, int B, int cap, float nms_radius, int max_keypoints, void* work, int64_t work_bytes,
+                   int* sel, int* n_sel, void* stream) {
+  OG_CHECK_ARG(kp && count && work && sel && n_sel, "sift_select: null pointer");
+  const int64_t need = og_sift_select_workspace_bytes(B, cap);
+  if (need < 0) return (int)need;
+  OG_CHECK_ARG(work_bytes >= need, "sift_select: workspace of %lld bytes, %lld needed", (long long)work_bytes, (long long)need);
+  OG_CHECK_ARG(nms_radius == nms_radius, "sift_select: nms_radius is NaN");
+  int n2 = 1;
+  while (n2 < cap) n2 <<= 1;
+  return OG_LAUNCH(sift_select_kernel, B, 1024, 0, (cudaStream_t)stream, kp, count, cap, nms_radius, max_keypoints, n2,
+                   static_cast<int*>(work), sel, n_sel);
+}
+int og_sift_describe(const void* ws, int B, int H, int W, int cap, const float* kp, const int* octave, const int* sel, const int* n_sel,
+                     int out_cap, int max_n, int rootsift, float* lafs, float* scores, float* desc, float* raw_desc, void* stream) {
+  OG_CHECK_ARG(ws && kp && octave && sel && n_sel && lafs && scores && desc, "sift_describe: null pointer");
+  OG_CHECK_ARG(out_cap > 0 && max_n >= 0, "sift_describe: bad sizes");
+  SiftLayout L;
+  if (og_sift_workspace_bytes(B, H, W, cap) < 0) return OG_EINVAL;
+  sift_layout(B, H, W, cap, L);
+  if (max_n == 0) return OG_OK;
+  const SiftPyramid P = sift_pyramid(static_cast<unsigned char*>(const_cast<void*>(ws)), L, B);
+  return OG_LAUNCH(sift_describe_kernel, dim3(cdiv(std::min(max_n, out_cap), 8), B), 256, 0, (cudaStream_t)stream, P, kp, octave, cap, sel, n_sel,
+                   out_cap, rootsift, lafs, scores, desc, raw_desc);
+}
+int og_sift_rootsift_laf(const float* kp, const float* raw_desc, int64_t N, int rootsift, float* lafs, float* scores, float* desc, void* stream) {
+  OG_CHECK_ARG(kp && raw_desc && lafs && scores && desc && N >= 0, "sift_rootsift_laf: bad arguments");
+  if (N == 0) return OG_OK;
+  return OG_LAUNCH(sift_rootsift_laf_kernel, (unsigned)((N + 7) / 8), 256, 0, (cudaStream_t)stream, kp, raw_desc, N, rootsift, lafs, scores, desc);
+}
+int og_sift_fast_atan2(const float* y, const float* x, int64_t n, int fused, float* out, void* stream) {
+  OG_CHECK_ARG(y && x && out && n >= 0, "sift_fast_atan2: bad arguments");
+  if (n == 0) return OG_OK;
+  return OG_LAUNCH(sift_fast_atan2_kernel, sift_grid(n), 256, 0, (cudaStream_t)stream, y, x, n, fused, out);
 }
 
 // ---- local features -> matcher inputs, matches -> compact list (csrc/features.cuh) ----
