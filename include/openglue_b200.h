@@ -141,6 +141,29 @@ int og_superglue_forward_f16(const og_config* cfg, const float* packed_weights,
                              int64_t* matches1, float* mscores1,
                              void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Padded batch: pairs with their own keypoint counts in one call, in every precision (packed_hi16 / packed_lo16 / meta16 may be
+ * NULL unless cfg->precision == OG_PREC_FP16X3).  kpts, side, desc, ctx, scores and matches are laid out as in
+ * og_superglue_forward at the capacity n, m; pair b owns rows [0, n_b) of image 0 and [0, m_b) of image 1, and each pair's result
+ * is the whole path run on that pair alone.
+ *   lengths      device int32 [2B]: n_0 .. n_{B-1}, then m_0 .. m_{B-1}.  Not checked: the kernels clamp each into [1, n] / [1, m].
+ *   image_sizes  device float [B, 4]: (W0, H0, W1, H1) of each pair
+ *   The padding slots of kpts, side and desc may hold anything (NaN, inf); they influence no valid output.  Outputs past the
+ *   lengths: scores -inf (each pair's dustbin row is row n_b, its dustbin column m_b), matches -1, mscores 0, ctx 0.
+ *   n <= 65536, batch <= 65535;  workspace >= og_workspace_bytes_padded(cfg, B, n, m), 256-byte aligned.
+ *   The first padded call on a device uploads the Sinkhorn's constant tables synchronously: it must not be stream-captured. */
+int64_t og_workspace_bytes_padded(const og_config* cfg, int batch, int n, int m);
+int og_superglue_forward_padded(const og_config* cfg, const float* packed_weights,
+                                const float* packed_hi, const float* packed_lo,
+                                const void* packed_hi16, const void* packed_lo16, const float* meta16,
+                                int batch, int n, int m, const int* lengths, const float* image_sizes,
+                                const float* kpts0, const float* kpts1,
+                                const float* side0, const float* side1,
+                                const float* desc0, const float* desc1,
+                                float* ctx0, float* ctx1, float* scores,
+                                int64_t* matches0, float* mscores0,
+                                int64_t* matches1, float* mscores1,
+                                void* workspace, int64_t workspace_bytes, void* stream);
+
 /* Number of kernels this thread has enqueued since the last og_superglue_forward (or _f16) began, that forward's own
  * launches included.  Every operator entry point adds the kernels it launches.                                      */
 int og_last_forward_launches(void);
@@ -232,6 +255,27 @@ int og_attention_f16_fwd(const float* q, int64_t ldq, int64_t strideq, const flo
                          float* out, int64_t ldo, int64_t strideo, float* out_amax,
                          int batch, int nq, int nk, int num_heads, int head_dim, int swap_halves, void* stream);
 
+/* Padded forms of the three attention operators: sequence b attends to its first key_lengths[b] keys (device int32 [batch],
+ * clamped into [1, nk]); the operands keep the layout of the capacity nk.  Every query row is computed. */
+int og_attention_fwd_padded(const float* q, int64_t ldq, int64_t strideq,
+                            const float* k, int64_t ldk, int64_t stridek,
+                            const float* v, int64_t ldv, int64_t stridev,
+                            float* out, int64_t ldo, int64_t strideo,
+                            int batch, int nq, int nk, int num_heads, int head_dim,
+                            const int* key_lengths, void* stream);
+int og_attention_tc_fwd_padded(const float* q, int64_t ldq, int64_t strideq,
+                               const float* khi, const float* klo, int64_t ldk,
+                               const float* vthi, const float* vtlo, int64_t ldvt,
+                               float* out, int64_t ldo, int64_t strideo,
+                               int batch, int nq, int nk, int num_heads, int head_dim,
+                               const int* key_lengths, void* stream);
+int og_attention_f16_fwd_padded(const float* q, int64_t ldq, int64_t strideq, const float* q_amax,
+                                const void* khi, const void* klo, int64_t ldk, const float* k_scale,
+                                const void* vthi, const void* vtlo, int64_t ldvt, const float* v_scale,
+                                float* out, int64_t ldo, int64_t strideo, float* out_amax,
+                                int batch, int nq, int nk, int num_heads, int head_dim,
+                                const int* key_lengths, void* stream);
+
 /* Dustbin-augmented log-domain Sinkhorn.  Replaces SuperGlue.get_matching_probs
  * (superglue.py:88-111) + log_otp_solver (optimal_transport.py:4-28).
  *   S       [B][n, lds]  inner score block (lds >= m, multiple of 4, 16-byte aligned rows)
@@ -250,6 +294,16 @@ int og_sinkhorn_plan(int batch, int n, int m, int64_t* plan);
 int og_sinkhorn_fwd(const float* S, int64_t lds, int64_t strideS, const float* dustbin,
                     int batch, int n, int m, int iters, float reg,
                     float* scores, void* workspace, int64_t workspace_bytes, void* stream);
+/* Padded form: pair b is the [n_b, m_b] block of the capacity n x m (lengths: device int32 [2B], n_0 .. n_{B-1}, m_0 .. m_{B-1},
+ * clamped into [1, n] / [1, m]; n <= 65536); scores[b, :n_b+1, :m_b+1] is its augmented log-assignment (dustbin row n_b, column
+ * m_b), -inf elsewhere.  The plan and workspace are the capacity's.  og_sinkhorn_consts: the host's (norm, log_a_last,
+ * log_b_last) of an n x m pair; og_sinkhorn_consts_padded: out [B, 3] (device), what the padded kernels use for each pair, bit
+ * for bit the host's.  The first padded call on a device uploads tables synchronously: it must not be stream-captured.  */
+int og_sinkhorn_fwd_padded(const float* S, int64_t lds, int64_t strideS, const float* dustbin,
+                           int batch, int n, int m, const int* lengths, int iters, float reg,
+                           float* scores, void* workspace, int64_t workspace_bytes, void* stream);
+int og_sinkhorn_consts(int n, int m, float* out);
+int og_sinkhorn_consts_padded(const int* lengths, int batch, int n, int m, float* out, void* stream);
 
 /* Training form of the Sinkhorn operator (SURVEY.md section 8, row f1).  og_sinkhorn_train_fwd = og_sinkhorn_fwd that also
  * records the scaling vectors of every iteration (hist: og_sinkhorn_hist_floats floats: u [B][T][n+1], v [B][T+1][m+1]);
@@ -274,6 +328,10 @@ int64_t og_match_workspace_bytes(int batch, int n, int m);
 int og_match_fwd(const float* scores, int batch, int n, int m, float threshold,
                  int64_t* matches0, float* mscores0, int64_t* matches1, float* mscores1,
                  void* workspace, int64_t workspace_bytes, void* stream);
+/* Padded form (lengths as og_sinkhorn_fwd_padded; batch <= 65535): pair b's matches on scores[b, :n_b, :m_b]; -1 / 0 past them. */
+int og_match_fwd_padded(const float* scores, int batch, int n, int m, const int* lengths, float threshold,
+                        int64_t* matches0, float* mscores0, int64_t* matches1, float* mscores1,
+                        void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Ground-truth match generation: the step immediately BEFORE the matching core in the reference's

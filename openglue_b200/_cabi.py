@@ -67,6 +67,9 @@ SYMBOLS = {
                                   _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
     'og_superglue_forward_f16': (_I, [_CFG, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_float),
                                       _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
+    'og_workspace_bytes_padded': (_L, [_CFG, _I, _I, _I]),
+    'og_superglue_forward_padded': (_I, [_CFG, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P,
+                                         _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
     'og_f16_meta_floats': (_L, [_CFG]),
     'og_pack_f16': (_I, [_CFG, _P, _P, _P, _P, _P]),
     'og_weight_split_f16': (_I, [_P, _P, _I, _I, _P, _P, _P, _P]),
@@ -79,16 +82,23 @@ SYMBOLS = {
     'og_linear_fwd': (_I, [C.POINTER(OgLinearArgs), _I, _P]),
     'og_attention_fwd': (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _L, _I, _I, _I, _I, _I, _I, _P]),
     'og_attention_tc_fwd': (_I, [_P, _L, _L, _P, _P, _L, _P, _P, _L, _P, _L, _L, _I, _I, _I, _I, _I, _P]),
+    'og_attention_fwd_padded': (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _L, _I, _I, _I, _I, _I, _P, _P]),
+    'og_attention_tc_fwd_padded': (_I, [_P, _L, _L, _P, _P, _L, _P, _P, _L, _P, _L, _L, _I, _I, _I, _I, _I, _P, _P]),
+    'og_attention_f16_fwd_padded': (_I, [_P, _L, _L, _P, _P, _P, _L, _P, _P, _P, _L, _P, _P, _L, _L, _P, _I, _I, _I, _I, _I, _P, _P]),
     'og_sinkhorn_workspace_bytes': (_L, [_I, _I, _I]),
     'og_set_sinkhorn_resident': (_I, [_I]),
     'og_sinkhorn_plan': (_I, [_I, _I, _I, _P]),
     'og_sinkhorn_fwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _L, _P]),
+    'og_sinkhorn_fwd_padded': (_I, [_P, _L, _L, _P, _I, _I, _I, _P, _I, _F, _P, _P, _L, _P]),
+    'og_sinkhorn_consts': (_I, [_I, _I, C.POINTER(C.c_float)]),
+    'og_sinkhorn_consts_padded': (_I, [_P, _I, _I, _I, _P, _P]),
     'og_sinkhorn_hist_floats': (_L, [_I, _I, _I, _I]),
     'og_sinkhorn_train_fwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _P, _L, _P]),
     'og_sinkhorn_bwd_workspace_bytes': (_L, [_I, _I, _I, _I]),
     'og_sinkhorn_bwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P, _L, _P]),
     'og_match_workspace_bytes': (_L, [_I, _I, _I]),
     'og_match_fwd': (_I, [_P, _I, _I, _I, _F, _P, _P, _P, _P, _P, _L, _P]),
+    'og_match_fwd_padded': (_I, [_P, _I, _I, _I, _P, _F, _P, _P, _P, _P, _P, _L, _P]),
     'og_gt_matches_workspace_bytes': (_L, [_I, _I, _I]),
     'og_collate_fwd': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'og_criterion_workspace_bytes': (_L, [_I]),

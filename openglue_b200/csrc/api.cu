@@ -36,6 +36,53 @@ __global__ void __launch_bounds__(256) kenc_input_kernel(const float* __restrict
   for (int s = 0; s < S; ++s) o[2 + s] = __ldg(side + (int64_t)r * S + s);
 }
 
+// Padded batch: row r of one image's [B, cap] rows is slot r % cap of pair b = r / cap, real below len[b] (clamped into [1, cap]).
+__device__ __forceinline__ bool padded_row_real(int64_t r, int cap, const int* len) {
+  const int b = (int)(r / cap);
+  return (int)(r - (int64_t)b * cap) < min(max(__ldg(len + b), 1), cap);
+}
+
+// kenc_input_kernel for a padded batch: each pair's (W - 1, H - 1) from wh (rows 4 floats apart: the image's (W, H) of the pair),
+// zero rows past its length (whatever the padding slots hold, every row from here on is finite)
+__global__ void __launch_bounds__(256) kenc_input_padded_kernel(const float* __restrict__ kpts, const float* __restrict__ side,
+                                                                 int rows, int cap, int S, const int* __restrict__ len,
+                                                                 const float* __restrict__ wh, float* __restrict__ out) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  float* o = out + (int64_t)r * (2 + S);
+  if (!padded_row_real(r, cap, len)) {
+    for (int s = 0; s < 2 + S; ++s) o[s] = 0.f;
+    return;
+  }
+  const int b = r / cap;
+  o[0] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r), __ldg(wh + 4 * b) - 1.f) - 1.f;
+  o[1] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r + 1), __ldg(wh + 4 * b + 1) - 1.f) - 1.f;
+  for (int s = 0; s < S; ++s) o[2 + s] = __ldg(side + (int64_t)r * S + s);
+}
+
+// dst = src [rows, d] with the rows past each pair's length zeroed (the descriptors a padded batch's residuals read)
+__global__ void __launch_bounds__(256) mask_padded_rows_kernel(const float* __restrict__ src, int64_t rows, int cap, int d,
+                                                                const int* __restrict__ len, float* __restrict__ dst) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows * d; i += (int64_t)gridDim.x * blockDim.x)
+    dst[i] = padded_row_real(i / d, cap, len) ? __ldg(src + i) : 0.f;
+}
+
+// ctx [B, d, cap] (channel-first context descriptors): zero the columns past each pair's length
+__global__ void __launch_bounds__(256) zero_padded_cols_kernel(float* __restrict__ ctx, int B, int d, int cap, const int* __restrict__ len) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (int64_t)B * d * cap; i += (int64_t)gridDim.x * blockDim.x) {
+    const int b = (int)(i / ((int64_t)d * cap));
+    if ((int)(i % cap) >= min(max(__ldg(len + b), 1), cap)) ctx[i] = 0.f;
+  }
+}
+
+// out[b] = the Sinkhorn constants (norm, log_a_last, log_b_last) the padded kernels derive for pair b
+__global__ void sinkhorn_consts_kernel(SinkArgs a, float* out) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.B) return;
+  const SinkPair<true> p(a, b);
+  out[3 * b] = p.norm(); out[3 * b + 1] = p.log_a_last(); out[3 * b + 2] = p.log_b_last();
+}
+
 struct Layout {           // float offsets of the packed weights
   std::vector<int64_t> kenc_w, kenc_b;
   std::vector<int64_t> qkv_w, qkv_b, fc1_w, fc1_b, fc2_w, fc2_b;
@@ -84,10 +131,11 @@ struct Workspace {
   void *sink, *match;
   float* slots;                           // amax / scale scalars of the fp16 path (zeroed at the start of a forward pass)
   int nslots;
+  float* desc;                            // padded batch: the descriptors of both images with their padding rows zeroed
   int64_t lds, sink_bytes, match_bytes, total;
 };
 
-static int plan_workspace(const og_config* c, int B, int n, int m, void* base, Workspace* w) {
+static int plan_workspace(const og_config* c, int B, int n, int m, void* base, Workspace* w, bool padded = false) {
   const int64_t d = c->descriptor_dim, R = (int64_t)B * (n + m);
   int maxh = (int)d;
   for (int i = 0; i < c->num_hidden; ++i) maxh = std::max(maxh, c->hidden[i]);
@@ -123,6 +171,7 @@ static int plan_workspace(const og_config* c, int B, int n, int m, void* base, W
   w->sink = take(w->sink_bytes);
   w->match_bytes = match_workspace_bytes(B, n, m);
   w->match = take(w->match_bytes);
+  w->desc = padded ? (float*)take(R * d * 4) : nullptr;
   w->total = off;
   return OG_OK;
 }
@@ -324,27 +373,57 @@ int og_split_tf32(const float* src, float* hi, float* lo, int64_t n, void* strea
   return OG_LAUNCH(split_tf32_kernel, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, src, hi, lo, n);
 }
 
-int og_attention_fwd(const float* q, int64_t ldq, int64_t strideq, const float* k, int64_t ldk, int64_t stridek,
-                     const float* v, int64_t ldv, int64_t stridev, float* out, int64_t ldo, int64_t strideo,
-                     int batch, int nq, int nk, int num_heads, int head_dim, int precision, void* stream) {
+static int attention_fwd_impl(const float* q, int64_t ldq, int64_t strideq, const float* k, int64_t ldk, int64_t stridek,
+                              const float* v, int64_t ldv, int64_t stridev, float* out, int64_t ldo, int64_t strideo,
+                              int batch, int nq, int nk, int num_heads, int head_dim, const int* klen, void* stream) {
   OG_CHECK_ARG(q && k && v && out, "attention: null pointer");
   OG_CHECK_ARG(batch > 0 && nq > 0 && nk > 0 && num_heads > 0 && head_dim > 0, "attention: bad sizes");
-  (void)precision;                                   // raw fp32 operands: always the exact kernel (see the header)
   AttnArgs a{q, ldq, strideq, k, ldk, stridek, v, ldv, stridev, out, ldo, strideo, batch, nq, nk, num_heads,
-             (float)pow((double)head_dim, -0.5)};
+             (float)pow((double)head_dim, -0.5), klen};
   return attention_simt_launch(a, head_dim, (cudaStream_t)stream);
 }
 
-int og_attention_tc_fwd(const float* q, int64_t ldq, int64_t strideq, const float* khi, const float* klo, int64_t ldk,
-                        const float* vthi, const float* vtlo, int64_t ldvt, float* out, int64_t ldo, int64_t strideo,
-                        int batch, int nq, int nk, int num_heads, int head_dim, void* stream) {
+int og_attention_fwd(const float* q, int64_t ldq, int64_t strideq, const float* k, int64_t ldk, int64_t stridek,
+                     const float* v, int64_t ldv, int64_t stridev, float* out, int64_t ldo, int64_t strideo,
+                     int batch, int nq, int nk, int num_heads, int head_dim, int precision, void* stream) {
+  (void)precision;                                   // raw fp32 operands: always the exact kernel (see the header)
+  return attention_fwd_impl(q, ldq, strideq, k, ldk, stridek, v, ldv, stridev, out, ldo, strideo, batch, nq, nk, num_heads, head_dim,
+                            nullptr, stream);
+}
+
+int og_attention_fwd_padded(const float* q, int64_t ldq, int64_t strideq, const float* k, int64_t ldk, int64_t stridek,
+                            const float* v, int64_t ldv, int64_t stridev, float* out, int64_t ldo, int64_t strideo,
+                            int batch, int nq, int nk, int num_heads, int head_dim, const int* key_lengths, void* stream) {
+  OG_CHECK_ARG(key_lengths, "attention_padded: null key_lengths");
+  return attention_fwd_impl(q, ldq, strideq, k, ldk, stridek, v, ldv, stridev, out, ldo, strideo, batch, nq, nk, num_heads, head_dim,
+                            key_lengths, stream);
+}
+
+static int attention_tc_fwd_impl(const float* q, int64_t ldq, int64_t strideq, const float* khi, const float* klo, int64_t ldk,
+                                 const float* vthi, const float* vtlo, int64_t ldvt, float* out, int64_t ldo, int64_t strideo,
+                                 int batch, int nq, int nk, int num_heads, int head_dim, const int* klen, void* stream) {
   OG_CHECK_ARG(q && khi && klo && vthi && vtlo && out, "attention_tc: null pointer");
   OG_CHECK_ARG(batch > 0 && nq > 0 && nk > 0 && num_heads > 0, "attention_tc: bad sizes");
   if (!attention_tc_eligible(head_dim, ldq, ldk, ldvt, ldo))
     return fail(OG_EUNSUPPORTED, "attention_tc: head_dim in {32, 64} and 16-byte aligned rows required");
   TcAttnArgs a{q, ldq, strideq, out, ldo, strideo, batch, nq, nk, num_heads, num_heads * head_dim,
-               (float)pow((double)head_dim, -0.5)};
+               (float)pow((double)head_dim, -0.5), klen};
   return attention_tc_launch(a, khi, klo, ldk, vthi, vtlo, ldvt, head_dim, (cudaStream_t)stream);
+}
+
+int og_attention_tc_fwd(const float* q, int64_t ldq, int64_t strideq, const float* khi, const float* klo, int64_t ldk,
+                        const float* vthi, const float* vtlo, int64_t ldvt, float* out, int64_t ldo, int64_t strideo,
+                        int batch, int nq, int nk, int num_heads, int head_dim, void* stream) {
+  return attention_tc_fwd_impl(q, ldq, strideq, khi, klo, ldk, vthi, vtlo, ldvt, out, ldo, strideo, batch, nq, nk, num_heads, head_dim,
+                               nullptr, stream);
+}
+
+int og_attention_tc_fwd_padded(const float* q, int64_t ldq, int64_t strideq, const float* khi, const float* klo, int64_t ldk,
+                               const float* vthi, const float* vtlo, int64_t ldvt, float* out, int64_t ldo, int64_t strideo,
+                               int batch, int nq, int nk, int num_heads, int head_dim, const int* key_lengths, void* stream) {
+  OG_CHECK_ARG(key_lengths, "attention_tc_padded: null key_lengths");
+  return attention_tc_fwd_impl(q, ldq, strideq, khi, klo, ldk, vthi, vtlo, ldvt, out, ldo, strideo, batch, nq, nk, num_heads, head_dim,
+                               key_lengths, stream);
 }
 
 int64_t og_sinkhorn_workspace_bytes(int batch, int n, int m) { return sinkhorn_workspace_bytes(batch, n, m); }
@@ -376,6 +455,34 @@ int og_sinkhorn_fwd(const float* S, int64_t lds, int64_t strideS, const float* d
   OG_CHECK_ARG(batch > 0 && n > 0 && m > 0 && iters >= 0 && reg > 0.f, "sinkhorn: bad sizes");
   return sinkhorn_launch(S, lds, strideS, dustbin, batch, n, m, iters, reg, scores, workspace, workspace_bytes,
                          (cudaStream_t)stream);
+}
+
+int og_sinkhorn_fwd_padded(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int batch, int n, int m,
+                           const int* lengths, int iters, float reg, float* scores, void* workspace, int64_t workspace_bytes,
+                           void* stream) {
+  OG_CHECK_ARG(S && dustbin && lengths && scores && workspace, "sinkhorn_padded: null pointer");
+  OG_CHECK_ARG(batch > 0 && n > 0 && m > 0 && iters >= 0 && reg > 0.f, "sinkhorn_padded: bad sizes");
+  return sinkhorn_launch(S, lds, strideS, dustbin, batch, n, m, iters, reg, scores, workspace, workspace_bytes,
+                         (cudaStream_t)stream, nullptr, nullptr, lengths);
+}
+
+int og_sinkhorn_consts(int n, int m, float* out) {
+  OG_CHECK_ARG(out && n > 0 && m > 0, "sinkhorn_consts: bad arguments");
+  const SinkConsts k = sinkhorn_consts(n, m);
+  out[0] = k.norm; out[1] = k.log_a_last; out[2] = k.log_b_last;
+  return OG_OK;
+}
+
+int og_sinkhorn_consts_padded(const int* lengths, int batch, int n, int m, float* out, void* stream) {
+  OG_CHECK_ARG(lengths && out && batch > 0 && n > 0 && m > 0, "sinkhorn_consts_padded: bad arguments");
+  OG_CHECK_ARG(n <= SINK_MAX_ROWS && m <= SINK_MAX_COLS, "sinkhorn_consts_padded: at most %d rows and %d columns", SINK_MAX_ROWS,
+               SINK_MAX_COLS);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (const int rc = sinkhorn_log_tables(st)) return rc;
+  SinkArgs a;
+  memset(&a, 0, sizeof(a));
+  a.B = batch; a.n = n; a.m = m; a.len_n = lengths; a.len_m = lengths + batch;
+  return OG_LAUNCH(sinkhorn_consts_kernel, cdiv(batch, 256), 256, 0, st, a, out);
 }
 
 int64_t og_sinkhorn_hist_floats(int batch, int n, int m, int iters) {
@@ -411,6 +518,14 @@ int og_match_fwd(const float* scores, int batch, int n, int m, float threshold, 
   OG_CHECK_ARG(batch > 0 && n > 0 && m > 0, "match: bad sizes");
   return match_launch(scores, batch, n, m, threshold, matches0, mscores0, matches1, mscores1, workspace,
                       workspace_bytes, (cudaStream_t)stream);
+}
+
+int og_match_fwd_padded(const float* scores, int batch, int n, int m, const int* lengths, float threshold, int64_t* matches0,
+                        float* mscores0, int64_t* matches1, float* mscores1, void* workspace, int64_t workspace_bytes, void* stream) {
+  OG_CHECK_ARG(scores && lengths && workspace, "match_padded: null pointer");
+  OG_CHECK_ARG(batch > 0 && batch <= 65535 && n > 0 && m > 0, "match_padded: bad sizes");
+  return match_launch(scores, batch, n, m, threshold, matches0, mscores0, matches1, mscores1, workspace,
+                      workspace_bytes, (cudaStream_t)stream, lengths);
 }
 
 int64_t og_gt_matches_workspace_bytes(int batch, int n, int m) {
@@ -818,10 +933,13 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
                          const float* kpts1, const float* side0, const float* side1, const float* desc0,
                          const float* desc1, const float* img_wh, float* ctx0, float* ctx1, float* scores,
                          int64_t* matches0, float* mscores0, int64_t* matches1, float* mscores1, void* workspace,
-                         int64_t workspace_bytes, void* stream_) {
+                         int64_t workspace_bytes, void* stream_, const int* lens = nullptr, const float* pair_wh = nullptr) {
   int rc = check_config(cfg);
   if (rc != OG_OK) return rc;
-  OG_CHECK_ARG(Wp && kpts0 && kpts1 && desc0 && desc1 && img_wh && scores && workspace, "forward: null pointer");
+  // padded batch (lens, pair_wh): pair b owns rows [0, lens[b]) of image 0 and [0, lens[B + b]) of image 1 of the capacity n, m
+  const bool padded = lens != nullptr;
+  OG_CHECK_ARG(Wp && kpts0 && kpts1 && desc0 && desc1 && (padded ? pair_wh != nullptr : img_wh != nullptr) && scores && workspace,
+               "forward: null pointer");
   OG_CHECK_ARG(cfg->side_info_size == 0 || (side0 && side1), "forward: side info missing");
   OG_CHECK_ARG(B > 0 && n > 0 && m > 0, "forward: batch, n, m must be positive");
   OG_CHECK_ARG(cfg->precision == OG_PREC_FP32 || (Whi && Wlo), "forward: the tensor-core modes need packed_hi / packed_lo");
@@ -838,7 +956,7 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
   const int prec = cfg->precision == OG_PREC_FP16X3 ? OG_PREC_TF32X3 : cfg->precision;     // what the non-f16 launches run as
   const Layout L = make_layout(cfg);
   Workspace w;
-  rc = plan_workspace(cfg, B, n, m, workspace, &w);
+  rc = plan_workspace(cfg, B, n, m, workspace, &w, padded);
   if (rc != OG_OK) return rc;
   if (workspace_bytes < w.total) return fail(OG_EWORKSPACE, "forward: workspace %lld < %lld bytes",
                                              (long long)workspace_bytes, (long long)w.total);
@@ -848,11 +966,28 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
   float* x0 = w.x; float* x1 = w.x + (int64_t)R0 * d;
 
   // ---- keypoint encoder (positional_encoding.py:16-19) + descriptors (superglue.py:52-55) ----
-  if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, S, img_wh[0] - 1.f, img_wh[1] - 1.f, w.in0)) != OG_OK)
-    return rc;
-  if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, S, img_wh[2] - 1.f, img_wh[3] - 1.f,
-                      w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
-    return rc;
+  // A padded batch zeroes its padding rows here and reads its descriptors from a copy with them zeroed: from the first kernel on
+  // every row is finite (the fp16 amax slots see every row, and a masked key with a NaN value would poison P.V: 0 * NaN = NaN).
+  const float* dsc0 = desc0;
+  const float* dsc1 = desc1;
+  if (padded) {
+    if ((rc = OG_LAUNCH(kenc_input_padded_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, n, S, lens, pair_wh, w.in0)) != OG_OK) return rc;
+    if ((rc = OG_LAUNCH(kenc_input_padded_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, m, S, lens + B, pair_wh + 2,
+                        w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
+      return rc;
+    float* d1m = w.desc + (int64_t)R0 * d;
+    if ((rc = OG_LAUNCH(mask_padded_rows_kernel, eltwise_grid((int64_t)R0 * d), 256, 0, st, desc0, (int64_t)R0, n, d, lens, w.desc)) != OG_OK)
+      return rc;
+    if ((rc = OG_LAUNCH(mask_padded_rows_kernel, eltwise_grid((int64_t)R1 * d), 256, 0, st, desc1, (int64_t)R1, m, d, lens + B, d1m)) != OG_OK)
+      return rc;
+    dsc0 = w.desc; dsc1 = d1m;
+  } else {
+    if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, S, img_wh[0] - 1.f, img_wh[1] - 1.f, w.in0)) != OG_OK)
+      return rc;
+    if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, S, img_wh[2] - 1.f, img_wh[3] - 1.f,
+                        w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
+      return rc;
+  }
   {
     const float* cur = w.in0;
     float* bufs[2] = {w.h0, w.h1};
@@ -866,10 +1001,10 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
         cur = bufs[i & 1];
       } else {                        // last layer: + local descriptors, per image (separate user tensors)
         og_linear_args a = lin(cur, kin, kin, Wp + L.kenc_w[i], Wp + L.kenc_b[i], R0, kout, x0, d);
-        if (!cfg->no_descriptors) { a.R = desc0; a.ldr = d; }          // superglue.py:45-55
+        if (!cfg->no_descriptors) { a.R = dsc0; a.ldr = d; }           // superglue.py:45-55
         if ((rc = linear_dispatch(a, OG_PREC_FP32, st)) != OG_OK) return rc;
         og_linear_args b = lin(cur + (int64_t)R0 * kin, kin, kin, Wp + L.kenc_w[i], Wp + L.kenc_b[i], R1, kout, x1, d);
-        if (!cfg->no_descriptors) { b.R = desc1; b.ldr = d; }
+        if (!cfg->no_descriptors) { b.R = dsc1; b.ldr = d; }
         if ((rc = linear_dispatch(b, OG_PREC_FP32, st)) != OG_OK) return rc;
       }
     }
@@ -978,19 +1113,21 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
     return OG_OK;
   };
 
-  // o[q] = attention of the queries q over the keys / values kv
+  // o[q] = attention of the queries q over the keys / values kv.  A padded batch gives each sequence its keys' length: lens is
+  // n_0 .. n_{B-1}, m_0 .. m_{B-1}, so image 0 (or both images as 2B sequences) starts at lens, image 1 at lens + B.
   auto attend = [&](const Seqs& q, const Seqs& kv) -> int {
     const float scale = (float)pow((double)dh, -0.5);
+    const int* klen = padded ? lens + (kv.img == 1 ? B : 0) : nullptr;
     if (att == Att::FP32) {
       const float* qkv_q = w.qkv + (int64_t)q.row0 * 3 * d;
       const float* qkv_kv = w.qkv + (int64_t)kv.row0 * 3 * d;
       AttnArgs a{qkv_q, 3 * d, (int64_t)q.len * 3 * d, qkv_kv + d, 3 * d, (int64_t)kv.len * 3 * d, qkv_kv + 2 * d, 3 * d,
-                 (int64_t)kv.len * 3 * d, w.o + (int64_t)q.row0 * d, d, (int64_t)q.len * d, q.count, q.len, kv.len, H, scale};
+                 (int64_t)kv.len * 3 * d, w.o + (int64_t)q.row0 * d, d, (int64_t)q.len * d, q.count, q.len, kv.len, H, scale, klen};
       return attention_simt_launch(a, dh, st);
     }
     const int64_t ldv = vt_ld(kv), voff = vt_off(kv), k0 = (int64_t)kv.row0 * d;
     TcAttnArgs a{w.q + (int64_t)q.row0 * d, d, (int64_t)q.len * d, w.o + (int64_t)q.row0 * d, d, (int64_t)q.len * d,
-                 q.count, q.len, kv.len, H, d, scale};
+                 q.count, q.len, kv.len, H, d, scale, klen};
     if (att == Att::TF32) return attention_tc_launch(a, w.khi + k0, w.klo + k0, d, w.vthi + voff, w.vtlo + voff, ldv, dh, st);
     const SeqSlots& s = ss[q.img == 1];
     return attention_f16_launch(a, F16AttnScales{s.q, s.k, s.v, s.o, 0}, kh16 + k0, kl16 + k0, d, vth16 + voff, vtl16 + voff, ldv, dh, st);
@@ -1053,12 +1190,15 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
     float* gr = w.g + (img ? (int64_t)R0 * d : 0);
     og_linear_args a = lin(xr, d, d, Wp + L.proj_w, Wp + L.proj_b, nn, d, gr, d);
     a.batch = B; a.strideA = (int64_t)nn * d; a.strideY = (int64_t)nn * d;
-    a.R = img ? desc1 : desc0; a.ldr = d; a.strideR = (int64_t)nn * d; a.rscale = Wp + L.proj_rmix;
+    a.R = img ? dsc1 : dsc0; a.ldr = d; a.strideR = (int64_t)nn * d; a.rscale = Wp + L.proj_rmix;
     float* ctx = img ? ctx1 : ctx0;
     if (ctx) { a.Yt = ctx; a.ldyt = nn; a.strideYt = (int64_t)d * nn; }
     SplitOut so;
     if (tcp && img == 1) { so.Yhi = w.ghi; so.Ylo = w.glo; }      // image-1 descriptors are the score GEMM's B operand
     if ((rc = linear_dispatch(a, prec, st, WH(L.proj_w), WL(L.proj_w), so)) != OG_OK) return rc;
+    if (padded && ctx &&
+        (rc = OG_LAUNCH(zero_padded_cols_kernel, eltwise_grid((int64_t)B * d * nn), 256, 0, st, ctx, B, d, nn, lens + (img ? B : 0))) != OG_OK)
+      return rc;
   }
   // ---- score matrix (superglue.py:64,80-86): S = g0^T g1 * d^-0.5, written with padded rows ----
   {
@@ -1069,11 +1209,11 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
   }
   // ---- optimal transport (superglue.py:88-111) + matches (matching_module.py:174-187) ----
   rc = sinkhorn_launch(w.sbuf, w.lds, (int64_t)n * w.lds, Wp + L.dustbin, B, n, m, cfg->sinkhorn_iters,
-                       cfg->sinkhorn_reg, scores, w.sink, w.sink_bytes, st);
+                       cfg->sinkhorn_reg, scores, w.sink, w.sink_bytes, st, nullptr, nullptr, lens);
   if (rc != OG_OK) return rc;
   if (matches0 || mscores0 || matches1 || mscores1) {
     rc = match_launch(scores, B, n, m, cfg->match_threshold, matches0, mscores0, matches1, mscores1, w.match,
-                      w.match_bytes, st);
+                      w.match_bytes, st, lens);
     if (rc != OG_OK) return rc;
   }
   return OG_OK;
@@ -1098,6 +1238,27 @@ int og_superglue_forward_f16(const og_config* cfg, const float* Wp, const float*
   return forward_impl(cfg, Wp, Whi, Wlo, static_cast<const __half*>(W16h), static_cast<const __half*>(W16l), meta16, B, n, m, kpts0, kpts1,
                       side0, side1, desc0, desc1, img_wh, ctx0, ctx1, scores, matches0, mscores0, matches1, mscores1, workspace,
                       workspace_bytes, stream);
+}
+
+int64_t og_workspace_bytes_padded(const og_config* cfg, int batch, int n, int m) {
+  if (check_config(cfg) != OG_OK) return -1;
+  if (batch <= 0 || n <= 0 || m <= 0) return fail(OG_EINVAL, "batch, n, m must be positive");
+  Workspace w;
+  if (plan_workspace(cfg, batch, n, m, nullptr, &w, true) != OG_OK) return -1;
+  return w.total;
+}
+
+int og_superglue_forward_padded(const og_config* cfg, const float* Wp, const float* Whi, const float* Wlo, const void* W16h,
+                                const void* W16l, const float* meta16, int B, int n, int m, const int* lengths,
+                                const float* image_sizes, const float* kpts0, const float* kpts1, const float* side0,
+                                const float* side1, const float* desc0, const float* desc1, float* ctx0, float* ctx1, float* scores,
+                                int64_t* matches0, float* mscores0, int64_t* matches1, float* mscores1, void* workspace,
+                                int64_t workspace_bytes, void* stream) {
+  OG_CHECK_ARG(lengths && image_sizes, "forward_padded: null lengths / image_sizes");
+  OG_CHECK_ARG(B <= 65535, "forward_padded: batch %d > 65535", B);
+  return forward_impl(cfg, Wp, Whi, Wlo, static_cast<const __half*>(W16h), static_cast<const __half*>(W16l), meta16, B, n, m, kpts0, kpts1,
+                      side0, side1, desc0, desc1, nullptr, ctx0, ctx1, scores, matches0, mscores0, matches1, mscores1, workspace,
+                      workspace_bytes, stream, lengths, image_sizes);
 }
 
 int64_t og_f16_meta_floats(const og_config* cfg) {
@@ -1159,18 +1320,36 @@ int og_linear_f16_fwd(const og_linear_args* a, const void* Wh16, const void* Wl1
                          "needs K >= 64, 16-byte aligned rows, exactly one output kind (Y | Yh,Yl | Yth,Ytl)", (cudaStream_t)stream);
 }
 
-int og_attention_f16_fwd(const float* q, int64_t ldq, int64_t strideq, const float* q_amax, const void* khi, const void* klo,
-                         int64_t ldk, const float* k_scale, const void* vthi, const void* vtlo, int64_t ldvt, const float* v_scale,
-                         float* out, int64_t ldo, int64_t strideo, float* out_amax, int batch, int nq, int nk, int num_heads,
-                         int head_dim, int swap_halves, void* stream) {
+static int attention_f16_fwd_impl(const float* q, int64_t ldq, int64_t strideq, const float* q_amax, const void* khi, const void* klo,
+                                  int64_t ldk, const float* k_scale, const void* vthi, const void* vtlo, int64_t ldvt,
+                                  const float* v_scale, float* out, int64_t ldo, int64_t strideo, float* out_amax, int batch, int nq,
+                                  int nk, int num_heads, int head_dim, int swap_halves, const int* klen, void* stream) {
   OG_CHECK_ARG(q && q_amax && khi && klo && k_scale && vthi && vtlo && v_scale && out, "attention_f16: null pointer");
   OG_CHECK_ARG(batch > 0 && nq > 0 && nk > 0 && num_heads > 0, "attention_f16: bad sizes");
   if (!attention_f16_eligible(head_dim, ldq, ldk, ldvt, ldo))
     return fail(OG_EUNSUPPORTED, "attention_f16: head_dim 64 and 16-byte aligned rows required");
-  TcAttnArgs a{q, ldq, strideq, out, ldo, strideo, batch, nq, nk, num_heads, num_heads * head_dim, (float)pow((double)head_dim, -0.5)};
+  TcAttnArgs a{q, ldq, strideq, out, ldo, strideo, batch, nq, nk, num_heads, num_heads * head_dim, (float)pow((double)head_dim, -0.5),
+               klen};
   F16AttnScales sc{q_amax, k_scale, v_scale, out_amax, swap_halves};
   return attention_f16_launch(a, sc, static_cast<const __half*>(khi), static_cast<const __half*>(klo), ldk,
                                 static_cast<const __half*>(vthi), static_cast<const __half*>(vtlo), ldvt, head_dim, (cudaStream_t)stream);
+}
+
+int og_attention_f16_fwd(const float* q, int64_t ldq, int64_t strideq, const float* q_amax, const void* khi, const void* klo,
+                         int64_t ldk, const float* k_scale, const void* vthi, const void* vtlo, int64_t ldvt, const float* v_scale,
+                         float* out, int64_t ldo, int64_t strideo, float* out_amax, int batch, int nq, int nk, int num_heads,
+                         int head_dim, int swap_halves, void* stream) {
+  return attention_f16_fwd_impl(q, ldq, strideq, q_amax, khi, klo, ldk, k_scale, vthi, vtlo, ldvt, v_scale, out, ldo, strideo, out_amax,
+                                batch, nq, nk, num_heads, head_dim, swap_halves, nullptr, stream);
+}
+
+int og_attention_f16_fwd_padded(const float* q, int64_t ldq, int64_t strideq, const float* q_amax, const void* khi, const void* klo,
+                                int64_t ldk, const float* k_scale, const void* vthi, const void* vtlo, int64_t ldvt,
+                                const float* v_scale, float* out, int64_t ldo, int64_t strideo, float* out_amax, int batch, int nq,
+                                int nk, int num_heads, int head_dim, const int* key_lengths, void* stream) {
+  OG_CHECK_ARG(key_lengths, "attention_f16_padded: null key_lengths");
+  return attention_f16_fwd_impl(q, ldq, strideq, q_amax, khi, klo, ldk, k_scale, vthi, vtlo, ldvt, v_scale, out, ldo, strideo, out_amax,
+                                batch, nq, nk, num_heads, head_dim, 0, key_lengths, stream);
 }
 
 }  // extern "C"

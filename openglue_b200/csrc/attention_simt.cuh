@@ -15,11 +15,13 @@ struct AttnArgs {
   float* out; int64_t ldo, strideo;
   int batch, nq, nk, num_heads;
   float scale;
+  const int* klen;           // padded batch (device, may be null): keys of sequence b = klen[b], clamped into [1, nk]
 };
+
 
 constexpr int ATQ = 64, ATK = 64;
 
-template <int DH>
+template <int DH, bool RAGGED>
 __global__ void __launch_bounds__(256) attention_simt_kernel(AttnArgs a) {
   constexpr int CPT = (DH >= 64) ? 4 : (DH >= 32 ? 2 : 1);     // output columns per thread
   extern __shared__ __align__(16) float og_attn_smem[];          // 64 KB at DH=64: dynamic
@@ -30,6 +32,7 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(AttnArgs a) {
 
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ATQ;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  const int nk = attention_keys<RAGGED>(a.klen, b, a.nk);
   const float* __restrict__ Q = a.q + (int64_t)b * a.strideq + h * DH;
   const float* __restrict__ Kp = a.k + (int64_t)b * a.stridek + h * DH;
   const float* __restrict__ Vp = a.v + (int64_t)b * a.stridev + h * DH;
@@ -49,16 +52,16 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(AttnArgs a) {
   }
   const bool pv_active = (tx * CPT < DH);
 
-  for (int k0 = 0; k0 < a.nk; k0 += ATK) {
+  for (int k0 = 0; k0 < nk; k0 += ATK) {
     __syncthreads();                                   // previous tile fully consumed (and Qt visible)
     for (int idx = tid; idx < ATK * DH; idx += 256) {
       const int r = idx % ATK, c = idx / ATK;
-      const bool ok = (k0 + r < a.nk);
+      const bool ok = (k0 + r < nk);
       Kt[c][r] = ok ? __ldg(Kp + (int64_t)(k0 + r) * a.ldk + c) : 0.f;
     }
     for (int idx = tid; idx < ATK * DH; idx += 256) {
       const int r = idx / DH, c = idx % DH;
-      Vs[r][c] = (k0 + r < a.nk) ? __ldg(Vp + (int64_t)(k0 + r) * a.ldv + c) : 0.f;
+      Vs[r][c] = (k0 + r < nk) ? __ldg(Vp + (int64_t)(k0 + r) * a.ldv + c) : 0.f;
     }
     __syncthreads();
 
@@ -83,7 +86,7 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(AttnArgs a) {
       float mx = -CUDART_INF_F;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        s[i][j] = (k0 + tx * 4 + j < a.nk) ? s[i][j] * a.scale : -CUDART_INF_F;
+        s[i][j] = (k0 + tx * 4 + j < nk) ? s[i][j] * a.scale : -CUDART_INF_F;
         mx = fmaxf(mx, s[i][j]);
       }
 #pragma unroll
@@ -137,8 +140,12 @@ inline int attention_simt_launch(const AttnArgs& a, int head_dim, cudaStream_t s
 #define OG_ATTN_CASE(DH_)                                                                        \
   case DH_: {                                                                                    \
     constexpr int smem = (DH_ * (ATQ + ATK) + ATK * DH_ + ATK * ATQ) * (int)sizeof(float);       \
-    if (const int rc = smem_opt_in<attention_simt_kernel<DH_>>(smem)) return rc;                 \
-    return OG_LAUNCH(attention_simt_kernel<DH_>, grid, 256, smem, stream, a);                    \
+    if (a.klen) {                                                                                \
+      if (const int rc = smem_opt_in<attention_simt_kernel<DH_, true>>(smem)) return rc;         \
+      return OG_LAUNCH((attention_simt_kernel<DH_, true>), grid, 256, smem, stream, a);          \
+    }                                                                                            \
+    if (const int rc = smem_opt_in<attention_simt_kernel<DH_, false>>(smem)) return rc;          \
+    return OG_LAUNCH((attention_simt_kernel<DH_, false>), grid, 256, smem, stream, a);           \
   }
   switch (head_dim) {
     OG_ATTN_CASE(8) OG_ATTN_CASE(16) OG_ATTN_CASE(32) OG_ATTN_CASE(64)

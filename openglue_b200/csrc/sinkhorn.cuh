@@ -27,7 +27,9 @@
 #include "tc_common.cuh"
 #include <math_constants.h>
 #include <algorithm>
+#include <mutex>
 #include <type_traits>
+#include <vector>
 
 namespace og {
 
@@ -47,6 +49,8 @@ struct SinkArgs {
   float* vglob;                          // resident kernel: [B, mpad] 64-bit words, v as each strip publishes its columns
   float* hist_u;                         // optional [B][iters][n+1]: u_t of every iteration  (kept for the backward pass,
   float* hist_v;                         // optional [B][iters+1][m+1]: v_t, row 0 = v_0 = 0   csrc/sinkhorn_bwd.cuh)
+  const int* len_n;                      // padded batch (the RAGGED kernels): pair b has len_n[b] rows and len_m[b] columns of the
+  const int* len_m;                      // capacity n x m (clamped into [1, n] / [1, m])
 };
 
 constexpr int SINK_WARPS = 8;
@@ -93,10 +97,13 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
 // W C columns; the warps exchange what they know of their segments through shared memory and one named barrier per row);
 // G = SINK_WARPS / W row groups = rows in progress per CTA.  A warp works on rows r0 + grp, r0 + grp + G, ... of its strip
 // [r0, r1) (row n is the dustbin row), columns [c0, c0 + C) of each.
-template <int V, int W>
+// n(a), m(a): the pair's rows and columns, a.n and a.m or, in a padded batch (R), its own lengths (set_lengths: r1 <= r0 for a
+// strip past them).
+template <int V, int W, bool R = false>
 struct SinkStrip {
   static constexpr int C = 128 * V, MC = W * C, G = SINK_WARPS / W;
   int b, strip, tid, lane, grp, sub, c0, r0, r1;
+  int n_ = 0, m_ = 0;
   template <class Args>
   __device__ __forceinline__ explicit SinkStrip(const Args& a) {
     b = blockIdx.x / a.SP; strip = blockIdx.x % a.SP;
@@ -106,6 +113,45 @@ struct SinkStrip {
     r0 = strip * a.rows_per_strip;
     r1 = min(r0 + a.rows_per_strip, a.n + 1);
   }
+  __device__ __forceinline__ void set_lengths(int n, int m, int rows_per_strip) {
+    n_ = n; m_ = m;
+    r1 = min(r0 + rows_per_strip, n + 1);
+  }
+  template <class Args> __device__ __forceinline__ int n(const Args& a) const { if constexpr (R) return n_; else return a.n; }
+  template <class Args> __device__ __forceinline__ int m(const Args& a) const { if constexpr (R) return m_; else return a.m; }
+};
+
+// The pair's lengths and the constants of its marginals (SinkConsts): the arguments' own, or in a padded batch (RAGGED) the pair's
+// from the tables of the host's logarithms (sinkhorn_log_tables), so that a pair at the capacity gets the very bits the uniform
+// kernel gets.
+constexpr int SINK_MAX_ROWS = 65536;                   // rows of a padded batch's capacity at most (the size of the tables)
+__device__ float og_sink_logf_tab[SINK_MAX_ROWS + SINK_MAX_COLS + 1];   // [k] = logf((float)k), the host's libm
+__device__ float og_sink_log_tab[SINK_MAX_ROWS + 1];                    // [k] = (float)log((double)k)
+template <bool RAGGED> struct SinkPair;
+template <> struct SinkPair<false> {                   // reads the arguments, as the uniform kernels always have
+  const SinkArgs& a;
+  __device__ __forceinline__ SinkPair(const SinkArgs& args, int) : a(args) {}
+  __device__ __forceinline__ int n() const { return a.n; }
+  __device__ __forceinline__ int m() const { return a.m; }
+  __device__ __forceinline__ float norm() const { return a.norm; }
+  __device__ __forceinline__ float log_a_last() const { return a.log_a_last; }
+  __device__ __forceinline__ float log_b_last() const { return a.log_b_last; }
+};
+template <> struct SinkPair<true> {
+  int n_, m_;
+  float norm_, la_, lb_;
+  __device__ __forceinline__ SinkPair(const SinkArgs& a, int b) {
+    n_ = min(max(__ldg(a.len_n + b), 1), a.n);
+    m_ = min(max(__ldg(a.len_m + b), 1), a.m);
+    norm_ = -og_sink_logf_tab[n_ + m_];
+    la_ = norm_ + og_sink_log_tab[m_];
+    lb_ = norm_ + og_sink_log_tab[n_];
+  }
+  __device__ __forceinline__ int n() const { return n_; }
+  __device__ __forceinline__ int m() const { return m_; }
+  __device__ __forceinline__ float norm() const { return norm_; }
+  __device__ __forceinline__ float log_a_last() const { return la_; }
+  __device__ __forceinline__ float log_b_last() const { return lb_; }
 };
 
 // One warp's slice of the shared-memory row ring, fed by bulk async copies (TMA 1-D) so that HBM latency overlaps the math of
@@ -113,26 +159,28 @@ struct SinkStrip {
 // `consumed` counts the real rows taken so far and gives each its slot and phase.  EVICT_FIRST loads with the L2 evict_first
 // policy (the forward pass): at the headline shape the score matrix is five times the 50 MB L2 and is swept cyclically, so
 // its lines would hit nothing and only push out those of the kernels that follow.
-template <int V, int W, int SLOTS, bool EVICT_FIRST, class Args>
+template <int V, int W, int SLOTS, bool EVICT_FIRST, class Args, bool R = false>
 struct SinkRowRing {
   static constexpr int C = 128 * V, G = SINK_WARPS / W;
   float* slot;                                         // [SLOTS][C]
   uint64_t* bar;                                       // [SLOTS]
   const Args& a;
   const float* seg;                                    // this warp's column segment of row 0 of the pair
-  int first, end_real, c0, lane;                       // first row of the warp; rows >= end_real do not exist in memory
+  int first, end_real, n, c0, lane;                    // first row of the warp; rows >= end_real do not exist in memory; row n: dustbin
+                                                       // (R; a.n otherwise)
   uint32_t bytes, consumed;                            // bytes of a segment: 0 when it lies beyond the last column
   bool full;                                           // the whole segment lies inside the row (warp-uniform)
   float dz;                                            // the dustbin score divided by reg, Z = M / reg
   uint64_t policy;
 
-  __device__ __forceinline__ SinkRowRing(const Args& args, const SinkStrip<V, W>& s, float* ring, uint64_t* bars) : a(args) {
+  __device__ __forceinline__ SinkRowRing(const Args& args, const SinkStrip<V, W, R>& s, float* ring, uint64_t* bars) : a(args) {
     const int warp = s.grp * W + s.sub;
     slot = ring + warp * SLOTS * C;
     bar = bars + warp * SLOTS;
     seg = a.S + (int64_t)s.b * a.strideS + s.c0;
     first = s.r0 + s.grp;
-    end_real = min(s.r1, a.n);
+    end_real = min(s.r1, s.n(a));
+    n = s.n(a);
     c0 = s.c0; lane = s.lane;
     const int seg_cols = min(a.m, c0 + C) - c0;        // <= 0: this warp's segment lies beyond the last column
     bytes = seg_cols > 0 ? (uint32_t)(((seg_cols + 3) / 4) * 16) : 0u;     // <= 4 * (lds - c0): inside the padded row
@@ -168,10 +216,10 @@ struct SinkRowRing {
     }
   }
 
-  // This warp's segment of row `row` in registers (columns >= m zero, divided by reg), and the slot refilled with the row SLOTS
+  // This warp's segment of row `row` in registers (columns >= a.m zero, divided by reg), and the slot refilled with the row SLOTS
   // ahead.  The dustbin row is the constant dustbin score.
   __device__ __forceinline__ void take(int row, float4 (&z)[V]) {
-    if (row >= a.n) {
+    if (row >= (R ? n : a.n)) {
 #pragma unroll
       for (int k = 0; k < V; ++k) z[k] = make_float4(dz, dz, dz, dz);
       return;
@@ -220,8 +268,8 @@ struct SinkRowRing {
 // The W warps of a row group publish one value each (`mine`) and meet at the group's named barrier; the returned W values are
 // in warp order, the same in every warp.  The buffer xr [2][G][W] alternates halves row by row (rowpar), so a warp that runs
 // ahead into the next row cannot overwrite values another warp has yet to read.
-template <int V, int W, class X>
-__device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkStrip<V, W>& s, uint32_t& rowpar) {
+template <int V, int W, bool R, class X>
+__device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkStrip<V, W, R>& s, uint32_t& rowpar) {
   X* x = xr + (rowpar * SinkStrip<V, W>::G + s.grp) * W;
   if (s.lane == 0) x[s.sub] = mine;
   asm volatile("bar.sync %0, %1;" ::"r"(1 + s.grp), "n"(W * 32) : "memory");
@@ -234,10 +282,10 @@ __device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkS
 // memory (buffer k & 1 of two) -> barrier among the SP CTAs of the pair -> every CTA of the pair rebuilds the sums in the same
 // fixed order (bitwise identical across CTAs) and calls update(j, sum) for j < m and update(MC, sum) for the dustbin column.
 // sink_strip_sums is its first part: the strip's column sums, passed to store(j, sum) for j <= m.
-template <int V, int W, class Args, class Store>
-__device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
+template <int V, int W, bool R, class Args, class Store>
+__device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V, W, R>& s, float* red, const float4 (&cacc)[V],
                                                 float cacc_m, Store store) {
-  const int m = a.m;
+  const int m = s.m(a);
   float* myred = red + s.grp * a.mpad;
 #pragma unroll
   for (int q = 0; q < V; ++q) {
@@ -255,10 +303,10 @@ __device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V
   }
 }
 
-template <int V, int W, class Args, class Update>
-__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
+template <int V, int W, bool R, class Args, class Update>
+__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W, R>& s, float* red, const float4 (&cacc)[V],
                                                    float cacc_m, int k, Update update) {
-  const int m = a.m;
+  const int m = s.m(a);
   const int64_t buf = (int64_t)(k & 1) * a.B * a.SP + (int64_t)s.b * a.SP;
   float* part = a.partial + (buf + s.strip) * a.mpad;
   sink_strip_sums(a, s, red, cacc, cacc_m, [&](int j, float sum) { part[j] = sum; });
@@ -293,12 +341,12 @@ template <int NR> using SinkRowStat = std::conditional_t<NR == 1, float2, float4
 // share e_ij a_i / S_i of the column sums, added to cacc (cacc_m: the dustbin column, counted by segment 0) row by row in order.
 // v_s: v of the pair in shared memory, v_m = v_s[MC].  Two rows share one read of v and one exchange, and their reduction chains
 // are independent, so one row's shuffles run under the other's exponentials; each row's arithmetic is the same for NR = 1 and 2.
-template <int V, int W, int NR>
-__device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkStrip<V, W>& s, const float4 (*q)[V], const float* v_s,
-                                              float v_m, float dz, float a_reg, float a_last, SinkRowStat<NR>* xr, uint32_t& rowpar,
-                                              int row0, int it, f32x2 (&cacc)[2 * V], float& cacc_m) {
+template <int V, int W, int NR, bool R>
+__device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkPair<R>& P, const SinkStrip<V, W, R>& s, const float4 (*q)[V],
+                                              const float* v_s, float v_m, float dz, float a_reg, float a_last, SinkRowStat<NR>* xr,
+                                              uint32_t& rowpar, int row0, int it, f32x2 (&cacc)[2 * V], float& cacc_m) {
   static_assert(NR == 1 || NR == 2, "one or two rows at a time");
-  const int n = a.n, c0 = s.c0, lane = s.lane, sub = s.sub;
+  const int n = P.n(), c0 = s.c0, lane = s.lane, sub = s.sub;
   const f32x2 log2e2 = pk2(LOG2E_F, LOG2E_F);
   f32x2 z[NR][2 * V];
 #pragma unroll
@@ -372,9 +420,9 @@ __device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkStrip
 #pragma unroll
     for (int r = 0; r < NR; ++r) {
       const int row = row0 + r * SinkStrip<V, W>::G;
-      const float u_i = ((row < n) ? a.norm : a.log_a_last) - (mxg[r] + logf(s_i[r]));
-      if (it == a.iters - 1) a.u[(int64_t)s.b * (n + 1) + row] = u_i;
-      if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (n + 1) + row] = u_i;
+      const float u_i = ((row < n) ? P.norm() : P.log_a_last()) - (mxg[r] + logf(s_i[r]));
+      if (it == a.iters - 1) a.u[(int64_t)s.b * (a.n + 1) + row] = u_i;
+      if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (a.n + 1) + row] = u_i;
     }
   }
 #pragma unroll
@@ -386,37 +434,48 @@ __device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkStrip
   }
 }
 
-// The final pass over one row: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111)
-template <int V, int W>
-__device__ __forceinline__ void sink_fwd_score_row(const SinkArgs& a, const SinkStrip<V, W>& s, const float4 (&z)[V], const float* v_s,
-                                                   float v_m, float dz, int row) {
-  const int n = a.n, m = a.m, c0 = s.c0, lane = s.lane;
+// The final pass over one row: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111).  Rows are a.m + 1 apart.
+template <int V, int W, bool R>
+__device__ __forceinline__ void sink_fwd_score_row(const SinkArgs& a, const SinkPair<R>& P, const SinkStrip<V, W, R>& s, const float4 (&z)[V],
+                                                   const float* v_s, float v_m, float dz, int row) {
+  const int m = P.m(), c0 = s.c0, lane = s.lane;
   float u_i = 0.f;
   if (a.iters > 0) {
-    if (lane == 0) u_i = __ldcg(a.u + (int64_t)s.b * (n + 1) + row);
+    if (lane == 0) u_i = __ldcg(a.u + (int64_t)s.b * (a.n + 1) + row);
     u_i = __shfl_sync(0xffffffffu, u_i, 0);
   }
-  float* out = a.scores + ((int64_t)s.b * (n + 1) + row) * (m + 1);
+  float* out = a.scores + ((int64_t)s.b * (a.n + 1) + row) * (a.m + 1);
 #pragma unroll
   for (int k = 0; k < V; ++k) {
     const int c = c0 + 4 * (lane + 32 * k);
     if (c < m) {
       const float4 vv = *reinterpret_cast<const float4*>(v_s + c);
-      if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - a.norm;
-      if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - a.norm;
-      if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - a.norm;
-      if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - a.norm;
+      if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - P.norm();
+      if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - P.norm();
+      if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - P.norm();
+      if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - P.norm();
     }
   }
-  if (s.sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - a.norm;
+  if (s.sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - P.norm();
+}
+
+// Padded batch, after the final pass: -inf over the strip's share of the padding of the pair's [a.n + 1, a.m + 1] block, the
+// columns past its dustbin column in its rows and every column of the capacity's rows past its dustbin row.
+template <int V, int W>
+__device__ __forceinline__ void sink_fill_padding(const SinkArgs& a, const SinkStrip<V, W, true>& s) {
+  const int rend = min(s.r0 + a.rows_per_strip, a.n + 1);
+  for (int row = s.r0; row < rend; ++row) {
+    float* out = a.scores + ((int64_t)s.b * (a.n + 1) + row) * (a.m + 1);
+    for (int c = (row <= s.n_ ? s.m_ + 1 : 0) + s.tid; c <= a.m; c += blockDim.x) out[c] = -CUDART_INF_F;
+  }
 }
 
 // SLOTS: ring depth per warp.  Configurations with V <= 8 need <= 128 registers and <= 106 KB of shared memory: two CTAs per
 // SM, so one CTA streams while the other sits in its per-iteration reduction / barrier phase.
-template <int V, int W, int SLOTS>
-__global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_kernel(SinkArgs a) {
+template <int V, int W, int SLOTS, bool RAGGED>
+__device__ __forceinline__ void sinkhorn_sweeps(const SinkArgs& a) {
   extern __shared__ __align__(128) float og_sink_smem[];
-  using Strip = SinkStrip<V, W>;
+  using Strip = SinkStrip<V, W, RAGGED>;
   constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G;
   float* v_s = og_sink_smem;                           // [MC + 4]  v_j for j < m, -inf for m <= j < MC (masks the padding
                                                        //           columns in the sweep without per-element selects), v_s[MC] = v_dustbin
@@ -424,10 +483,13 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
   float* ring = red + G * a.mpad;                      // [SINK_WARPS][SLOTS][C]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);   // [SINK_WARPS][SLOTS]
   float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS * SLOTS);             // [2][G][W] (max, sum) of a segment
-  const Strip s(a);
-  const int m = a.m;
-  const float a_reg = expf(a.norm), a_last = expf(a.log_a_last);
-  SinkRowRing<V, W, SLOTS, true, SinkArgs> rows(a, s, ring, bars);
+  Strip strip(a);
+  const SinkPair<RAGGED> P(a, strip.b);
+  if (RAGGED) strip.set_lengths(P.n(), P.m(), a.rows_per_strip);
+  const Strip& s = strip;
+  const int m = P.m();
+  const float a_reg = expf(P.norm()), a_last = expf(P.log_a_last());
+  SinkRowRing<V, W, SLOTS, true, SinkArgs, RAGGED> rows(a, s, ring, bars);
   const float dz = rows.dz;
 
   for (int j = s.tid; j < MC; j += blockDim.x) v_s[j] = (j < m) ? 0.f : -CUDART_INF_F;
@@ -446,14 +508,14 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
     for (int row = s.r0 + s.grp; row < s.r1; row += G) {
       float4 q[V];
       rows.take(row, q);
-      sink_fwd_rows<V, W, 1>(a, s, &q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
+      sink_fwd_rows<V, W, 1>(a, P, s, &q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
     }
     rows.prime();                                      // next sweep's (or the final pass's) first rows fly during the reduction
     float4 c4[V];
 #pragma unroll
     for (int k = 0; k < V; ++k) { upk2(cacc[2 * k], c4[k].x, c4[k].y); upk2(cacc[2 * k + 1], c4[k].z, c4[k].w); }
     sink_column_reduce(a, s, red, c4, cacc_m, it, [&](int j, float c) {
-      v_s[j] = ((j < MC) ? a.norm : a.log_b_last) + v_s[j] - logf(c);
+      v_s[j] = ((j < MC) ? P.norm() : P.log_b_last()) + v_s[j] - logf(c);
     });
     if (a.hist_v && s.strip == 0) {                   // every CTA of the pair holds the same v: one of them records it
       float* hv = a.hist_v + ((int64_t)s.b * (a.iters + 1) + it + 1) * (m + 1);
@@ -465,8 +527,18 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
   for (int row = s.r0 + s.grp; row < s.r1; row += G) {
     float4 z[V];
     rows.take(row, z);
-    sink_fwd_score_row(a, s, z, v_s, v_m, dz, row);
+    sink_fwd_score_row(a, P, s, z, v_s, v_m, dz, row);
   }
+  if constexpr (RAGGED) sink_fill_padding(a, s);
+}
+template <int V, int W, int SLOTS>
+__global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_kernel(SinkArgs a) {
+  sinkhorn_sweeps<V, W, SLOTS, false>(a);
+}
+// The padded batch's form: each pair's own lengths (SinkArgs::len_n / len_m) in the capacity's layout and plan.
+template <int V, int W, int SLOTS>
+__global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_padded_kernel(SinkArgs a) {
+  sinkhorn_sweeps<V, W, SLOTS, true>(a);
 }
 
 // A value and the iteration (from 1) it belongs to, as one 64-bit word: a single-copy-atomic store and load carry both, so a reader
@@ -504,11 +576,11 @@ __device__ __forceinline__ void sink_take(float (&x)[N], At at, uint32_t tag) {
 // The resident kernel's form of sink_strip_sums, in half the shared memory: the upper half of the row groups parks its column sums
 // in red [G/2][mpad] (the dustbin column in redm [G]), the lower half adds its own to them, and store(j, sum) gets the G/2 folded
 // sums added in order (a fixed order: the same bits in every run).
-template <int V, int W, class Args, class Store>
-__device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const SinkStrip<V, W>& s, float* red, float* redm,
+template <int V, int W, bool R, class Args, class Store>
+__device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const SinkStrip<V, W, R>& s, float* red, float* redm,
                                                        const float4 (&cacc)[V], float cacc_m, Store store) {
   constexpr int H = SinkStrip<V, W>::G / 2;
-  const int m = a.m;
+  const int m = s.m(a);
   float4* fold = reinterpret_cast<float4*>(red + (s.grp % H) * a.mpad);
   if (s.grp >= H) {
 #pragma unroll
@@ -551,11 +623,11 @@ __device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const Sink
 // v back.  Partials and v travel as (value, iteration + 1) words (sink_put / sink_take), so a reader waits for exactly the words it
 // needs and the pair needs no barrier: a strip writes its next partials only after it has read all of v, which every owner
 // publishes only after it has read all partials of its columns, so one buffer of each suffices.  Both are zeroed before each launch.
-template <int V, int W, int RR>
-__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(SinkArgs a) {
+template <int V, int W, int RR, bool RAGGED>
+__device__ __forceinline__ void sinkhorn_resident_sweeps(const SinkArgs& a) {
   static_assert(RR % 2 == 0, "the register rows go two at a time");
   extern __shared__ __align__(128) float og_sink_smem[];
-  using Strip = SinkStrip<V, W>;
+  using Strip = SinkStrip<V, W, RAGGED>;
   constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G, NT = SINK_WARPS * 32, HS = SINK_WARPS * (C / 4);
   const int slots = max(a.rows_smem, 1);
   float* v_s = og_sink_smem;                                              // [MC + 4]  as in sinkhorn_kernel
@@ -566,11 +638,14 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
   float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS);             // [2][G][W]  one row's (max, sum)
   float4* xr2 = reinterpret_cast<float4*>(xr + 2 * G * W);               // [2][G][W]  two rows'
   float* redm = reinterpret_cast<float*>(xr2 + 2 * G * W);               // [G]
-  const Strip s(a);
-  const int m = a.m, lane = s.lane, row0 = s.r0 + s.grp;
-  const float a_reg = expf(a.norm), a_last = expf(a.log_a_last);
+  Strip strip(a);
+  const SinkPair<RAGGED> P(a, strip.b);
+  if (RAGGED) strip.set_lengths(P.n(), P.m(), a.rows_per_strip);
+  const Strip& s = strip;
+  const int m = P.m(), lane = s.lane, row0 = s.r0 + s.grp;
+  const float a_reg = expf(P.norm()), a_last = expf(P.log_a_last());
   float4* mine = held + (s.grp * W + s.sub) * (C / 4);
-  SinkRowRing<V, W, 1, true, SinkArgs> rows(a, s, reinterpret_cast<float*>(held + (size_t)(slots - 1) * HS), bars);
+  SinkRowRing<V, W, 1, true, SinkArgs, RAGGED> rows(a, s, reinterpret_cast<float*>(held + (size_t)(slots - 1) * HS), bars);
   const float dz = rows.dz;
   uint64_t* vg = reinterpret_cast<uint64_t*>(a.vglob) + (int64_t)s.b * a.mpad;
 
@@ -589,11 +664,11 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
     float cacc_m = 0.f;
     const float v_m = v_s[MC];
     auto one = [&](int row, const float4 (*q)[V]) {
-      sink_fwd_rows<V, W, 1>(a, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
+      sink_fwd_rows<V, W, 1>(a, P, s, q, v_s, v_m, dz, a_reg, a_last, xr, rowpar, row, it, cacc, cacc_m);
     };
     if (it == 0 || last) {
       auto visit = [&](int row, const float4 (&q)[V]) {
-        if (last) sink_fwd_score_row(a, s, q, v_s, v_m, dz, row);
+        if (last) sink_fwd_score_row(a, P, s, q, v_s, v_m, dz, row);
         else one(row, &q);
       };
 #pragma unroll
@@ -617,10 +692,13 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
         }
         visit(row, q);
       }
-      if (last) break;
+      if (last) {
+        if constexpr (RAGGED) sink_fill_padding(a, s);
+        break;
+      }
     } else {
       auto two = [&](int row, const float4 (*q)[V]) {
-        sink_fwd_rows<V, W, 2>(a, s, q, v_s, v_m, dz, a_reg, a_last, xr2, rowpar, row, it, cacc, cacc_m);
+        sink_fwd_rows<V, W, 2>(a, P, s, q, v_s, v_m, dz, a_reg, a_last, xr2, rowpar, row, it, cacc, cacc_m);
       };
 #pragma unroll
       for (int k = 0; k < RR; k += 2) {
@@ -656,7 +734,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
     // order (a fixed order: the same bits in every run)
     const int S = cdiv(m + 1, a.SP), lo = s.strip * S, NG = S >= NT ? 1 : NT / S;
     auto publish = [&](int j, float c) {
-      sink_put(vg + j, ((j < m) ? a.norm + v_s[j] : a.log_b_last + v_s[MC]) - logf(c), tag);
+      sink_put(vg + j, ((j < m) ? P.norm() + v_s[j] : P.log_b_last() + v_s[MC]) - logf(c), tag);
     };
     for (int i = s.tid; i < S * NG; i += NT) {
       const int j = lo + i % S;
@@ -691,6 +769,14 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(S
     }
     __syncthreads();
   }
+}
+template <int V, int W, int RR>
+__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(SinkArgs a) {
+  sinkhorn_resident_sweeps<V, W, RR, false>(a);
+}
+template <int V, int W, int RR>
+__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_padded_kernel(SinkArgs a) {
+  sinkhorn_resident_sweeps<V, W, RR, true>(a);
 }
 
 // resident: the plan is for sinkhorn_resident_kernel (slots = 1, occ = 1); rows_reg / rows_smem: rows per warp in registers /
@@ -832,17 +918,62 @@ inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
   return SINK_BARRIER_BYTES + align_up((int64_t)B * (n + 1) * 4, 256) + align_up(rows * p.mpad * 4, 256);
 }
 
-template <int V, int W>
+// The tables sink_pair<true> reads, from the host's own logf / log (bit for bit what sinkhorn_consts computes), copied to the
+// current device at its first padded Sinkhorn.  That copy is synchronous, so it cannot be part of a stream capture: a capture
+// needs one padded call on the device before it.
+inline int sinkhorn_log_tables(cudaStream_t stream) {
+  static bool done[OG_MAX_DEVICES] = {};
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  bool& d = done[current_device()];
+  if (d) return OG_OK;
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  OG_CUDA(cudaStreamIsCapturing(stream, &cap));
+  if (cap != cudaStreamCaptureStatusNone)
+    return fail(OG_EUNSUPPORTED, "sinkhorn (padded): the first padded call on a device uploads its tables and cannot be captured; "
+                                 "run one padded call before the capture");
+  static std::vector<float> lf, l;
+  if (lf.empty()) {
+    lf.resize(SINK_MAX_ROWS + SINK_MAX_COLS + 1); l.resize(SINK_MAX_ROWS + 1);
+    for (size_t k = 0; k < lf.size(); ++k) lf[k] = logf((float)k);
+    for (size_t k = 0; k < l.size(); ++k) l[k] = (float)log((double)k);
+  }
+  OG_CUDA(cudaMemcpyToSymbol(og_sink_logf_tab, lf.data(), lf.size() * sizeof(float)));
+  OG_CUDA(cudaMemcpyToSymbol(og_sink_log_tab, l.data(), l.size() * sizeof(float)));
+  d = true;
+  return OG_OK;
+}
+
+template <int V, int W, bool RAGGED>
 inline int sinkhorn_resident_launch(const SinkArgs& a, const SinkPlan& p, cudaStream_t stream) {
-  constexpr auto kernel = sinkhorn_resident_kernel<V, W, 16 / V>;
+  constexpr auto kernel = RAGGED ? sinkhorn_resident_padded_kernel<V, W, 16 / V> : sinkhorn_resident_kernel<V, W, 16 / V>;
   if (const int rc = smem_opt_in<kernel>((int)OG_SMEM_OPTIN_MAX)) return rc;
   return launch("sinkhorn_resident_kernel", kernel, LaunchAttr::cooperative, dim3(a.B * a.SP), dim3(SINK_WARPS * 32), p.smem,
                 stream, a);
 }
 
+template <bool RAGGED>
+inline int sinkhorn_kernel_launch(const SinkArgs& a, const SinkPlan& p, cudaStream_t stream) {
+  if (p.resident) {
+    if (p.W == 1) return sinkhorn_resident_launch<4, 1, RAGGED>(a, p, stream);
+    return p.V == 4 ? sinkhorn_resident_launch<4, 2, RAGGED>(a, p, stream) : sinkhorn_resident_launch<8, 2, RAGGED>(a, p, stream);
+  }
+  if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<4, 1, 2> : sinkhorn_kernel<4, 1, 2>, 4, 1, 2>(a, p, stream);
+  if (p.V == 4)             return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<4, 2, 2> : sinkhorn_kernel<4, 2, 2>, 4, 2, 2>(a, p, stream);
+  if (p.V == 8)             return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<8, 2, 2> : sinkhorn_kernel<8, 2, 2>, 8, 2, 2>(a, p, stream);
+  if (p.W == 2)
+    return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<16, 2, 2> : sinkhorn_kernel<16, 2, 2>, 16, 2, 2>(a, p, stream);
+  return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<16, 4, 1> : sinkhorn_kernel<16, 4, 1>, 16, 4, 1>(a, p, stream);
+}
+
+// lens (padded batch, device): n_0 .. n_{B-1}, then m_0 .. m_{B-1}; n, m are the capacity and the plan is the capacity's.
 inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int B, int n, int m,
                            int iters, float reg, float* scores, void* ws, int64_t ws_bytes, cudaStream_t stream,
-                           float* hist_u = nullptr, float* hist_v = nullptr) {
+                           float* hist_u = nullptr, float* hist_v = nullptr, const int* lens = nullptr) {
+  if (lens && (hist_u || hist_v)) return fail(OG_EUNSUPPORTED, "sinkhorn: no training form for a padded batch");
+  if (lens && n > SINK_MAX_ROWS) return fail(OG_EUNSUPPORTED, "sinkhorn: a padded batch has at most %d rows, not %d", SINK_MAX_ROWS, n);
+  if (lens)
+    if (const int rc = sinkhorn_log_tables(stream)) return rc;
   SinkPlan p;
   const bool resident = !hist_u && !hist_v && sink_resident_mode() && sinkhorn_resident_plan(B, n, m, &p);
   if (!resident) {
@@ -870,15 +1001,9 @@ inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const f
     if (p.resident) OG_CUDA(cudaMemsetAsync(partial, 0, 8LL * (p.SP + 1) * p.pairs_per_launch * p.mpad, stream));
     a.hist_u = hist_u ? hist_u + (int64_t)b0 * iters * (n + 1) : nullptr;
     a.hist_v = hist_v ? hist_v + (int64_t)b0 * (iters + 1) * (m + 1) : nullptr;
-    if (p.resident) {
-      if (p.W == 1) return sinkhorn_resident_launch<4, 1>(a, p, stream);
-      return p.V == 4 ? sinkhorn_resident_launch<4, 2>(a, p, stream) : sinkhorn_resident_launch<8, 2>(a, p, stream);
-    }
-    if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<sinkhorn_kernel<4, 1, 2>, 4, 1, 2>(a, p, stream);
-    if (p.V == 4)             return sinkhorn_coop_launch<sinkhorn_kernel<4, 2, 2>, 4, 2, 2>(a, p, stream);
-    if (p.V == 8)             return sinkhorn_coop_launch<sinkhorn_kernel<8, 2, 2>, 8, 2, 2>(a, p, stream);
-    if (p.W == 2)             return sinkhorn_coop_launch<sinkhorn_kernel<16, 2, 2>, 16, 2, 2>(a, p, stream);
-    return sinkhorn_coop_launch<sinkhorn_kernel<16, 4, 1>, 16, 4, 1>(a, p, stream);
+    a.len_n = lens ? lens + b0 : nullptr;
+    a.len_m = lens ? lens + B + b0 : nullptr;
+    return lens ? sinkhorn_kernel_launch<true>(a, p, stream) : sinkhorn_kernel_launch<false>(a, p, stream);
   });
 }
 

@@ -17,7 +17,7 @@ CUDA tensors only, and no autograd: the reference never differentiates these out
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn as nn
@@ -26,7 +26,8 @@ from . import _cabi
 from ._cabi import ptr, stream
 from .superglue import SuperGlue
 
-__all__ = ['LAFConverter', 'get_laf_to_sideinfo_converter', 'prepare_features_output', 'compact_matches', 'OpenGlueMatcher']
+__all__ = ['LAFConverter', 'get_laf_to_sideinfo_converter', 'prepare_features_output', 'compact_matches', 'pad_features',
+           'OpenGlueMatcher']
 
 # method name -> (og_laf_method, side-information columns after the response)
 _METHODS = {'none': (0, 0), 'scale': (1, 1), 'rotation': (2, 2), 'scale_rotation': (3, 3), 'affine': (4, 5)}
@@ -136,6 +137,41 @@ def compact_matches(matches0: torch.Tensor, mscores0: torch.Tensor, lafs0: torch
             'lafs0': l0[:nc][None], 'lafs1': l1[:nc][None], 'keypoints0': k0[:nc], 'keypoints1': k1[:nc]}
 
 
+def pad_features(features: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]], capacity: Optional[int] = None
+                 ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """One batch from images with their own keypoint counts, without dropping any: the lossless counterpart of the reference's
+    ``min_stack`` (models/features/utils.py:28-52), which trims every image to the smallest count.  ``features``: one
+    ``(lafs [1,N_b,2,3] | [N_b,2,3], responses [1,N_b] | [N_b], descriptors [1,N_b,D] | [N_b,D])`` per image, as
+    ``OpenCVSIFT.extract_batch`` returns them.  -> zero-padded ``lafs`` [B,N,2,3], ``responses`` [B,N], ``descriptors`` [B,N,D]
+    with N = ``capacity`` (default: the largest N_b), and ``num_keypoints`` [B] (int64, on the host): the matcher's
+    ``num_keypoints0`` / ``num_keypoints1``."""
+    feats: List[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = []
+    for lafs, resp, desc in features:
+        if lafs.dim() == 4:
+            lafs, resp, desc = lafs[0], resp[0], desc[0]
+        if lafs.dim() != 3 or lafs.shape[1:] != (2, 3) or resp.shape != lafs.shape[:1] or desc.dim() != 2 or desc.shape[0] != lafs.shape[0]:
+            raise ValueError('each feature set must be (lafs [N,2,3], responses [N], descriptors [N,D]), optionally with a leading 1')
+        feats.append((lafs, resp, desc))
+    if not feats:
+        raise ValueError('pad_features needs at least one feature set')
+    counts = [f[0].shape[0] for f in feats]
+    D = feats[0][2].shape[1]
+    if any(f[2].shape[1] != D for f in feats):
+        raise ValueError('descriptors of different widths')
+    N = max(counts) if capacity is None else int(capacity)
+    if N < max(counts):
+        raise ValueError(f'capacity {N} is below the largest keypoint count {max(counts)}')
+    dev = feats[0][0].device
+    B = len(feats)
+    lafs = torch.zeros(B, N, 2, 3, dtype=torch.float32, device=dev)
+    resp = torch.zeros(B, N, dtype=torch.float32, device=dev)
+    desc = torch.zeros(B, N, D, dtype=torch.float32, device=dev)
+    for b, (l, r, d) in enumerate(feats):
+        k = l.shape[0]
+        lafs[b, :k], resp[b, :k], desc[b, :k] = l, r, d
+    return lafs, resp, desc, torch.tensor(counts, dtype=torch.int64)
+
+
 class OpenGlueMatcher(nn.Module):
     """Drop-in for the reference's ``inference.OpenGlueMatcher`` (inference.py:81-211): correspondences between two images from
     local features followed by SuperGlue.
@@ -145,7 +181,9 @@ class OpenGlueMatcher(nn.Module):
     optional ``superglue.log_transform_response`` and ``inference.match_threshold``.
 
     ``forward(data)`` takes ``image0`` / ``image1`` [B,1,H,W] and, optionally, pre-extracted ``lafs{0,1}``, ``descriptors{0,1}``,
-    ``responses{0,1}`` (the images then only give their sizes); it sets ``data['image{0,1}_size']`` as the reference does and
+    ``responses{0,1}`` (the images then only give their sizes) - padded to a capacity with ``num_keypoints0`` /
+    ``num_keypoints1`` (``pad_features``), they are matched as one batch with each pair's own counts; it sets
+    ``data['image{0,1}_size']`` as the reference does and
     returns ``original_matching_idxs`` [NC,2], ``batch_indexes`` [NC], ``confidence`` [NC], ``lafs0`` / ``lafs1`` [1,NC,2,3],
     ``keypoints0`` / ``keypoints1`` [NC,2]."""
 

@@ -21,7 +21,7 @@ from . import _cabi
 from ._cabi import ptr, stream
 from .packing import pack_weights
 
-__all__ = ['SuperGlue', 'MatchingCore', 'PendingMatches']
+__all__ = ['SuperGlue', 'MatchingCore', 'PendingMatches', 'is_padded', 'padded_inputs']
 
 # Counts (re)registrations of parameters, buffers and submodules on any module: ``conv.weight = nn.Parameter(...)`` or
 # ``bn.running_mean = t`` replaces a tensor object, which a cached list of a SuperGlue's tensors would not see.
@@ -37,6 +37,41 @@ for _register in (torch.nn.modules.module.register_module_parameter_registration
                   torch.nn.modules.module.register_module_buffer_registration_hook,
                   torch.nn.modules.module.register_module_module_registration_hook):
     _register(_count_registration)
+
+
+def is_padded(data: dict) -> bool:
+    """Whether ``data`` is a padded batch: pairs with their own keypoint counts ``num_keypoints0`` / ``num_keypoints1``."""
+    return 'num_keypoints0' in data or 'num_keypoints1' in data
+
+
+def padded_inputs(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]:
+    """A padded batch's per-pair inputs, where the caller keeps them: ``num_keypoints0`` / ``num_keypoints1`` as int32 [B] and
+    ``image0_size`` / ``image1_size`` as float32 [B, 2] (W, H) per pair (a batch-wide size, or the image tensors' own, broadcast).
+    Host lengths are checked against the capacities n, m; device lengths are not (the kernels clamp them into range)."""
+    if 'num_keypoints0' not in data or 'num_keypoints1' not in data:
+        raise ValueError('a padded batch needs both num_keypoints0 and num_keypoints1')
+    out = {}
+    for idx, cap in ((0, n), (1, m)):
+        t = data[f'num_keypoints{idx}']
+        t = t.detach() if torch.is_tensor(t) else torch.as_tensor(t)
+        if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool or tuple(t.shape) != (B,):
+            raise ValueError(f'num_keypoints{idx} must be an integer tensor of shape [{B}], got {t.dtype} {tuple(t.shape)}')
+        if t.device.type == 'cpu':
+            lo, hi = int(t.min()), int(t.max())
+            if lo < 1 or hi > cap:
+                raise ValueError(f'num_keypoints{idx} must lie in [1, {cap}] (the capacity), got values in [{lo}, {hi}]')
+        out[f'num_keypoints{idx}'] = t.to(torch.int32)
+        size = data.get(f'image{idx}_size')
+        if 'image0' in data and 'image1' in data:
+            size = None
+        if torch.is_tensor(size) and size.dim() == 2:
+            if tuple(size.shape) != (B, 2):
+                raise ValueError(f'image{idx}_size must be [{B}, 2] (W, H per pair), got {tuple(size.shape)}')
+            out[f'image{idx}_size'] = size.detach().to(torch.float32)
+        else:
+            w, h = SuperGlue._image_wh(data, idx)
+            out[f'image{idx}_size'] = torch.tensor([[w, h]], dtype=torch.float32).expand(B, 2)
+    return out
 
 
 def _feed_forward_params(*sizes: int) -> nn.Sequential:
@@ -209,6 +244,14 @@ class SuperGlue(nn.Module):
 
     def run(self, data: dict, want_matches: bool, want_context: bool = True,
             match_threshold: Optional[float] = None) -> Dict[str, torch.Tensor]:
+        """The eval-mode forward pass (and the matches of ``MatchingCore``).  A padded batch (``data`` with ``num_keypoints0`` /
+        ``num_keypoints1``) has the capacities N, M as its keypoint dimensions; pair b owns rows [0, n_b) / [0, m_b), and its
+        outputs are those of the pair run alone: ``scores[b, :n_b+1, :m_b+1]`` (dustbins at n_b and m_b), ``-inf`` elsewhere;
+        matches -1 and matching scores 0 past the lengths; context-descriptor columns past them 0."""
+        padded = is_padded(data)
+        if self.training and padded:
+            raise NotImplementedError('openglue_b200: padded batches (num_keypoints0 / num_keypoints1) run in eval mode only: the '
+                                      'inference forward pass, match extraction and MatchingCore are built for them, training is not')
         if self.training:
             raise RuntimeError('openglue_b200.SuperGlue.run is the fused eval-mode path; in train() mode call forward() '
                                '(openglue_b200.training: batch-statistics BatchNorm + the explicit backward pass)')
@@ -237,8 +280,13 @@ class SuperGlue(nn.Module):
             raise ValueError('inconsistent batch / keypoint counts in data')
         if n == 0 or m == 0:
             raise ValueError('empty keypoint set')
-        w0, h0 = self._image_wh(data, 0)
-        w1, h1 = self._image_wh(data, 1)
+        if padded:
+            extra = padded_inputs(data, B, n, m)
+            lens = torch.cat([extra['num_keypoints0'].to(dev), extra['num_keypoints1'].to(dev)])
+            pair_wh = torch.cat([extra['image0_size'].to(dev), extra['image1_size'].to(dev)], 1).contiguous()
+        else:
+            w0, h0 = self._image_wh(data, 0)
+            w1, h1 = self._image_wh(data, 1)
 
         lib = _cabi.lib()
         with torch.cuda.device(dev):
@@ -247,7 +295,8 @@ class SuperGlue(nn.Module):
             if match_threshold is not None and float(match_threshold) != cfg.match_threshold:
                 cfg = _cabi.OgConfig.from_buffer_copy(cfg)             # per call: never written back into the shared config
                 cfg.match_threshold = float(match_threshold)
-            ws_bytes = _cabi.check_size(lib.og_workspace_bytes(cfg, B, n, m), 'og_workspace_bytes')
+            ws_query = lib.og_workspace_bytes_padded if padded else lib.og_workspace_bytes
+            ws_bytes = _cabi.check_size(ws_query(cfg, B, n, m), 'og_workspace_bytes')
             if self._workspace is None or self._workspace.numel() < ws_bytes or self._workspace.device != dev:
                 self._workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
                 self._bump_alloc()
@@ -265,9 +314,16 @@ class SuperGlue(nn.Module):
                 m1 = torch.empty(B, m, dtype=torch.int64, device=dev)
                 ms1 = torch.empty(B, m, dtype=torch.float32, device=dev)
                 out.update(matches0=m0, matching_scores0=ms0, matches1=m1, matching_scores1=ms1)
+            outs = (ptr(ctx0), ptr(ctx1), ptr(scores), ptr(m0), ptr(ms0), ptr(m1), ptr(ms1), ptr(self._workspace), ws_bytes, stream(dev))
+            if padded:
+                rc = lib.og_superglue_forward_padded(cfg, ptr(packed), ptr(self._packed_hi), ptr(self._packed_lo), ptr(self._packed_h16),
+                                                     ptr(self._packed_l16), ptr(self._meta16), B, n, m, ptr(lens), ptr(pair_wh), ptr(k0),
+                                                     ptr(k1), ptr(s0), ptr(s1), ptr(d0), ptr(d1), *outs)
+                _cabi.check(rc, 'og_superglue_forward_padded')
+                self.last_launches = lib.og_last_forward_launches()
+                return out
             wh = (C.c_float * 4)(w0, h0, w1, h1)
-            tail = (B, n, m, ptr(k0), ptr(k1), ptr(s0), ptr(s1), ptr(d0), ptr(d1), wh, ptr(ctx0), ptr(ctx1), ptr(scores), ptr(m0), ptr(ms0),
-                    ptr(m1), ptr(ms1), ptr(self._workspace), ws_bytes, stream(dev))
+            tail = (B, n, m, ptr(k0), ptr(k1), ptr(s0), ptr(s1), ptr(d0), ptr(d1), wh, *outs)
             if cfg.precision == _cabi.OG_PREC_FP16X3:
                 rc = lib.og_superglue_forward_f16(cfg, ptr(packed), ptr(self._packed_hi), ptr(self._packed_lo), ptr(self._packed_h16),
                                                   ptr(self._packed_l16), ptr(self._meta16), *tail)
@@ -282,6 +338,10 @@ class SuperGlue(nn.Module):
         In ``train()`` mode the outputs are differentiable with respect to every parameter and the local descriptors
         (BatchNorm uses batch statistics and updates its running buffers, as the reference module does in training_step)."""
         if self.training:
+            if is_padded(data):
+                raise NotImplementedError('openglue_b200: padded batches (num_keypoints0 / num_keypoints1) run in eval mode only: '
+                                          'the inference forward pass, match extraction and MatchingCore are built for them, '
+                                          'training is not')
             from .training import train_forward
             return train_forward(self, data)
         return self.run(data, want_matches=False)
@@ -306,7 +366,11 @@ class MatchingCore(nn.Module):
 
     ``use_cuda_graph=True`` captures the whole launch schedule (~177 kernels at 9 stages) once per
     (batch, N, M) into a CUDA graph with static input / output buffers and replays it: for small
-    batches the path is launch-latency-bound (1 pair, N=M=512: 3.3 ms eager)."""
+    batches the path is launch-latency-bound (1 pair, N=M=512: 3.3 ms eager).
+
+    Padded batches (``num_keypoints0`` / ``num_keypoints1``, see :meth:`SuperGlue.run`) take every path; their lengths and
+    per-pair image sizes are copied into the graph's static buffers like the other inputs, so one graph per capacity (B, N, M)
+    serves every set of lengths and sizes."""
 
     def __init__(self, superglue: SuperGlue, match_threshold: float = 0.2, device: Optional[torch.device] = None,
                  use_cuda_graph: bool = False):
@@ -324,7 +388,13 @@ class MatchingCore(nn.Module):
     def _run_graph(self, data: dict, dev: torch.device) -> Dict[str, torch.Tensor]:
         """Replay (capturing on first use) the CUDA graph for this shape; inputs are copied into its static buffers."""
         shapes = tuple(tuple(data[k].shape) for k in self._TENSOR_KEYS)
-        sizes = (SuperGlue._image_wh(data, 0), SuperGlue._image_wh(data, 1))       # plain floats (collated sizes are tensors)
+        extra = {}
+        if is_padded(data):                      # lengths and sizes go through static buffers: not part of the key
+            k0, k1 = data['keypoints0'], data['keypoints1']
+            extra = padded_inputs(data, k0.shape[0], k0.shape[1], k1.shape[1])
+            sizes = 'padded'
+        else:
+            sizes = (SuperGlue._image_wh(data, 0), SuperGlue._image_wh(data, 1))   # plain floats (collated sizes are tensors)
         # the precision picks the captured kernels and packed-weight forms: a switch in config['precision'] repacks only at the
         # next run, so the alloc-gen check below cannot see it yet
         key = (shapes, sizes, str(dev), self.superglue._weights_version(), self.superglue._precision(), self.match_threshold)
@@ -336,9 +406,15 @@ class MatchingCore(nn.Module):
             entry = None
         if entry is None:
             static = dict(data)
+            if extra:                                                                # sizes come from image*_size alone
+                static.pop('image0', None)
+                static.pop('image1', None)
             for k in self._TENSOR_KEYS:
                 static[k] = torch.empty(data[k].shape, dtype=torch.float32, device=dev)
                 static[k].copy_(data[k], non_blocking=True)
+            for k, v in extra.items():
+                static[k] = torch.empty(v.shape, dtype=v.dtype, device=dev)
+                static[k].copy_(v, non_blocking=True)
             run = lambda: self.superglue.run(static, want_matches=True, want_context=False, match_threshold=self.match_threshold)
             run()                                                                    # warm-up: builds weights, workspace, attributes
             torch.cuda.synchronize(dev)
@@ -351,6 +427,8 @@ class MatchingCore(nn.Module):
         graph, static, out, _ = entry
         for k in self._TENSOR_KEYS:
             static[k].copy_(data[k], non_blocking=True)
+        for k, v in extra.items():
+            static[k].copy_(v, non_blocking=True)
         graph.replay()
         return out
 

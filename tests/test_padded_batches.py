@@ -1,0 +1,355 @@
+"""Padded batches on the H100: pairs with their own keypoint counts n_b, m_b in one call at the capacity N, M
+(``num_keypoints0`` / ``num_keypoints1``).  A pair's result must be the path run on that pair alone; at full lengths the padded
+path must be the uniform path bit for bit; the padding slots must not matter, and the padding outputs are exactly -inf / -1 / 0.
+The operators are checked one by one: attention per sequence against float64 torch, the Sinkhorn pair by pair against the
+oracle in float64, match extraction pair by pair against the oracle exactly."""
+import ctypes as C
+
+import pytest
+import torch
+
+from openglue_b200 import _cabi
+from openglue_b200._cabi import ptr, stream
+from openglue_b200.features import OpenGlueMatcher, pad_features
+from openglue_b200.sift import OpenCVSIFT
+from openglue_b200.superglue import MatchingCore
+from openglue_b200.synthetic import default_config, synthetic_pairs, synthetic_state_dict
+from oracle import superglue_oracle as O
+from test_gpu_parity import DEV, TOL, _model, check_matches
+
+pytestmark = pytest.mark.gpu
+
+KEYS = ('keypoints', 'side_info', 'local_descriptors')
+CONFIGS = {
+    'd256_h4': dict(descriptor_dim=256, num_heads=4, num_stages=2, num_iters=20),     # head_dim 64: the fp16 GNN
+    'd64_h2': dict(descriptor_dim=64, num_heads=2, num_stages=2, num_iters=20),       # head_dim 32: tf32 attention
+    'd32_h4': dict(descriptor_dim=32, num_heads=4, num_stages=1, num_iters=20),       # head_dim 8: fp32 attention in every precision
+}
+PRECISIONS = ('fp32', 'tf32x3', 'fp16x3')
+
+
+def _cfg_model(name, precision, seed=3):
+    cfg = default_config(**CONFIGS[name])
+    return cfg, _model(cfg, synthetic_state_dict(cfg, seed=seed), precision)
+
+
+def _pair(cfg, n, m, seed, wh=(640, 480)):
+    d = synthetic_pairs(1, n, m, cfg['descriptor_dim'], cfg['positional_encoding']['side_info_size'], seed=seed, image_wh=wh)
+    d['image0_size'] = d['image1_size'] = wh
+    return d
+
+
+def _padded(pairs, N, M, fill=0.0):
+    """One padded batch of single-pair dicts at capacity N, M; the padding slots hold `fill`."""
+    B = len(pairs)
+    data = {}
+    for i, cap in ((0, N), (1, M)):
+        for k in KEYS:
+            src = [p[f'{k}{i}'][0] for p in pairs]
+            t = torch.full((B, cap, src[0].shape[-1]), fill, dtype=torch.float32)
+            for b, s in enumerate(src):
+                t[b, :s.shape[0]] = s
+            data[f'{k}{i}'] = t.to(DEV)
+        data[f'num_keypoints{i}'] = torch.tensor([p[f'keypoints{i}'].shape[1] for p in pairs])
+        data[f'image{i}_size'] = torch.tensor([list(p[f'image{i}_size']) for p in pairs], dtype=torch.float32)
+    return data
+
+
+def _alone(model, pair, thr=0.2):
+    out = model.run({k: (v.to(DEV) if torch.is_tensor(v) else v) for k, v in pair.items()}, want_matches=True,
+                    match_threshold=thr)
+    return {k: v.cpu() for k, v in out.items()}
+
+
+def _run(model, data, thr=0.2):
+    return {k: v.cpu() for k, v in model.run(data, want_matches=True, match_threshold=thr).items()}
+
+
+def _check_pair(got, b, n, m, ref, ctx_tol=1e-4):
+    """Pair b of a padded run against the pair alone: parity bounds inside, exact padding outside."""
+    s = got['scores'][b]
+    inner = s[:n + 1, :m + 1]
+    assert (inner.double() - ref['scores'][0].double()).abs().max() <= TOL
+    pad = s.clone()
+    pad[:n + 1, :m + 1] = -float('inf')
+    assert torch.isneginf(pad).all()
+    one = {'matches0': got['matches0'][b:b + 1, :n], 'matching_scores0': got['matching_scores0'][b:b + 1, :n]}
+    check_matches(one, ref, ref['scores'], TOL)
+    assert (got['matches0'][b, n:] == -1).all() and (got['matching_scores0'][b, n:] == 0).all()
+    assert (got['matches1'][b, m:] == -1).all() and (got['matching_scores1'][b, m:] == 0).all()
+    for i, L in ((0, n), (1, m)):
+        c = got[f'context_descriptors{i}'][b]
+        assert (c[:, :L] - ref[f'context_descriptors{i}'][0]).abs().max() <= ctx_tol
+        assert (c[:, L:] == 0).all()
+
+
+def _same(a, b, keys):
+    for k in keys:
+        assert torch.equal(a[k], b[k]), f'{k}: {int((a[k] != b[k]).sum())} elements differ'
+
+
+OUT_KEYS = ('scores', 'matches0', 'matching_scores0', 'matches1', 'matching_scores1', 'context_descriptors0', 'context_descriptors1')
+
+
+# --------------------------------------------------------------------------- 1. full lengths = the uniform path, bit for bit
+@pytest.mark.parametrize('precision', PRECISIONS)
+@pytest.mark.parametrize('name', ['d256_h4', 'd64_h2', 'C3_planted'])
+def test_full_lengths_equal_uniform_path(golden, name, precision):
+    if name == 'C3_planted':
+        fx = golden(name)
+        cfg, model = fx['config'], _model(fx['config'], fx['state_dict'], precision)
+        data = {k: (v[:4].to(DEV) if torch.is_tensor(v) else v) for k, v in fx['data'].items()}
+    else:
+        cfg, model = _cfg_model(name, precision)
+        data = {k: (v.to(DEV) if torch.is_tensor(v) else v) for k, v in
+                synthetic_pairs(3, 200, 143, cfg['descriptor_dim'], cfg['positional_encoding']['side_info_size'], seed=5).items()}
+    B, N, M = data['keypoints0'].shape[0], data['keypoints0'].shape[1], data['keypoints1'].shape[1]
+    uniform = _run(model, data)
+    padded = _run(model, dict(data, num_keypoints0=torch.full((B,), N), num_keypoints1=torch.full((B,), M)))
+    _same(padded, uniform, OUT_KEYS)
+
+
+# --------------------------------------------------------------------------- 2. each pair equals itself alone
+LENGTHS = [(1, 300), (300, 1), (127, 128), (128, 129), (129, 127), (255, 256), (256, 257), (257, 255), (300, 300)]
+SIZES = [(640, 480), (320, 240), (1024, 768)]
+
+
+@pytest.mark.parametrize('precision', PRECISIONS)
+@pytest.mark.parametrize('name', list(CONFIGS))
+def test_each_pair_equals_itself_alone(name, precision):
+    cfg, model = _cfg_model(name, precision)
+    pairs = [_pair(cfg, n, m, seed=10 + i, wh=SIZES[i % 3]) for i, (n, m) in enumerate(LENGTHS)]
+    got = _run(model, _padded(pairs, 300, 300))
+    for b, ((n, m), p) in enumerate(zip(LENGTHS, pairs)):
+        _check_pair(got, b, n, m, _alone(model, p))
+        if precision == 'fp32' and name != 'd256_h4':
+            ref = O.run(synthetic_state_dict(cfg, seed=3), cfg, p)
+            assert (got['scores'][b, :n + 1, :m + 1] - ref['scores'][0]).abs().max() <= TOL
+
+
+@pytest.mark.parametrize('resident', [1, 0])
+@pytest.mark.parametrize('M', [512, 1024, 2048, 4096, 8192])
+def test_each_pair_alone_at_every_sinkhorn_band(M, resident):
+    """Capacities that select every Sinkhorn instantiation, in the resident and the streaming form."""
+    cfg, model = _cfg_model('d64_h2', 'tf32x3')
+    lib = _cabi.lib()
+    prev = lib.og_set_sinkhorn_resident(resident)
+    try:
+        lengths = [(200, M), (57, M // 2 + 3), (129, 1)]
+        pairs = [_pair(cfg, n, m, seed=40 + i) for i, (n, m) in enumerate(lengths)]
+        got = _run(model, _padded(pairs, 200, M))
+        for b, ((n, m), p) in enumerate(zip(lengths, pairs)):
+            _check_pair(got, b, n, m, _alone(model, p))
+    finally:
+        lib.og_set_sinkhorn_resident(prev)
+
+
+# --------------------------------------------------------------------------- 3. padding contents do not matter
+@pytest.mark.parametrize('precision', PRECISIONS)
+@pytest.mark.parametrize('fill', [float('nan'), float('inf'), -float('inf'), 1e30])
+def test_padding_contents_do_not_matter(precision, fill):
+    cfg, model = _cfg_model('d256_h4', precision)
+    lengths = [(1, 150), (129, 77), (150, 150)]
+    pairs = [_pair(cfg, n, m, seed=60 + i, wh=SIZES[i]) for i, (n, m) in enumerate(lengths)]
+    zero = _run(model, _padded(pairs, 150, 150, 0.0))
+    junk = _run(model, _padded(pairs, 150, 150, fill))
+    _same(junk, zero, OUT_KEYS)
+    for b, (n, m) in enumerate(lengths):
+        assert torch.isneginf(zero['scores'][b, n + 1:]).all() and torch.isneginf(zero['scores'][b, :, m + 1:]).all()
+        assert torch.isfinite(zero['scores'][b, :n + 1, :m + 1]).all()
+
+
+# --------------------------------------------------------------------------- 4. capacity independence
+@pytest.mark.parametrize('precision', PRECISIONS)
+def test_capacity_independence(precision):
+    cfg, model = _cfg_model('d256_h4', precision)
+    lengths = [(90, 120), (128, 64), (33, 129)]
+    pairs = [_pair(cfg, n, m, seed=80 + i) for i, (n, m) in enumerate(lengths)]
+    a = _run(model, _padded(pairs, 130, 130))
+    b = _run(model, _padded(pairs, 520, 260))
+    for i, (n, m) in enumerate(lengths):
+        assert (a['scores'][i, :n + 1, :m + 1] - b['scores'][i, :n + 1, :m + 1]).abs().max() <= TOL
+        ref = {'scores': a['scores'][i:i + 1, :n + 1, :m + 1], 'matches0': a['matches0'][i:i + 1, :n],
+               'matching_scores0': a['matching_scores0'][i:i + 1, :n]}
+        check_matches({'matches0': b['matches0'][i:i + 1, :n], 'matching_scores0': b['matching_scores0'][i:i + 1, :n]}, ref,
+                      ref['scores'], TOL)
+
+
+# --------------------------------------------------------------------------- 5. operators alone
+def _attention_ref(q, k, v, H, L):
+    dh = q.shape[1] // H
+    qh = q.double().view(-1, H, dh).transpose(0, 1)
+    kh = k[:L].double().view(L, H, dh).transpose(0, 1)
+    vh = v[:L].double().view(L, H, dh).transpose(0, 1)
+    p = torch.softmax(qh @ kh.transpose(1, 2) * dh ** -0.5, -1)
+    return (p @ vh).transpose(0, 1).reshape(q.shape[0], -1)
+
+
+@pytest.mark.parametrize('form', ['fp32', 'tf32'])
+@pytest.mark.parametrize('dh', [32, 64])
+def test_attention_key_lengths(form, dh):
+    H, nq, nk = 2, 130, 300
+    d = H * dh
+    lens = [1, 63, 64, 65, 127, 128, 129, 255, 256, 257, 300]
+    B = len(lens)
+    g = torch.Generator().manual_seed(7)
+    q, k, v = (torch.randn(B, n, d, generator=g) for n in (nq, nk, nk))
+    k[:-1, 280:] = float('nan')                          # keys past every length but the last one's: never read or masked
+    qd, kd, vd = q.to(DEV), k.to(DEV), v.to(DEV)
+    kl = torch.tensor(lens, dtype=torch.int32, device=DEV)
+    out = torch.empty(B, nq, d, device=DEV)
+    lib = _cabi.lib()
+    if form == 'fp32':
+        rc = lib.og_attention_fwd_padded(ptr(qd), d, nq * d, ptr(kd), d, nk * d, ptr(vd), d, nk * d, ptr(out), d, nq * d, B, nq, nk, H, dh,
+                                         ptr(kl), stream())
+    else:
+        kd = torch.nan_to_num(kd)                        # the tf32 operands are finite (the forward pass guarantees it)
+        khi, klo = torch.empty_like(kd), torch.empty_like(kd)
+        _cabi.check(lib.og_split_tf32(ptr(kd), ptr(khi), ptr(klo), kd.numel(), stream()), 'og_split_tf32')
+        ldvt = (nk + 3) // 4 * 4
+        vt = torch.zeros(B, d, ldvt, device=DEV)
+        vt[:, :, :nk] = vd.transpose(1, 2)
+        vthi, vtlo = torch.empty_like(vt), torch.empty_like(vt)
+        _cabi.check(lib.og_split_tf32(ptr(vt), ptr(vthi), ptr(vtlo), vt.numel(), stream()), 'og_split_tf32')
+        rc = lib.og_attention_tc_fwd_padded(ptr(qd), d, nq * d, ptr(khi), ptr(klo), d, ptr(vthi), ptr(vtlo), ldvt, ptr(out), d, nq * d,
+                                            B, nq, nk, H, dh, ptr(kl), stream())
+    _cabi.check(rc, 'attention_padded')
+    torch.cuda.synchronize()
+    for b, L in enumerate(lens):
+        ref = _attention_ref(q[b], k[b], v[b], H, L)
+        assert (out[b].cpu().double() - ref).abs().max() <= 2e-5, (b, L)
+
+
+def _sinkhorn_padded(S, dust, lens, iters, reg):
+    B, N, M = S.shape
+    lib = _cabi.lib()
+    lds = (M + 3) // 4 * 4
+    Sp = torch.zeros(B, N, lds, device=DEV)
+    Sp[:, :, :M] = S.to(DEV)
+    scores = torch.empty(B, N + 1, M + 1, device=DEV)
+    wsb = _cabi.check_size(lib.og_sinkhorn_workspace_bytes(B, N, M), 'og_sinkhorn_workspace_bytes')
+    ws = torch.empty(wsb, dtype=torch.uint8, device=DEV)
+    ld = torch.tensor(lens, dtype=torch.int32, device=DEV)
+    _cabi.check(lib.og_sinkhorn_fwd_padded(ptr(Sp), lds, N * lds, ptr(dust.to(DEV)), B, N, M, ptr(ld), iters, reg, ptr(scores), ptr(ws),
+                                           wsb, stream()), 'og_sinkhorn_fwd_padded')
+    return scores.cpu()
+
+
+@pytest.mark.parametrize('resident', [1, 0])
+@pytest.mark.parametrize('N,M', [(300, 500), (200, 1000), (150, 2000), (100, 4000), (60, 8192)])
+def test_sinkhorn_lengths_against_oracle(N, M, resident):
+    lib = _cabi.lib()
+    prev = lib.og_set_sinkhorn_resident(resident)
+    try:
+        ns, ms = [N, 1, N // 2 + 1, 17], [M, M // 2 - 1, 1, M - 5]
+        g = torch.Generator().manual_seed(N + M)
+        S = torch.randn(len(ns), N, M, generator=g) * 3
+        dust = torch.tensor([0.7])
+        got = _sinkhorn_padded(S, dust, ns + ms, 50, 1.0)
+        for b, (n, m) in enumerate(zip(ns, ms)):
+            ref = O.matching_log_probs(S[b:b + 1, :n, :m].double(), dust.double()[0], 50, 1.0)[0]
+            assert (got[b, :n + 1, :m + 1].double() - ref).abs().max() <= 1e-3
+            pad = got[b].clone()
+            pad[:n + 1, :m + 1] = -float('inf')
+            assert torch.isneginf(pad).all()
+    finally:
+        lib.og_set_sinkhorn_resident(prev)
+
+
+def test_sinkhorn_device_constants_equal_host():
+    lib = _cabi.lib()
+    N, M = 65536, 8192
+    pairs = [(n, 1) for n in range(1, N + 1)] + [(N, m) for m in range(1, M + 1)] + [(n, M) for n in range(1, N + 1, 7)] + \
+            [(1, m) for m in range(1, M + 1)]
+    lens = torch.tensor([p[0] for p in pairs] + [p[1] for p in pairs], dtype=torch.int32, device=DEV)
+    out = torch.empty(len(pairs), 3, device=DEV)
+    _cabi.check(lib.og_sinkhorn_consts_padded(ptr(lens), len(pairs), N, M, ptr(out), stream()), 'og_sinkhorn_consts_padded')
+    host = torch.empty(len(pairs), 3)
+    buf = (C.c_float * 3)()
+    for i, (n, m) in enumerate(pairs):
+        _cabi.check(lib.og_sinkhorn_consts(n, m, buf), 'og_sinkhorn_consts')
+        host[i] = torch.tensor(list(buf))
+    assert torch.equal(out.cpu().view(torch.int32), host.view(torch.int32))
+
+
+def test_match_lengths_equal_oracle_exactly():
+    B, N, M = 4, 200, 150
+    ns, ms = [200, 1, 64, 65], [150, 149, 1, 129]
+    g = torch.Generator().manual_seed(3)
+    scores = torch.randn(B, N + 1, M + 1, generator=g)
+    scores[:, :, :] = torch.log_softmax(scores, -1)
+    sd = scores.to(DEV)
+    lib = _cabi.lib()
+    wsb = _cabi.check_size(lib.og_match_workspace_bytes(B, N, M), 'og_match_workspace_bytes')
+    ws = torch.empty(wsb, dtype=torch.uint8, device=DEV)
+    m0, m1 = torch.empty(B, N, dtype=torch.int64, device=DEV), torch.empty(B, M, dtype=torch.int64, device=DEV)
+    s0, s1 = torch.empty(B, N, device=DEV), torch.empty(B, M, device=DEV)
+    ld = torch.tensor(ns + ms, dtype=torch.int32, device=DEV)
+    _cabi.check(lib.og_match_fwd_padded(ptr(sd), B, N, M, ptr(ld), 0.01, ptr(m0), ptr(s0), ptr(m1), ptr(s1), ptr(ws), wsb, stream()),
+                'og_match_fwd_padded')
+    for b, (n, m) in enumerate(zip(ns, ms)):
+        sub = scores[b:b + 1, :n + 1, :m + 1].clone()
+        ref = O.extract_matches(sub, 0.01)
+        assert torch.equal(m0[b, :n].cpu(), ref['matches0'][0]) and torch.equal(m1[b, :m].cpu(), ref['matches1'][0])
+        # the scores are exp of the same maxima: expf on the device and torch's exp on the host may differ in the last bit
+        torch.testing.assert_close(s0[b, :n].cpu(), ref['matching_scores0'][0], rtol=3e-7, atol=0)
+        torch.testing.assert_close(s1[b, :m].cpu(), ref['matching_scores1'][0], rtol=3e-7, atol=0)
+        assert (m0[b, n:] == -1).all() and (s0[b, n:] == 0).all() and (m1[b, m:] == -1).all() and (s1[b, m:] == 0).all()
+
+
+# --------------------------------------------------------------------------- 6. serving
+@pytest.mark.parametrize('precision', PRECISIONS)
+def test_graph_serves_every_length_set(precision, monkeypatch):
+    cfg, model = _cfg_model('d256_h4', precision)
+    captured = [0]
+    orig = torch.cuda.CUDAGraph.capture_end
+
+    def counting(self):
+        captured[0] += 1
+        return orig(self)
+    monkeypatch.setattr(torch.cuda.CUDAGraph, 'capture_end', counting)
+    core = MatchingCore(model, 0.2, use_cuda_graph=True)
+    eager = MatchingCore(model, 0.2)
+    for i, lengths in enumerate([[(160, 160), (1, 7), (80, 129)], [(17, 160), (160, 3), (129, 128)], [(64, 65), (65, 64), (5, 5)]]):
+        pairs = [_pair(cfg, n, m, seed=100 + 3 * i + j, wh=SIZES[(i + j) % 3]) for j, (n, m) in enumerate(lengths)]
+        data = _padded(pairs, 160, 160)
+        want = eager(data, want_scores=True)
+        got = core(data, want_scores=True)
+        _same({k: v.cpu() for k, v in got.items()}, {k: v.cpu() for k, v in want.items()}, want.keys())
+        host = {k: (v.cpu() if torch.is_tensor(v) else v) for k, v in data.items()}
+        res = core.submit(host).wait()
+        _same({k: res[k] for k in core._OUT_KEYS}, {k: want[k].cpu() for k in core._OUT_KEYS}, core._OUT_KEYS)
+    assert captured[0] == 1
+
+
+# --------------------------------------------------------------------------- 7. end to end: SIFT -> pad_features -> one batched matcher call
+def test_sift_padded_batch_matches_each_pair_alone():
+    g = torch.Generator().manual_seed(0)
+    H = W = 240
+    yy, xx = torch.meshgrid(torch.arange(H), torch.arange(W), indexing='ij')
+    busy = torch.rand(H, W, generator=g) * 255
+    blobs = 127 + 100 * torch.sin(xx / 9.0) * torch.cos(yy / 13.0)
+    calm = 127 + 40 * torch.sin(xx / 40.0) + torch.rand(H, W, generator=g) * 10
+    imgs0 = torch.stack([busy, blobs, calm])[:, None].round().clamp(0, 255).to(DEV)
+    imgs1 = torch.stack([torch.roll(busy, 3, 1), torch.roll(blobs, 5, 0), torch.roll(calm, 4, 1)])[:, None].round().clamp(0, 255).to(DEV)
+    sift = OpenCVSIFT(max_keypoints=400)
+    f0, f1 = sift.extract_batch(imgs0), sift.extract_batch(imgs1)
+    assert len({f[0].shape[1] for f in f0 + f1}) > 1, 'the images should give different keypoint counts'
+    cfg = default_config(descriptor_dim=128, num_heads=4, num_stages=2, num_iters=20, side_info_size=1)
+    model = _model(cfg, synthetic_state_dict(cfg, seed=1), 'tf32x3')
+    mc = {'superglue': {'laf_to_sideinfo_method': 'none'}, 'inference': {'match_threshold': 0.0}}
+    matcher = OpenGlueMatcher(sift, model, mc)
+    l0, r0, d0, n0 = pad_features(f0)
+    l1, r1, d1, n1 = pad_features(f1)
+    batched = matcher({'image0': imgs0, 'image1': imgs1, 'lafs0': l0, 'responses0': r0, 'descriptors0': d0, 'num_keypoints0': n0,
+                       'lafs1': l1, 'responses1': r1, 'descriptors1': d1, 'num_keypoints1': n1})
+    for b in range(3):
+        one = {'image0': imgs0[b:b + 1], 'image1': imgs1[b:b + 1]}
+        for i, f in ((0, f0[b]), (1, f1[b])):
+            one.update({f'lafs{i}': f[0], f'responses{i}': f[1], f'descriptors{i}': f[2]})
+        alone = matcher(one)
+        sel = batched['batch_indexes'] == b
+        got = {tuple(x) for x in batched['original_matching_idxs'][sel].tolist()}
+        want = {tuple(x) for x in alone['original_matching_idxs'].tolist()}
+        # decisions within the parity bound of the threshold or of a tie may flip; the lists must agree on the rest
+        assert len(got ^ want) <= max(2, len(want) // 50), (b, len(got), len(want), len(got ^ want))
