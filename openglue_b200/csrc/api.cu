@@ -24,39 +24,33 @@
 
 namespace og {
 
-// keypoint normalisation + concat with side info:  in0[r] = [2*x/(W-1) - 1, 2*y/(H-1) - 1, side...]
-// (reference superglue.py:74-78 and positional_encoding.py:16-18)
-__global__ void __launch_bounds__(256) kenc_input_kernel(const float* __restrict__ kpts, const float* __restrict__ side,
-                                                          int rows, int S, float wm1, float hm1, float* __restrict__ out) {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= rows) return;
-  float* o = out + (int64_t)r * (2 + S);
-  o[0] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r), wm1) - 1.f;
-  o[1] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r + 1), hm1) - 1.f;
-  for (int s = 0; s < S; ++s) o[2 + s] = __ldg(side + (int64_t)r * S + s);
-}
-
 // Padded batch: row r of one image's [B, cap] rows is slot r % cap of pair b = r / cap, real below len[b] (clamped into [1, cap]).
 __device__ __forceinline__ bool padded_row_real(int64_t r, int cap, const int* len) {
   const int b = (int)(r / cap);
-  return (int)(r - (int64_t)b * cap) < min(max(__ldg(len + b), 1), cap);
+  return (int)(r - (int64_t)b * cap) < padded_length(len, b, cap);
 }
 
-// kenc_input_kernel for a padded batch: each pair's (W - 1, H - 1) from wh (rows 4 floats apart: the image's (W, H) of the pair),
-// zero rows past its length (whatever the padding slots hold, every row from here on is finite)
-__global__ void __launch_bounds__(256) kenc_input_padded_kernel(const float* __restrict__ kpts, const float* __restrict__ side,
-                                                                 int rows, int cap, int S, const int* __restrict__ len,
-                                                                 const float* __restrict__ wh, float* __restrict__ out) {
+// keypoint normalisation + concat with side info:  in0[r] = [2*x/(W-1) - 1, 2*y/(H-1) - 1, side...]
+// (reference superglue.py:74-78 and positional_encoding.py:16-18).  A padded batch (len non-null) takes each pair's (W - 1, H - 1)
+// from wh (rows 4 floats apart: the image's (W, H) of the pair) and zeroes the rows past its length (whatever the padding slots
+// hold, every row from here on is finite).
+__global__ void __launch_bounds__(256) kenc_input_kernel(const float* __restrict__ kpts, const float* __restrict__ side,
+                                                          int rows, int S, float wm1, float hm1, int cap, const int* __restrict__ len,
+                                                          const float* __restrict__ wh, float* __restrict__ out) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= rows) return;
   float* o = out + (int64_t)r * (2 + S);
-  if (!padded_row_real(r, cap, len)) {
-    for (int s = 0; s < 2 + S; ++s) o[s] = 0.f;
-    return;
+  if (len) {
+    if (!padded_row_real(r, cap, len)) {
+      for (int s = 0; s < 2 + S; ++s) o[s] = 0.f;
+      return;
+    }
+    const int b = r / cap;
+    wm1 = __ldg(wh + 4 * b) - 1.f;
+    hm1 = __ldg(wh + 4 * b + 1) - 1.f;
   }
-  const int b = r / cap;
-  o[0] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r), __ldg(wh + 4 * b) - 1.f) - 1.f;
-  o[1] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r + 1), __ldg(wh + 4 * b + 1) - 1.f) - 1.f;
+  o[0] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r), wm1) - 1.f;
+  o[1] = __fdiv_rn(2.f * __ldg(kpts + 2 * (int64_t)r + 1), hm1) - 1.f;
   for (int s = 0; s < S; ++s) o[2 + s] = __ldg(side + (int64_t)r * S + s);
 }
 
@@ -71,7 +65,7 @@ __global__ void __launch_bounds__(256) mask_padded_rows_kernel(const float* __re
 __global__ void __launch_bounds__(256) zero_padded_cols_kernel(float* __restrict__ ctx, int B, int d, int cap, const int* __restrict__ len) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (int64_t)B * d * cap; i += (int64_t)gridDim.x * blockDim.x) {
     const int b = (int)(i / ((int64_t)d * cap));
-    if ((int)(i % cap) >= min(max(__ldg(len + b), 1), cap)) ctx[i] = 0.f;
+    if ((int)(i % cap) >= padded_length(len, b, cap)) ctx[i] = 0.f;
   }
 }
 
@@ -79,8 +73,8 @@ __global__ void __launch_bounds__(256) zero_padded_cols_kernel(float* __restrict
 __global__ void sinkhorn_consts_kernel(SinkArgs a, float* out) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= a.B) return;
-  const SinkPair<true> p(a, b);
-  out[3 * b] = p.norm(); out[3 * b + 1] = p.log_a_last(); out[3 * b + 2] = p.log_b_last();
+  const SinkPair p(a, b);
+  out[3 * b] = p.norm; out[3 * b + 1] = p.log_a_last; out[3 * b + 2] = p.log_b_last;
 }
 
 struct Layout {           // float offsets of the packed weights
@@ -691,7 +685,7 @@ int og_mix_param_grad(const float* colsum, const float* mix, float* dmix, int d,
 int og_kenc_input(const float* kpts, const float* side, int rows, int side_info_size, float width, float height, float* out, void* stream) {
   OG_CHECK_ARG(kpts && out && rows > 0 && side_info_size >= 0 && (side_info_size == 0 || side), "kenc_input: bad arguments");
   return OG_LAUNCH(kenc_input_kernel, cdiv(rows, 256), 256, 0, (cudaStream_t)stream, kpts, side, rows, side_info_size, width - 1.f,
-                   height - 1.f, out);
+                   height - 1.f, rows, nullptr, nullptr, out);
 }
 
 // ---- SuperPoint front-end operators (row f4; csrc/superpoint.cuh) ----
@@ -970,23 +964,24 @@ static int forward_impl(const og_config* cfg, const float* Wp, const float* Whi,
   // every row is finite (the fp16 amax slots see every row, and a masked key with a NaN value would poison P.V: 0 * NaN = NaN).
   const float* dsc0 = desc0;
   const float* dsc1 = desc1;
+  // each image's (W - 1, H - 1), or in a padded batch its lengths and per-pair sizes (the kernel reads these when len is set)
+  const float wm0 = padded ? 0.f : img_wh[0] - 1.f, hm0 = padded ? 0.f : img_wh[1] - 1.f;
+  const float wm1 = padded ? 0.f : img_wh[2] - 1.f, hm1 = padded ? 0.f : img_wh[3] - 1.f;
+  const int* len0 = padded ? lens : nullptr;
+  const int* len1 = padded ? lens + B : nullptr;
+  const float* wh0 = padded ? pair_wh : nullptr;
+  const float* wh1 = padded ? pair_wh + 2 : nullptr;
+  if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, S, wm0, hm0, n, len0, wh0, w.in0)) != OG_OK) return rc;
+  if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, S, wm1, hm1, m, len1, wh1,
+                      w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
+    return rc;
   if (padded) {
-    if ((rc = OG_LAUNCH(kenc_input_padded_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, n, S, lens, pair_wh, w.in0)) != OG_OK) return rc;
-    if ((rc = OG_LAUNCH(kenc_input_padded_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, m, S, lens + B, pair_wh + 2,
-                        w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
-      return rc;
     float* d1m = w.desc + (int64_t)R0 * d;
     if ((rc = OG_LAUNCH(mask_padded_rows_kernel, eltwise_grid((int64_t)R0 * d), 256, 0, st, desc0, (int64_t)R0, n, d, lens, w.desc)) != OG_OK)
       return rc;
     if ((rc = OG_LAUNCH(mask_padded_rows_kernel, eltwise_grid((int64_t)R1 * d), 256, 0, st, desc1, (int64_t)R1, m, d, lens + B, d1m)) != OG_OK)
       return rc;
     dsc0 = w.desc; dsc1 = d1m;
-  } else {
-    if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R0, 256), 256, 0, st, kpts0, side0, R0, S, img_wh[0] - 1.f, img_wh[1] - 1.f, w.in0)) != OG_OK)
-      return rc;
-    if ((rc = OG_LAUNCH(kenc_input_kernel, cdiv(R1, 256), 256, 0, st, kpts1, side1, R1, S, img_wh[2] - 1.f, img_wh[3] - 1.f,
-                        w.in0 + (int64_t)R0 * (2 + S))) != OG_OK)
-      return rc;
   }
   {
     const float* cur = w.in0;

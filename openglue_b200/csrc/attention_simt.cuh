@@ -18,10 +18,9 @@ struct AttnArgs {
   const int* klen;           // padded batch (device, may be null): keys of sequence b = klen[b], clamped into [1, nk]
 };
 
-
 constexpr int ATQ = 64, ATK = 64;
 
-template <int DH, bool RAGGED>
+template <int DH>
 __global__ void __launch_bounds__(256) attention_simt_kernel(AttnArgs a) {
   constexpr int CPT = (DH >= 64) ? 4 : (DH >= 32 ? 2 : 1);     // output columns per thread
   extern __shared__ __align__(16) float og_attn_smem[];          // 64 KB at DH=64: dynamic
@@ -32,7 +31,7 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(AttnArgs a) {
 
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ATQ;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int nk = attention_keys<RAGGED>(a.klen, b, a.nk);
+  const int nk = padded_length(a.klen, b, a.nk);
   const float* __restrict__ Q = a.q + (int64_t)b * a.strideq + h * DH;
   const float* __restrict__ Kp = a.k + (int64_t)b * a.stridek + h * DH;
   const float* __restrict__ Vp = a.v + (int64_t)b * a.stridev + h * DH;
@@ -140,12 +139,8 @@ inline int attention_simt_launch(const AttnArgs& a, int head_dim, cudaStream_t s
 #define OG_ATTN_CASE(DH_)                                                                        \
   case DH_: {                                                                                    \
     constexpr int smem = (DH_ * (ATQ + ATK) + ATK * DH_ + ATK * ATQ) * (int)sizeof(float);       \
-    if (a.klen) {                                                                                \
-      if (const int rc = smem_opt_in<attention_simt_kernel<DH_, true>>(smem)) return rc;         \
-      return OG_LAUNCH((attention_simt_kernel<DH_, true>), grid, 256, smem, stream, a);          \
-    }                                                                                            \
-    if (const int rc = smem_opt_in<attention_simt_kernel<DH_, false>>(smem)) return rc;          \
-    return OG_LAUNCH((attention_simt_kernel<DH_, false>), grid, 256, smem, stream, a);           \
+    if (const int rc = smem_opt_in<attention_simt_kernel<DH_>>(smem)) return rc;                 \
+    return OG_LAUNCH(attention_simt_kernel<DH_>, grid, 256, smem, stream, a);                    \
   }
   switch (head_dim) {
     OG_ATTN_CASE(8) OG_ATTN_CASE(16) OG_ATTN_CASE(32) OG_ATTN_CASE(64)

@@ -160,7 +160,7 @@ __device__ __forceinline__ float attention_store(const float (&acc)[DH / 2], con
 // while this one waits for its own, folds O_{i-1} and runs the softmax of S_i and the split of P_i.  (Starting that softmax as soon as S_i is done, while
 // O_{i-1} is still in the pipe, measured no faster on an H100.)  A stage is released by one thread per consumer once its P.V
 // has completed; three stages, because two leave the consumers waiting for TMA.
-template <int DH, bool RAGGED>
+template <int DH>
 __device__ __forceinline__ void attention_f16_ws(const CUtensorMap* mkh, const CUtensorMap* mkl, const CUtensorMap* mvh,
                                                  const CUtensorMap* mvl, const TcAttnArgs& a, const F16AttnScales& sc,
                                                  uint8_t* smem) {
@@ -176,7 +176,7 @@ __device__ __forceinline__ void attention_f16_ws(const CUtensorMap* mkh, const C
   volatile uint32_t* timeout_flag = reinterpret_cast<uint32_t*>(empty + S);   // a consumer's wait on `full` timed out
 
   const int q0 = blockIdx.x * BM, h = blockIdx.y, b = blockIdx.z;
-  const int nk = attention_keys<RAGGED>(a.klen, b, a.nk);      // the producer and both consumers run the same key blocks
+  const int nk = padded_length(a.klen, b, a.nk);      // the producer and both consumers run the same key blocks
   const int nblk = cdiv(nk, BNK);
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
@@ -320,7 +320,7 @@ __device__ __forceinline__ void attention_f16_ws(const CUtensorMap* mkh, const C
 
 // ---- 3xTF32 form: two warpgroups of 64 query rows, key blocks of 64.  Thread 0 stages the K / V^T hi/lo tiles; Q hi/lo stays in
 // registers for the whole CTA; each warpgroup waits for its Q.K^T chain, runs the softmax, then issues and waits for P.V.
-template <int DH, bool RAGGED>
+template <int DH>
 __device__ __forceinline__ void attention_tf32(const CUtensorMap* mkh, const CUtensorMap* mkl, const CUtensorMap* mvh,
                                                const CUtensorMap* mvl, const TcAttnArgs& a, uint8_t* smem) {
   using namespace tca;
@@ -332,7 +332,7 @@ __device__ __forceinline__ void attention_tf32(const CUtensorMap* mkh, const CUt
   uint64_t* empty = full + S;
 
   const int q0 = blockIdx.x * BM, h = blockIdx.y, b = blockIdx.z;
-  const int nk = attention_keys<RAGGED>(a.klen, b, a.nk);
+  const int nk = padded_length(a.klen, b, a.nk);
   const int nblk = cdiv(nk, BNK);
   const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   if (threadIdx.x == 0) {
@@ -444,32 +444,18 @@ __device__ __forceinline__ void attention_tf32(const CUtensorMap* mkh, const CUt
   attention_store<DH>(acc, l_run, 1.f, qr, t, a, h, b);
 }
 
-template <int DH, bool F16, bool RAGGED>
-__device__ __forceinline__ void attention_sm90(const CUtensorMap* mkh, const CUtensorMap* mkl, const CUtensorMap* mvh,
-                                               const CUtensorMap* mvl, const TcAttnArgs& a, const F16AttnScales& sc) {
-  static_assert(DH == 64 || (DH == 32 && !F16), "head_dim 64 (both forms) or 32 (tf32)");
-  tc::launch_dependents();
-  extern __shared__ uint8_t og_att_smem_raw[];
-  uint8_t* smem = tc::align_smem_1024(og_att_smem_raw);
-  if constexpr (F16) attention_f16_ws<DH, RAGGED>(mkh, mkl, mvh, mvl, a, sc, smem);
-  else attention_tf32<DH, RAGGED>(mkh, mkl, mvh, mvl, a, smem);
-}
 template <int DH, bool F16>
 __global__ void __launch_bounds__(tca::Cfg<DH, F16>::THREADS, 1) attention_sm90_kernel(const __grid_constant__ CUtensorMap map_khi,
                                                                                        const __grid_constant__ CUtensorMap map_klo,
                                                                                        const __grid_constant__ CUtensorMap map_vhi,
                                                                                        const __grid_constant__ CUtensorMap map_vlo,
                                                                                        TcAttnArgs a, F16AttnScales sc) {
-  attention_sm90<DH, F16, false>(&map_khi, &map_klo, &map_vhi, &map_vlo, a, sc);
-}
-// The padded batch's form: each sequence's keys from TcAttnArgs::klen
-template <int DH, bool F16>
-__global__ void __launch_bounds__(tca::Cfg<DH, F16>::THREADS, 1) attention_sm90_padded_kernel(const __grid_constant__ CUtensorMap map_khi,
-                                                                                              const __grid_constant__ CUtensorMap map_klo,
-                                                                                              const __grid_constant__ CUtensorMap map_vhi,
-                                                                                              const __grid_constant__ CUtensorMap map_vlo,
-                                                                                              TcAttnArgs a, F16AttnScales sc) {
-  attention_sm90<DH, F16, true>(&map_khi, &map_klo, &map_vhi, &map_vlo, a, sc);
+  static_assert(DH == 64 || (DH == 32 && !F16), "head_dim 64 (both forms) or 32 (tf32)");
+  tc::launch_dependents();
+  extern __shared__ uint8_t og_att_smem_raw[];
+  uint8_t* smem = tc::align_smem_1024(og_att_smem_raw);
+  if constexpr (F16) attention_f16_ws<DH>(&map_khi, &map_klo, &map_vhi, &map_vlo, a, sc, smem);
+  else attention_tf32<DH>(&map_khi, &map_klo, &map_vhi, &map_vlo, a, smem);
 }
 
 template <int DH, bool F16, class T>
@@ -483,15 +469,9 @@ inline int attention_sm90_launch(const TcAttnArgs& a, const F16AttnScales& sc, c
   if ((rc = tc::make_tmap_2d(&mkl, klo, (uint64_t)a.batch * a.nk, (uint64_t)a.d, (uint64_t)ldk, C::BNK)) != OG_OK) return rc;
   if ((rc = tc::make_tmap_2d(&mvh, vthi, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
   if ((rc = tc::make_tmap_2d(&mvl, vtlo, (uint64_t)a.batch * a.d, (uint64_t)a.nk, (uint64_t)ldvt, DH)) != OG_OK) return rc;
-  const dim3 grid(cdiv(a.nq, BM), a.num_heads, a.batch);
-  if (a.klen) {
-    if ((rc = smem_opt_in<attention_sm90_padded_kernel<DH, F16>>(C::SMEM_BYTES, true)) != OG_OK) return rc;
-    return launch("attention_sm90_padded_kernel", attention_sm90_padded_kernel<DH, F16>, LaunchAttr::pdl, grid, dim3(C::THREADS),
-                  C::SMEM_BYTES, stream, mkh, mkl, mvh, mvl, a, sc);
-  }
   if ((rc = smem_opt_in<attention_sm90_kernel<DH, F16>>(C::SMEM_BYTES, true)) != OG_OK) return rc;   // the GEMMs' configuration
-  return launch("attention_sm90_kernel", attention_sm90_kernel<DH, F16>, LaunchAttr::pdl, grid, dim3(C::THREADS), C::SMEM_BYTES,
-                stream, mkh, mkl, mvh, mvl, a, sc);
+  return launch("attention_sm90_kernel", attention_sm90_kernel<DH, F16>, LaunchAttr::pdl, dim3(cdiv(a.nq, BM), a.num_heads, a.batch),
+                dim3(C::THREADS), C::SMEM_BYTES, stream, mkh, mkl, mvh, mvl, a, sc);
 }
 
 inline bool attention_tc_eligible(int head_dim, int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo) {

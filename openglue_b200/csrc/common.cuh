@@ -106,11 +106,10 @@ __host__ __device__ inline int64_t align_up(int64_t x, int64_t a) { return (x + 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// The keys of attention sequence b: nk, or in a padded batch (RAGGED) its own length klen[b], clamped into [1, nk]
-template <bool RAGGED>
-__device__ __forceinline__ int attention_keys(const int* klen, int b, int nk) {
-  if constexpr (RAGGED) return min(max(__ldg(klen + b), 1), nk);
-  else return nk;
+// The length of sequence b of a batch with capacity cap: cap, or in a padded batch (len non-null) its own length len[b], clamped
+// into [1, cap]
+__device__ __forceinline__ int padded_length(const int* len, int b, int cap) {
+  return len ? min(max(__ldg(len + b), 1), cap) : cap;
 }
 
 __device__ __forceinline__ float warp_max(float v) {

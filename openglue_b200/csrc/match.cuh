@@ -9,20 +9,18 @@ namespace og {
 
 constexpr int MATCH_ROW_CHUNK = 64;     // rows per column-pass chunk
 
-// Padded batch (RAGGED): pair b's rows and columns, lens[b] and lens[B + b] clamped into [1, n] / [1, m]; n, m otherwise.
-template <bool RAGGED>
-__device__ __forceinline__ int2 match_lengths(const int* lens, int b, int n, int m) {
-  if constexpr (!RAGGED) return make_int2(n, m);
-  else return make_int2(min(max(__ldg(lens + b), 1), n), min(max(__ldg(lens + gridDim.y + b), 1), m));
+// Pair b's rows and columns: n, m, or in a padded batch of B pairs (lens non-null) lens[b] and lens[B + b] clamped into [1, n] / [1, m]
+__device__ __forceinline__ int2 match_lengths(const int* lens, int b, int B, int n, int m) {
+  if (!lens) return make_int2(n, m);
+  return make_int2(padded_length(lens, b, n), padded_length(lens + B, b, m));
 }
 
 // one warp per row: (max, first argmax) over columns 0..m-1 (the pair's; a padded batch's rows past its length are skipped)
-template <bool RAGGED>
 __global__ void __launch_bounds__(256) match_rowmax_kernel(const float* __restrict__ scores, int n, int m, const int* lens,
                                                             float* __restrict__ rowval, int* __restrict__ rowidx) {
   const int b = blockIdx.y;
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int2 len = match_lengths<RAGGED>(lens, b, n, m);
+  const int2 len = match_lengths(lens, b, gridDim.y, n, m);
   if (row >= len.x) return;
   const float* src = scores + ((int64_t)b * (n + 1) + row) * (m + 1);
   float best = -CUDART_INF_F; int bi = 0x7fffffff;
@@ -41,15 +39,14 @@ __global__ void __launch_bounds__(256) match_rowmax_kernel(const float* __restri
 
 // one thread per column per row-chunk: partial (max, first argmax) over the chunk's rows (a chunk past a padded pair's rows: -inf,
 // which never wins the strict comparison of match_colreduce_kernel)
-template <bool RAGGED>
 __global__ void __launch_bounds__(256) match_colmax_kernel(const float* __restrict__ scores, int n, int m, const int* lens, int chunks,
                                                             float* __restrict__ pval, int* __restrict__ pidx) {
   const int b = blockIdx.z, chunk = blockIdx.y;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  const int2 len = RAGGED ? make_int2(min(max(__ldg(lens + b), 1), n), min(max(__ldg(lens + gridDim.z + b), 1), m)) : make_int2(n, m);
+  const int2 len = match_lengths(lens, b, gridDim.z, n, m);
   if (c >= len.y) return;
   const int r0 = chunk * MATCH_ROW_CHUNK, r1 = min(r0 + MATCH_ROW_CHUNK, len.x);
-  if (RAGGED && r0 >= r1) {
+  if (r0 >= r1) {
     pval[((int64_t)b * chunks + chunk) * m + c] = -CUDART_INF_F;
     pidx[((int64_t)b * chunks + chunk) * m + c] = r0;
     return;
@@ -78,7 +75,6 @@ __global__ void __launch_bounds__(256) match_colreduce_kernel(int n, int m, int 
 }
 
 // padded batch: -1 / 0 past the pair's lengths
-template <bool RAGGED>
 __global__ void __launch_bounds__(256) match_finalize_kernel(int n, int m, const int* lens, float thr, const float* __restrict__ rowval,
                                                               const int* __restrict__ rowidx, const int* __restrict__ colidx,
                                                               int64_t* __restrict__ matches0, float* __restrict__ mscores0,
@@ -88,12 +84,12 @@ __global__ void __launch_bounds__(256) match_finalize_kernel(int n, int m, const
   const int* ri = rowidx + (int64_t)b * n;
   const int* ci = colidx + (int64_t)b * m;
   const float* rv = rowval + (int64_t)b * n;
-  const int2 len = match_lengths<RAGGED>(lens, b, n, m);       // rows / columns past them: -1 / 0
-  if (RAGGED && t >= len.x && t < n) {
+  const int2 len = match_lengths(lens, b, gridDim.y, n, m);    // rows / columns past them: -1 / 0
+  if (t >= len.x && t < n) {
     if (matches0) matches0[(int64_t)b * n + t] = -1;
     if (mscores0) mscores0[(int64_t)b * n + t] = 0.f;
   }
-  if (RAGGED && t >= len.y && t < m) {
+  if (t >= len.y && t < m) {
     if (matches1) matches1[(int64_t)b * m + t] = -1;
     if (mscores1) mscores1[(int64_t)b * m + t] = 0.f;
   }
@@ -124,9 +120,8 @@ inline int64_t match_workspace_bytes(int B, int n, int m) {
 }
 
 // lens (padded batch, device): n_0 .. n_{B-1}, then m_0 .. m_{B-1}; n, m are the capacity
-template <bool RAGGED>
-inline int match_launch_impl(const float* scores, int B, int n, int m, const int* lens, float thr, int64_t* matches0, float* mscores0,
-                             int64_t* matches1, float* mscores1, void* ws, int64_t ws_bytes, cudaStream_t stream) {
+inline int match_launch(const float* scores, int B, int n, int m, float thr, int64_t* matches0, float* mscores0, int64_t* matches1,
+                        float* mscores1, void* ws, int64_t ws_bytes, cudaStream_t stream, const int* lens = nullptr) {
   if (ws_bytes < match_workspace_bytes(B, n, m)) return fail(OG_EWORKSPACE, "match: workspace too small");
   const int chunks = cdiv(n, MATCH_ROW_CHUNK);
   char* w = static_cast<char*>(ws);
@@ -136,18 +131,12 @@ inline int match_launch_impl(const float* scores, int B, int n, int m, const int
   float* pval = reinterpret_cast<float*>(w); w += align_up((int64_t)B * chunks * m * 4, 256);
   int* pidx = reinterpret_cast<int*>(w);
   int rc;
-  if ((rc = OG_LAUNCH(match_rowmax_kernel<RAGGED>, dim3(cdiv(n, 8), B), 256, 0, stream, scores, n, m, lens, rowval, rowidx))) return rc;
-  if ((rc = OG_LAUNCH(match_colmax_kernel<RAGGED>, dim3(cdiv(m, 256), chunks, B), 256, 0, stream, scores, n, m, lens, chunks, pval, pidx)))
+  if ((rc = OG_LAUNCH(match_rowmax_kernel, dim3(cdiv(n, 8), B), 256, 0, stream, scores, n, m, lens, rowval, rowidx))) return rc;
+  if ((rc = OG_LAUNCH(match_colmax_kernel, dim3(cdiv(m, 256), chunks, B), 256, 0, stream, scores, n, m, lens, chunks, pval, pidx)))
     return rc;
   if ((rc = OG_LAUNCH(match_colreduce_kernel, dim3(cdiv(m, 256), B), 256, 0, stream, n, m, chunks, pval, pidx, colidx))) return rc;
-  return OG_LAUNCH(match_finalize_kernel<RAGGED>, dim3(cdiv(std::max(n, m), 256), B), 256, 0, stream, n, m, lens, thr, rowval, rowidx,
+  return OG_LAUNCH(match_finalize_kernel, dim3(cdiv(std::max(n, m), 256), B), 256, 0, stream, n, m, lens, thr, rowval, rowidx,
                    colidx, matches0, mscores0, matches1, mscores1);
-}
-
-inline int match_launch(const float* scores, int B, int n, int m, float thr, int64_t* matches0, float* mscores0, int64_t* matches1,
-                        float* mscores1, void* ws, int64_t ws_bytes, cudaStream_t stream, const int* lens = nullptr) {
-  if (lens) return match_launch_impl<true>(scores, B, n, m, lens, thr, matches0, mscores0, matches1, mscores1, ws, ws_bytes, stream);
-  return match_launch_impl<false>(scores, B, n, m, nullptr, thr, matches0, mscores0, matches1, mscores1, ws, ws_bytes, stream);
 }
 
 }  // namespace og

@@ -49,7 +49,7 @@ struct SinkArgs {
   float* vglob;                          // resident kernel: [B, mpad] 64-bit words, v as each strip publishes its columns
   float* hist_u;                         // optional [B][iters][n+1]: u_t of every iteration  (kept for the backward pass,
   float* hist_v;                         // optional [B][iters+1][m+1]: v_t, row 0 = v_0 = 0   csrc/sinkhorn_bwd.cuh)
-  const int* len_n;                      // padded batch (the RAGGED kernels): pair b has len_n[b] rows and len_m[b] columns of the
+  const int* len_n;                      // padded batch (null otherwise): pair b has len_n[b] rows and len_m[b] columns of the
   const int* len_m;                      // capacity n x m (clamped into [1, n] / [1, m])
 };
 
@@ -97,61 +97,42 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
 // W C columns; the warps exchange what they know of their segments through shared memory and one named barrier per row);
 // G = SINK_WARPS / W row groups = rows in progress per CTA.  A warp works on rows r0 + grp, r0 + grp + G, ... of its strip
 // [r0, r1) (row n is the dustbin row), columns [c0, c0 + C) of each.
-// n(a), m(a): the pair's rows and columns, a.n and a.m or, in a padded batch (R), its own lengths (set_lengths: r1 <= r0 for a
-// strip past them).
-template <int V, int W, bool R = false>
+// n, m: the pair's rows and columns, a.n and a.m or, in a padded batch, its own lengths (r1 <= r0 for a strip past them).
+template <int V, int W>
 struct SinkStrip {
   static constexpr int C = 128 * V, MC = W * C, G = SINK_WARPS / W;
-  int b, strip, tid, lane, grp, sub, c0, r0, r1;
-  int n_ = 0, m_ = 0;
+  int b, strip, tid, lane, grp, sub, c0, r0, r1, n, m;
   template <class Args>
-  __device__ __forceinline__ explicit SinkStrip(const Args& a) {
+  __device__ __forceinline__ SinkStrip(const Args& a, int rows, int cols) : n(rows), m(cols) {
     b = blockIdx.x / a.SP; strip = blockIdx.x % a.SP;
     tid = threadIdx.x; lane = tid & 31;
     grp = (tid >> 5) / W; sub = (tid >> 5) % W;
     c0 = sub * C;
     r0 = strip * a.rows_per_strip;
-    r1 = min(r0 + a.rows_per_strip, a.n + 1);
+    r1 = min(r0 + a.rows_per_strip, n + 1);
   }
-  __device__ __forceinline__ void set_lengths(int n, int m, int rows_per_strip) {
-    n_ = n; m_ = m;
-    r1 = min(r0 + rows_per_strip, n + 1);
-  }
-  template <class Args> __device__ __forceinline__ int n(const Args& a) const { if constexpr (R) return n_; else return a.n; }
-  template <class Args> __device__ __forceinline__ int m(const Args& a) const { if constexpr (R) return m_; else return a.m; }
 };
 
-// The pair's lengths and the constants of its marginals (SinkConsts): the arguments' own, or in a padded batch (RAGGED) the pair's
-// from the tables of the host's logarithms (sinkhorn_log_tables), so that a pair at the capacity gets the very bits the uniform
-// kernel gets.
+// The lengths of pair b and the constants of its marginals (SinkConsts): the arguments' own, or in a padded batch (a.len_n set) the
+// pair's, from the tables of the host's logarithms (sinkhorn_log_tables), so that a pair at the capacity gets the very bits a
+// uniform batch gets.  A uniform batch never reads the tables.
 constexpr int SINK_MAX_ROWS = 65536;                   // rows of a padded batch's capacity at most (the size of the tables)
 __device__ float og_sink_logf_tab[SINK_MAX_ROWS + SINK_MAX_COLS + 1];   // [k] = logf((float)k), the host's libm
 __device__ float og_sink_log_tab[SINK_MAX_ROWS + 1];                    // [k] = (float)log((double)k)
-template <bool RAGGED> struct SinkPair;
-template <> struct SinkPair<false> {                   // reads the arguments, as the uniform kernels always have
-  const SinkArgs& a;
-  __device__ __forceinline__ SinkPair(const SinkArgs& args, int) : a(args) {}
-  __device__ __forceinline__ int n() const { return a.n; }
-  __device__ __forceinline__ int m() const { return a.m; }
-  __device__ __forceinline__ float norm() const { return a.norm; }
-  __device__ __forceinline__ float log_a_last() const { return a.log_a_last; }
-  __device__ __forceinline__ float log_b_last() const { return a.log_b_last; }
-};
-template <> struct SinkPair<true> {
-  int n_, m_;
-  float norm_, la_, lb_;
+struct SinkPair {
+  int n, m;
+  float norm, log_a_last, log_b_last;
   __device__ __forceinline__ SinkPair(const SinkArgs& a, int b) {
-    n_ = min(max(__ldg(a.len_n + b), 1), a.n);
-    m_ = min(max(__ldg(a.len_m + b), 1), a.m);
-    norm_ = -og_sink_logf_tab[n_ + m_];
-    la_ = norm_ + og_sink_log_tab[m_];
-    lb_ = norm_ + og_sink_log_tab[n_];
+    n = padded_length(a.len_n, b, a.n);
+    m = padded_length(a.len_m, b, a.m);
+    if (a.len_n) {
+      norm = -og_sink_logf_tab[n + m];
+      log_a_last = norm + og_sink_log_tab[m];
+      log_b_last = norm + og_sink_log_tab[n];
+    } else {
+      norm = a.norm; log_a_last = a.log_a_last; log_b_last = a.log_b_last;
+    }
   }
-  __device__ __forceinline__ int n() const { return n_; }
-  __device__ __forceinline__ int m() const { return m_; }
-  __device__ __forceinline__ float norm() const { return norm_; }
-  __device__ __forceinline__ float log_a_last() const { return la_; }
-  __device__ __forceinline__ float log_b_last() const { return lb_; }
 };
 
 // One warp's slice of the shared-memory row ring, fed by bulk async copies (TMA 1-D) so that HBM latency overlaps the math of
@@ -159,7 +140,7 @@ template <> struct SinkPair<true> {
 // `consumed` counts the real rows taken so far and gives each its slot and phase.  EVICT_FIRST loads with the L2 evict_first
 // policy (the forward pass): at the headline shape the score matrix is five times the 50 MB L2 and is swept cyclically, so
 // its lines would hit nothing and only push out those of the kernels that follow.
-template <int V, int W, int SLOTS, bool EVICT_FIRST, class Args, bool R = false>
+template <int V, int W, int SLOTS, bool EVICT_FIRST, class Args>
 struct SinkRowRing {
   static constexpr int C = 128 * V, G = SINK_WARPS / W;
   float* slot;                                         // [SLOTS][C]
@@ -167,20 +148,19 @@ struct SinkRowRing {
   const Args& a;
   const float* seg;                                    // this warp's column segment of row 0 of the pair
   int first, end_real, n, c0, lane;                    // first row of the warp; rows >= end_real do not exist in memory; row n: dustbin
-                                                       // (R; a.n otherwise)
   uint32_t bytes, consumed;                            // bytes of a segment: 0 when it lies beyond the last column
   bool full;                                           // the whole segment lies inside the row (warp-uniform)
   float dz;                                            // the dustbin score divided by reg, Z = M / reg
   uint64_t policy;
 
-  __device__ __forceinline__ SinkRowRing(const Args& args, const SinkStrip<V, W, R>& s, float* ring, uint64_t* bars) : a(args) {
+  __device__ __forceinline__ SinkRowRing(const Args& args, const SinkStrip<V, W>& s, float* ring, uint64_t* bars) : a(args) {
     const int warp = s.grp * W + s.sub;
     slot = ring + warp * SLOTS * C;
     bar = bars + warp * SLOTS;
     seg = a.S + (int64_t)s.b * a.strideS + s.c0;
     first = s.r0 + s.grp;
-    end_real = min(s.r1, s.n(a));
-    n = s.n(a);
+    end_real = min(s.r1, s.n);
+    n = s.n;
     c0 = s.c0; lane = s.lane;
     const int seg_cols = min(a.m, c0 + C) - c0;        // <= 0: this warp's segment lies beyond the last column
     bytes = seg_cols > 0 ? (uint32_t)(((seg_cols + 3) / 4) * 16) : 0u;     // <= 4 * (lds - c0): inside the padded row
@@ -219,7 +199,7 @@ struct SinkRowRing {
   // This warp's segment of row `row` in registers (columns >= a.m zero, divided by reg), and the slot refilled with the row SLOTS
   // ahead.  The dustbin row is the constant dustbin score.
   __device__ __forceinline__ void take(int row, float4 (&z)[V]) {
-    if (row >= (R ? n : a.n)) {
+    if (row >= n) {
 #pragma unroll
       for (int k = 0; k < V; ++k) z[k] = make_float4(dz, dz, dz, dz);
       return;
@@ -251,8 +231,12 @@ struct SinkRowRing {
       }
     }
     ++consumed;
-    __syncwarp();                                      // every lane has its part of the row in registers
+    // The refill is an async-proxy write to the slot the lanes have just read through the generic proxy.  The memory model orders
+    // the two only through a proxy fence; without it, whether the bulk copy can overtake the reads depends on the schedule nvcc
+    // emits (16 pairs of 2048 x 2048 gave run-to-run differences on an H100 for a schedule that did not hide it).
     const int nxt = row + SLOTS * G;
+    if (nxt < end_real) tc::fence_proxy_async();
+    __syncwarp();                                      // every lane has its part of the row in registers
     if (lane == 0 && nxt < end_real) copy(sl, nxt);
     if (a.reg != 1.0f) {
       const float reg = a.reg;
@@ -268,8 +252,8 @@ struct SinkRowRing {
 // The W warps of a row group publish one value each (`mine`) and meet at the group's named barrier; the returned W values are
 // in warp order, the same in every warp.  The buffer xr [2][G][W] alternates halves row by row (rowpar), so a warp that runs
 // ahead into the next row cannot overwrite values another warp has yet to read.
-template <int V, int W, bool R, class X>
-__device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkStrip<V, W, R>& s, uint32_t& rowpar) {
+template <int V, int W, class X>
+__device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkStrip<V, W>& s, uint32_t& rowpar) {
   X* x = xr + (rowpar * SinkStrip<V, W>::G + s.grp) * W;
   if (s.lane == 0) x[s.sub] = mine;
   asm volatile("bar.sync %0, %1;" ::"r"(1 + s.grp), "n"(W * 32) : "memory");
@@ -282,10 +266,10 @@ __device__ __forceinline__ const X* sink_row_exchange(X* xr, X mine, const SinkS
 // memory (buffer k & 1 of two) -> barrier among the SP CTAs of the pair -> every CTA of the pair rebuilds the sums in the same
 // fixed order (bitwise identical across CTAs) and calls update(j, sum) for j < m and update(MC, sum) for the dustbin column.
 // sink_strip_sums is its first part: the strip's column sums, passed to store(j, sum) for j <= m.
-template <int V, int W, bool R, class Args, class Store>
-__device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V, W, R>& s, float* red, const float4 (&cacc)[V],
+template <int V, int W, class Args, class Store>
+__device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
                                                 float cacc_m, Store store) {
-  const int m = s.m(a);
+  const int m = s.m;
   float* myred = red + s.grp * a.mpad;
 #pragma unroll
   for (int q = 0; q < V; ++q) {
@@ -303,10 +287,10 @@ __device__ __forceinline__ void sink_strip_sums(const Args& a, const SinkStrip<V
   }
 }
 
-template <int V, int W, bool R, class Args, class Update>
-__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W, R>& s, float* red, const float4 (&cacc)[V],
+template <int V, int W, class Args, class Update>
+__device__ __forceinline__ void sink_column_reduce(const Args& a, const SinkStrip<V, W>& s, float* red, const float4 (&cacc)[V],
                                                    float cacc_m, int k, Update update) {
-  const int m = s.m(a);
+  const int m = s.m;
   const int64_t buf = (int64_t)(k & 1) * a.B * a.SP + (int64_t)s.b * a.SP;
   float* part = a.partial + (buf + s.strip) * a.mpad;
   sink_strip_sums(a, s, red, cacc, cacc_m, [&](int j, float sum) { part[j] = sum; });
@@ -341,12 +325,12 @@ template <int NR> using SinkRowStat = std::conditional_t<NR == 1, float2, float4
 // share e_ij a_i / S_i of the column sums, added to cacc (cacc_m: the dustbin column, counted by segment 0) row by row in order.
 // v_s: v of the pair in shared memory, v_m = v_s[MC].  Two rows share one read of v and one exchange, and their reduction chains
 // are independent, so one row's shuffles run under the other's exponentials; each row's arithmetic is the same for NR = 1 and 2.
-template <int V, int W, int NR, bool R>
-__device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkPair<R>& P, const SinkStrip<V, W, R>& s, const float4 (*q)[V],
+template <int V, int W, int NR>
+__device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkPair& P, const SinkStrip<V, W>& s, const float4 (*q)[V],
                                               const float* v_s, float v_m, float dz, float a_reg, float a_last, SinkRowStat<NR>* xr,
                                               uint32_t& rowpar, int row0, int it, f32x2 (&cacc)[2 * V], float& cacc_m) {
   static_assert(NR == 1 || NR == 2, "one or two rows at a time");
-  const int n = P.n(), c0 = s.c0, lane = s.lane, sub = s.sub;
+  const int n = P.n, c0 = s.c0, lane = s.lane, sub = s.sub;
   const f32x2 log2e2 = pk2(LOG2E_F, LOG2E_F);
   f32x2 z[NR][2 * V];
 #pragma unroll
@@ -420,7 +404,7 @@ __device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkPair<
 #pragma unroll
     for (int r = 0; r < NR; ++r) {
       const int row = row0 + r * SinkStrip<V, W>::G;
-      const float u_i = ((row < n) ? P.norm() : P.log_a_last()) - (mxg[r] + logf(s_i[r]));
+      const float u_i = ((row < n) ? P.norm : P.log_a_last) - (mxg[r] + logf(s_i[r]));
       if (it == a.iters - 1) a.u[(int64_t)s.b * (a.n + 1) + row] = u_i;
       if (a.hist_u) a.hist_u[((int64_t)s.b * a.iters + it) * (a.n + 1) + row] = u_i;
     }
@@ -435,10 +419,10 @@ __device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkPair<
 }
 
 // The final pass over one row: scores = Z + u + v - norm   (optimal_transport.py:28, superglue.py:111).  Rows are a.m + 1 apart.
-template <int V, int W, bool R>
-__device__ __forceinline__ void sink_fwd_score_row(const SinkArgs& a, const SinkPair<R>& P, const SinkStrip<V, W, R>& s, const float4 (&z)[V],
+template <int V, int W>
+__device__ __forceinline__ void sink_fwd_score_row(const SinkArgs& a, const SinkPair& P, const SinkStrip<V, W>& s, const float4 (&z)[V],
                                                    const float* v_s, float v_m, float dz, int row) {
-  const int m = P.m(), c0 = s.c0, lane = s.lane;
+  const int m = P.m, c0 = s.c0, lane = s.lane;
   float u_i = 0.f;
   if (a.iters > 0) {
     if (lane == 0) u_i = __ldcg(a.u + (int64_t)s.b * (a.n + 1) + row);
@@ -450,32 +434,32 @@ __device__ __forceinline__ void sink_fwd_score_row(const SinkArgs& a, const Sink
     const int c = c0 + 4 * (lane + 32 * k);
     if (c < m) {
       const float4 vv = *reinterpret_cast<const float4*>(v_s + c);
-      if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - P.norm();
-      if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - P.norm();
-      if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - P.norm();
-      if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - P.norm();
+      if (c + 0 < m) out[c + 0] = (z[k].x + u_i) + vv.x - P.norm;
+      if (c + 1 < m) out[c + 1] = (z[k].y + u_i) + vv.y - P.norm;
+      if (c + 2 < m) out[c + 2] = (z[k].z + u_i) + vv.z - P.norm;
+      if (c + 3 < m) out[c + 3] = (z[k].w + u_i) + vv.w - P.norm;
     }
   }
-  if (s.sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - P.norm();
+  if (s.sub == 0 && lane == 0) out[m] = (dz + u_i) + v_m - P.norm;
 }
 
 // Padded batch, after the final pass: -inf over the strip's share of the padding of the pair's [a.n + 1, a.m + 1] block, the
 // columns past its dustbin column in its rows and every column of the capacity's rows past its dustbin row.
 template <int V, int W>
-__device__ __forceinline__ void sink_fill_padding(const SinkArgs& a, const SinkStrip<V, W, true>& s) {
+__device__ __forceinline__ void sink_fill_padding(const SinkArgs& a, const SinkStrip<V, W>& s) {
   const int rend = min(s.r0 + a.rows_per_strip, a.n + 1);
   for (int row = s.r0; row < rend; ++row) {
     float* out = a.scores + ((int64_t)s.b * (a.n + 1) + row) * (a.m + 1);
-    for (int c = (row <= s.n_ ? s.m_ + 1 : 0) + s.tid; c <= a.m; c += blockDim.x) out[c] = -CUDART_INF_F;
+    for (int c = (row <= s.n ? s.m + 1 : 0) + s.tid; c <= a.m; c += blockDim.x) out[c] = -CUDART_INF_F;
   }
 }
 
 // SLOTS: ring depth per warp.  Configurations with V <= 8 need <= 128 registers and <= 106 KB of shared memory: two CTAs per
 // SM, so one CTA streams while the other sits in its per-iteration reduction / barrier phase.
-template <int V, int W, int SLOTS, bool RAGGED>
-__device__ __forceinline__ void sinkhorn_sweeps(const SinkArgs& a) {
+template <int V, int W, int SLOTS>
+__global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_kernel(SinkArgs a) {
   extern __shared__ __align__(128) float og_sink_smem[];
-  using Strip = SinkStrip<V, W, RAGGED>;
+  using Strip = SinkStrip<V, W>;
   constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G;
   float* v_s = og_sink_smem;                           // [MC + 4]  v_j for j < m, -inf for m <= j < MC (masks the padding
                                                        //           columns in the sweep without per-element selects), v_s[MC] = v_dustbin
@@ -483,13 +467,11 @@ __device__ __forceinline__ void sinkhorn_sweeps(const SinkArgs& a) {
   float* ring = red + G * a.mpad;                      // [SINK_WARPS][SLOTS][C]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);   // [SINK_WARPS][SLOTS]
   float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS * SLOTS);             // [2][G][W] (max, sum) of a segment
-  Strip strip(a);
-  const SinkPair<RAGGED> P(a, strip.b);
-  if (RAGGED) strip.set_lengths(P.n(), P.m(), a.rows_per_strip);
-  const Strip& s = strip;
-  const int m = P.m();
-  const float a_reg = expf(P.norm()), a_last = expf(P.log_a_last());
-  SinkRowRing<V, W, SLOTS, true, SinkArgs, RAGGED> rows(a, s, ring, bars);
+  const SinkPair P(a, blockIdx.x / a.SP);
+  const Strip s(a, P.n, P.m);
+  const int m = P.m;
+  const float a_reg = expf(P.norm), a_last = expf(P.log_a_last);
+  SinkRowRing<V, W, SLOTS, true, SinkArgs> rows(a, s, ring, bars);
   const float dz = rows.dz;
 
   for (int j = s.tid; j < MC; j += blockDim.x) v_s[j] = (j < m) ? 0.f : -CUDART_INF_F;
@@ -515,7 +497,7 @@ __device__ __forceinline__ void sinkhorn_sweeps(const SinkArgs& a) {
 #pragma unroll
     for (int k = 0; k < V; ++k) { upk2(cacc[2 * k], c4[k].x, c4[k].y); upk2(cacc[2 * k + 1], c4[k].z, c4[k].w); }
     sink_column_reduce(a, s, red, c4, cacc_m, it, [&](int j, float c) {
-      v_s[j] = ((j < MC) ? P.norm() : P.log_b_last()) + v_s[j] - logf(c);
+      v_s[j] = ((j < MC) ? P.norm : P.log_b_last) + v_s[j] - logf(c);
     });
     if (a.hist_v && s.strip == 0) {                   // every CTA of the pair holds the same v: one of them records it
       float* hv = a.hist_v + ((int64_t)s.b * (a.iters + 1) + it + 1) * (m + 1);
@@ -529,16 +511,7 @@ __device__ __forceinline__ void sinkhorn_sweeps(const SinkArgs& a) {
     rows.take(row, z);
     sink_fwd_score_row(a, P, s, z, v_s, v_m, dz, row);
   }
-  if constexpr (RAGGED) sink_fill_padding(a, s);
-}
-template <int V, int W, int SLOTS>
-__global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_kernel(SinkArgs a) {
-  sinkhorn_sweeps<V, W, SLOTS, false>(a);
-}
-// The padded batch's form: each pair's own lengths (SinkArgs::len_n / len_m) in the capacity's layout and plan.
-template <int V, int W, int SLOTS>
-__global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_padded_kernel(SinkArgs a) {
-  sinkhorn_sweeps<V, W, SLOTS, true>(a);
+  if (a.len_n) sink_fill_padding(a, s);
 }
 
 // A value and the iteration (from 1) it belongs to, as one 64-bit word: a single-copy-atomic store and load carry both, so a reader
@@ -576,11 +549,11 @@ __device__ __forceinline__ void sink_take(float (&x)[N], At at, uint32_t tag) {
 // The resident kernel's form of sink_strip_sums, in half the shared memory: the upper half of the row groups parks its column sums
 // in red [G/2][mpad] (the dustbin column in redm [G]), the lower half adds its own to them, and store(j, sum) gets the G/2 folded
 // sums added in order (a fixed order: the same bits in every run).
-template <int V, int W, bool R, class Args, class Store>
-__device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const SinkStrip<V, W, R>& s, float* red, float* redm,
+template <int V, int W, class Args, class Store>
+__device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const SinkStrip<V, W>& s, float* red, float* redm,
                                                        const float4 (&cacc)[V], float cacc_m, Store store) {
   constexpr int H = SinkStrip<V, W>::G / 2;
-  const int m = s.m(a);
+  const int m = s.m;
   float4* fold = reinterpret_cast<float4*>(red + (s.grp % H) * a.mpad);
   if (s.grp >= H) {
 #pragma unroll
@@ -623,11 +596,11 @@ __device__ __forceinline__ void sink_strip_sums_folded(const Args& a, const Sink
 // v back.  Partials and v travel as (value, iteration + 1) words (sink_put / sink_take), so a reader waits for exactly the words it
 // needs and the pair needs no barrier: a strip writes its next partials only after it has read all of v, which every owner
 // publishes only after it has read all partials of its columns, so one buffer of each suffices.  Both are zeroed before each launch.
-template <int V, int W, int RR, bool RAGGED>
-__device__ __forceinline__ void sinkhorn_resident_sweeps(const SinkArgs& a) {
+template <int V, int W, int RR>
+__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(SinkArgs a) {
   static_assert(RR % 2 == 0, "the register rows go two at a time");
   extern __shared__ __align__(128) float og_sink_smem[];
-  using Strip = SinkStrip<V, W, RAGGED>;
+  using Strip = SinkStrip<V, W>;
   constexpr int C = Strip::C, MC = Strip::MC, G = Strip::G, NT = SINK_WARPS * 32, HS = SINK_WARPS * (C / 4);
   const int slots = max(a.rows_smem, 1);
   float* v_s = og_sink_smem;                                              // [MC + 4]  as in sinkhorn_kernel
@@ -638,14 +611,12 @@ __device__ __forceinline__ void sinkhorn_resident_sweeps(const SinkArgs& a) {
   float2* xr = reinterpret_cast<float2*>(bars + SINK_WARPS);             // [2][G][W]  one row's (max, sum)
   float4* xr2 = reinterpret_cast<float4*>(xr + 2 * G * W);               // [2][G][W]  two rows'
   float* redm = reinterpret_cast<float*>(xr2 + 2 * G * W);               // [G]
-  Strip strip(a);
-  const SinkPair<RAGGED> P(a, strip.b);
-  if (RAGGED) strip.set_lengths(P.n(), P.m(), a.rows_per_strip);
-  const Strip& s = strip;
-  const int m = P.m(), lane = s.lane, row0 = s.r0 + s.grp;
-  const float a_reg = expf(P.norm()), a_last = expf(P.log_a_last());
+  const SinkPair P(a, blockIdx.x / a.SP);
+  const Strip s(a, P.n, P.m);
+  const int m = P.m, lane = s.lane, row0 = s.r0 + s.grp;
+  const float a_reg = expf(P.norm), a_last = expf(P.log_a_last);
   float4* mine = held + (s.grp * W + s.sub) * (C / 4);
-  SinkRowRing<V, W, 1, true, SinkArgs, RAGGED> rows(a, s, reinterpret_cast<float*>(held + (size_t)(slots - 1) * HS), bars);
+  SinkRowRing<V, W, 1, true, SinkArgs> rows(a, s, reinterpret_cast<float*>(held + (size_t)(slots - 1) * HS), bars);
   const float dz = rows.dz;
   uint64_t* vg = reinterpret_cast<uint64_t*>(a.vglob) + (int64_t)s.b * a.mpad;
 
@@ -693,7 +664,7 @@ __device__ __forceinline__ void sinkhorn_resident_sweeps(const SinkArgs& a) {
         visit(row, q);
       }
       if (last) {
-        if constexpr (RAGGED) sink_fill_padding(a, s);
+        if (a.len_n) sink_fill_padding(a, s);
         break;
       }
     } else {
@@ -734,7 +705,7 @@ __device__ __forceinline__ void sinkhorn_resident_sweeps(const SinkArgs& a) {
     // order (a fixed order: the same bits in every run)
     const int S = cdiv(m + 1, a.SP), lo = s.strip * S, NG = S >= NT ? 1 : NT / S;
     auto publish = [&](int j, float c) {
-      sink_put(vg + j, ((j < m) ? P.norm() + v_s[j] : P.log_b_last() + v_s[MC]) - logf(c), tag);
+      sink_put(vg + j, ((j < m) ? P.norm + v_s[j] : P.log_b_last + v_s[MC]) - logf(c), tag);
     };
     for (int i = s.tid; i < S * NG; i += NT) {
       const int j = lo + i % S;
@@ -769,14 +740,6 @@ __device__ __forceinline__ void sinkhorn_resident_sweeps(const SinkArgs& a) {
     }
     __syncthreads();
   }
-}
-template <int V, int W, int RR>
-__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_kernel(SinkArgs a) {
-  sinkhorn_resident_sweeps<V, W, RR, false>(a);
-}
-template <int V, int W, int RR>
-__global__ void __launch_bounds__(SINK_WARPS * 32, 1) sinkhorn_resident_padded_kernel(SinkArgs a) {
-  sinkhorn_resident_sweeps<V, W, RR, true>(a);
 }
 
 // resident: the plan is for sinkhorn_resident_kernel (slots = 1, occ = 1); rows_reg / rows_smem: rows per warp in registers /
@@ -918,7 +881,7 @@ inline int64_t sinkhorn_workspace_bytes(int B, int n, int m) {
   return SINK_BARRIER_BYTES + align_up((int64_t)B * (n + 1) * 4, 256) + align_up(rows * p.mpad * 4, 256);
 }
 
-// The tables sink_pair<true> reads, from the host's own logf / log (bit for bit what sinkhorn_consts computes), copied to the
+// The tables SinkPair reads in a padded batch, from the host's own logf / log (bit for bit what sinkhorn_consts computes), copied to the
 // current device at its first padded Sinkhorn.  That copy is synchronous, so it cannot be part of a stream capture: a capture
 // needs one padded call on the device before it.
 inline int sinkhorn_log_tables(cudaStream_t stream) {
@@ -944,26 +907,24 @@ inline int sinkhorn_log_tables(cudaStream_t stream) {
   return OG_OK;
 }
 
-template <int V, int W, bool RAGGED>
+template <int V, int W>
 inline int sinkhorn_resident_launch(const SinkArgs& a, const SinkPlan& p, cudaStream_t stream) {
-  constexpr auto kernel = RAGGED ? sinkhorn_resident_padded_kernel<V, W, 16 / V> : sinkhorn_resident_kernel<V, W, 16 / V>;
+  constexpr auto kernel = sinkhorn_resident_kernel<V, W, 16 / V>;
   if (const int rc = smem_opt_in<kernel>((int)OG_SMEM_OPTIN_MAX)) return rc;
   return launch("sinkhorn_resident_kernel", kernel, LaunchAttr::cooperative, dim3(a.B * a.SP), dim3(SINK_WARPS * 32), p.smem,
                 stream, a);
 }
 
-template <bool RAGGED>
 inline int sinkhorn_kernel_launch(const SinkArgs& a, const SinkPlan& p, cudaStream_t stream) {
   if (p.resident) {
-    if (p.W == 1) return sinkhorn_resident_launch<4, 1, RAGGED>(a, p, stream);
-    return p.V == 4 ? sinkhorn_resident_launch<4, 2, RAGGED>(a, p, stream) : sinkhorn_resident_launch<8, 2, RAGGED>(a, p, stream);
+    if (p.W == 1) return sinkhorn_resident_launch<4, 1>(a, p, stream);
+    return p.V == 4 ? sinkhorn_resident_launch<4, 2>(a, p, stream) : sinkhorn_resident_launch<8, 2>(a, p, stream);
   }
-  if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<4, 1, 2> : sinkhorn_kernel<4, 1, 2>, 4, 1, 2>(a, p, stream);
-  if (p.V == 4)             return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<4, 2, 2> : sinkhorn_kernel<4, 2, 2>, 4, 2, 2>(a, p, stream);
-  if (p.V == 8)             return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<8, 2, 2> : sinkhorn_kernel<8, 2, 2>, 8, 2, 2>(a, p, stream);
-  if (p.W == 2)
-    return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<16, 2, 2> : sinkhorn_kernel<16, 2, 2>, 16, 2, 2>(a, p, stream);
-  return sinkhorn_coop_launch<RAGGED ? sinkhorn_padded_kernel<16, 4, 1> : sinkhorn_kernel<16, 4, 1>, 16, 4, 1>(a, p, stream);
+  if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<sinkhorn_kernel<4, 1, 2>, 4, 1, 2>(a, p, stream);
+  if (p.V == 4)             return sinkhorn_coop_launch<sinkhorn_kernel<4, 2, 2>, 4, 2, 2>(a, p, stream);
+  if (p.V == 8)             return sinkhorn_coop_launch<sinkhorn_kernel<8, 2, 2>, 8, 2, 2>(a, p, stream);
+  if (p.W == 2)             return sinkhorn_coop_launch<sinkhorn_kernel<16, 2, 2>, 16, 2, 2>(a, p, stream);
+  return sinkhorn_coop_launch<sinkhorn_kernel<16, 4, 1>, 16, 4, 1>(a, p, stream);
 }
 
 // lens (padded batch, device): n_0 .. n_{B-1}, then m_0 .. m_{B-1}; n, m are the capacity and the plan is the capacity's.
@@ -1003,7 +964,7 @@ inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const f
     a.hist_v = hist_v ? hist_v + (int64_t)b0 * (iters + 1) * (m + 1) : nullptr;
     a.len_n = lens ? lens + b0 : nullptr;
     a.len_m = lens ? lens + B + b0 : nullptr;
-    return lens ? sinkhorn_kernel_launch<true>(a, p, stream) : sinkhorn_kernel_launch<false>(a, p, stream);
+    return sinkhorn_kernel_launch(a, p, stream);
   });
 }
 

@@ -52,7 +52,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
   float* ring = red + G * a.mpad;                      // [SINK_WARPS][SLOTS][C]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);
   float* xr = reinterpret_cast<float*>(bars + SINK_WARPS * SLOTS);               // [2][G][W] partial row sums
-  const Strip s(a);
+  const Strip s(a, a.n, a.m);
   const int n = a.n, m = a.m, T = a.iters, b = s.b, tid = s.tid;
   const float ia_reg = expf(-a.norm), ia_last = expf(-a.log_a_last);      // 1 / a_i
   SinkRowRing<V, W, SLOTS, false, SinkBwdArgs> rows(a, s, ring, bars);

@@ -106,6 +106,51 @@ def test_resident_is_deterministic(B, n, m, iters):
     assert torch.equal(_sinkhorn(S, m, iters, 1), _sinkhorn(S, m, iters, 1))
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize('form', ['uniform', 'padded', 'backward'])
+@pytest.mark.parametrize('B,n,m,iters', [(16, 2048, 2048, 100), (32, 1024, 1024, 20)])
+def test_streaming_is_deterministic(B, n, m, iters, form):
+    """The streaming kernels (forward, padded forward at full lengths, backward) give the same bits in every run.  Their row ring
+    refills a shared-memory slot by bulk copy right after the warp has read it: without the proxy fence between the two, several
+    pairs of 2048 x 2048 gave run-to-run differences of up to 15 in the scores."""
+    lib = _cabi.lib()
+    g = torch.Generator(device=DEV).manual_seed(13)
+    lds = (m + 3) // 4 * 4
+    S = torch.randn(B, n, lds, device=DEV, generator=g) * 4
+    dust = torch.full((1,), 1.3, device=DEV)
+    wsb = lib.og_sinkhorn_workspace_bytes(B, n, m)
+    ws = torch.empty(wsb, dtype=torch.uint8, device=DEV)
+    lens = torch.tensor([n] * B + [m] * B, dtype=torch.int32, device=DEV)
+    hist = torch.empty(lib.og_sinkhorn_hist_floats(B, n, m, iters), device=DEV)
+    G = torch.randn(B, n + 1, m + 1, device=DEV, generator=g)
+    bwsb = lib.og_sinkhorn_bwd_workspace_bytes(B, n, m, iters)
+    bws = torch.empty(bwsb if form == 'backward' else 0, dtype=torch.uint8, device=DEV)
+
+    def run():
+        scores = torch.empty(B, n + 1, m + 1, device=DEV)
+        with _Mode(0):
+            if form == 'uniform':
+                _cabi.check(lib.og_sinkhorn_fwd(_ptr(S), lds, n * lds, _ptr(dust), B, n, m, iters, 1.0, _ptr(scores), _ptr(ws), wsb,
+                                                _stream()), 'og_sinkhorn_fwd')
+            elif form == 'padded':
+                _cabi.check(lib.og_sinkhorn_fwd_padded(_ptr(S), lds, n * lds, _ptr(dust), B, n, m, _ptr(lens), iters, 1.0,
+                                                       _ptr(scores), _ptr(ws), wsb, _stream()), 'og_sinkhorn_fwd_padded')
+            else:
+                _cabi.check(lib.og_sinkhorn_train_fwd(_ptr(S), lds, n * lds, _ptr(dust), B, n, m, iters, 1.0, _ptr(scores), _ptr(hist),
+                                                      _ptr(ws), wsb, _stream()), 'og_sinkhorn_train_fwd')
+                dS, dd = torch.empty(B, n + 1, m + 1, device=DEV), torch.empty(1, device=DEV)
+                _cabi.check(lib.og_sinkhorn_bwd(_ptr(S), lds, n * lds, _ptr(dust), B, n, m, iters, 1.0, _ptr(hist), _ptr(G), _ptr(dS),
+                                                _ptr(dd), _ptr(bws), bwsb, _stream()), 'og_sinkhorn_bwd')
+                scores = torch.cat([scores.flatten(), dS.flatten(), dd])
+        torch.cuda.synchronize()
+        return scores
+
+    first = run()
+    assert torch.isfinite(first).all()
+    for _ in range(4):
+        assert torch.equal(run(), first)
+
+
 # BASELINE.json configs as the Sinkhorn sees them on one H100 (132 SMs): (pairs per GPU, n, m) -> resident, strips, rows per
 # strip, pairs per launch.  C2's 1024-column rows pay more per held row than streaming them costs, so it streams.
 BASELINE_PLANS = {

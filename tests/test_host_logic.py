@@ -166,7 +166,9 @@ def test_tensor_core_kernels_are_hopper_native_and_address_shared_memory_directl
 def test_sinkhorn_kernels_are_the_planned_instantiations_without_spills():
     """Static check of the built library (cuobjdump, no GPU; OG_LIB names another build): it holds exactly the five forward and
     five backward cooperative Sinkhorn instantiations sinkhorn_plan can select, and none touches local memory (STL / LDL:
-    spills) - the V = 16 forms sit within a few registers of the 255 limit."""
+    spills) - the V = 16 forms sit within a few registers of the 255 limit.  Uniform and padded batches run the same kernels
+    (the per-pair lengths are a runtime argument), so every Sinkhorn, attention, match and encoder-input kernel is one of the
+    planned instantiations, with no second, padded form beside it."""
     import re
     import shutil
     import subprocess
@@ -196,6 +198,21 @@ def test_sinkhorn_kernels_are_the_planned_instantiations_without_spills():
     assert set(funcs) == fwd | bwd, sorted(funcs)
     for name, ops in funcs.items():
         assert 'STL' not in ops and 'LDL' not in ops, name
+
+    def kernel(mangled):                                   # _ZN2og<len><name>[I<L{i,b}<value>E>...E]E...: (name, template values)
+        m = re.match(r'_ZN2og(\d+)', mangled)
+        name = mangled[m.end():m.end() + int(m.group(1))]
+        targs = re.match(r'I((?:L[ib]\d+E)+)E', mangled[m.end() + len(name):])
+        return name, tuple(int(v) for v in re.findall(r'\d+', targs.group(1))) if targs else ()
+    operators = {kernel(k) for k in re.findall(r'^\s*Function : (_ZN2og\S+)$', res.stdout, re.M)}
+    operators = {k for k in operators if re.match(r'(sinkhorn|attention|match|kenc)_', k[0])}
+    planned = ({('sinkhorn_kernel', k[1:]) for k in fwd} | {('sinkhorn_bwd_kernel', k[1:]) for k in bwd} |
+               {('sinkhorn_resident_kernel', (v, w, 16 // v)) for v, w in [(4, 1), (4, 2), (8, 2)]} |
+               {('attention_sm90_kernel', k) for k in [(32, 0), (64, 0), (64, 1)]} |
+               {('attention_simt_kernel', (dh,)) for dh in (8, 16, 32, 64)} |
+               {(f'match_{op}_kernel', ()) for op in ('rowmax', 'colmax', 'colreduce', 'finalize', 'compact')} |
+               {('sinkhorn_consts_kernel', ()), ('kenc_input_kernel', ())})
+    assert operators == planned, sorted(operators ^ planned)
 
 
 def test_bench_work_accounting_reproduces_the_survey_table():

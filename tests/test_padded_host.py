@@ -86,7 +86,7 @@ def test_padded_workspace_holds_the_masked_descriptors():
 
 
 def test_host_sinkhorn_constants_are_the_references():
-    """og_sinkhorn_consts is what the uniform kernels use and what the padded kernels' tables must reproduce bit for bit:
+    """og_sinkhorn_consts is what the Sinkhorn uses for a uniform batch and what a padded batch's tables must reproduce bit for bit:
     norm = -log(n + m) in float32 (the host's logf), log_a_last = norm + log(m), log_b_last = norm + log(n)."""
     lib = _cabi.lib()
     libm = C.CDLL(ctypes.util.find_library('m'))

@@ -2,9 +2,10 @@
 
     python tools/sinkhorn_timing.py [--launches 20] [--rounds 3] [--out DIR] [--against OTHER_LIB]
 
-For each shape (the BASELINE workloads' Sinkhorn, and one pair at the headline size) it prints the plan of each form, the median
-over `rounds` rounds of the mean CUDA-event time of `launches` back-to-back launches, the largest score difference between the
-two forms and whether two resident launches gave identical bits.  --against measures the same shapes in a second process on
+For each shape (the BASELINE workloads' Sinkhorn, one pair at the headline size, and two pairs of 2048 x 4096 for the band
+2048 < m <= 4096, which only the streaming kernel runs) it prints the plan of each form, the median over `rounds` rounds of the
+mean CUDA-event time of `launches` back-to-back launches, the largest score difference between the two forms and whether two
+resident launches gave identical bits.  --against measures the same shapes in a second process on
 another build of the library (OG_LIB, such as a parent commit's) and prints both builds' times and whether their streaming
 outputs are bit-identical.  Needs a CUDA device."""
 from __future__ import annotations
@@ -26,7 +27,7 @@ from openglue_b200._cabi import ptr, stream  # noqa: E402
 
 # (label, pairs, n, m, iterations)
 SHAPES = [('C3', 16, 2048, 2048, 100), ('C2', 32, 1024, 1024, 100), ('C5', 1, 4096, 1024, 50), ('C1', 1, 512, 512, 20),
-          ('1 pair 2048', 1, 2048, 2048, 100)]
+          ('1 pair 2048', 1, 2048, 2048, 100), ('2048x4096', 2, 2048, 4096, 100)]
 
 
 def plan(lib, B, n, m):
