@@ -716,11 +716,10 @@ int og_sp_select(const int* cand_idx, const float* cand_score, const int* count,
                  int out_cap, int max_count, float* kpts, float* scores, void* stream) {
   OG_CHECK_ARG(cand_idx && cand_score && count && n_out && mode && kpts && scores, "sp_select: null pointer");
   OG_CHECK_ARG(B > 0 && cap > 0 && W > 0 && out_cap > 0 && max_count >= 0, "sp_select: bad sizes");
-  if (max_count > SP_MAX_CAND) return fail(OG_EUNSUPPORTED, "sp_select: %d candidates in one image exceed the sort capacity %d", max_count, SP_MAX_CAND);
-  int n2 = 1;
-  while (n2 < max_count) n2 <<= 1;
-  const int smem = 2 * n2 * 4;
-  if (const int rc = smem_opt_in<sp_select_kernel>(2 * SP_MAX_CAND * 4)) return rc;
+  size_t smem;
+  if (const int rc = cta_topk_smem<sp_select_kernel>(max_count, "sp_select: %d candidates in one image exceed the sort capacity %d",
+                                                     &smem))
+    return rc;
   return OG_LAUNCH(sp_select_kernel, B, 1024, smem, (cudaStream_t)stream, cand_idx, cand_score, count, n_out, mode, cap, W, out_cap, kpts,
                    scores);
 }
@@ -819,9 +818,7 @@ int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, v
 }
 int64_t og_sift_select_workspace_bytes(int B, int cap) {
   if (B <= 0 || B > 65535 || cap <= 0 || cap > (1 << 24)) return fail(OG_EINVAL, "sift_select_workspace_bytes: bad sizes");
-  int n2 = 1;
-  while (n2 < cap) n2 <<= 1;
-  return (int64_t)B * 4 * n2 * 4;
+  return (int64_t)B * 4 * pow2_ceil(cap) * 4;
 }
 int og_sift_select(const float* kp, const int* count, int B, int cap, float nms_radius, int max_keypoints, void* work, int64_t work_bytes,
                    int* sel, int* n_sel, void* stream) {
@@ -830,9 +827,7 @@ int og_sift_select(const float* kp, const int* count, int B, int cap, float nms_
   if (need < 0) return (int)need;
   OG_CHECK_ARG(work_bytes >= need, "sift_select: workspace of %lld bytes, %lld needed", (long long)work_bytes, (long long)need);
   OG_CHECK_ARG(nms_radius == nms_radius, "sift_select: nms_radius is NaN");
-  int n2 = 1;
-  while (n2 < cap) n2 <<= 1;
-  return OG_LAUNCH(sift_select_kernel, B, 1024, 0, (cudaStream_t)stream, kp, count, cap, nms_radius, max_keypoints, n2,
+  return OG_LAUNCH(sift_select_kernel, B, 1024, 0, (cudaStream_t)stream, kp, count, cap, nms_radius, max_keypoints, pow2_ceil(cap),
                    static_cast<int*>(work), sel, n_sel);
 }
 int og_sift_describe(const void* ws, int B, int H, int W, int cap, const float* kp, const int* octave, const int* sel, const int* n_sel,

@@ -11,7 +11,6 @@
 // rest is a gather: HBM-bound, ~(6 + 1 + D) floats in and out per kept keypoint.  Index work: bit-exact.
 #pragma once
 #include "common.cuh"
-#include <math_constants.h>
 
 namespace og {
 
@@ -32,7 +31,6 @@ struct CollateArgs {
 };
 
 constexpr int COLLATE_THREADS = 256;
-constexpr int COLLATE_MAX_KPTS = 16384;
 
 __global__ void __launch_bounds__(COLLATE_THREADS) collate_kernel(CollateArgs a) {
   extern __shared__ __align__(16) unsigned char og_collate_smem[];
@@ -43,31 +41,7 @@ __global__ void __launch_bounds__(COLLATE_THREADS) collate_kernel(CollateArgs a)
   const int first = a.offsets[i], cnt = a.offsets[i + 1] - first;
   const int K = a.K, D = a.D;
   const int keep = min(cnt, K);
-  const bool topk = cnt > K && a.select == nullptr;
-  if (topk) {
-    int n2 = 1;
-    while (n2 < cnt) n2 <<= 1;
-    for (int j = threadIdx.x; j < n2; j += COLLATE_THREADS) {
-      key[j] = (j < cnt) ? a.scores[first + j] : -CUDART_INF_F;
-      val[j] = (j < cnt) ? j : 0x7fffffff;
-    }
-    __syncthreads();
-    // bitonic sort, descending by score, ascending by index among equal scores
-    for (int size = 2; size <= n2; size <<= 1) {
-      for (int stride = size >> 1; stride > 0; stride >>= 1) {
-        for (int t = threadIdx.x; t < (n2 >> 1); t += COLLATE_THREADS) {
-          const int lo = 2 * t - (t & (stride - 1));
-          const int hi = lo + stride;
-          const bool desc_dir = ((lo & size) == 0);
-          const float k0 = key[lo], k1 = key[hi];
-          const int v0 = val[lo], v1 = val[hi];
-          const bool first_before = (k0 > k1) || (k0 == k1 && v0 < v1);     // lo already ahead of hi in descending order
-          if (first_before != desc_dir) { key[lo] = k1; key[hi] = k0; val[lo] = v1; val[hi] = v0; }
-        }
-        __syncthreads();
-      }
-    }
-  }
+  if (cnt > K && a.select == nullptr) cta_topk_sort<COLLATE_THREADS>(a.scores + first, cnt, key, val);
   float* o_lafs = (img ? a.out_lafs1 : a.out_lafs0) + (int64_t)b * K * 6;
   float* o_sc = (img ? a.out_scores1 : a.out_scores0) + (int64_t)b * K;
   float* o_desc = (img ? a.out_desc1 : a.out_desc0) + (int64_t)b * K * D;
@@ -110,12 +84,9 @@ __global__ void __launch_bounds__(COLLATE_THREADS) collate_kernel(CollateArgs a)
 }
 
 inline int collate_launch(CollateArgs a, int max_count, cudaStream_t stream) {
-  if (max_count > COLLATE_MAX_KPTS) return fail(OG_EUNSUPPORTED, "collate: %d keypoints in one image > %d", max_count, COLLATE_MAX_KPTS);
-  int n2 = 1;
-  while (n2 < max_count) n2 <<= 1;
-  a.sort_n = n2;
-  const size_t smem = (size_t)n2 * 8;
-  if (const int rc = smem_opt_in<collate_kernel>(COLLATE_MAX_KPTS * 8)) return rc;
+  size_t smem;
+  if (const int rc = cta_topk_smem<collate_kernel>(max_count, "collate: %d keypoints in one image > %d", &smem)) return rc;
+  a.sort_n = pow2_ceil(max_count);
   return OG_LAUNCH(collate_kernel, dim3(a.B, 2), COLLATE_THREADS, smem, stream, a);
 }
 

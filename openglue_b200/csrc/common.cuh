@@ -1,6 +1,8 @@
 // Shared helpers for the openglue_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
+#include <math_constants.h>
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
@@ -117,10 +119,93 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-__device__ __forceinline__ float warp_sum(float v) {
+template <class T>
+__device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+// Sum of v over a CTA of THREADS threads in a fixed order: a warp butterfly, then thread 0 adds the warp totals in warp order.
+// Valid in thread 0.  red: shared, THREADS / 32 slots; the __syncthreads() before it is written lets consecutive calls reuse it.
+template <int THREADS, class T>
+__device__ __forceinline__ T cta_sum(T v, T* red) {
+  v = warp_sum(v);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  T t = 0;
+  if (threadIdx.x == 0) for (int w = 0; w < THREADS / 32; ++w) t += red[w];
+  return t;
+}
+
+// The last CTA of a grid finishes a reduction: every CTA stores its partial, then its thread 0 calls last_cta_arrive(), which
+// fences that store device-wide before it arrives on `counter` and returns whether every other CTA has already arrived.  The
+// last CTA fences again before any of its threads reads the partials; last_cta_sum() does both for one thread.  `counter`
+// starts at 0; resetting it for the next launch is the caller's.
+__device__ __forceinline__ bool last_cta_arrive(unsigned int* counter) {
+  __threadfence();
+  return atomicAdd(counter, 1u) == gridDim.x - 1;
+}
+// partial[0 .. n) summed in index order (deterministic), by one thread of the last CTA
+template <class T>
+__device__ __forceinline__ T last_cta_sum(const T* partial, int n) {
+  __threadfence();
+  T t = 0;
+  for (int p = 0; p < n; ++p) t += __ldcg(partial + p);
+  return t;
+}
+
+// The smallest power of two >= x (1 for x <= 1): the length of a bitonic sort of x keys
+__host__ __device__ __forceinline__ int pow2_ceil(int x) {
+  int n = 1;
+  while (n < x) n <<= 1;
+  return n;
+}
+// CTA-wide bitonic sort of positions [0, n2), n2 a power of two, into the order of before(lo, hi): "the element at position lo
+// goes first".  swap(lo, hi) exchanges two positions.  Every thread of the CTA calls it; one __syncthreads() per stride.
+// THREADS: the CTA's size where every launch uses that constant (the compiler then unrolls the loop), or 0: blockDim.x.
+template <int THREADS = 0, class Before, class Swap>
+__device__ __forceinline__ void cta_bitonic_sort(int n2, Before before, Swap swap) {
+  for (int size = 2; size <= n2; size <<= 1)
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = threadIdx.x; t < (n2 >> 1); t += THREADS ? THREADS : blockDim.x) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        if (before(lo, hi) != ((lo & size) == 0)) swap(lo, hi);
+      }
+      __syncthreads();
+    }
+}
+// Top-k order (torch.topk, the reference's nms_keypoints): the higher score first, on equal scores the lower index
+__device__ __forceinline__ bool topk_before(float a, int ia, float b, int ib) { return a > b || (a == b && ia < ib); }
+
+// Shared-memory top-k sort of scores[0 .. cnt): key / val [pow2_ceil(cnt)] receive the scores and their indices in top-k order,
+// padded with (-inf, INT_MAX).  Every thread of the CTA calls it; THREADS as for cta_bitonic_sort.  CTA_TOPK_MAX keys at most
+// (cta_topk_smem).
+constexpr int CTA_TOPK_MAX = 16384;
+template <int THREADS>
+__device__ __forceinline__ void cta_topk_sort(const float* scores, int cnt, float* key, int* val) {
+  const int n2 = pow2_ceil(cnt);
+  for (int j = threadIdx.x; j < n2; j += THREADS ? THREADS : blockDim.x) {
+    key[j] = j < cnt ? scores[j] : -CUDART_INF_F;
+    val[j] = j < cnt ? j : INT_MAX;
+  }
+  __syncthreads();
+  cta_bitonic_sort<THREADS>(n2, [&](int lo, int hi) { return topk_before(key[lo], val[lo], key[hi], val[hi]); },
+                   [&](int lo, int hi) {
+                     const float k0 = key[lo], k1 = key[hi];
+                     const int v0 = val[lo], v1 = val[hi];
+                     key[lo] = k1; key[hi] = k0; val[lo] = v1; val[hi] = v0;
+                   });
+}
+// Host side of cta_topk_sort for Kernel: refuses more than CTA_TOPK_MAX keys (the error message is too_many % (max_count,
+// CTA_TOPK_MAX)), opts Kernel in to the capacity's shared memory and sets *bytes to what a sort of max_count keys needs (key and
+// val back to back).
+template <auto Kernel>
+inline int cta_topk_smem(int max_count, const char* too_many, size_t* bytes) {
+  if (max_count > CTA_TOPK_MAX) return fail(OG_EUNSUPPORTED, too_many, max_count, CTA_TOPK_MAX);
+  *bytes = (size_t)pow2_ceil(max_count) * 8;
+  return smem_opt_in<Kernel>(CTA_TOPK_MAX * 8);
 }
 // One step of an ordered (stable) compaction by one CTA: every thread holds one element of a chunk, in thread order, flagged by
 // `on`.  Returns the element's output slot (meaningful where `on`): `base` + the number of flagged elements before it in the

@@ -29,17 +29,6 @@ struct CritArgs {
   float grad_scale;             // upstream gradient of 'loss' (nll_weight)
 };
 
-__device__ __forceinline__ float block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-  if (threadIdx.x == 0) for (int w = 0; w < CRIT_THREADS / 32; ++w) t += red[w];   // fixed order
-  return t;                                                                         // valid in thread 0
-}
-
 __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
   __shared__ float red[CRIT_THREADS / 32];
   __shared__ float s_cnt[3];
@@ -57,8 +46,8 @@ __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
   }
   for (int j = threadIdx.x; j < m; j += CRIT_THREADS)
     if (g1[j] == -1) { su1 += S[(int64_t)n * (m + 1) + j]; cu1 += 1.f; }
-  const float tm = block_sum(sm, red), tu0 = block_sum(su0, red), tu1 = block_sum(su1, red);
-  const float nm = block_sum(cm, red), nu0 = block_sum(cu0, red), nu1 = block_sum(cu1, red);
+  const float tm = cta_sum<CRIT_THREADS>(sm, red), tu0 = cta_sum<CRIT_THREADS>(su0, red), tu1 = cta_sum<CRIT_THREADS>(su1, red);
+  const float nm = cta_sum<CRIT_THREADS>(cm, red), nu0 = cta_sum<CRIT_THREADS>(cu0, red), nu1 = cta_sum<CRIT_THREADS>(cu1, red);
   if (threadIdx.x == 0) {
     float l = 0.f;
     if (nm > 0.f) l -= tm / nm;
@@ -66,8 +55,7 @@ __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
     if (nu1 > 0.f) l -= 0.5f * tu1 / nu1;
     a.per_pair[b] = l;
     s_cnt[0] = nm; s_cnt[1] = nu0; s_cnt[2] = nu1;
-    __threadfence();
-    last = atomicAdd(a.counter, 1u) == (unsigned int)(gridDim.x - 1);
+    last = last_cta_arrive(a.counter);
   }
   __syncthreads();
   if (a.dscores) {                                          // d loss / d scores: the same gather, scattered
@@ -84,10 +72,7 @@ __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
       if (g1[j] == -1) D[(int64_t)n * (m + 1) + j] = w1;
   }
   if (last && threadIdx.x == 0) {
-    __threadfence();
-    float t = 0.f;
-    for (int p = 0; p < a.B; ++p) t += __ldcg(a.per_pair + p);     // pair order: deterministic
-    a.loss[0] = t / (float)a.B;
+    a.loss[0] = last_cta_sum(a.per_pair, a.B) / (float)a.B;       // pair order: deterministic
     a.loss[1] = 0.f;                                               // metric_loss with margin = None (utils/losses.py:56-58, 83-85)
   }
 }

@@ -158,17 +158,6 @@ __global__ void __launch_bounds__(256) metric_cols_merge_kernel(MetricArgs a) {
   a.n1[t] = im; a.u1[t] = iu; a.dn1[t] = bm; a.du1[t] = bu;
 }
 
-__device__ __forceinline__ float metric_block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-  if (threadIdx.x == 0) for (int w = 0; w < METRIC_THREADS / 32; ++w) t += red[w];   // fixed order
-  return t;                                                                           // valid in thread 0
-}
-
 // the hinge arguments, one expression each (the loss and its gradient read the same values)
 __device__ __forceinline__ float pos_arg(float dpos, float dneg, float mu) { return __fadd_rn(__fsub_rn(dpos, dneg), mu); }
 __device__ __forceinline__ float neg_arg(float dneg, float mu) { return __fsub_rn(mu, dneg); }
@@ -201,9 +190,9 @@ __global__ void __launch_bounds__(METRIC_THREADS) metric_loss_kernel(MetricArgs 
   }
   for (int j = threadIdx.x; j < m; j += METRIC_THREADS)
     if (g1[j] == -1) { su1 += hinge(neg_arg(a.du1[co + j], mu)); cu1 += 1.f; }
-  const float t0 = metric_block_sum(s0, red), t1 = metric_block_sum(s1, red);
-  const float tu0 = metric_block_sum(su0, red), tu1 = metric_block_sum(su1, red);
-  const float nm = metric_block_sum(cm, red), nu0 = metric_block_sum(cu0, red), nu1 = metric_block_sum(cu1, red);
+  const float t0 = cta_sum<METRIC_THREADS>(s0, red), t1 = cta_sum<METRIC_THREADS>(s1, red);
+  const float tu0 = cta_sum<METRIC_THREADS>(su0, red), tu1 = cta_sum<METRIC_THREADS>(su1, red);
+  const float nm = cta_sum<METRIC_THREADS>(cm, red), nu0 = cta_sum<METRIC_THREADS>(cu0, red), nu1 = cta_sum<METRIC_THREADS>(cu1, red);
   if (threadIdx.x == 0) {
     float l = 0.f;
     if (nm > 0.f) l += (t0 + t1) / nm;
@@ -214,8 +203,7 @@ __global__ void __launch_bounds__(METRIC_THREADS) metric_loss_kernel(MetricArgs 
     s_w[0] = nm > 0.f ? gB / nm : 0.f;
     s_w[1] = nu0 > 0.f ? gB / nu0 : 0.f;
     s_w[2] = nu1 > 0.f ? gB / nu1 : 0.f;
-    __threadfence();
-    last = atomicAdd(a.counter, 1u) == (unsigned int)(gridDim.x - 1);
+    last = last_cta_arrive(a.counter);
   }
   __syncthreads();
   if (a.want_grad) {
@@ -243,12 +231,7 @@ __global__ void __launch_bounds__(METRIC_THREADS) metric_loss_kernel(MetricArgs 
       a.u1c[co + j] = g1[j] == -1 ? -w1 * hinge_grad(neg_arg(a.du1[co + j], mu)) : 0.f;
     }
   }
-  if (last && threadIdx.x == 0) {
-    __threadfence();
-    float t = 0.f;
-    for (int p = 0; p < a.B; ++p) t += __ldcg(a.per_pair + p);     // pair order: deterministic
-    a.loss[0] = t / (float)a.B;
-  }
+  if (last && threadIdx.x == 0) a.loss[0] = last_cta_sum(a.per_pair, a.B) / (float)a.B;     // pair order: deterministic
 }
 
 // D = d loss / d dist (TRANS = 0: [B, n, ldo] rows i) or D^T (TRANS = 1: [B, m, ldo] rows j), one warp per output row, pad

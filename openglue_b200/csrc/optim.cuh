@@ -56,18 +56,6 @@ __device__ __forceinline__ float clip_coefficient(float norm, double max_norm) {
   return isnan(c) ? c : fminf(c, 1.f);
 }
 
-__device__ __forceinline__ double block_sum_f64(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x == 0) for (int w = 0; w < OPT_THREADS / 32; ++w) t += red[w];   // fixed order
-  return t;                                                                         // valid in thread 0
-}
-
 __global__ void __launch_bounds__(OPT_THREADS) optim_norm_kernel(const og_optim_segment* __restrict__ segs, int nseg, int64_t ntiles,
                                                                  OptHyper h, og_optim_state* state, double* partial, float2* scal) {
   tc::launch_dependents();                                    // the update kernel's CTAs may become resident; they wait for us
@@ -97,18 +85,17 @@ __global__ void __launch_bounds__(OPT_THREADS) optim_norm_kernel(const og_optim_
       }
     }
   }
-  const double tot = block_sum_f64(acc, red);
+  const double tot = cta_sum<OPT_THREADS>(acc, red);
   if (threadIdx.x == 0) {
     partial[blockIdx.x] = tot;
-    __threadfence();
-    last = atomicAdd(&state->counter, 1u) == (unsigned)(OPT_NORM_CTAS - 1);
+    last = last_cta_arrive(&state->counter);
   }
   __syncthreads();
   if (!last) return;
   __threadfence();
   double p = 0.0;
   for (int c = threadIdx.x; c < OPT_NORM_CTAS; c += OPT_THREADS) p += __ldcg(partial + c);
-  const double sumsq = block_sum_f64(p, red);
+  const double sumsq = cta_sum<OPT_THREADS>(p, red);
   if (threadIdx.x == 0) {
     const float norm = (float)sqrt(sumsq);
     state->grad_norm = norm;

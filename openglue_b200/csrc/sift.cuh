@@ -383,23 +383,15 @@ __global__ void __launch_bounds__(256) sift_orientation_kernel(SiftPyramid pyr, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// CTA-wide bitonic sort of idx[0 .. n2) (n2 a power of two, entries >= n are padding that sorts last) by before(a, b) in global
+// CTA-wide sort of the indices idx[0 .. pow2_ceil(n)) (entries >= n are padding that sorts last) by before(a, b), in global
 // memory; every thread of the CTA calls it.
 template <class Before>
-__device__ void sift_cta_sort(int* idx, int n, int n2, Before before) {
+__device__ void sift_cta_sort(int* idx, int n, Before before) {
+  const int n2 = pow2_ceil(n);
   for (int t = threadIdx.x; t < n2; t += blockDim.x) idx[t] = t;
   __syncthreads();
-  for (int size = 2; size <= n2; size <<= 1)
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = threadIdx.x; t < (n2 >> 1); t += blockDim.x) {
-        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-        const int a = idx[lo], c = idx[hi];
-        const bool a_first = c >= n || (a < n && before(a, c));
-        const bool asc = (lo & size) == 0;
-        if (a_first != asc) { idx[lo] = c; idx[hi] = a; }
-      }
-      __syncthreads();
-    }
+  cta_bitonic_sort(n2, [&](int lo, int hi) { const int a = idx[lo], c = idx[hi]; return c >= n || (a < n && before(a, c)); },
+                   [&](int lo, int hi) { const int a = idx[lo], c = idx[hi]; idx[lo] = c; idx[hi] = a; });
 }
 
 // cv2's KeyPoint12_LessThan
@@ -422,12 +414,10 @@ __global__ void __launch_bounds__(1024) sift_sort_unique_kernel(const float* __r
   __shared__ int base;
   const int b = blockIdx.x;
   const int raw = kp_count[b], n = min(raw, cap);
-  int n2 = 1;
-  while (n2 < n) n2 <<= 1;
   int* idx = work + (int64_t)b * n2max;
   const float* kb = kp + (int64_t)b * cap * 5;
   const int* ob = kp_oct + (int64_t)b * cap;
-  sift_cta_sort(idx, n, n2, [&](int p, int q) { return sift_cv_before(sift_load_kp(kb, ob, p), sift_load_kp(kb, ob, q)); });
+  sift_cta_sort(idx, n, [&](int p, int q) { return sift_cv_before(sift_load_kp(kb, ob, p), sift_load_kp(kb, ob, q)); });
   if (threadIdx.x == 0) base = 0;
   __syncthreads();
   for (int j0 = 0; j0 < n; j0 += 1024) {
@@ -460,8 +450,6 @@ __global__ void __launch_bounds__(1024) sift_select_kernel(const float* __restri
   __shared__ int base, changed;
   const int b = blockIdx.x;
   const int n = max(0, min(count[b], cap));
-  int n2 = 1;
-  while (n2 < n) n2 <<= 1;
   int* ord = work + (int64_t)b * 4 * n2max;
   int* xo = ord + n2max;
   int* rank = xo + n2max;
@@ -470,11 +458,11 @@ __global__ void __launch_bounds__(1024) sift_select_kernel(const float* __restri
   auto X = [&](int i) { return kb[(int64_t)i * 5 + 0]; };
   auto Y = [&](int i) { return kb[(int64_t)i * 5 + 1]; };
   auto S = [&](int i) { return kb[(int64_t)i * 5 + 4]; };
-  sift_cta_sort(ord, n, n2, [&](int p, int q) { const float sp = S(p), sq = S(q); return sp > sq || (sp == sq && p < q); });
+  sift_cta_sort(ord, n, [&](int p, int q) { return topk_before(S(p), p, S(q), q); });
   for (int j = threadIdx.x; j < n; j += blockDim.x) { rank[ord[j]] = j; state[j] = radius > 0.f ? 0 : 1; }
   __syncthreads();
   if (radius > 0.f) {
-    sift_cta_sort(xo, n, n2, [&](int p, int q) { const float xp = X(p), xq = X(q); return xp < xq || (xp == xq && p < q); });
+    sift_cta_sort(xo, n, [&](int p, int q) { const float xp = X(p), xq = X(q); return xp < xq || (xp == xq && p < q); });
     const double r = (double)radius, r2 = r * r;
     volatile int* vstate = state;
     for (;;) {
@@ -756,10 +744,8 @@ inline bool sift_layout(int B, int H, int W, int cap, SiftLayout& L) {
   L.kp_off = off; off += align_up((int64_t)B * cap * 5 * 4, 256);
   L.oct_off = off; off += align_up((int64_t)B * cap * 4, 256);
   L.cnt_off = off; off += align_up((int64_t)2 * B * 4, 256);
-  int n2 = 1;
-  while (n2 < cap) n2 <<= 1;
-  L.n2max = n2;
-  L.work_off = off; off += align_up((int64_t)B * 4 * n2 * 4, 256);
+  L.n2max = pow2_ceil(cap);
+  L.work_off = off; off += align_up((int64_t)B * 4 * L.n2max * 4, 256);
   L.total = off;
   return true;
 }

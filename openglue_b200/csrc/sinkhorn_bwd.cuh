@@ -234,27 +234,15 @@ __global__ void __launch_bounds__(256) sinkb_dz_kernel(SinkBwdArgs a, const floa
 __global__ void __launch_bounds__(256) sinkb_dustbin_kernel(const float* __restrict__ dZ, int B, int n, int m, float* __restrict__ per_pair,
                                                             unsigned int* counter, float* __restrict__ out) {
   __shared__ float red[8];
-  __shared__ bool last;
   const int b = blockIdx.x;
   const float* d = dZ + (int64_t)b * (n + 1) * (m + 1);
   float s = 0.f;
   for (int j = threadIdx.x; j <= m; j += 256) s += d[(int64_t)n * (m + 1) + j];
   for (int i = threadIdx.x; i < n; i += 256) s += d[(int64_t)i * (m + 1) + m];
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
+  const float t = cta_sum<256>(s, red);
   if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int w = 0; w < 8; ++w) t += red[w];
     per_pair[b] = t;
-    __threadfence();
-    last = atomicAdd(counter, 1u) == (unsigned int)(gridDim.x - 1);
-    if (last) {
-      __threadfence();
-      float tt = 0.f;
-      for (int p = 0; p < B; ++p) tt += __ldcg(per_pair + p);
-      *out = tt;
-    }
+    if (last_cta_arrive(counter)) *out = last_cta_sum(per_pair, B);
   }
 }
 

@@ -14,7 +14,6 @@
 //   keep x[p] iff x[p] > max(0, x[q] for the k*k - 1 other offsets q of the window, coordinates clamped to the image (replicate padding)).
 #pragma once
 #include "common.cuh"
-#include <math_constants.h>
 #include <algorithm>
 
 namespace og {
@@ -126,10 +125,9 @@ __global__ void __launch_bounds__(1024) sp_compact_kernel(const float* __restric
 
 // selection of n_out[b] keypoints of image b from its candidate list: mode[b] = 0 keep the (row-major) order, 1 = the n_out largest
 // scores in descending order (torch.topk; equal scores: lower index first).  Outputs keypoints as (x, y) floats (model.py:108),
-// scores, both [B, out_cap, ...].  One CTA per image; the sort is a bitonic sort of (score, position) in shared memory.
+// scores, both [B, out_cap, ...].  One CTA per image; the sort is cta_topk_sort's, of (score, position) in shared memory.
 // Caller contract (not checked on the device): n_out[b] <= min(count[b], cap) and n_out[b] <= out_cap, and max_count >= every count[b]
 // (it sizes the shared memory); a larger n_out reads candidate slots that were never written.
-constexpr int SP_MAX_CAND = 16384;
 __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__ cand_idx, const float* __restrict__ cand_score,
                                                          const int* __restrict__ count, const int* __restrict__ n_out, const int* __restrict__ mode,
                                                          int cap, int W, int out_cap, float* __restrict__ kpts, float* __restrict__ scores) {
@@ -139,26 +137,10 @@ __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__
   const int cnt = min(count[b], cap), n = n_out[b];
   const int* ci = cand_idx + (int64_t)b * cap;
   const float* cs = cand_score + (int64_t)b * cap;
-  int n2 = 1;
-  while (n2 < cnt) n2 <<= 1;
-  int* val = reinterpret_cast<int*>(key + n2);
-  if (mode[b]) {
-    for (int j = tid; j < n2; j += 1024) { key[j] = j < cnt ? cs[j] : -CUDART_INF_F; val[j] = j < cnt ? j : 0x7fffffff; }
-    __syncthreads();
-    for (int size = 2; size <= n2; size <<= 1) {
-      for (int stride = size >> 1; stride > 0; stride >>= 1) {
-        for (int t = tid; t < (n2 >> 1); t += 1024) {
-          const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-          const bool desc = (lo & size) == 0;
-          const float ka = key[lo], kb = key[hi];
-          const int va = val[lo], vb = val[hi];
-          const bool a_first = ka > kb || (ka == kb && va < vb);        // a before b in descending-score / ascending-position order
-          if (a_first != desc) { key[lo] = kb; key[hi] = ka; val[lo] = vb; val[hi] = va; }
-        }
-        __syncthreads();
-      }
-    }
-  }
+  int* val = reinterpret_cast<int*>(key + pow2_ceil(cnt));
+  // <0>: the sort strides by blockDim.x.  Here that runs faster than the loop unrolled for the constant 1024 (collate is the
+  // other way round), so the choice is deliberate.
+  if (mode[b]) cta_topk_sort<0>(cs, cnt, key, val);
   for (int j = tid; j < n; j += 1024) {
     const int src = mode[b] ? val[j] : j;
     const int p = ci[src];

@@ -28,7 +28,7 @@ DEV = 'cuda:0'
 U = 2.0 ** -24                  # unit roundoff of float32
 GUARD = 1024                    # poisoned elements after every output buffer
 INT_POISON = -0x5a5a5a5a
-SP_MAX_CAND = 16384             # csrc/superpoint.cuh: the sort capacity of og_sp_select
+SP_MAX_CAND = 16384             # csrc/common.cuh (CTA_TOPK_MAX): the sort capacity of og_sp_select
 OG_EUNSUPPORTED = -2
 
 
