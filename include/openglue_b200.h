@@ -320,6 +320,17 @@ int og_sinkhorn_bwd(const float* S, int64_t lds, int64_t strideS, const float* d
                     int batch, int n, int m, int iters, float reg, const float* hist,
                     const float* dscores, float* dS_aug, float* ddustbin,
                     void* workspace, int64_t workspace_bytes, void* stream);
+/* Padded forms (lengths as og_sinkhorn_fwd_padded; same hist size and workspace): pair b runs on its [n_b, m_b] block with its own
+ * marginals; hist keeps the capacity's strides (pair b's dustbin entries at n_b / m_b).  The backward pass reads dscores on each
+ * pair's [n_b + 1, m_b + 1] block only, writes dS_aug there and 0 on the rest of the capacity, and ddustbin sums each pair's own
+ * dustbin row and column.  Both need the tables og_sinkhorn_fwd_padded uploads (one padded call before a stream capture). */
+int og_sinkhorn_train_fwd_padded(const float* S, int64_t lds, int64_t strideS, const float* dustbin,
+                                 int batch, int n, int m, const int* lengths, int iters, float reg, float* scores, float* hist,
+                                 void* workspace, int64_t workspace_bytes, void* stream);
+int og_sinkhorn_bwd_padded(const float* S, int64_t lds, int64_t strideS, const float* dustbin,
+                           int batch, int n, int m, const int* lengths, int iters, float reg, const float* hist,
+                           const float* dscores, float* dS_aug, float* ddustbin,
+                           void* workspace, int64_t workspace_bytes, void* stream);
 
 /* Mutual-argmax match extraction on scores[:, :n, :m].  Replaces
  * models/matching_module.py:174-187 and inference.py:176-190 (ties -> lowest index).
@@ -359,6 +370,11 @@ int64_t og_gt_matches_workspace_bytes(int batch, int n, int m);
  * (index of the match, -1 unmatched, -2 ignore).  All pointers are device memory.                  */
 int og_gt_matches_fwd(const float* kpts0, const float* kpts1, int batch, int n, int m, const og_gt_transform* tf,
                       int64_t* gt_matches0, int64_t* gt_matches1, void* workspace, int64_t workspace_bytes, void* stream);
+/* Padded form (lengths as og_sinkhorn_fwd_padded): pair b's nearest neighbours and mutual check run over its first n_b / m_b
+ * keypoints; its labels past them are -2 (ignore).  Per-keypoint depths keep the capacity's layout [B,n] / [B,m].            */
+int og_gt_matches_fwd_padded(const float* kpts0, const float* kpts1, int batch, int n, int m, const int* lengths,
+                             const og_gt_transform* tf, int64_t* gt_matches0, int64_t* gt_matches1, void* workspace,
+                             int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Batch collation of cached local features: the step that FEEDS the path from the cached-feature dataset.  Replaces
@@ -385,6 +401,11 @@ int og_collate_fwd(const float* lafs, const float* scores, const float* desc, co
 int64_t og_criterion_workspace_bytes(int batch);
 int og_criterion_fwd(const float* scores, const int64_t* gt_matches0, const int64_t* gt_matches1, int batch, int n, int m,
                      float* loss, float* dscores, float grad_scale, void* workspace, int64_t workspace_bytes, void* stream);
+/* Padded form (lengths as og_sinkhorn_fwd_padded): pair b's loss reads its [n_b + 1, m_b + 1] block of scores (dustbins at n_b,
+ * m_b) and its first n_b / m_b labels; loss[0] is the mean of the B pairs' losses.  dscores outside each block stays 0.        */
+int og_criterion_fwd_padded(const float* scores, const int64_t* gt_matches0, const int64_t* gt_matches1, int batch, int n, int m,
+                            const int* lengths, float* loss, float* dscores, float grad_scale, void* workspace,
+                            int64_t workspace_bytes, void* stream);
 
 /* Metric terms of the same loss for a margin mu: criterion(..., margin=mu)['metric_loss'] (utils/losses.py:56-99 on the
  * half cosine distance of utils/misc.py:106-113, dist = 0.25 |normalize(c0_i) - normalize(c1_j)|^2).
@@ -450,6 +471,27 @@ int og_mix_bwd(const float* dm, const float* mix, float* dg, float* dl, int64_t 
 int og_mix_param_grad(const float* colsum, const float* mix, float* dmix, int d, void* stream);
 int og_kenc_input(const float* kpts, const float* side, int rows, int side_info_size, float width, float height,
                   float* out, void* stream);
+/* Padded forms of the training-step operators.  Rows are [batch, cap]: row r is slot r % cap of pair r / cap, real below
+ * lengths[r / cap] (device int32 [batch], clamped into [1, cap]).
+ *   og_bn_train_fwd_padded / _bwd_padded  batch statistics over the real rows of every pair: mean and biased variance over
+ *                       sum_b n_b rows, running_var with the unbiased factor sum n / (sum n - 1); dgamma / dbeta over the real
+ *                       rows; da = 0 on the padding rows.  Padding rows of y are finite when a is.
+ *   og_softmax_rows_padded / og_softmax_bwd_rows_padded   rows [batch, seq_rows]: sequence b's rows take its first
+ *                       key_lengths[b] columns of `cols`; P = 0 (dS = 0) on the others
+ *   og_kenc_input_padded   og_kenc_input with each pair's (W, H) from pair_wh (rows 4 floats apart) and the padding rows 0
+ *   og_mask_padded_rows    dst = src [batch * cap, cols] with the padding rows 0 (dst may not alias src)                  */
+int og_bn_train_fwd_padded(const float* a, int64_t lda, int batch, int cap, const int* lengths, int cols, int relu, const float* gamma,
+                           const float* beta, float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
+                           float* running_mean, float* running_var, float* workspace, void* stream);
+int og_bn_train_bwd_padded(const float* dy, int64_t lddy, const float* a, int64_t lda, int batch, int cap, const int* lengths, int cols,
+                           int relu, const float* gamma, const float* save_mean, const float* save_invstd,
+                           float* da, int64_t ldda, float* dgamma, float* dbeta, float* workspace, void* stream);
+int og_softmax_rows_padded(float* S, int64_t ld, int batch, int64_t seq_rows, int cols, const int* key_lengths, void* stream);
+int og_softmax_bwd_rows_padded(const float* P, float* dP, int64_t ld, int batch, int64_t seq_rows, int cols, float scale,
+                               const int* key_lengths, void* stream);
+int og_kenc_input_padded(const float* kpts, const float* side, int batch, int cap, const int* lengths, int side_info_size,
+                         const float* pair_wh, float* out, void* stream);
+int og_mask_padded_rows(const float* src, int batch, int cap, int cols, const int* lengths, float* dst, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * SuperPoint front-end operators (SURVEY.md section 8, row f4): SuperPointNet.forward (models/features/superpoint/model.py:61-129)

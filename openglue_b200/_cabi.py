@@ -96,6 +96,8 @@ SYMBOLS = {
     'og_sinkhorn_train_fwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _P, _L, _P]),
     'og_sinkhorn_bwd_workspace_bytes': (_L, [_I, _I, _I, _I]),
     'og_sinkhorn_bwd': (_I, [_P, _L, _L, _P, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P, _L, _P]),
+    'og_sinkhorn_train_fwd_padded': (_I, [_P, _L, _L, _P, _I, _I, _I, _P, _I, _F, _P, _P, _P, _L, _P]),
+    'og_sinkhorn_bwd_padded': (_I, [_P, _L, _L, _P, _I, _I, _I, _P, _I, _F, _P, _P, _P, _P, _P, _L, _P]),
     'og_match_workspace_bytes': (_L, [_I, _I, _I]),
     'og_match_fwd': (_I, [_P, _I, _I, _I, _F, _P, _P, _P, _P, _P, _L, _P]),
     'og_match_fwd_padded': (_I, [_P, _I, _I, _I, _P, _F, _P, _P, _P, _P, _P, _L, _P]),
@@ -103,9 +105,11 @@ SYMBOLS = {
     'og_collate_fwd': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'og_criterion_workspace_bytes': (_L, [_I]),
     'og_criterion_fwd': (_I, [_P, _P, _P, _I, _I, _I, _P, _P, _F, _P, _L, _P]),
+    'og_criterion_fwd_padded': (_I, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _F, _P, _L, _P]),
     'og_metric_loss_workspace_bytes': (_L, [_I, _I, _I, _I, _I, _I]),
     'og_metric_loss_fwd': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P, _P, _P, _P, _P, _P, _P, _F, _P, _L, _P]),
     'og_gt_matches_fwd': (_I, [_P, _P, _I, _I, _I, C.POINTER(OgGtTransform), _P, _P, _P, _L, _P]),
+    'og_gt_matches_fwd_padded': (_I, [_P, _P, _I, _I, _I, _P, C.POINTER(OgGtTransform), _P, _P, _P, _L, _P]),
     # training-step operators (row f1)
     'og_train_workspace_floats': (_L, [_I]),
     'og_linear_auto_scratch_floats': (_L, [C.POINTER(OgLinearArgs)]),
@@ -122,6 +126,12 @@ SYMBOLS = {
     'og_mix_bwd': (_I, [_P, _P, _P, _P, _L, _I, _P]),
     'og_mix_param_grad': (_I, [_P, _P, _P, _I, _P]),
     'og_kenc_input': (_I, [_P, _P, _I, _I, _F, _F, _P, _P]),
+    'og_bn_train_fwd_padded': (_I, [_P, _L, _I, _I, _P, _I, _I, _P, _P, _F, _F, _P, _L, _P, _P, _P, _P, _P, _P]),
+    'og_bn_train_bwd_padded': (_I, [_P, _L, _P, _L, _I, _I, _P, _I, _I, _P, _P, _P, _P, _L, _P, _P, _P, _P]),
+    'og_softmax_rows_padded': (_I, [_P, _L, _I, _L, _I, _P, _P]),
+    'og_softmax_bwd_rows_padded': (_I, [_P, _P, _L, _I, _L, _I, _F, _P, _P]),
+    'og_kenc_input_padded': (_I, [_P, _P, _I, _I, _P, _I, _P, _P, _P]),
+    'og_mask_padded_rows': (_I, [_P, _I, _I, _I, _P, _P, _P]),
     # SuperPoint front-end operators (row f4)
     'og_sp_im2col3x3': (_I, [_P, _I, _I, _I, _I, _P, _P]),
     'og_sp_maxpool2x2': (_I, [_P, _I, _I, _I, _I, _P, _P]),

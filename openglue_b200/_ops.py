@@ -17,7 +17,10 @@ def _pad4(n: int) -> int:
 
 
 class _Ops:
-    """ctypes wrappers of the training operators on the current stream of ``dev`` (fp32 CUDA tensors in, out)."""
+    """ctypes wrappers of the training operators on the current stream of ``dev`` (fp32 CUDA tensors in, out).
+
+    A padded batch passes per-pair lengths ``lens`` (device int32 [B]: the first ``lens[b]`` of pair b's ``cap`` rows are real;
+    for the Sinkhorn, the B row lengths then the B column lengths); without them every operator runs its uniform form."""
 
     def __init__(self, dev: torch.device, precision: int):
         self.dev, self.prec = dev, precision
@@ -95,14 +98,28 @@ class _Ops:
         _cabi.check(self.lib.og_transpose(ptr(X, x_off), ld_in, stride_in, ptr(out), ld_out, stride_out, batch, rows, cols, int(transpose), self.st()),
                     'og_transpose')
 
-    def kenc_input(self, kpts, side, rows, S, width, height):
+    def kenc_input(self, kpts, side, rows, S, width, height, lens=None, pair_wh=None):
+        """``pair_wh``: padded batch, (W, H) of pair b's image at pair_wh[b, :2] (rows 4 floats apart)"""
         out = self.empty(rows, 2 + S)
+        if lens is not None:
+            B = lens.numel()
+            _cabi.check(self.lib.og_kenc_input_padded(ptr(kpts), ptr(side) if S else None, B, rows // B, ptr(lens), S, ptr(pair_wh), ptr(out),
+                                                      self.st()), 'og_kenc_input_padded')
+            return out
         _cabi.check(self.lib.og_kenc_input(ptr(kpts), ptr(side) if S else None, rows, S, float(width), float(height), ptr(out), self.st()), 'og_kenc_input')
         return out
 
-    def attention(self, q, k, v, B, nq, nk, H, dh):
+    def mask_rows(self, X, lens):
+        """X [B * cap, cols] -> a copy with the rows past each pair's length zeroed"""
+        rows, cols = X.shape
+        B = lens.numel()
+        out = self.empty(rows, cols)
+        _cabi.check(self.lib.og_mask_padded_rows(ptr(X), B, rows // B, cols, ptr(lens), ptr(out), self.st()), 'og_mask_padded_rows')
+        return out
+
+    def attention(self, q, k, v, B, nq, nk, H, dh, klen=None):
         """fused softmax attention (forward): the wgmma 3xTF32 kernel for head_dim 32 / 64 (K and V^T as tf32 hi/lo operands),
-        the fp32 CUDA-core kernel otherwise / in fp32 mode"""
+        the fp32 CUDA-core kernel otherwise / in fp32 mode; ``klen``: sequence b attends to its first klen[b] keys"""
         d = H * dh
         o = self.empty(B * nq, d)
         if self.prec != _cabi.OG_PREC_FP32 and dh in (32, 64):
@@ -111,17 +128,35 @@ class _Ops:
             vt = self.transpose(v, batch=B, rows=nk, cols=d)            # [B, d, pad4(nk)], zero padded
             vthi, vtlo = torch.empty_like(vt), torch.empty_like(vt)
             _cabi.check(self.lib.og_split_tf32(ptr(vt), ptr(vthi), ptr(vtlo), vt.numel(), self.st()), 'og_split_tf32')
+            if klen is not None:
+                _cabi.check(self.lib.og_attention_tc_fwd_padded(ptr(q), d, nq * d, ptr(khi), ptr(klo), d, ptr(vthi), ptr(vtlo), vt.shape[2], ptr(o),
+                                                                d, nq * d, B, nq, nk, H, dh, ptr(klen), self.st()), 'og_attention_tc_fwd_padded')
+                return o
             _cabi.check(self.lib.og_attention_tc_fwd(ptr(q), d, nq * d, ptr(khi), ptr(klo), d, ptr(vthi), ptr(vtlo), vt.shape[2], ptr(o), d, nq * d,
                                                      B, nq, nk, H, dh, self.st()), 'og_attention_tc_fwd')
+            return o
+        if klen is not None:
+            _cabi.check(self.lib.og_attention_fwd_padded(ptr(q), d, nq * d, ptr(k), d, nk * d, ptr(v), d, nk * d, ptr(o), d, nq * d, B, nq, nk, H,
+                                                         dh, ptr(klen), self.st()), 'og_attention_fwd_padded')
             return o
         _cabi.check(self.lib.og_attention_fwd(ptr(q), d, nq * d, ptr(k), d, nk * d, ptr(v), d, nk * d, ptr(o), d, nq * d, B, nq, nk, H, dh,
                                               _cabi.OG_PREC_FP32, self.st()), 'og_attention_fwd')
         return o
 
-    def softmax_rows(self, P, ld, rows, cols):
+    def softmax_rows(self, P, ld, rows, cols, klen=None):
+        """``klen``: rows are [B, rows / B] and sequence b's rows take its first klen[b] columns (P = 0 past them)"""
+        if klen is not None:
+            B = klen.numel()
+            _cabi.check(self.lib.og_softmax_rows_padded(ptr(P), ld, B, rows // B, cols, ptr(klen), self.st()), 'og_softmax_rows_padded')
+            return
         _cabi.check(self.lib.og_softmax_rows(ptr(P), ld, rows, cols, self.st()), 'og_softmax_rows')
 
-    def softmax_bwd_rows(self, P, dP, ld, rows, cols, scale):
+    def softmax_bwd_rows(self, P, dP, ld, rows, cols, scale, klen=None):
+        if klen is not None:
+            B = klen.numel()
+            _cabi.check(self.lib.og_softmax_bwd_rows_padded(ptr(P), ptr(dP), ld, B, rows // B, cols, float(scale), ptr(klen), self.st()),
+                        'og_softmax_bwd_rows_padded')
+            return
         _cabi.check(self.lib.og_softmax_bwd_rows(ptr(P), ptr(dP), ld, rows, cols, float(scale), self.st()), 'og_softmax_bwd_rows')
 
     def mix_fwd(self, g, l, mix):
@@ -142,35 +177,57 @@ class _Ops:
         _cabi.check(self.lib.og_mix_param_grad(ptr(csum), ptr(mix), ptr(out), d, self.st()), 'og_mix_param_grad')
         return out
 
-    def bn_fwd(self, a, gamma, beta, eps, momentum, running_mean, running_var):
+    def bn_fwd(self, a, gamma, beta, eps, momentum, running_mean, running_var, lens=None):
+        """``lens``: statistics over the real rows of every pair (rows [B, cap])"""
         rows, cols = a.shape
         y, mean, invstd = self.empty(rows, cols), self.empty(cols), self.empty(cols)
+        if lens is not None:
+            B = lens.numel()
+            _cabi.check(self.lib.og_bn_train_fwd_padded(ptr(a), a.stride(0), B, rows // B, ptr(lens), cols, 1, ptr(gamma), ptr(beta), float(eps),
+                                                        float(momentum), ptr(y), cols, ptr(mean), ptr(invstd), ptr(running_mean),
+                                                        ptr(running_var), ptr(self.ws(cols)), self.st()), 'og_bn_train_fwd_padded')
+            return y, mean, invstd
         _cabi.check(self.lib.og_bn_train_fwd(ptr(a), a.stride(0), rows, cols, 1, ptr(gamma), ptr(beta), float(eps), float(momentum), ptr(y), cols,
                                              ptr(mean), ptr(invstd), ptr(running_mean), ptr(running_var), ptr(self.ws(cols)), self.st()), 'og_bn_train_fwd')
         return y, mean, invstd
 
-    def bn_bwd(self, dy, a, gamma, mean, invstd):
+    def bn_bwd(self, dy, a, gamma, mean, invstd, lens=None):
         rows, cols = a.shape
         da, dgamma, dbeta = self.empty(rows, cols), self.empty(cols), self.empty(cols)
+        if lens is not None:
+            B = lens.numel()
+            _cabi.check(self.lib.og_bn_train_bwd_padded(ptr(dy), dy.stride(0), ptr(a), a.stride(0), B, rows // B, ptr(lens), cols, 1, ptr(gamma),
+                                                        ptr(mean), ptr(invstd), ptr(da), cols, ptr(dgamma), ptr(dbeta), ptr(self.ws(cols)),
+                                                        self.st()), 'og_bn_train_bwd_padded')
+            return da, dgamma, dbeta
         _cabi.check(self.lib.og_bn_train_bwd(ptr(dy), dy.stride(0), ptr(a), a.stride(0), rows, cols, 1, ptr(gamma), ptr(mean), ptr(invstd), ptr(da), cols,
                                              ptr(dgamma), ptr(dbeta), ptr(self.ws(cols)), self.st()), 'og_bn_train_bwd')
         return da, dgamma, dbeta
 
-    def sinkhorn_fwd(self, Sp, dust, B, n, m, iters, reg):
+    def sinkhorn_fwd(self, Sp, dust, B, n, m, iters, reg, lens=None):
+        """``lens``: [2B] row then column lengths of a padded batch"""
         lib, lds = self.lib, Sp.shape[2]
         scores = self.empty(B, n + 1, m + 1)
         hist = self.empty(max(int(lib.og_sinkhorn_hist_floats(B, n, m, iters)), 1))
         wsb = _cabi.check_size(lib.og_sinkhorn_workspace_bytes(B, n, m), 'og_sinkhorn_workspace_bytes')
         ws = torch.empty(wsb, dtype=torch.uint8, device=self.dev)
+        if lens is not None:
+            _cabi.check(lib.og_sinkhorn_train_fwd_padded(ptr(Sp), lds, n * lds, ptr(dust), B, n, m, ptr(lens), iters, reg, ptr(scores), ptr(hist),
+                                                         ptr(ws), wsb, self.st()), 'og_sinkhorn_train_fwd_padded')
+            return scores, hist
         _cabi.check(lib.og_sinkhorn_train_fwd(ptr(Sp), lds, n * lds, ptr(dust), B, n, m, iters, reg, ptr(scores), ptr(hist), ptr(ws), wsb, self.st()),
                     'og_sinkhorn_train_fwd')
         return scores, hist
 
-    def sinkhorn_bwd(self, Sp, dust, hist, G, B, n, m, iters, reg):
+    def sinkhorn_bwd(self, Sp, dust, hist, G, B, n, m, iters, reg, lens=None):
         lib, lds = self.lib, Sp.shape[2]
         dZ, dd = self.empty(B, n + 1, m + 1), self.empty(1)
         wsb = _cabi.check_size(lib.og_sinkhorn_bwd_workspace_bytes(B, n, m, iters), 'og_sinkhorn_bwd_workspace_bytes')
         ws = torch.empty(wsb, dtype=torch.uint8, device=self.dev)
+        if lens is not None:
+            _cabi.check(lib.og_sinkhorn_bwd_padded(ptr(Sp), lds, n * lds, ptr(dust), B, n, m, ptr(lens), iters, reg, ptr(hist), ptr(G), ptr(dZ),
+                                                   ptr(dd), ptr(ws), wsb, self.st()), 'og_sinkhorn_bwd_padded')
+            return dZ, dd
         _cabi.check(lib.og_sinkhorn_bwd(ptr(Sp), lds, n * lds, ptr(dust), B, n, m, iters, reg, ptr(hist), ptr(G), ptr(dZ), ptr(dd), ptr(ws), wsb, self.st()),
                     'og_sinkhorn_bwd')
         return dZ, dd

@@ -491,6 +491,15 @@ int og_sinkhorn_train_fwd(const float* S, int64_t lds, int64_t strideS, const fl
                          hist, hist + (int64_t)batch * iters * (n + 1));
 }
 
+int og_sinkhorn_train_fwd_padded(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int batch, int n, int m,
+                                 const int* lengths, int iters, float reg, float* scores, float* hist, void* workspace,
+                                 int64_t workspace_bytes, void* stream) {
+  OG_CHECK_ARG(S && dustbin && lengths && scores && workspace && hist, "sinkhorn_train_fwd_padded: null pointer");
+  OG_CHECK_ARG(batch > 0 && n > 0 && m > 0 && iters >= 0 && reg > 0.f, "sinkhorn_train_fwd_padded: bad sizes");
+  return sinkhorn_launch(S, lds, strideS, dustbin, batch, n, m, iters, reg, scores, workspace, workspace_bytes, (cudaStream_t)stream,
+                         hist, hist + (int64_t)batch * iters * (n + 1), lengths);
+}
+
 int64_t og_sinkhorn_bwd_workspace_bytes(int batch, int n, int m, int iters) {
   return (batch > 0 && n > 0 && m > 0 && iters >= 0) ? sinkhorn_bwd_workspace_bytes(batch, n, m, iters) : -1;
 }
@@ -502,6 +511,15 @@ int og_sinkhorn_bwd(const float* S, int64_t lds, int64_t strideS, const float* d
   OG_CHECK_ARG(batch > 0 && n > 0 && m > 0 && iters >= 0 && reg > 0.f, "sinkhorn_bwd: bad sizes");
   return sinkhorn_bwd_launch(S, lds, strideS, dustbin, batch, n, m, iters, reg, hist, dscores, dS_aug, ddustbin, workspace,
                              workspace_bytes, (cudaStream_t)stream);
+}
+
+int og_sinkhorn_bwd_padded(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int batch, int n, int m,
+                           const int* lengths, int iters, float reg, const float* hist, const float* dscores, float* dS_aug,
+                           float* ddustbin, void* workspace, int64_t workspace_bytes, void* stream) {
+  OG_CHECK_ARG(S && dustbin && lengths && hist && dscores && dS_aug && ddustbin && workspace, "sinkhorn_bwd_padded: null pointer");
+  OG_CHECK_ARG(batch > 0 && n > 0 && m > 0 && iters >= 0 && reg > 0.f, "sinkhorn_bwd_padded: bad sizes");
+  return sinkhorn_bwd_launch(S, lds, strideS, dustbin, batch, n, m, iters, reg, hist, dscores, dS_aug, ddustbin, workspace,
+                             workspace_bytes, (cudaStream_t)stream, lengths);
 }
 
 int64_t og_match_workspace_bytes(int batch, int n, int m) { return match_workspace_bytes(batch, n, m); }
@@ -527,8 +545,8 @@ int64_t og_gt_matches_workspace_bytes(int batch, int n, int m) {
   return gt_matches_workspace_bytes(batch, n, m);
 }
 
-int og_gt_matches_fwd(const float* kpts0, const float* kpts1, int batch, int n, int m, const og_gt_transform* tf,
-                      int64_t* gt_matches0, int64_t* gt_matches1, void* workspace, int64_t workspace_bytes, void* stream) {
+static int gt_matches_impl(const float* kpts0, const float* kpts1, int batch, int n, int m, const int* lens, const og_gt_transform* tf,
+                           int64_t* gt_matches0, int64_t* gt_matches1, void* workspace, int64_t workspace_bytes, void* stream) {
   OG_CHECK_ARG(kpts0 && kpts1 && tf && gt_matches0 && gt_matches1 && workspace, "gt_matches: null pointer");
   OG_CHECK_ARG(batch > 0 && n > 0 && m > 0, "gt_matches: bad sizes (the reference returns (None, None) for an empty keypoint set)");
   OG_CHECK_ARG(tf->type == OG_GT_PERSPECTIVE || tf->type == OG_GT_3D_REPROJECTION, "gt_matches: unknown transformation type %d", tf->type);
@@ -539,7 +557,20 @@ int og_gt_matches_fwd(const float* kpts0, const float* kpts1, int batch, int n, 
     OG_CHECK_ARG(!tf->depth_is_image || (tf->depth0_h > 0 && tf->depth0_w > 0 && tf->depth1_h > 0 && tf->depth1_w > 0),
                  "gt_matches: depth image sizes");
   }
-  return gt_matches_launch(kpts0, kpts1, batch, n, m, *tf, gt_matches0, gt_matches1, workspace, workspace_bytes, (cudaStream_t)stream);
+  return gt_matches_launch(kpts0, kpts1, batch, n, m, *tf, gt_matches0, gt_matches1, workspace, workspace_bytes, (cudaStream_t)stream,
+                           lens);
+}
+
+int og_gt_matches_fwd(const float* kpts0, const float* kpts1, int batch, int n, int m, const og_gt_transform* tf,
+                      int64_t* gt_matches0, int64_t* gt_matches1, void* workspace, int64_t workspace_bytes, void* stream) {
+  return gt_matches_impl(kpts0, kpts1, batch, n, m, nullptr, tf, gt_matches0, gt_matches1, workspace, workspace_bytes, stream);
+}
+
+int og_gt_matches_fwd_padded(const float* kpts0, const float* kpts1, int batch, int n, int m, const int* lengths,
+                             const og_gt_transform* tf, int64_t* gt_matches0, int64_t* gt_matches1, void* workspace,
+                             int64_t workspace_bytes, void* stream) {
+  OG_CHECK_ARG(lengths, "gt_matches_padded: null lengths");
+  return gt_matches_impl(kpts0, kpts1, batch, n, m, lengths, tf, gt_matches0, gt_matches1, workspace, workspace_bytes, stream);
 }
 
 int og_collate_fwd(const float* lafs, const float* scores, const float* desc, const int* offsets, const int* select, int max_count,
@@ -569,6 +600,15 @@ int og_criterion_fwd(const float* scores, const int64_t* gt_matches0, const int6
   OG_CHECK_ARG(batch > 0 && n > 0 && m > 0, "criterion: bad sizes");
   return criterion_launch(scores, gt_matches0, gt_matches1, batch, n, m, loss, dscores, grad_scale, workspace, workspace_bytes,
                           (cudaStream_t)stream);
+}
+
+int og_criterion_fwd_padded(const float* scores, const int64_t* gt_matches0, const int64_t* gt_matches1, int batch, int n, int m,
+                            const int* lengths, float* loss, float* dscores, float grad_scale, void* workspace, int64_t workspace_bytes,
+                            void* stream) {
+  OG_CHECK_ARG(scores && gt_matches0 && gt_matches1 && lengths && loss && workspace, "criterion_padded: null pointer");
+  OG_CHECK_ARG(batch > 0 && n > 0 && m > 0, "criterion_padded: bad sizes");
+  return criterion_launch(scores, gt_matches0, gt_matches1, batch, n, m, loss, dscores, grad_scale, workspace, workspace_bytes,
+                          (cudaStream_t)stream, lengths);
 }
 
 static bool metric_sizes_ok(int batch, int d, int n, int m, int precision) {
@@ -607,52 +647,100 @@ int og_colsum(const float* x, int64_t ldx, const float* y, int64_t ldy, const fl
   return colreduce_launch<0>(a, (cudaStream_t)stream);
 }
 
-int og_bn_train_fwd(const float* a_, int64_t lda, int rows, int cols, int relu, const float* gamma, const float* beta,
-                    float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
-                    float* running_mean, float* running_var, float* workspace, void* stream) {
+static int bn_train_fwd_impl(const float* a_, int64_t lda, int rows, int cols, int relu, const float* gamma, const float* beta,
+                             float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
+                             float* running_mean, float* running_var, float* workspace, const int* len, int cap, void* stream) {
   OG_CHECK_ARG(a_ && gamma && beta && y && save_mean && save_invstd && workspace, "bn_train_fwd: null pointer");
   OG_CHECK_ARG(rows > 0 && cols > 0, "bn_train_fwd: bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
   float* var = workspace;                                   // [cols]
   ColReduceArgs r = {};
   r.x = a_; r.ldx = lda; r.rows = rows; r.cols = cols; r.relu = relu; r.partial = workspace + 2 * (int64_t)cols; r.out0 = save_mean;
+  r.len = len; r.cap = cap;
   int rc = colreduce_launch<1>(r, st);
   if (rc != OG_OK) return rc;
   r.mu = save_mean; r.out0 = var;
   if ((rc = colreduce_launch<2>(r, st)) != OG_OK) return rc;
-  if ((rc = OG_LAUNCH(bn_finish_stats_kernel, cdiv(cols, 256), 256, 0, st, save_mean, var, cols, rows, eps, momentum, save_invstd,
+  if ((rc = OG_LAUNCH(bn_finish_stats_kernel, cdiv(cols, 256), 256, 0, st, save_mean, var, cols, rows, len, cap, eps, momentum, save_invstd,
                       running_mean, running_var)) != OG_OK) return rc;
   return OG_LAUNCH(bn_apply_kernel, eltwise_grid((int64_t)rows * cols), 256, 0, st, a_, lda, rows, cols, relu, save_mean, save_invstd, gamma,
                    beta, y, ldy);
 }
 
-int og_bn_train_bwd(const float* dy, int64_t lddy, const float* a_, int64_t lda, int rows, int cols, int relu,
-                    const float* gamma, const float* save_mean, const float* save_invstd,
-                    float* da, int64_t ldda, float* dgamma, float* dbeta, float* workspace, void* stream) {
+int og_bn_train_fwd(const float* a_, int64_t lda, int rows, int cols, int relu, const float* gamma, const float* beta,
+                    float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
+                    float* running_mean, float* running_var, float* workspace, void* stream) {
+  return bn_train_fwd_impl(a_, lda, rows, cols, relu, gamma, beta, eps, momentum, y, ldy, save_mean, save_invstd, running_mean, running_var,
+                           workspace, nullptr, rows, stream);
+}
+
+int og_bn_train_fwd_padded(const float* a_, int64_t lda, int batch, int cap, const int* lengths, int cols, int relu, const float* gamma,
+                           const float* beta, float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
+                           float* running_mean, float* running_var, float* workspace, void* stream) {
+  OG_CHECK_ARG(lengths && batch > 0 && cap > 0 && (int64_t)batch * cap <= INT32_MAX, "bn_train_fwd_padded: bad lengths or sizes");
+  return bn_train_fwd_impl(a_, lda, batch * cap, cols, relu, gamma, beta, eps, momentum, y, ldy, save_mean, save_invstd, running_mean,
+                           running_var, workspace, lengths, cap, stream);
+}
+
+static int bn_train_bwd_impl(const float* dy, int64_t lddy, const float* a_, int64_t lda, int rows, int cols, int relu,
+                             const float* gamma, const float* save_mean, const float* save_invstd,
+                             float* da, int64_t ldda, float* dgamma, float* dbeta, float* workspace, const int* len, int cap, void* stream) {
   OG_CHECK_ARG(dy && a_ && gamma && save_mean && save_invstd && da && dgamma && dbeta && workspace, "bn_train_bwd: null pointer");
   OG_CHECK_ARG(rows > 0 && cols > 0, "bn_train_bwd: bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
   ColReduceArgs r = {};
   r.x = dy; r.ldx = lddy; r.y = a_; r.ldy = lda; r.mu = save_mean; r.invstd = save_invstd; r.rows = rows; r.cols = cols; r.relu = relu;
   r.partial = workspace + 2 * (int64_t)cols; r.out0 = dbeta; r.out1 = dgamma;
+  r.len = len; r.cap = cap;
   int rc = colreduce_launch<3>(r, st);
   if (rc != OG_OK) return rc;
   return OG_LAUNCH(bn_bwd_apply_kernel, eltwise_grid((int64_t)rows * cols), 256, 0, st, dy, lddy, a_, lda, rows, cols, relu, save_mean,
-                   save_invstd, gamma, dgamma, dbeta, da, ldda);
+                   save_invstd, gamma, dgamma, dbeta, da, ldda, len, cap);
+}
+
+int og_bn_train_bwd(const float* dy, int64_t lddy, const float* a_, int64_t lda, int rows, int cols, int relu,
+                    const float* gamma, const float* save_mean, const float* save_invstd,
+                    float* da, int64_t ldda, float* dgamma, float* dbeta, float* workspace, void* stream) {
+  return bn_train_bwd_impl(dy, lddy, a_, lda, rows, cols, relu, gamma, save_mean, save_invstd, da, ldda, dgamma, dbeta, workspace,
+                           nullptr, rows, stream);
+}
+
+int og_bn_train_bwd_padded(const float* dy, int64_t lddy, const float* a_, int64_t lda, int batch, int cap, const int* lengths, int cols,
+                           int relu, const float* gamma, const float* save_mean, const float* save_invstd,
+                           float* da, int64_t ldda, float* dgamma, float* dbeta, float* workspace, void* stream) {
+  OG_CHECK_ARG(lengths && batch > 0 && cap > 0 && (int64_t)batch * cap <= INT32_MAX, "bn_train_bwd_padded: bad lengths or sizes");
+  return bn_train_bwd_impl(dy, lddy, a_, lda, batch * cap, cols, relu, gamma, save_mean, save_invstd, da, ldda, dgamma, dbeta, workspace,
+                           lengths, cap, stream);
 }
 
 int og_softmax_rows(float* S, int64_t ld, int64_t rows, int cols, void* stream) {
   OG_CHECK_ARG(S && rows >= 0 && cols > 0 && ld >= cols, "softmax_rows: bad arguments");
   if (rows == 0) return OG_OK;
   OG_CHECK_ARG((rows + 7) / 8 <= 0x7fffffffLL, "softmax_rows: too many rows");
-  return OG_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, S, ld, rows, cols);
+  return OG_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, S, ld, rows, cols, nullptr, rows);
+}
+
+int og_softmax_rows_padded(float* S, int64_t ld, int batch, int64_t seq_rows, int cols, const int* key_lengths, void* stream) {
+  OG_CHECK_ARG(S && key_lengths && batch > 0 && seq_rows > 0 && cols > 0 && ld >= cols, "softmax_rows_padded: bad arguments");
+  const int64_t rows = (int64_t)batch * seq_rows;
+  OG_CHECK_ARG((rows + 7) / 8 <= 0x7fffffffLL, "softmax_rows_padded: too many rows");
+  return OG_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, S, ld, rows, cols, key_lengths, seq_rows);
 }
 
 int og_softmax_bwd_rows(const float* P, float* dP, int64_t ld, int64_t rows, int cols, float scale, void* stream) {
   OG_CHECK_ARG(P && dP && rows >= 0 && cols > 0 && ld >= cols, "softmax_bwd_rows: bad arguments");
   if (rows == 0) return OG_OK;
   OG_CHECK_ARG((rows + 7) / 8 <= 0x7fffffffLL, "softmax_bwd_rows: too many rows");
-  return OG_LAUNCH(softmax_bwd_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, P, dP, ld, rows, cols, scale);
+  return OG_LAUNCH(softmax_bwd_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, P, dP, ld, rows, cols, scale, nullptr, rows);
+}
+
+int og_softmax_bwd_rows_padded(const float* P, float* dP, int64_t ld, int batch, int64_t seq_rows, int cols, float scale,
+                               const int* key_lengths, void* stream) {
+  OG_CHECK_ARG(P && dP && key_lengths && batch > 0 && seq_rows > 0 && cols > 0 && ld >= cols, "softmax_bwd_rows_padded: bad arguments");
+  const int64_t rows = (int64_t)batch * seq_rows;
+  OG_CHECK_ARG((rows + 7) / 8 <= 0x7fffffffLL, "softmax_bwd_rows_padded: too many rows");
+  return OG_LAUNCH(softmax_bwd_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, P, dP, ld, rows, cols, scale,
+                   key_lengths, seq_rows);
 }
 
 int og_sum_batches(const float* part, int S, int rows, int cols, float* out, int64_t ld_out, int accumulate, void* stream) {
@@ -686,6 +774,21 @@ int og_kenc_input(const float* kpts, const float* side, int rows, int side_info_
   OG_CHECK_ARG(kpts && out && rows > 0 && side_info_size >= 0 && (side_info_size == 0 || side), "kenc_input: bad arguments");
   return OG_LAUNCH(kenc_input_kernel, cdiv(rows, 256), 256, 0, (cudaStream_t)stream, kpts, side, rows, side_info_size, width - 1.f,
                    height - 1.f, rows, nullptr, nullptr, out);
+}
+
+int og_kenc_input_padded(const float* kpts, const float* side, int batch, int cap, const int* lengths, int side_info_size,
+                         const float* pair_wh, float* out, void* stream) {
+  OG_CHECK_ARG(kpts && out && lengths && pair_wh && batch > 0 && cap > 0 && (int64_t)batch * cap <= INT32_MAX && side_info_size >= 0 &&
+               (side_info_size == 0 || side), "kenc_input_padded: bad arguments");
+  const int rows = batch * cap;
+  return OG_LAUNCH(kenc_input_kernel, cdiv(rows, 256), 256, 0, (cudaStream_t)stream, kpts, side, rows, side_info_size, 0.f, 0.f, cap,
+                   lengths, pair_wh, out);
+}
+
+int og_mask_padded_rows(const float* src, int batch, int cap, int cols, const int* lengths, float* dst, void* stream) {
+  OG_CHECK_ARG(src && dst && lengths && batch > 0 && cap > 0 && cols > 0, "mask_padded_rows: bad arguments");
+  const int64_t rows = (int64_t)batch * cap;
+  return OG_LAUNCH(mask_padded_rows_kernel, eltwise_grid(rows * cols), 256, 0, (cudaStream_t)stream, src, rows, cap, cols, lengths, dst);
 }
 
 // ---- SuperPoint front-end operators (row f4; csrc/superpoint.cuh) ----

@@ -27,6 +27,8 @@ struct CritArgs {
   float* loss;                  // [2]: {loss, metric_loss}
   float* dscores;               // optional [B, n+1, m+1], zero-filled by the caller: receives d loss / d scores
   float grad_scale;             // upstream gradient of 'loss' (nll_weight)
+  const int* lens;              // padded batch (null otherwise): n_0 .. n_{B-1}, m_0 .. m_{B-1}; pair b is the [n_b + 1, m_b + 1] block of
+                                // its capacity-strided scores (dustbins at n_b, m_b), its labels past the lengths are ignored
 };
 
 __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
@@ -34,18 +36,19 @@ __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
   __shared__ float s_cnt[3];
   __shared__ bool last;
   const int b = blockIdx.x;
-  const int n = a.n, m = a.m;
-  const float* S = a.scores + (int64_t)b * (n + 1) * (m + 1);
-  const int64_t* g0 = a.gt0 + (int64_t)b * n;
-  const int64_t* g1 = a.gt1 + (int64_t)b * m;
+  const int n = a.lens ? padded_length(a.lens, b, a.n) : a.n, m = a.lens ? padded_length(a.lens + a.B, b, a.m) : a.m;
+  const int64_t ld = a.m + 1;
+  const float* S = a.scores + (int64_t)b * (a.n + 1) * ld;
+  const int64_t* g0 = a.gt0 + (int64_t)b * a.n;
+  const int64_t* g1 = a.gt1 + (int64_t)b * a.m;
   float sm = 0.f, su0 = 0.f, su1 = 0.f, cm = 0.f, cu0 = 0.f, cu1 = 0.f;
   for (int i = threadIdx.x; i < n; i += CRIT_THREADS) {
     const int64_t g = g0[i];
-    if (g >= 0 && g < m) { sm += S[(int64_t)i * (m + 1) + g]; cm += 1.f; }
-    else if (g == -1)    { su0 += S[(int64_t)i * (m + 1) + m]; cu0 += 1.f; }
+    if (g >= 0 && g < m) { sm += S[(int64_t)i * ld + g]; cm += 1.f; }
+    else if (g == -1)    { su0 += S[(int64_t)i * ld + m]; cu0 += 1.f; }
   }
   for (int j = threadIdx.x; j < m; j += CRIT_THREADS)
-    if (g1[j] == -1) { su1 += S[(int64_t)n * (m + 1) + j]; cu1 += 1.f; }
+    if (g1[j] == -1) { su1 += S[(int64_t)n * ld + j]; cu1 += 1.f; }
   const float tm = cta_sum<CRIT_THREADS>(sm, red), tu0 = cta_sum<CRIT_THREADS>(su0, red), tu1 = cta_sum<CRIT_THREADS>(su1, red);
   const float nm = cta_sum<CRIT_THREADS>(cm, red), nu0 = cta_sum<CRIT_THREADS>(cu0, red), nu1 = cta_sum<CRIT_THREADS>(cu1, red);
   if (threadIdx.x == 0) {
@@ -59,17 +62,17 @@ __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
   }
   __syncthreads();
   if (a.dscores) {                                          // d loss / d scores: the same gather, scattered
-    float* D = a.dscores + (int64_t)b * (n + 1) * (m + 1);
+    float* D = a.dscores + (int64_t)b * (a.n + 1) * ld;
     const float wm = s_cnt[0] > 0.f ? -a.grad_scale / (s_cnt[0] * a.B) : 0.f;
     const float w0 = s_cnt[1] > 0.f ? -0.5f * a.grad_scale / (s_cnt[1] * a.B) : 0.f;
     const float w1 = s_cnt[2] > 0.f ? -0.5f * a.grad_scale / (s_cnt[2] * a.B) : 0.f;
     for (int i = threadIdx.x; i < n; i += CRIT_THREADS) {
       const int64_t g = g0[i];
-      if (g >= 0 && g < m) D[(int64_t)i * (m + 1) + g] = wm;       // a row holds at most one of the two
-      else if (g == -1)    D[(int64_t)i * (m + 1) + m] = w0;
+      if (g >= 0 && g < m) D[(int64_t)i * ld + g] = wm;       // a row holds at most one of the two
+      else if (g == -1)    D[(int64_t)i * ld + m] = w0;
     }
     for (int j = threadIdx.x; j < m; j += CRIT_THREADS)
-      if (g1[j] == -1) D[(int64_t)n * (m + 1) + j] = w1;
+      if (g1[j] == -1) D[(int64_t)n * ld + j] = w1;
   }
   if (last && threadIdx.x == 0) {
     a.loss[0] = last_cta_sum(a.per_pair, a.B) / (float)a.B;       // pair order: deterministic
@@ -80,13 +83,14 @@ __global__ void __launch_bounds__(CRIT_THREADS) criterion_kernel(CritArgs a) {
 inline int64_t criterion_workspace_bytes(int B) { return 256 + align_up((int64_t)B * 4, 256); }
 
 inline int criterion_launch(const float* scores, const int64_t* gt0, const int64_t* gt1, int B, int n, int m, float* loss,
-                            float* dscores, float grad_scale, void* ws, int64_t ws_bytes, cudaStream_t stream) {
+                            float* dscores, float grad_scale, void* ws, int64_t ws_bytes, cudaStream_t stream,
+                            const int* lens = nullptr) {
   if (ws_bytes < criterion_workspace_bytes(B)) return fail(OG_EWORKSPACE, "criterion: workspace too small");
   CritArgs a;
   a.scores = scores; a.gt0 = gt0; a.gt1 = gt1; a.B = B; a.n = n; a.m = m;
   a.counter = static_cast<unsigned int*>(ws);
   a.per_pair = reinterpret_cast<float*>(static_cast<char*>(ws) + 256);
-  a.loss = loss; a.dscores = dscores; a.grad_scale = grad_scale;
+  a.loss = loss; a.dscores = dscores; a.grad_scale = grad_scale; a.lens = lens;
   OG_CUDA(cudaMemsetAsync(a.counter, 0, 4, stream));
   return OG_LAUNCH(criterion_kernel, B, CRIT_THREADS, 0, stream, a);
 }

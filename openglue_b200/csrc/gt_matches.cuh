@@ -102,14 +102,16 @@ __global__ void gt_reproject_kernel(const float* __restrict__ kpts, int n, int d
   mask[(int64_t)b * n + i] = ok ? 1 : 0;
 }
 
-// nearest target of every query point (first index on ties, like torch.min); targets stream through shared memory
+// nearest target of every query point (first index on ties, like torch.min); targets stream through shared memory.
+// A padded batch (tlen set) searches each pair's first tlen[b] targets only.
 constexpr int GT_TILE = 2048;
-__global__ void __launch_bounds__(256) gt_nearest_kernel(const float2* __restrict__ q, int nq, const float* __restrict__ targets, int nt,
-                                                         int* __restrict__ nn) {
+__global__ void __launch_bounds__(256) gt_nearest_kernel(const float2* __restrict__ q, int nq, const float* __restrict__ targets, int nt_cap,
+                                                         const int* __restrict__ tlen, int* __restrict__ nn) {
   __shared__ float2 tile[GT_TILE];
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   const float2 me = i < nq ? q[(int64_t)b * nq + i] : make_float2(0.f, 0.f);
-  const float2* tg = reinterpret_cast<const float2*>(targets) + (int64_t)b * nt;
+  const float2* tg = reinterpret_cast<const float2*>(targets) + (int64_t)b * nt_cap;
+  const int nt = tlen ? padded_length(tlen, b, nt_cap) : nt_cap;
   float best = CUDART_INF_F;
   int best_j = 0;
   for (int j0 = 0; j0 < nt; j0 += GT_TILE) {
@@ -127,11 +129,13 @@ __global__ void __launch_bounds__(256) gt_nearest_kernel(const float2* __restric
   if (i < nq) nn[(int64_t)b * nq + i] = best_j;
 }
 
-// gt[i] = nn[i] if the neighbour points back, else -1; -2 where the reprojection was invalid   (:45-51, :72-73)
+// gt[i] = nn[i] if the neighbour points back, else -1; -2 where the reprojection was invalid   (:45-51, :72-73), and in a padded
+// batch (alen set) past the pair's length
 __global__ void gt_mutual_kernel(const int* __restrict__ nn_a, const int* __restrict__ nn_b, const uint8_t* __restrict__ mask_a,
-                                 int na, int nb, int64_t* __restrict__ gt_a) {
+                                 int na, int nb, const int* __restrict__ alen, int64_t* __restrict__ gt_a) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= na) return;
+  if (alen && i >= padded_length(alen, b, na)) { gt_a[(int64_t)b * na + i] = -2; return; }
   const int j = nn_a[(int64_t)b * na + i];
   int64_t g = (nn_b[(int64_t)b * nb + j] == i) ? (int64_t)j : -1;
   if (!mask_a[(int64_t)b * na + i]) g = -2;
@@ -144,7 +148,9 @@ inline int64_t gt_matches_workspace_bytes(int B, int n, int m) {
 }
 
 inline int gt_matches_launch(const float* kpts0, const float* kpts1, int B, int n, int m, const og_gt_transform& tf,
-                             int64_t* gt0, int64_t* gt1, void* ws, int64_t ws_bytes, cudaStream_t st) {
+                             int64_t* gt0, int64_t* gt1, void* ws, int64_t ws_bytes, cudaStream_t st, const int* lens = nullptr) {
+  const int* len0 = lens;                              // padded batch: n_0 .. n_{B-1}, m_0 .. m_{B-1}
+  const int* len1 = lens ? lens + B : nullptr;
   if (ws_bytes < gt_matches_workspace_bytes(B, n, m)) return fail(OG_EWORKSPACE, "gt_matches: workspace too small");
   char* w = static_cast<char*>(ws);
   auto take = [&](int64_t bytes) { char* p = w; w += align_up(bytes, 256); return p; };
@@ -159,10 +165,10 @@ inline int gt_matches_launch(const float* kpts0, const float* kpts1, int B, int 
   if ((rc = OG_LAUNCH(gt_prepare_kernel, cdiv(2 * B, 64), 64, 0, st, tf, B, prep))) return rc;
   if ((rc = OG_LAUNCH(gt_reproject_kernel, dim3(cdiv(n, 256), B), 256, 0, st, kpts0, n, 0, tf, prep, k0t, mask0))) return rc;
   if ((rc = OG_LAUNCH(gt_reproject_kernel, dim3(cdiv(m, 256), B), 256, 0, st, kpts1, m, 1, tf, prep, k1t, mask1))) return rc;
-  if ((rc = OG_LAUNCH(gt_nearest_kernel, dim3(cdiv(n, 256), B), 256, 0, st, k0t, n, kpts1, m, nn0))) return rc;
-  if ((rc = OG_LAUNCH(gt_nearest_kernel, dim3(cdiv(m, 256), B), 256, 0, st, k1t, m, kpts0, n, nn1))) return rc;
-  if ((rc = OG_LAUNCH(gt_mutual_kernel, dim3(cdiv(n, 256), B), 256, 0, st, nn0, nn1, mask0, n, m, gt0))) return rc;
-  return OG_LAUNCH(gt_mutual_kernel, dim3(cdiv(m, 256), B), 256, 0, st, nn1, nn0, mask1, m, n, gt1);
+  if ((rc = OG_LAUNCH(gt_nearest_kernel, dim3(cdiv(n, 256), B), 256, 0, st, k0t, n, kpts1, m, len1, nn0))) return rc;
+  if ((rc = OG_LAUNCH(gt_nearest_kernel, dim3(cdiv(m, 256), B), 256, 0, st, k1t, m, kpts0, n, len0, nn1))) return rc;
+  if ((rc = OG_LAUNCH(gt_mutual_kernel, dim3(cdiv(n, 256), B), 256, 0, st, nn0, nn1, mask0, n, m, len0, gt0))) return rc;
+  return OG_LAUNCH(gt_mutual_kernel, dim3(cdiv(m, 256), B), 256, 0, st, nn1, nn0, mask1, m, n, len1, gt1);
 }
 
 }  // namespace og

@@ -122,7 +122,8 @@ __device__ float og_sink_log_tab[SINK_MAX_ROWS + 1];                    // [k] =
 struct SinkPair {
   int n, m;
   float norm, log_a_last, log_b_last;
-  __device__ __forceinline__ SinkPair(const SinkArgs& a, int b) {
+  template <class Args>
+  __device__ __forceinline__ SinkPair(const Args& a, int b) {
     n = padded_length(a.len_n, b, a.n);
     m = padded_length(a.len_m, b, a.m);
     if (a.len_n) {
@@ -500,7 +501,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_ke
       v_s[j] = ((j < MC) ? P.norm : P.log_b_last) + v_s[j] - logf(c);
     });
     if (a.hist_v && s.strip == 0) {                   // every CTA of the pair holds the same v: one of them records it
-      float* hv = a.hist_v + ((int64_t)s.b * (a.iters + 1) + it + 1) * (m + 1);
+      float* hv = a.hist_v + (int64_t)(a.m + 1) * (s.b * (a.iters + 1) + it + 1);     // capacity rows; the pair's dustbin at m
       for (int j = s.tid; j <= m; j += blockDim.x) hv[j] = (j < m) ? v_s[j] : v_s[MC];
     }
   }
@@ -931,7 +932,6 @@ inline int sinkhorn_kernel_launch(const SinkArgs& a, const SinkPlan& p, cudaStre
 inline int sinkhorn_launch(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int B, int n, int m,
                            int iters, float reg, float* scores, void* ws, int64_t ws_bytes, cudaStream_t stream,
                            float* hist_u = nullptr, float* hist_v = nullptr, const int* lens = nullptr) {
-  if (lens && (hist_u || hist_v)) return fail(OG_EUNSUPPORTED, "sinkhorn: no training form for a padded batch");
   if (lens && n > SINK_MAX_ROWS) return fail(OG_EUNSUPPORTED, "sinkhorn: a padded batch has at most %d rows, not %d", SINK_MAX_ROWS, n);
   if (lens)
     if (const int rc = sinkhorn_log_tables(stream)) return rc;

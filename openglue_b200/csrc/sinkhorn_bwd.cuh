@@ -38,6 +38,8 @@ struct SinkBwdArgs {
   float* partial;                        // [2][B][SP][mpad]
   unsigned int* barrier;
   int SP, rows_per_strip, mpad;
+  const int* len_n;                      // padded batch (null otherwise), as SinkArgs: pair b is the [len_n[b], len_m[b]] block of the
+  const int* len_m;                      // capacity; every history row and G keep the capacity's strides (n + 1, m + 1)
 };
 
 template <int V, int W, int SLOTS>
@@ -52,16 +54,18 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
   float* ring = red + G * a.mpad;                      // [SINK_WARPS][SLOTS][C]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SINK_WARPS * SLOTS * C);
   float* xr = reinterpret_cast<float*>(bars + SINK_WARPS * SLOTS);               // [2][G][W] partial row sums
-  const Strip s(a, a.n, a.m);
-  const int n = a.n, m = a.m, T = a.iters, b = s.b, tid = s.tid;
-  const float ia_reg = expf(-a.norm), ia_last = expf(-a.log_a_last);      // 1 / a_i
+  const SinkPair P(a, blockIdx.x / a.SP);
+  const Strip s(a, P.n, P.m);
+  const int n = P.n, m = P.m, T = a.iters, b = s.b, tid = s.tid;
+  const int64_t n1 = a.n + 1, m1 = a.m + 1;           // the capacity's row lengths of the histories
+  const float ia_reg = expf(-P.norm), ia_last = expf(-P.log_a_last);      // 1 / a_i
   SinkRowRing<V, W, SLOTS, false, SinkBwdArgs> rows(a, s, ring, bars);
   const float dz = rows.dz;
 
   for (int j = tid; j <= MC; j += blockDim.x) {        // vbar_T = column sums of G
     float vb = 0.f;
-    if (j < m) vb = __ldg(a.vbar_init + (int64_t)b * (m + 1) + j);
-    else if (j == MC) vb = __ldg(a.vbar_init + (int64_t)b * (m + 1) + m);
+    if (j < m) vb = __ldg(a.vbar_init + b * m1 + j);
+    else if (j == MC) vb = __ldg(a.vbar_init + b * m1 + m);
     vbar_s[j] = vb;
   }
   __syncthreads();
@@ -70,13 +74,13 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
   uint32_t rowpar = 0;
   for (int it = T - 1; it >= 0; --it) {
     // column constants of iteration t = it + 1 (every CTA of the pair builds the same values)
-    const float* vt = a.hist_v + ((int64_t)b * (T + 1) + it + 1) * (m + 1);
-    const float* vtm1 = vt - (m + 1);
+    const float* vt = a.hist_v + ((int64_t)b * (T + 1) + it + 1) * m1;
+    const float* vtm1 = vt - m1;
     for (int j = tid; j <= MC; j += blockDim.x) {
       float cv = -CUDART_INF_F, wq = 0.f;
       const int jj = (j < m) ? j : (j == MC ? m : -1);
       if (jj >= 0) {
-        const float lb = (jj < m) ? a.norm : a.log_b_last;
+        const float lb = (jj < m) ? P.norm : P.log_b_last;
         cv = __ldcg(vt + jj) - lb;
         wq = expf(__ldcg(vtm1 + jj) - cv);
       }
@@ -84,7 +88,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
     }
     __syncthreads();
     if (s.strip == 0) {                                // history for the matrix-gradient pass
-      const int64_t o = ((int64_t)b * T + it) * (m + 1);
+      const int64_t o = ((int64_t)b * T + it) * m1;
       for (int j = tid; j <= m; j += blockDim.x) {
         const int js = (j < m) ? j : MC;
         a.hist_cvec[o + j] = cvec_s[js]; a.hist_vbar[o + j] = vbar_s[js]; a.hist_wq[o + j] = wq_s[js];
@@ -95,7 +99,7 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
     for (int k = 0; k < V; ++k) cacc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
     float cacc_m = 0.f;
     const float cv_m = cvec_s[MC], vb_m = vbar_s[MC];
-    const float* ut = a.hist_u + ((int64_t)b * T + it) * (n + 1);
+    const float* ut = a.hist_u + ((int64_t)b * T + it) * n1;
 
     for (int row = s.r0 + s.grp; row < s.r1; row += G) {
       float4 z[V];
@@ -121,9 +125,9 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
 #pragma unroll
         for (int w2 = 0; w2 < W; ++w2) r_i += x[w2];
       }
-      const float ub0 = (it == T - 1) ? __ldg(a.ubar_init + (int64_t)b * (n + 1) + row) : 0.f;
+      const float ub0 = (it == T - 1) ? __ldg(a.ubar_init + b * n1 + row) : 0.f;
       const float coef = (ub0 - r_i) * ((row < n) ? ia_reg : ia_last);      // ubar_t,i / a_i
-      if (s.sub == 0 && s.lane == 0) a.hist_coef[((int64_t)b * T + it) * (n + 1) + row] = coef;
+      if (s.sub == 0 && s.lane == 0) a.hist_coef[((int64_t)b * T + it) * n1 + row] = coef;
 #pragma unroll
       for (int k = 0; k < V; ++k) {
         cacc[k].x = fmaf(z[k].x, coef, cacc[k].x); cacc[k].y = fmaf(z[k].y, coef, cacc[k].y);
@@ -138,11 +142,13 @@ __global__ void __launch_bounds__(SINK_WARPS * 32, (V <= 8) ? 2 : 1) sinkhorn_bw
 }
 
 // ---- small kernels around the sweeps ------------------------------------------------------------------------------
-// row sums of G [B, n+1, m+1]: one warp per row
-__global__ void __launch_bounds__(256) sinkb_rowsum_kernel(const float* __restrict__ G, int rows_total, int m1, float* __restrict__ out) {
+// row sums of G [B, n+1, m+1]: one warp per row (a padded batch: over the pair's m_b + 1 columns, len_m set)
+__global__ void __launch_bounds__(256) sinkb_rowsum_kernel(const float* __restrict__ G, int rows_total, int m1_cap, int n1,
+                                                           const int* __restrict__ len_m, float* __restrict__ out) {
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= rows_total) return;
-  const float* g = G + (int64_t)row * m1;
+  const float* g = G + (int64_t)row * m1_cap;
+  const int m1 = len_m ? padded_length(len_m, row / n1, m1_cap - 1) + 1 : m1_cap;
   float s = 0.f;
   for (int j = lane; j < m1; j += 32) s += __ldg(g + j);
   s = warp_sum(s);
@@ -150,10 +156,12 @@ __global__ void __launch_bounds__(256) sinkb_rowsum_kernel(const float* __restri
 }
 // column sums of G, two deterministic stages: strips of 64 rows -> partial [B][RS][m+1] -> out [B][m+1]
 constexpr int SINKB_RS_ROWS = 64;
-__global__ void __launch_bounds__(256) sinkb_colsum_kernel(const float* __restrict__ G, int n1, int m1, float* __restrict__ partial) {
+__global__ void __launch_bounds__(256) sinkb_colsum_kernel(const float* __restrict__ G, int n1, int m1, const int* __restrict__ len_n,
+                                                           float* __restrict__ partial) {
   const int b = blockIdx.z, rs = blockIdx.y, j = blockIdx.x * 256 + threadIdx.x;
   if (j >= m1) return;
-  const int i0 = rs * SINKB_RS_ROWS, i1 = min(i0 + SINKB_RS_ROWS, n1);
+  const int i0 = rs * SINKB_RS_ROWS;
+  const int i1 = min(i0 + SINKB_RS_ROWS, len_n ? padded_length(len_n, b, n1 - 1) + 1 : n1);
   const float* g = G + ((int64_t)b * n1 + i0) * m1 + j;
   float s = 0.f;
   for (int i = i0; i < i1; ++i, g += m1) s += __ldg(g);
@@ -171,7 +179,8 @@ __global__ void __launch_bounds__(256) sinkb_colsum_finish_kernel(const float* _
 constexpr int SINKB_TR = 64, SINKB_TC = 128;
 __global__ void __launch_bounds__(256) sinkb_dz_kernel(SinkBwdArgs a, const float* __restrict__ G, float* __restrict__ dZ, float inv_reg) {
   const int b = blockIdx.z;
-  const int n = a.n, m = a.m, T = a.iters;
+  const int n = padded_length(a.len_n, b, a.n), m = padded_length(a.len_m, b, a.m), T = a.iters;
+  const int64_t n1 = a.n + 1, m1 = a.m + 1;                  // capacity strides (a padded pair's block is [n + 1, m + 1] of it)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i0 = blockIdx.y * SINKB_TR + warp * 8;            // my 8 rows
   const int j0 = blockIdx.x * SINKB_TC + lane * 4;            // my 4 columns
@@ -194,9 +203,9 @@ __global__ void __launch_bounds__(256) sinkb_dz_kernel(SinkBwdArgs a, const floa
     }
   }
   for (int it = 0; it < T; ++it) {
-    const float* ut = a.hist_u + ((int64_t)b * T + it) * (n + 1);
-    const float* cf = a.hist_coef + ((int64_t)b * T + it) * (n + 1);
-    const int64_t co = ((int64_t)b * T + it) * (m + 1);
+    const float* ut = a.hist_u + ((int64_t)b * T + it) * n1;
+    const float* cf = a.hist_coef + ((int64_t)b * T + it) * n1;
+    const int64_t co = ((int64_t)b * T + it) * m1;
     float cv[4], vb[4], wq[4];
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -220,25 +229,28 @@ __global__ void __launch_bounds__(256) sinkb_dz_kernel(SinkBwdArgs a, const floa
 #pragma unroll
   for (int r = 0; r < 8; ++r) {
     const int i = i0 + r;
-    if (i > n) continue;
+    if (i > a.n) continue;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       const int j = j0 + c;
-      if (j > m) continue;
-      const int64_t o = ((int64_t)b * (n + 1) + i) * (m + 1) + j;
-      dZ[o] = (__ldg(G + o) - acc[r][c]) * inv_reg;
+      if (j > a.m) continue;
+      const int64_t o = ((int64_t)b * n1 + i) * m1 + j;
+      dZ[o] = (i <= n && j <= m) ? (__ldg(G + o) - acc[r][c]) * inv_reg : 0.f;     // 0 outside a padded pair's block
     }
   }
 }
-// d loss / d dustbin = sum of dZ's last row and last column (the corner once): one CTA per pair, fixed order, then pairs in order
-__global__ void __launch_bounds__(256) sinkb_dustbin_kernel(const float* __restrict__ dZ, int B, int n, int m, float* __restrict__ per_pair,
-                                                            unsigned int* counter, float* __restrict__ out) {
+// d loss / d dustbin = sum of dZ's last row and last column (the corner once): one CTA per pair, fixed order, then pairs in order.
+// A padded pair (lens set) sums its own dustbin row n_b and column m_b.
+__global__ void __launch_bounds__(256) sinkb_dustbin_kernel(const float* __restrict__ dZ, int B, int n_cap, int m_cap, const int* __restrict__ lens,
+                                                            float* __restrict__ per_pair, unsigned int* counter, float* __restrict__ out) {
   __shared__ float red[8];
   const int b = blockIdx.x;
-  const float* d = dZ + (int64_t)b * (n + 1) * (m + 1);
+  const int64_t ld = m_cap + 1;
+  const int n = lens ? padded_length(lens, b, n_cap) : n_cap, m = lens ? padded_length(lens + B, b, m_cap) : m_cap;
+  const float* d = dZ + (int64_t)b * (n_cap + 1) * ld;
   float s = 0.f;
-  for (int j = threadIdx.x; j <= m; j += 256) s += d[(int64_t)n * (m + 1) + j];
-  for (int i = threadIdx.x; i < n; i += 256) s += d[(int64_t)i * (m + 1) + m];
+  for (int j = threadIdx.x; j <= m; j += 256) s += d[(int64_t)n * ld + j];
+  for (int i = threadIdx.x; i < n; i += 256) s += d[(int64_t)i * ld + m];
   const float t = cta_sum<256>(s, red);
   if (threadIdx.x == 0) {
     per_pair[b] = t;
@@ -264,11 +276,14 @@ inline int64_t sinkhorn_bwd_workspace_bytes(int B, int n, int m, int T) {
 // G = d loss / d scores [B, n+1, m+1] (dense) -> dZ = d loss / d S_aug [B, n+1, m+1], ddustbin [1]
 inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, const float* dustbin, int B, int n, int m, int iters, float reg,
                                const float* hist, const float* G, float* dZ, float* ddustbin, void* ws, int64_t ws_bytes,
-                               cudaStream_t stream) {
+                               cudaStream_t stream, const int* lens = nullptr) {
   SinkPlan p;
   if (const int rc = sinkhorn_plan(true, B, n, m, &p)) return rc;
   if (ws_bytes < sinkhorn_bwd_workspace_bytes(B, n, m, iters)) return fail(OG_EWORKSPACE, "sinkhorn_bwd: workspace too small");
   if (const int rc = sinkhorn_check_rows("sinkhorn_bwd", S, lds, strideS, m)) return rc;
+  if (lens && n > SINK_MAX_ROWS) return fail(OG_EUNSUPPORTED, "sinkhorn_bwd: a padded batch has at most %d rows, not %d", SINK_MAX_ROWS, n);
+  if (lens)
+    if (const int rc = sinkhorn_log_tables(stream)) return rc;
   const int T = iters;
   const int64_t nrs = cdiv(n + 1, SINKB_RS_ROWS);
   char* w = static_cast<char*>(ws);
@@ -288,8 +303,10 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   const SinkConsts k = sinkhorn_consts(n, m);
   const int m1 = m + 1, n1 = n + 1;
   int rc;
-  if ((rc = OG_LAUNCH(sinkb_rowsum_kernel, cdiv(B * n1, 8), 256, 0, stream, G, B * n1, m1, ubar_init))) return rc;
-  if ((rc = OG_LAUNCH(sinkb_colsum_kernel, dim3(cdiv(m1, 256), (unsigned)nrs, B), 256, 0, stream, G, n1, m1, colpart))) return rc;
+  const int* len_n = lens;
+  const int* len_m = lens ? lens + B : nullptr;
+  if ((rc = OG_LAUNCH(sinkb_rowsum_kernel, cdiv(B * n1, 8), 256, 0, stream, G, B * n1, m1, n1, len_m, ubar_init))) return rc;
+  if ((rc = OG_LAUNCH(sinkb_colsum_kernel, dim3(cdiv(m1, 256), (unsigned)nrs, B), 256, 0, stream, G, n1, m1, len_n, colpart))) return rc;
   if ((rc = OG_LAUNCH(sinkb_colsum_finish_kernel, dim3(cdiv(m1, 256), B), 256, 0, stream, colpart, (int)nrs, m1, vbar_init))) return rc;
   SinkBwdArgs a;
   a.S = S; a.lds = lds; a.strideS = strideS; a.dustbin = dustbin; a.B = B; a.n = n; a.m = m; a.iters = T; a.reg = reg;
@@ -298,6 +315,7 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   a.ubar_init = ubar_init; a.vbar_init = vbar_init;
   a.hist_coef = hist_coef; a.hist_cvec = hist_cvec; a.hist_vbar = hist_vbar; a.hist_wq = hist_wq;
   a.partial = partial; a.barrier = barrier; a.SP = p.SP; a.rows_per_strip = p.rows_per_strip; a.mpad = p.mpad;
+  a.len_n = len_n; a.len_m = len_m;
   if (T > 0) {
     rc = sinkhorn_for_each_launch(p, B, barrier, stream, [&](int b0, int nb) {
       SinkBwdArgs g = a;
@@ -307,6 +325,7 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
       g.ubar_init = ubar_init + (int64_t)b0 * n1; g.vbar_init = vbar_init + (int64_t)b0 * m1;
       g.hist_coef = hist_coef + (int64_t)b0 * T * n1; g.hist_cvec = hist_cvec + (int64_t)b0 * T * m1;
       g.hist_vbar = hist_vbar + (int64_t)b0 * T * m1; g.hist_wq = hist_wq + (int64_t)b0 * T * m1;
+      g.len_n = lens ? len_n + b0 : nullptr; g.len_m = lens ? len_m + b0 : nullptr;
       if (p.V == 4 && p.W == 1) return sinkhorn_coop_launch<sinkhorn_bwd_kernel<4, 1, 2>, 4, 1, 2>(g, p, stream);
       if (p.V == 4)             return sinkhorn_coop_launch<sinkhorn_bwd_kernel<4, 2, 2>, 4, 2, 2>(g, p, stream);
       if (p.V == 8)             return sinkhorn_coop_launch<sinkhorn_bwd_kernel<8, 2, 2>, 8, 2, 2>(g, p, stream);
@@ -317,7 +336,7 @@ inline int sinkhorn_bwd_launch(const float* S, int64_t lds, int64_t strideS, con
   }
   if ((rc = OG_LAUNCH(sinkb_dz_kernel, dim3(cdiv(m1, SINKB_TC), cdiv(n1, SINKB_TR), B), 256, 0, stream, a, G, dZ, 1.f / reg))) return rc;
   OG_CUDA(cudaMemsetAsync(counter, 0, 4, stream));
-  return OG_LAUNCH(sinkb_dustbin_kernel, B, 256, 0, stream, dZ, B, n, m, per_pair, counter, ddustbin);
+  return OG_LAUNCH(sinkb_dustbin_kernel, B, 256, 0, stream, dZ, B, n, m, lens, per_pair, counter, ddustbin);
 }
 
 }  // namespace og

@@ -62,6 +62,8 @@ inline int transpose_launch(const float* in, int64_t ld_in, int64_t stride_in, f
 //   MODE 1  mean     o0 = mean relu?(x)                                                 BN statistics, pass 1
 //   MODE 2  var      o0 = mean (relu?(x) - mu[c])^2                                     BN statistics, pass 2
 //   MODE 3  bn-bwd   o0 = sum dy,  o1 = sum dy xhat,  xhat = (relu?(a) - mu) invstd     d beta, d gamma
+// A padded batch (len set) reduces over the real rows only: row r is slot r % cap of pair r / cap, real below len[r / cap], and the
+// means divide by their count, sum_b len[b].
 struct ColReduceArgs {
   const float* x; int64_t ldx;         // MODE 3: dy
   const float* y; int64_t ldy;         // MODE 0: optional factor; MODE 3: a (pre-activation)
@@ -71,8 +73,20 @@ struct ColReduceArgs {
   float* partial;                      // [chunks][2][cols]
   float* out0; float* out1;
   int chunks, rows_per_chunk;
+  const int* len; int cap;             // padded batch (null otherwise): per-pair lengths [rows / cap], clamped into [1, cap]
 };
 constexpr int COLRED_MAX_CHUNKS = 256;
+
+// rows a padded reduction counts: sum_b len[b] (rows when len is null)
+__device__ __forceinline__ int padded_count(const int* len, int rows, int cap) {
+  if (!len) return rows;
+  int t = 0;
+  for (int b = 0; b < rows / cap; ++b) t += padded_length(len, b, cap);
+  return t;
+}
+__device__ __forceinline__ bool padded_real(const int* len, int r, int cap) {
+  return !len || r % cap < padded_length(len, r / cap, cap);
+}
 
 template <int MODE>
 __global__ void __launch_bounds__(256) colreduce_stage1(ColReduceArgs a) {
@@ -86,6 +100,7 @@ __global__ void __launch_bounds__(256) colreduce_stage1(ColReduceArgs a) {
     if (MODE == 2 || MODE == 3) mu = __ldg(a.mu + c);
     if (MODE == 3) is = __ldg(a.invstd + c);
     for (int r = rb + ty; r < re; r += 4) {
+      if (a.len && !padded_real(a.len, r, a.cap)) continue;
       float v = a.x[(int64_t)r * a.ldx + c];
       if (MODE == 0) {
         if (a.y) { float f = a.y[(int64_t)r * a.ldy + c]; if (a.z) f -= a.z[(int64_t)r * a.ldz + c]; v *= f; }
@@ -122,7 +137,7 @@ __global__ void __launch_bounds__(256) colreduce_stage2(ColReduceArgs a) {
     t0 += a.partial[(int64_t)k * 2 * a.cols + c];
     if (MODE == 3) t1 += a.partial[(int64_t)k * 2 * a.cols + a.cols + c];
   }
-  if (MODE == 1 || MODE == 2) t0 = __fdiv_rn(t0, (float)a.rows);
+  if (MODE == 1 || MODE == 2) t0 = __fdiv_rn(t0, (float)padded_count(a.len, a.rows, a.cap));
   a.out0[c] = t0;
   if (MODE == 3) a.out1[c] = t1;
 }
@@ -141,12 +156,14 @@ inline int colreduce_launch(ColReduceArgs a, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------------------------------
 // BatchNorm1d with batch statistics (torch.nn.functional.batch_norm, training=True): y = gamma (r - mu) / sqrt(var + eps) + beta,
 // r = relu(a) when the ReLU in front of the norm is fused in; var is the biased variance; the running statistics move by
-// `momentum` towards (mu, unbiased var).
-__global__ void __launch_bounds__(256) bn_finish_stats_kernel(const float* __restrict__ mean, const float* __restrict__ var, int cols, int rows,
-                                                              float eps, float momentum, float* __restrict__ invstd,
-                                                              float* __restrict__ running_mean, float* __restrict__ running_var) {
+// `momentum` towards (mu, unbiased var).  A padded batch (len set) counts its real rows, sum_b len[b] (ColReduceArgs).
+__global__ void __launch_bounds__(256) bn_finish_stats_kernel(const float* __restrict__ mean, const float* __restrict__ var, int cols, int rows_all,
+                                                              const int* __restrict__ len, int cap, float eps, float momentum,
+                                                              float* __restrict__ invstd, float* __restrict__ running_mean,
+                                                              float* __restrict__ running_var) {
   const int c = blockIdx.x * 256 + threadIdx.x;
   if (c >= cols) return;
+  const int rows = padded_count(len, rows_all, cap);
   const float v = var[c];
   invstd[c] = __fdiv_rn(1.f, __fsqrt_rn(v + eps));
   if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean[c];
@@ -167,16 +184,17 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__
     y[(int64_t)r * ldy + c] = fmaf((v - mean[c]) * invstd[c], gamma[c], beta[c]);
   }
 }
-// da = [a > 0] gamma invstd (dy - dbeta / n - xhat dgamma / n)
+// da = [a > 0] gamma invstd (dy - dbeta / n - xhat dgamma / n);  a padded batch (len set): n = sum_b len[b], da = 0 on its padding rows
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float* __restrict__ dy, int64_t lddy, const float* __restrict__ a, int64_t lda,
                                                            int rows, int cols, int relu, const float* __restrict__ mean,
                                                            const float* __restrict__ invstd, const float* __restrict__ gamma,
                                                            const float* __restrict__ dgamma, const float* __restrict__ dbeta,
-                                                           float* __restrict__ da, int64_t ldda) {
+                                                           float* __restrict__ da, int64_t ldda, const int* __restrict__ len, int cap) {
   const int64_t n = (int64_t)rows * cols;
-  const float inv_n = __fdiv_rn(1.f, (float)rows);
+  const float inv_n = __fdiv_rn(1.f, (float)padded_count(len, rows, cap));
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) {
     const int r = (int)(i / cols), c = (int)(i % cols);
+    if (len && !padded_real(len, r, cap)) { da[(int64_t)r * ldda + c] = 0.f; continue; }
     const float pre = a[(int64_t)r * lda + c];
     const float act = relu ? fmaxf(pre, 0.f) : pre;
     const float xhat = (act - mean[c]) * invstd[c];
@@ -189,12 +207,19 @@ inline unsigned eltwise_grid(int64_t n) { return (unsigned)std::min<int64_t>((n 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // row softmax of a materialised [rows, cols] matrix (in place) and its backward  dS = scale P (dP - sum_j P dP)  (in place of dP).
-// One warp per row.
-__global__ void __launch_bounds__(256) softmax_rows_kernel(float* __restrict__ S, int64_t ld, int64_t rows, int cols) {
+// One warp per row.  Padded keys (len set): row r belongs to sequence r / seq_rows, whose first len[r / seq_rows] columns are its
+// keys; P = 0 and dS = 0 over the other columns of the capacity `cols`.
+__device__ __forceinline__ int softmax_row_cols(const int* len, int64_t row, int64_t seq_rows, int cols) {
+  return len ? padded_length(len, (int)(row / seq_rows), cols) : cols;
+}
+__global__ void __launch_bounds__(256) softmax_rows_kernel(float* __restrict__ S, int64_t ld, int64_t rows, int cols_all,
+                                                           const int* __restrict__ len, int64_t seq_rows) {
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
   float* s = S + row * ld;
+  const int cols = softmax_row_cols(len, row, seq_rows, cols_all);
+  for (int j = cols + lane; j < cols_all; j += 32) s[j] = 0.f;
   float mx = -CUDART_INF_F;
   for (int j = lane; j < cols; j += 32) mx = fmaxf(mx, s[j]);
   mx = warp_max(mx);
@@ -204,13 +229,15 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(float* __restrict__ S
   const float inv = __fdiv_rn(1.f, sum);
   for (int j = lane; j < cols; j += 32) s[j] *= inv;
 }
-__global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __restrict__ P, float* __restrict__ dP, int64_t ld, int64_t rows, int cols,
-                                                               float scale) {
+__global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __restrict__ P, float* __restrict__ dP, int64_t ld, int64_t rows,
+                                                               int cols_all, float scale, const int* __restrict__ len, int64_t seq_rows) {
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
   const float* p = P + row * ld;
   float* g = dP + row * ld;
+  const int cols = softmax_row_cols(len, row, seq_rows, cols_all);
+  for (int j = cols + lane; j < cols_all; j += 32) g[j] = 0.f;
   float dot = 0.f;
   for (int j = lane; j < cols; j += 32) dot = fmaf(p[j], g[j], dot);
   dot = warp_sum(dot);

@@ -14,6 +14,7 @@ from typing import Any, Dict, Optional, Tuple
 import torch
 
 from . import _cabi
+from .superglue import is_padded, padded_lengths
 
 UNMATCHED_INDEX = -1      # reference models/gt_matches_generation.py:13
 IGNORE_INDEX = -2         # reference models/gt_matches_generation.py:14
@@ -25,8 +26,11 @@ def _f32(t: torch.Tensor, dev: torch.device) -> torch.Tensor:
     return t.detach().to(device=dev, dtype=torch.float32).contiguous()
 
 
-def gt_matches(kpts0: torch.Tensor, kpts1: torch.Tensor, transformation: Dict[str, Any]) -> Tuple[torch.Tensor, torch.Tensor]:
-    """-> (gt_matches0 [B, N] int64, gt_matches1 [B, M] int64) on the keypoints' (CUDA) device."""
+def gt_matches(kpts0: torch.Tensor, kpts1: torch.Tensor, transformation: Dict[str, Any],
+               lengths: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """-> (gt_matches0 [B, N] int64, gt_matches1 [B, M] int64) on the keypoints' (CUDA) device.  ``lengths`` (padded batch,
+    int32 [2B] on the device: n_0 .. n_{B-1}, m_0 .. m_{B-1}): pair b's labels come from its first n_b / m_b keypoints alone and
+    are ``IGNORE_INDEX`` past them."""
     dev = kpts0.device
     if dev.type != 'cuda':
         raise RuntimeError('openglue_b200.gt_matches needs CUDA tensors (sm_90a); there is no CPU path')
@@ -70,10 +74,16 @@ def gt_matches(kpts0: torch.Tensor, kpts1: torch.Tensor, transformation: Dict[st
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         gt0 = torch.empty(B, n, dtype=torch.int64, device=dev)
         gt1 = torch.empty(B, m, dtype=torch.int64, device=dev)
-        rc = lib.og_gt_matches_fwd(_cabi.ptr(k0), _cabi.ptr(k1), B, n, m, C.byref(tf), _cabi.ptr(gt0), _cabi.ptr(gt1), _cabi.ptr(ws), ws_bytes,
-                                   _cabi.stream(dev))
-        _cabi.check(rc, 'og_gt_matches_fwd')
-        for t in keep + [k0, k1, ws]:                      # the kernels are only enqueued: keep their inputs alive on this stream
+        if lengths is not None:
+            rc = lib.og_gt_matches_fwd_padded(_cabi.ptr(k0), _cabi.ptr(k1), B, n, m, _cabi.ptr(lengths), C.byref(tf), _cabi.ptr(gt0),
+                                              _cabi.ptr(gt1), _cabi.ptr(ws), ws_bytes, _cabi.stream(dev))
+            _cabi.check(rc, 'og_gt_matches_fwd_padded')
+        else:
+            rc = lib.og_gt_matches_fwd(_cabi.ptr(k0), _cabi.ptr(k1), B, n, m, C.byref(tf), _cabi.ptr(gt0), _cabi.ptr(gt1), _cabi.ptr(ws),
+                                       ws_bytes, _cabi.stream(dev))
+            _cabi.check(rc, 'og_gt_matches_fwd')
+        # the kernels are only enqueued: keep their inputs alive on this stream
+        for t in keep + [k0, k1, ws] + ([lengths] if lengths is not None else []):
             t.record_stream(torch.cuda.current_stream(dev))
     return gt0, gt1
 
@@ -81,13 +91,20 @@ def gt_matches(kpts0: torch.Tensor, kpts1: torch.Tensor, transformation: Dict[st
 def generate_gt_matches(data: Dict[str, Any], features0: Dict[str, torch.Tensor], features1: Dict[str, torch.Tensor],
                         positive_threshold: float, negative_threshold: Optional[float] = None
                         ) -> Tuple[Optional[Dict[str, Any]], Optional[Dict[str, torch.Tensor]]]:
-    """Same contract as the reference function (models/gt_matches_generation.py:17-93)."""
+    """Same contract as the reference function (models/gt_matches_generation.py:17-93).  A padded batch (``data`` with
+    ``num_keypoints0`` / ``num_keypoints1``) labels each pair from its own keypoints, and ``y_true`` carries the lengths on to
+    :func:`~openglue_b200.criterion`."""
     kpts0, kpts1 = features0['keypoints'], features1['keypoints']
     if kpts0.size(1) == 0 or kpts1.size(1) == 0:           # reference :33-35
         return None, None
-    gt0, gt1 = gt_matches(kpts0, kpts1, data['transformation'])
+    lengths, y_len = None, {}
+    if is_padded(data):
+        y_len = padded_lengths(data, kpts0.shape[0], kpts0.shape[1], kpts1.shape[1])
+        lengths = torch.cat([y_len['num_keypoints0'].to(kpts0.device), y_len['num_keypoints1'].to(kpts0.device)]).contiguous()
+        y_len = {k: data[k] for k in y_len}
+    gt0, gt1 = gt_matches(kpts0, kpts1, data['transformation'], lengths)
     data = {**data,
             'keypoints0': kpts0, 'keypoints1': kpts1,
             'local_descriptors0': features0['local_descriptors'], 'local_descriptors1': features1['local_descriptors'],
             'side_info0': features0['side_info'], 'side_info1': features1['side_info']}
-    return data, {'gt_matches0': gt0, 'gt_matches1': gt1}
+    return data, {'gt_matches0': gt0, 'gt_matches1': gt1, **y_len}

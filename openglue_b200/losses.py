@@ -17,6 +17,7 @@ import torch
 
 from . import _cabi
 from ._cabi import ptr, stream
+from .superglue import is_padded, padded_lengths
 
 __all__ = ['criterion', 'criterion_with_grad', 'metric_loss_with_grad']
 
@@ -32,12 +33,21 @@ def _run(y_true: Dict[str, torch.Tensor], y_pred: Dict[str, torch.Tensor], want_
     gt1 = y_true['gt_matches1'].to(device=dev, dtype=torch.int64).contiguous()
     if gt0.shape != (B, n1 - 1) or gt1.shape != (B, m1 - 1):
         raise ValueError(f'gt_matches shapes {tuple(gt0.shape)}, {tuple(gt1.shape)} do not fit scores {tuple(scores.shape)}')
+    lens = None
+    if is_padded(y_true):                                  # each pair's loss on its own block, dustbins at its lengths
+        ln = padded_lengths(y_true, B, n1 - 1, m1 - 1)
+        lens = torch.cat([ln['num_keypoints0'].to(dev), ln['num_keypoints1'].to(dev)]).contiguous()
     lib = _cabi.lib()
     with torch.cuda.device(dev):
         wsb = _cabi.check_size(lib.og_criterion_workspace_bytes(B), 'og_criterion_workspace_bytes')
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         loss = torch.empty(2, dtype=torch.float32, device=dev)
         dscores = torch.zeros_like(scores) if want_grad else None
+        if lens is not None:
+            rc = lib.og_criterion_fwd_padded(ptr(scores), ptr(gt0), ptr(gt1), B, n1 - 1, m1 - 1, ptr(lens), ptr(loss), ptr(dscores),
+                                             float(grad_scale), ptr(ws), wsb, stream(dev))
+            _cabi.check(rc, 'og_criterion_fwd_padded')
+            return loss, dscores
         rc = lib.og_criterion_fwd(ptr(scores), ptr(gt0), ptr(gt1), B, n1 - 1, m1 - 1, ptr(loss), ptr(dscores), float(grad_scale), ptr(ws), wsb,
                                   stream(dev))
         _cabi.check(rc, 'og_criterion_fwd')
@@ -48,8 +58,8 @@ class _Criterion(torch.autograd.Function):
     """loss = criterion(scores): the same kernel call also writes d loss / d scores, which the backward pass scales."""
 
     @staticmethod
-    def forward(ctx, scores, gt0, gt1):
-        loss, dscores = _run({'gt_matches0': gt0, 'gt_matches1': gt1}, {'scores': scores}, True, 1.0)
+    def forward(ctx, scores, y_true):
+        loss, dscores = _run(y_true, {'scores': scores}, True, 1.0)
         ctx.save_for_backward(dscores)
         ctx.dtype = scores.dtype
         return loss
@@ -57,7 +67,7 @@ class _Criterion(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gloss):
         dscores, = ctx.saved_tensors
-        return (dscores * gloss[0]).to(ctx.dtype), None, None          # metric_loss (loss[1]) is identically 0
+        return (dscores * gloss[0]).to(ctx.dtype), None                # metric_loss (loss[1]) is identically 0
 
 
 def _metric_run(gt0: torch.Tensor, gt1: torch.Tensor, c0: torch.Tensor, c1: torch.Tensor, margin: float, want_grad: bool,
@@ -134,7 +144,13 @@ def criterion(y_true: Dict[str, torch.Tensor], y_pred: Dict[str, torch.Tensor], 
     """reference utils/losses.py:7-99 -> {'loss', 'metric_loss'} (0-dim tensors on the scores' device).  Differentiable
     with respect to ``y_pred['scores']`` (the sparse scatter the gather's backward pass is) and, with a margin, to
     ``y_pred['context_descriptors0/1']``, so ``(nll_weight * out['loss'] + metric_weight * out['metric_loss']).backward()``
-    drives the training step as it does in the reference (matching_module.py:101-105)."""
+    drives the training step as it does in the reference (matching_module.py:101-105).
+
+    A padded batch (``y_true`` with ``num_keypoints0`` / ``num_keypoints1``, as :func:`generate_gt_matches` returns it) takes
+    each pair's loss on its own block of ``scores`` (dustbins at its lengths), ignores its labels past them and averages the B
+    pairs; ``d loss / d scores`` is 0 outside the blocks.  The metric terms (``margin``) are not built for padded batches."""
+    if margin is not None and is_padded(y_true):
+        raise NotImplementedError('criterion(margin=...) on a padded batch (num_keypoints0 / num_keypoints1) is not built')
     if margin is not None:
         gt0, gt1, c0, c1 = _metric_inputs(y_true, y_pred)
         scores = y_pred['scores']
@@ -145,7 +161,7 @@ def criterion(y_true: Dict[str, torch.Tensor], y_pred: Dict[str, torch.Tensor], 
             _metric_run(gt0, gt1, _f32(c0), _f32(c1), float(margin), False, 1.0, out=loss[1:])
         return {'loss': loss[0], 'metric_loss': loss[1]}
     if torch.is_grad_enabled() and y_pred['scores'].requires_grad:
-        loss = _Criterion.apply(y_pred['scores'], y_true['gt_matches0'], y_true['gt_matches1'])
+        loss = _Criterion.apply(y_pred['scores'], y_true)
     else:
         loss, _ = _run(y_true, y_pred, False, 1.0)
     return {'loss': loss[0], 'metric_loss': loss[1]}

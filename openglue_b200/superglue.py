@@ -21,7 +21,7 @@ from . import _cabi
 from ._cabi import ptr, stream
 from .packing import pack_weights
 
-__all__ = ['SuperGlue', 'MatchingCore', 'PendingMatches', 'is_padded', 'padded_inputs']
+__all__ = ['SuperGlue', 'MatchingCore', 'PendingMatches', 'is_padded', 'padded_inputs', 'padded_lengths']
 
 # Counts (re)registrations of parameters, buffers and submodules on any module: ``conv.weight = nn.Parameter(...)`` or
 # ``bn.running_mean = t`` replaces a tensor object, which a cached list of a SuperGlue's tensors would not see.
@@ -44,10 +44,9 @@ def is_padded(data: dict) -> bool:
     return 'num_keypoints0' in data or 'num_keypoints1' in data
 
 
-def padded_inputs(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]:
-    """A padded batch's per-pair inputs, where the caller keeps them: ``num_keypoints0`` / ``num_keypoints1`` as int32 [B] and
-    ``image0_size`` / ``image1_size`` as float32 [B, 2] (W, H) per pair (a batch-wide size, or the image tensors' own, broadcast).
-    Host lengths are checked against the capacities n, m; device lengths are not (the kernels clamp them into range)."""
+def padded_lengths(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]:
+    """``num_keypoints0`` / ``num_keypoints1`` of a padded batch as int32 [B], where the caller keeps them.  Host lengths are
+    checked against the capacities n, m; device lengths are not (the kernels clamp them into range)."""
     if 'num_keypoints0' not in data or 'num_keypoints1' not in data:
         raise ValueError('a padded batch needs both num_keypoints0 and num_keypoints1')
     out = {}
@@ -61,6 +60,15 @@ def padded_inputs(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]
             if lo < 1 or hi > cap:
                 raise ValueError(f'num_keypoints{idx} must lie in [1, {cap}] (the capacity), got values in [{lo}, {hi}]')
         out[f'num_keypoints{idx}'] = t.to(torch.int32)
+    return out
+
+
+def padded_inputs(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]:
+    """A padded batch's per-pair inputs, where the caller keeps them: ``num_keypoints0`` / ``num_keypoints1`` as int32 [B]
+    (:func:`padded_lengths`) and ``image0_size`` / ``image1_size`` as float32 [B, 2] (W, H) per pair (a batch-wide size, or the
+    image tensors' own, broadcast)."""
+    out = padded_lengths(data, B, n, m)
+    for idx in (0, 1):
         size = data.get(f'image{idx}_size')
         if 'image0' in data and 'image1' in data:
             size = None
@@ -72,6 +80,13 @@ def padded_inputs(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]
             w, h = SuperGlue._image_wh(data, idx)
             out[f'image{idx}_size'] = torch.tensor([[w, h]], dtype=torch.float32).expand(B, 2)
     return out
+
+
+# The autograd drop-in's outputs feed losses written against the reference layout, which read every pair's dustbins at
+# scores[:, -1, :] / scores[:, :, -1]: wrong for a padded pair, whose dustbins sit at its own lengths.
+_TRAIN_PADDED_MSG = ('openglue_b200: SuperGlue.forward / run take padded batches (num_keypoints0 / num_keypoints1) in eval mode only. '
+                     'To train on a padded batch use openglue_b200.training.GraphedTrainStep or TrainStep with openglue_b200.criterion, whose '
+                     "loss reads each pair's own dustbin row and column")
 
 
 def _feed_forward_params(*sizes: int) -> nn.Sequential:
@@ -250,8 +265,7 @@ class SuperGlue(nn.Module):
         matches -1 and matching scores 0 past the lengths; context-descriptor columns past them 0."""
         padded = is_padded(data)
         if self.training and padded:
-            raise NotImplementedError('openglue_b200: padded batches (num_keypoints0 / num_keypoints1) run in eval mode only: the '
-                                      'inference forward pass, match extraction and MatchingCore are built for them, training is not')
+            raise NotImplementedError(_TRAIN_PADDED_MSG)
         if self.training:
             raise RuntimeError('openglue_b200.SuperGlue.run is the fused eval-mode path; in train() mode call forward() '
                                '(openglue_b200.training: batch-statistics BatchNorm + the explicit backward pass)')
@@ -339,9 +353,7 @@ class SuperGlue(nn.Module):
         (BatchNorm uses batch statistics and updates its running buffers, as the reference module does in training_step)."""
         if self.training:
             if is_padded(data):
-                raise NotImplementedError('openglue_b200: padded batches (num_keypoints0 / num_keypoints1) run in eval mode only: '
-                                          'the inference forward pass, match extraction and MatchingCore are built for them, '
-                                          'training is not')
+                raise NotImplementedError(_TRAIN_PADDED_MSG)
             from .training import train_forward
             return train_forward(self, data)
         return self.run(data, want_matches=False)

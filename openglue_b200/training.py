@@ -12,6 +12,11 @@ to the ``nn.Parameter`` objects (``_TrainFunction``).  There is no CPU path.
 Layout: every activation is row-major ``[rows, channels]`` with ``rows = batch x keypoints`` of ONE image - the reference's
 ``[B, C, N]`` tensors transposed; BatchNorm statistics therefore run over the rows of one call, exactly the reference's
 per-call ``(B, N)`` statistics (attention_gnn.py:58-77 calls the shared module once per image).
+
+Padded batches (``num_keypoints0`` / ``num_keypoints1`` in ``data``, as for inference): pair b owns rows [0, n_b) / [0, m_b) of
+the capacities N, M.  Attention, Sinkhorn and the loss run on each pair alone; BatchNorm pools the real rows of every pair in
+the call (mean and biased variance over sum_b n_b rows).  Local descriptors are read through a copy with the padding zeroed, so
+the padding's contents never reach a result, and every gradient at a padding row is 0.
 """
 from __future__ import annotations
 
@@ -21,6 +26,7 @@ import torch
 
 from . import _cabi
 from ._ops import _Ops, _pad4  # noqa: F401  (tests build their torch double of the kernels on _Ops' composite helpers)
+from .superglue import is_padded, padded_inputs
 
 __all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep']
 
@@ -28,8 +34,9 @@ __all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep']
 class _BN:
     """One BatchNorm1d call site: parameters, running buffers and what the backward pass needs."""
 
-    def __init__(self, mod: torch.nn.BatchNorm1d):
+    def __init__(self, mod: torch.nn.BatchNorm1d, lens: Optional[torch.Tensor] = None):
         self.mod = mod
+        self.pk = {} if lens is None else {'lens': lens}           # padded batch: statistics over the real rows of every pair
 
     def forward(self, ops: _Ops, a: torch.Tensor) -> torch.Tensor:
         m = self.mod
@@ -38,19 +45,24 @@ class _BN:
             raise NotImplementedError('BatchNorm1d(momentum=None) (cumulative average) is not built')
         track = m.track_running_stats and m.running_mean is not None
         y, self.mean, self.invstd = ops.bn_fwd(a, m.weight, m.bias, m.eps, m.momentum, m.running_mean if track else None,
-                                               m.running_var if track else None)
+                                               m.running_var if track else None, **self.pk)
         if track:
             m.num_batches_tracked += 1
         return y
 
     def backward(self, ops: _Ops, dy: torch.Tensor):
-        return ops.bn_bwd(dy, self.a, self.mod.weight, self.mean, self.invstd)
+        return ops.bn_bwd(dy, self.a, self.mod.weight, self.mean, self.invstd, **self.pk)
 
 
 class TrainStep:
     """One training-mode forward pass of ``model`` (an ``openglue_b200.SuperGlue`` in ``train()`` mode) with everything its
     backward pass needs.  ``forward()`` -> (scores [B,N+1,M+1], ctx0 [B,d,N], ctx1 [B,d,M]); ``backward(dscores, dctx0, dctx1)`` ->
-    ``{parameter name: gradient}`` (+ ``'local_descriptors0/1'``)."""
+    ``{parameter name: gradient}`` (+ ``'local_descriptors0/1'``).
+
+    A padded batch (``num_keypoints0`` / ``num_keypoints1``, per-pair ``image0_size`` / ``image1_size`` optional, validated by
+    :func:`~openglue_b200.superglue.padded_inputs`) gives each pair's outputs on its own block: ``scores[b, :n_b+1, :m_b+1]``
+    (dustbins at n_b, m_b) and ``-inf`` elsewhere, context descriptors 0 past the lengths.  ``backward`` reads ``dscores`` on
+    those blocks and ``dctx`` on the real columns only; the local-descriptor gradients are 0 on the padding rows."""
 
     def __init__(self, model, data: dict, ops=None):
         model._check_head_dim()                         # before the forward pass moves any BatchNorm running buffer
@@ -82,8 +94,28 @@ class TrainStep:
         self.N = [self.kpts[0].shape[1], self.kpts[1].shape[1]]
         if min(self.N) == 0:
             raise ValueError('empty keypoint set')
-        self.wh = [model._image_wh(data, 0), model._image_wh(data, 1)]
+        self.padded = is_padded(data)
+        self.lens = None
+        if self.padded:
+            extra = padded_inputs(data, self.B, self.N[0], self.N[1])
+            lh = [extra['num_keypoints0'], extra['num_keypoints1']]
+            for i, t in enumerate(lh):
+                if t.device.type == 'cpu' and int(t.sum()) < 2:
+                    # what BatchNorm1d raises for one value per channel: the statistics of a call pool the real rows
+                    raise ValueError(f'Expected more than 1 value per channel when training: num_keypoints{i} sums to 1')
+            self.lens = torch.cat([t.to(self.dev) for t in lh]).contiguous()          # [2B]: n_0 .. n_{B-1}, m_0 .. m_{B-1}
+            self.pair_wh = torch.cat([extra['image0_size'].to(self.dev), extra['image1_size'].to(self.dev)], 1).contiguous()   # [B, 4]
+            self.wh = [(0.0, 0.0), (0.0, 0.0)]
+        else:
+            self.wh = [model._image_wh(data, 0), model._image_wh(data, 1)]
         self.grads: Dict[str, torch.Tensor] = {}
+
+    def _len(self, i):
+        """image i's per-pair lengths (device int32 [B]), or None for a uniform batch"""
+        return None if self.lens is None else self.lens[i * self.B:(i + 1) * self.B]
+
+    def _lk(self):
+        return {} if self.lens is None else {'lens': self.lens}
 
     @staticmethod
     def _prep(t, last):
@@ -129,12 +161,17 @@ class TrainStep:
             nl = (len(enc) + 2) // 3                                   # Conv (ReLU BN Conv)*
             self.kenc = []                                             # per image: list of (input, _BN) per hidden layer + last input
             x = []
+            if self.padded:                                            # the residuals read the descriptors with the padding zeroed
+                self.ldesc = [ops.mask_rows(self.ldesc[i].view(B * self.N[i], d), self._len(i)).view(B, self.N[i], d) for i in range(2)]
             for i in range(2):
                 rows = B * self.N[i]
-                h = ops.kenc_input(self.kpts[i], self.side[i], rows, self.S, self.wh[i][0], self.wh[i][1])
+                if self.padded:
+                    h = ops.kenc_input(self.kpts[i], self.side[i], rows, self.S, 0.0, 0.0, lens=self._len(i), pair_wh=self.pair_wh[:, 2 * i:])
+                else:
+                    h = ops.kenc_input(self.kpts[i], self.side[i], rows, self.S, self.wh[i][0], self.wh[i][1])
                 rec = []
                 for j in range(nl - 1):
-                    conv, bn = enc[3 * j], _BN(enc[3 * j + 2])
+                    conv, bn = enc[3 * j], _BN(enc[3 * j + 2], self._len(i))
                     a = ops.linear(h, self._w2(conv), conv.bias)
                     rec.append((h, bn))
                     h = bn.forward(ops, a)
@@ -161,6 +198,8 @@ class TrainStep:
                 self.m = [ops.mix_fwd(self.g[i], self.ldesc[i].view(B * self.N[i], d), self.mix) for i in range(2)]
             else:
                 self.m = self.g
+            if self.padded:                                            # context descriptors are 0 past the lengths
+                self.m = [ops.mask_rows(self.m[i], self._len(i)) for i in range(2)]
             n, m_ = self.N
             # context descriptors in the reference's [B, d, N] layout; their zero-padded copies are the transposed operands of the backward pass
             self.mT = [ops.transpose(self.m[i], batch=B, rows=self.N[i], cols=d) for i in range(2)]          # [B, d, pad4(N)]
@@ -169,7 +208,7 @@ class TrainStep:
             self.Sp = ops.zeros(B, n, lds)
             ops.gemm(self.m[0], d, d, self.m[1], d, n, m_, self.Sp, lds, alpha=d ** -0.5, batch=B, strideA=n * d, strideW=m_ * d, strideY=n * lds)
             self.dust = model.dustbin_score.detach().reshape(1).contiguous()
-            scores, self.hist = ops.sinkhorn_fwd(self.Sp, self.dust, B, n, m_, self.iters, self.reg)
+            scores, self.hist = ops.sinkhorn_fwd(self.Sp, self.dust, B, n, m_, self.iters, self.reg, **self._lk())
         return scores, ctx[0], ctx[1]
 
     def _prop(self, name, mod, xq, xkv, iq, ikv):
@@ -180,15 +219,16 @@ class TrainStep:
         q = ops.linear(xq, self._w2(mha.in_proj_q), mha.in_proj_q.bias)
         k = ops.linear(xkv, self._w2(mha.in_proj_k), mha.in_proj_k.bias)
         v = ops.linear(xkv, self._w2(mha.in_proj_v), mha.in_proj_v.bias)
-        o = ops.attention(q, k, v, B, nq, nk, H, d // H)
+        kl = {} if self.lens is None else {'klen': self._len(ikv)}
+        o = ops.attention(q, k, v, B, nq, nk, H, d // H, **kl)
         msg = ops.linear(o, self._w2(mha.out_proj), mha.out_proj.bias)
         c1 = ops.axpby(xq, msg, 1.0, -1.0) if self.use_offset else xq
         fc = mod.fc
         a = ops.linear(c1, self._w2(fc[0]), fc[0].bias, A2=msg)
-        bn = _BN(fc[2])
+        bn = _BN(fc[2], self._len(iq))
         hbn = bn.forward(ops, a)
         out = ops.linear(hbn, self._w2(fc[3]), fc[3].bias, R=xq)
-        self.calls.append(dict(name=name, mod=mod, xq=xq, xkv=xkv, iq=iq, ikv=ikv, q=q, k=k, v=v, o=o, msg=msg, c1=c1, bn=bn, hbn=hbn))
+        self.calls.append(dict(name=name, mod=mod, xq=xq, xkv=xkv, iq=iq, ikv=ikv, q=q, k=k, v=v, o=o, msg=msg, c1=c1, bn=bn, hbn=hbn, **kl))
         return out
 
     # ------------------------------------------------------------------ backward
@@ -201,7 +241,7 @@ class TrainStep:
             dm = [ops.zeros(B * n, d), ops.zeros(B * m_, d)]
             if dscores is not None:
                 G = dscores.detach().float().contiguous()
-                dZ, dd = ops.sinkhorn_bwd(self.Sp, self.dust, self.hist, G, B, n, m_, self.iters, self.reg)
+                dZ, dd = ops.sinkhorn_bwd(self.Sp, self.dust, self.hist, G, B, n, m_, self.iters, self.reg, **self._lk())
                 self.grads['dustbin_score'] = dd.reshape(model.dustbin_score.shape)
                 # S = m0 m1^T d^-0.5:  dm0 = dS m1 d^-0.5,  dm1 = dS^T m0 d^-0.5   (superglue.py:64, 80-85)
                 mp, np_ = _pad4(m_), _pad4(n)
@@ -216,6 +256,8 @@ class TrainStep:
                 if dctx is not None:                                    # gradient arriving at the [B, d, N] context descriptors
                     t = ops.transpose(dctx.detach().float().contiguous(), batch=B, rows=d, cols=self.N[i], pad=False)     # -> [B, N, d]
                     ops.axpby(dm[i], t.view(B * self.N[i], d), 1.0, 1.0, out=dm[i])
+            if self.padded:     # backward of the forward's mask: drops the dustbin gradients at n_b, m_b and any dctx past the lengths
+                dm = [ops.mask_rows(dm[i], self._len(i)) for i in range(2)]
             dl = [None, None]
             if self.residual:
                 dg = []
@@ -312,14 +354,15 @@ class TrainStep:
         dq, dk, dv = ops.empty(B * nq, d), ops.empty(B * nk, d), ops.empty(B * nk, d)
         P, dP = ops.zeros(B, nq, nkp), ops.zeros(B, nq, nkp)
         PT, dST = ops.zeros(B, nk, nqp), ops.zeros(B, nk, nqp)
+        kl = {'klen': call['klen']} if 'klen' in call else {}   # P = 0 past each sequence's keys: dQ, dK, dV vanish there
         for h in range(H):
             c = h * dh
             ops.gemm(q, d, dh, k, d, nq, nk, P, nkp, a_off=c, w_off=c, alpha=scale, batch=B, strideA=nq * d, strideW=nk * d, strideY=nq * nkp)
-            ops.softmax_rows(P, nkp, B * nq, nk)
+            ops.softmax_rows(P, nkp, B * nq, nk, **kl)
             ops.gemm(do, d, dh, v, d, nq, nk, dP, nkp, a_off=c, w_off=c, batch=B, strideA=nq * d, strideW=nk * d, strideY=nq * nkp)
             ops.transpose_raw(P, 0, nkp, nq * nkp, PT, nqp, nk * nqp, B, nq, nk, True)
             ops.gemm(PT, nqp, nqp, doT, nqp, nk, dh, dv, d, w_off=c * nqp, y_off=c, batch=B, strideA=nk * nqp, strideW=d * nqp, strideY=nk * d)
-            ops.softmax_bwd_rows(P, dP, nkp, B * nq, nk, scale)
+            ops.softmax_bwd_rows(P, dP, nkp, B * nq, nk, scale, **kl)
             ops.gemm(dP, nkp, nkp, kT, nkp, nq, dh, dq, d, w_off=c * nkp, y_off=c, batch=B, strideA=nq * nkp, strideW=d * nkp, strideY=nq * d)
             ops.transpose_raw(dP, 0, nkp, nq * nkp, dST, nqp, nk * nqp, B, nq, nk, True)
             ops.gemm(dST, nqp, nqp, qT, nqp, nk, dh, dk, d, w_off=c * nqp, y_off=c, batch=B, strideA=nk * nqp, strideW=d * nqp, strideY=nk * d)
@@ -384,7 +427,12 @@ class GraphedTrainStep:
     ``margin`` / ``metric_weight`` (the reference's ``train.margin`` / ``train.metric_weight``, matching_module.py:101-105): with a
     margin the graph also computes ``metric_loss`` on the context descriptors (``og_metric_loss_fwd``) and backpropagates
     ``nll_weight * loss + metric_weight * metric_loss``, as ``criterion(..., margin=)`` does in the eager step; ``margin=None``
-    captures the margin-free step exactly as before."""
+    captures the margin-free step exactly as before.
+
+    Padded batches (``num_keypoints0`` / ``num_keypoints1`` in ``data`` and ``y_true``, per-pair ``image0_size`` /
+    ``image1_size`` optional): the lengths and sizes live in static device buffers like the other inputs, so one capture per
+    capacity (B, N, M) replays every set of lengths; the step is :class:`TrainStep`'s padded step with :func:`criterion`'s
+    per-pair loss.  ``margin`` is not built for padded batches."""
 
     _KEYS = ('keypoints0', 'keypoints1', 'side_info0', 'side_info1', 'local_descriptors0', 'local_descriptors1')
 
@@ -406,6 +454,15 @@ class GraphedTrainStep:
         for k in self._KEYS:
             self.static[k] = data[k].detach().float().contiguous().clone()
         self.gt = {k: y_true[k].to(device=dev, dtype=torch.int64).contiguous().clone() for k in ('gt_matches0', 'gt_matches1')}
+        self.padded = is_padded(data)
+        if self.padded:                                                  # lengths and sizes through static buffers: any set replays
+            if margin is not None:
+                raise NotImplementedError('GraphedTrainStep(margin=...) on a padded batch (num_keypoints0 / num_keypoints1) is not built')
+            self.static.pop('image0', None)
+            self.static.pop('image1', None)
+            for k, v in self._extra(data).items():
+                self.static[k] = v.to(dev).clone()
+            self.gt.update({k: self.static[k] for k in ('num_keypoints0', 'num_keypoints1')})
         self.params = list(model.named_parameters())
         for _, p in self.params:
             if p.grad is None:
@@ -450,12 +507,21 @@ class GraphedTrainStep:
                 self._opt_idx = optimizer._last_idx
                 optimizer._stepped = list(saved_opt[-1])
 
+    def _extra(self, data):
+        k0, k1 = data['keypoints0'], data['keypoints1']
+        return padded_inputs(data, k0.shape[0], k0.shape[1], k1.shape[1])
+
     def __call__(self, data: dict, y_true: dict) -> Dict[str, torch.Tensor]:
+        if is_padded(data) != self.padded:
+            raise ValueError('the batch must be padded (num_keypoints0 / num_keypoints1) exactly when the captured one was')
         for k in self._KEYS:
             if tuple(data[k].shape) != tuple(self.static[k].shape):
                 raise ValueError(f'{k}: shape {tuple(data[k].shape)} differs from the captured {tuple(self.static[k].shape)}')
             self.static[k].copy_(data[k], non_blocking=True)
-        for k in self.gt:
+        if self.padded:
+            for k, v in self._extra(data).items():
+                self.static[k].copy_(v, non_blocking=True)
+        for k in ('gt_matches0', 'gt_matches1'):
             self.gt[k].copy_(y_true[k], non_blocking=True)
         self.graph.replay()
         if self.optimizer is not None:                                   # the kernels wrote the parameters through raw pointers
