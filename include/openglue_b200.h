@@ -538,6 +538,9 @@ int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const f
  *                            (same B, H, W, cap), then normalize_descriptors (rootsift: L1 + sqrt, else L2) and lafs_from_opencv_kpts
  *                            (mr_size 6): lafs [B, out_cap, 2, 3], scores [B, out_cap], desc [B, out_cap, 128], raw_desc (optional)
  *                            [B, out_cap, 128] cv2's integer-valued descriptor.  max_n >= every n_sel[b] sizes the grid.
+ *   og_sift_detect_padded    og_sift_detect for outputs padded to a fixed capacity: count[b] is always the number of keypoints
+ *                            written (<= cap) and overflow[b] = 1 marks an image that exceeded a capacity (its keypoints are then
+ *                            incomplete), 0 otherwise.  Nothing is read back to the host.
  *   og_sift_rootsift_laf     normalize_descriptors + lafs_from_opencv_kpts of supplied kp [N, 5] and raw descriptors [N, 128]
  *   og_sift_fast_atan2       out[i] = cv2's fastAtan2(y[i], x[i]) in degrees: fused = cv::hal::fastAtan2's vector form, 0 = the
  *                            scalar one (cv2.fastAtan2)
@@ -546,6 +549,8 @@ int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const f
 int64_t og_sift_workspace_bytes(int B, int H, int W, int cap);
 int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
                    int* count, void* stream);
+int og_sift_detect_padded(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
+                          int* count, int* overflow, void* stream);
 int64_t og_sift_select_workspace_bytes(int B, int cap);
 int og_sift_select(const float* kp, const int* count, int B, int cap, float nms_radius, int max_keypoints, void* work, int64_t work_bytes,
                    int* sel, int* n_sel, void* stream);
@@ -577,7 +582,15 @@ int og_sift_gaussian_taps(double sigma, float* taps, int cap);
  *                          out_kpts0/1 [B n, 2] = their centres;  total [1] int64 = the number of matches (rows past it are
  *                          not written).  matches0 [B,n] int64, mscores0 [B,n], lafs0 [B,n,2,3], lafs1 [B,m,2,3].
  *                        The predicate is matches0 >= 0, never the score: a mutual match whose exp underflowed to 0 is kept
- *                        when the threshold is negative.                                                             */
+ *                        when the threshold is negative.
+ *   og_keypoint_counts   the kept keypoints of each image of a front-end output padded to K rows, on the device: of count[b]
+ *                        keypoints the first min(count[b], cap) were stored; max_keypoints >= 0 below that number keeps the
+ *                        max_keypoints best (mode[b] = 1), otherwise all are kept in stored order (mode[b] = 0); n_out[b] = the
+ *                        kept number clamped to K; overflow[b] |= 1 when count[b] > cap or the kept number exceeds K (the caller
+ *                        initialises overflow).  count, n_out, mode (may be NULL), overflow: int32 [B].
+ *   og_mask_empty_pairs  matches0 / mscores0 [B,n] and matches1 / mscores1 [B,m] (og_match_fwd_padded's outputs) = -1 / 0 in every
+ *                        slot of a pair whose len0[b] or len1[b] (int32 [B], device) is 0: the padded kernels clamp lengths to
+ *                        at least 1, so they match row 0 of an image without keypoints.                               */
 typedef enum og_laf_method {
   OG_LAF_NONE = 0, OG_LAF_SCALE = 1, OG_LAF_ROTATION = 2, OG_LAF_SCALE_ROTATION = 3, OG_LAF_AFFINE = 4
 } og_laf_method;
@@ -586,6 +599,9 @@ int og_prepare_features(const float* lafs, const float* responses, int64_t R, in
 int og_match_compact(const int64_t* matches0, const float* mscores0, const float* lafs0, const float* lafs1, int B, int n, int m,
                      int64_t* pair, int64_t* ij, float* confidence, float* out_lafs0, float* out_lafs1, float* out_kpts0,
                      float* out_kpts1, int64_t* total, void* stream);
+int og_keypoint_counts(const int* count, int B, int cap, int max_keypoints, int K, int* n_out, int* mode, int* overflow, void* stream);
+int og_mask_empty_pairs(const int* len0, const int* len1, int B, int n, int m, int64_t* matches0, float* mscores0, int64_t* matches1,
+                        float* mscores1, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Homography-pretraining image pairs (OxfordParis1MDataset.__getitem__, data/oxford_paris_dataset.py:27-66, without the decode,

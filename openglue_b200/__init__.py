@@ -15,12 +15,13 @@ and the steps either side of those:
     OpenCVSIFT(max_keypoints, nms_diameter, rootsift)(image) -> (lafs, scores, descriptors)   (OPENCV_SIFT: cv2's SIFT + radius NMS + RootSIFT)
     prepare_features_output(lafs, responses, desc, get_laf_to_sideinfo_converter(method), ...)   (front-end output -> SuperGlue input)
     OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
+    ImagePairMatcher(local_feature, superglue, match_config)(image0, image1) -> padded matches   (batches of pairs, one CUDA graph)
     synthesize_homography_pairs(images_u8, offset, warp_offset, generator)   (the homography-pretraining dataset's pairs, batched)
 """
 from .gt_matches import generate_gt_matches  # noqa: F401
 from .homography import synthesize_homography_pairs  # noqa: F401
 from .feature_cache import FeatureStore, collate_features  # noqa: F401
-from .features import OpenGlueMatcher, get_laf_to_sideinfo_converter, prepare_features_output  # noqa: F401
+from .features import ImagePairMatcher, OpenGlueMatcher, get_laf_to_sideinfo_converter, prepare_features_output  # noqa: F401
 from .losses import criterion  # noqa: F401
 from .optim import ClippedAdam  # noqa: F401
 from .sinkhorn import matching_log_probs  # noqa: F401

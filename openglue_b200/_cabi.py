@@ -143,6 +143,7 @@ SYMBOLS = {
     # OpenCV SIFT front-end (row f7)
     'og_sift_workspace_bytes': (_L, [_I, _I, _I, _I]),
     'og_sift_detect': (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P, _P]),
+    'og_sift_detect_padded': (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P, _P, _P]),
     'og_sift_select_workspace_bytes': (_L, [_I, _I]),
     'og_sift_select': (_I, [_P, _P, _I, _I, _F, _I, _P, _L, _P, _P, _P]),
     'og_sift_describe': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
@@ -152,6 +153,8 @@ SYMBOLS = {
     # local features -> matcher inputs, matches -> compact list
     'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'og_keypoint_counts': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'og_mask_empty_pairs': (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
     # homography-pretraining pairs
     'og_homography_pairs': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     # optimiser step: clip_grad_norm_ -> Adam -> StepLR

@@ -855,8 +855,9 @@ static int sift_blur(const float* src, int B, int h, int w, double sigma, float*
   if (const int rc = OG_LAUNCH(sift_blur_rows_kernel, sift_grid(n), 256, 0, st, src, B, h, w, t, tmp)) return rc;
   return OG_LAUNCH(sift_blur_cols_kernel, sift_grid(n), 256, 0, st, tmp, B, h, w, t, dst, src, dog);
 }
-int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
-                   int* count, void* stream) {
+// og_sift_detect, and with overflow non-null og_sift_detect_padded (see sift_sort_unique_kernel)
+static int sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
+                       int* count, int* overflow, void* stream) {
   OG_CHECK_ARG(image && ws && kp && octave && count, "sift_detect: null pointer");
   OG_CHECK_ARG(dtype == 0 || dtype == 1, "sift_detect: dtype must be 0 (uint8) or 1 (float32)");
   const int64_t need = og_sift_workspace_bytes(B, H, W, cap);
@@ -917,7 +918,16 @@ int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, v
                                (const int*)loc_count, kp_raw, oct_raw, cap, kp_count)) return rc;
   // KeyPointsFilter::removeDuplicatedSorted
   return OG_LAUNCH(sift_sort_unique_kernel, B, 1024, 0, st, (const float*)kp_raw, (const int*)oct_raw, (const int*)kp_count,
-                   (const int*)loc_count, L.loc_cap, cap, L.n2max, work, kp, octave, count);
+                   (const int*)loc_count, L.loc_cap, cap, L.n2max, work, kp, octave, count, overflow);
+}
+int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
+                   int* count, void* stream) {
+  return sift_detect(image, dtype, B, H, W, cap, ws, ws_bytes, kp, octave, count, nullptr, stream);
+}
+int og_sift_detect_padded(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
+                          int* count, int* overflow, void* stream) {
+  OG_CHECK_ARG(overflow, "sift_detect_padded: null pointer");
+  return sift_detect(image, dtype, B, H, W, cap, ws, ws_bytes, kp, octave, count, overflow, stream);
 }
 int64_t og_sift_select_workspace_bytes(int B, int cap) {
   if (B <= 0 || B > 65535 || cap <= 0 || cap > (1 << 24)) return fail(OG_EINVAL, "sift_select_workspace_bytes: bad sizes");
@@ -974,6 +984,21 @@ int og_match_compact(const int64_t* matches0, const float* mscores0, const float
   OG_CHECK_ARG(B > 0 && n > 0 && m > 0 && (int64_t)B * n <= INT32_MAX - 1024, "match_compact: bad sizes");
   return OG_LAUNCH(match_compact_kernel, 1, 1024, 0, (cudaStream_t)stream, matches0, mscores0, lafs0, lafs1, B * n, n, m, pair, ij, confidence,
                    out_lafs0, out_lafs1, out_kpts0, out_kpts1, total);
+}
+
+int og_keypoint_counts(const int* count, int B, int cap, int max_keypoints, int K, int* n_out, int* mode, int* overflow, void* stream) {
+  OG_CHECK_ARG(count && n_out && overflow, "keypoint_counts: null pointer");
+  OG_CHECK_ARG(B > 0 && cap > 0 && K > 0, "keypoint_counts: bad sizes");
+  return OG_LAUNCH(keypoint_counts_kernel, cdiv(B, 256), 256, 0, (cudaStream_t)stream, count, B, cap, max_keypoints, K, n_out, mode,
+                   overflow);
+}
+int og_mask_empty_pairs(const int* len0, const int* len1, int B, int n, int m, int64_t* matches0, float* mscores0, int64_t* matches1,
+                        float* mscores1, void* stream) {
+  OG_CHECK_ARG(len0 && len1 && matches0 && mscores0 && matches1 && mscores1, "mask_empty_pairs: null pointer");
+  OG_CHECK_ARG(B > 0 && n > 0 && m > 0, "mask_empty_pairs: bad sizes");
+  const int64_t total = (int64_t)B * ((int64_t)n + m);
+  return OG_LAUNCH(mask_empty_pairs_kernel, eltwise_grid(total), 256, 0, (cudaStream_t)stream, len0, len1, B, n, m, matches0, mscores0,
+                   matches1, mscores1);
 }
 
 // ---- homography-pretraining pairs (csrc/homography.cuh) ----

@@ -97,4 +97,36 @@ __global__ void __launch_bounds__(1024) match_compact_kernel(const int64_t* __re
   if (threadIdx.x == 0) total[0] = base;
 }
 
+// The kept count of image b of a front-end output padded to K rows, from its device count: of count[b] keypoints the first
+// min(count[b], cap) were stored; the top-k keeps max_keypoints of them when max_keypoints >= 0 cuts that number (mode[b] = 1: by
+// score) and all of them otherwise (mode[b] = 0: in stored order), as top_k_keypoints (superpoint/utils.py:34-39) decides per
+// image.  n_out[b] = that number clamped to K; overflow[b] |= 1 when count[b] > cap or the kept number exceeds K.  mode may be NULL.
+__global__ void __launch_bounds__(256) keypoint_counts_kernel(const int* __restrict__ count, int B, int cap, int max_keypoints, int K,
+                                                              int* __restrict__ n_out, int* __restrict__ mode, int* __restrict__ overflow) {
+  const int b = blockIdx.x * 256 + threadIdx.x;
+  if (b >= B) return;
+  const int c = count[b], stored = max(0, min(c, cap));
+  const bool top = max_keypoints >= 0 && max_keypoints < stored;
+  const int keep = top ? max_keypoints : stored;
+  n_out[b] = min(keep, K);
+  if (mode) mode[b] = top ? 1 : 0;
+  if (c > cap || keep > K) overflow[b] = 1;
+}
+
+// matches0 / mscores0 [B, n], matches1 / mscores1 [B, m]: -1 and 0 in every slot of a pair with no keypoint in either image
+// (len0[b] == 0 or len1[b] == 0).  The padded matcher clamps each length to at least 1, so it matches row 0 of an empty image.
+__global__ void __launch_bounds__(256) mask_empty_pairs_kernel(const int* __restrict__ len0, const int* __restrict__ len1, int B, int n, int m,
+                                                               int64_t* __restrict__ matches0, float* __restrict__ mscores0,
+                                                               int64_t* __restrict__ matches1, float* __restrict__ mscores1) {
+  const int64_t rows0 = (int64_t)B * n, total = rows0 + (int64_t)B * m;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const bool first = i < rows0;
+    const int64_t r = first ? i : i - rows0;
+    const int b = (int)(r / (first ? n : m));
+    if (__ldg(len0 + b) > 0 && __ldg(len1 + b) > 0) continue;
+    if (first) { matches0[r] = -1; mscores0[r] = 0.f; }
+    else { matches1[r] = -1; mscores1[r] = 0.f; }
+  }
+}
+
 }  // namespace og

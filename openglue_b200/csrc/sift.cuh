@@ -406,10 +406,12 @@ __device__ __forceinline__ bool sift_cv_before(const SiftKp& p, const SiftKp& q)
 
 // One CTA per image: the orientation kernel's keypoints -> cv2's order without exact duplicates (same x, y, size, angle) into
 // out_kp / out_oct [B, cap]; count[b] = the number kept, or a value > cap when a capacity was exceeded (the outputs are then
-// incomplete).  work: [B, n2max] ints.
+// incomplete).  With overflow non-null, count[b] is always the number of keypoints written and overflow[b] = 1 marks an image
+// whose outputs are incomplete.  work: [B, n2max] ints.
 __global__ void __launch_bounds__(1024) sift_sort_unique_kernel(const float* __restrict__ kp, const int* __restrict__ kp_oct, const int* __restrict__ kp_count,
                                                                 const int* __restrict__ loc_count, int loc_cap, int cap, int n2max, int* __restrict__ work,
-                                                                float* __restrict__ out_kp, int* __restrict__ out_oct, int* __restrict__ count) {
+                                                                float* __restrict__ out_kp, int* __restrict__ out_oct, int* __restrict__ count,
+                                                                int* __restrict__ overflow) {
   __shared__ int warp_tot[32];
   __shared__ int base;
   const int b = blockIdx.x;
@@ -435,7 +437,15 @@ __global__ void __launch_bounds__(1024) sift_sort_unique_kernel(const float* __r
     const int pos = cta_ordered_slot(on, warp_tot, base);
     if (on) sift_store_kp(out_kp, out_oct, (int64_t)b * cap + pos, k);
   }
-  if (threadIdx.x == 0) count[b] = (raw > cap || loc_count[b] > loc_cap) ? max(raw, cap + 1) : base;
+  if (threadIdx.x == 0) {
+    const bool over = raw > cap || loc_count[b] > loc_cap;
+    if (overflow) {
+      count[b] = base;
+      overflow[b] = over ? 1 : 0;
+    } else {
+      count[b] = over ? max(raw, cap + 1) : base;
+    }
+  }
 }
 
 // One CTA per image: detect_kpts_opencv's selection on keypoints kp [B, cap, 5] (x, y, size, angle, response), count[b] of them:

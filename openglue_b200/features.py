@@ -11,7 +11,9 @@ column except the logarithms equals the reference's fp32 result bit for bit (the
 ATen's vectorised CPU form misses by an ulp on a few frames in a thousand).  ``OpenGlueMatcher`` runs an image pair (or
 pre-extracted features) through the front-end, this step, ``SuperGlue`` with ``MatchingCore``'s match extraction, and the ordered
 compaction ``og_match_compact`` to the reference's compact match list; reading the number of matches is its one host
-synchronisation, where the reference's boolean indexing synchronises too.
+synchronisation, where the reference's boolean indexing synchronises too.  ``ImagePairMatcher`` runs batches of image pairs
+through the same chain on padded front-end outputs (``extract_padded``) with the keypoint counts on the device: no host
+synchronisation at all, so the whole chain replays as one CUDA graph.
 
 CUDA tensors only, and no autograd: the reference never differentiates these outputs.
 """
@@ -27,7 +29,7 @@ from ._cabi import ptr, stream
 from .superglue import SuperGlue
 
 __all__ = ['LAFConverter', 'get_laf_to_sideinfo_converter', 'prepare_features_output', 'compact_matches', 'pad_features',
-           'OpenGlueMatcher']
+           'padded_capacity', 'OpenGlueMatcher', 'ImagePairMatcher']
 
 # method name -> (og_laf_method, side-information columns after the response)
 _METHODS = {'none': (0, 0), 'scale': (1, 1), 'rotation': (2, 2), 'scale_rotation': (3, 3), 'affine': (4, 5)}
@@ -172,6 +174,17 @@ def pad_features(features: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tens
     return lafs, resp, desc, torch.tensor(counts, dtype=torch.int64)
 
 
+def padded_capacity(max_keypoints: int, capacity: Optional[int] = None) -> int:
+    """K, the rows per image of a front-end's ``extract_padded``: ``capacity``, by default ``max_keypoints``."""
+    if capacity is None:
+        if int(max_keypoints) == -1:
+            raise ValueError('extract_padded needs a capacity when max_keypoints is -1 (every keypoint kept)')
+        capacity = max_keypoints
+    if int(capacity) < 1:
+        raise ValueError(f'capacity must be at least 1, got {capacity}')
+    return int(capacity)
+
+
 class OpenGlueMatcher(nn.Module):
     """Drop-in for the reference's ``inference.OpenGlueMatcher`` (inference.py:81-211): correspondences between two images from
     local features followed by SuperGlue.
@@ -222,3 +235,121 @@ class OpenGlueMatcher(nn.Module):
         res = self.matcher.run(inputs, want_matches=True, want_context=False,
                                match_threshold=float(self.match_config['inference']['match_threshold']))
         return compact_matches(res['matches0'], res['matching_scores0'], lafs0, lafs1)
+
+
+def _frontend_version(module: nn.Module) -> tuple:
+    """Storage and version of every parameter and buffer: a captured graph has the front-end's packed weights baked in"""
+    return tuple((t.data_ptr(), t._version) for t in list(module.parameters()) + list(module.buffers()))
+
+
+class ImagePairMatcher(nn.Module):
+    """Batches of image pairs to matches with no host synchronisation, replayed as one CUDA graph by default.
+
+    ``local_feature``: an ``OpenCVSIFT`` or ``SuperPointNet`` / ``SuperPointNetBn``; ``matcher``: an ``openglue_b200.SuperGlue``;
+    ``match_config``: ``OpenGlueMatcher``'s (``superglue.laf_to_sideinfo_method``, optional ``superglue.log_transform_response``,
+    ``inference.match_threshold``).  ``capacity``: the keypoint rows K per image (default: the front-end's ``max_keypoints``).
+
+    ``forward(image0 [B,1,H0,W0], image1 [B,1,H1,W1])`` runs ``extract_padded`` on both images, ``prepare_features_output``,
+    ``SuperGlue.run`` on the padded batch with the device counts, and the match extraction.  Each pair's matches are those of
+    the pair matched alone.  It returns device tensors: ``matches0`` / ``matching_scores0`` [B,K], ``matches1`` /
+    ``matching_scores1`` [B,K] (-1 / 0 past the counts, and everywhere in a pair with no keypoint in either image),
+    ``lafs0`` / ``lafs1`` [B,K,2,3], ``keypoints0`` / ``keypoints1`` [B,K,2], ``num_keypoints0`` / ``num_keypoints1`` [B] int32 and
+    ``overflow0`` / ``overflow1`` [B] int32 (the front-ends' flags: an image cut to the capacity).  ``compact_matches(matches0,
+    matching_scores0, lafs0, lafs1)`` gives ``OpenGlueMatcher``'s list.
+
+    ``use_cuda_graph=True`` captures the chain once per (B, H0, W0, H1, W1, K, image dtype, device, precision, match threshold)
+    after one eager warm-up run, and replays it with the images copied into static buffers.  A graph is captured again when the
+    matcher's buffers are reallocated or a weight of the matcher or the front-end changes; at most ``max_graphs`` are kept.
+    The first call packs the weights and copies them to the device; every later call runs without a host synchronisation."""
+
+    _OUT_KEYS = ('matches0', 'matching_scores0', 'matches1', 'matching_scores1', 'lafs0', 'lafs1', 'keypoints0', 'keypoints1',
+                 'num_keypoints0', 'num_keypoints1', 'overflow0', 'overflow1')
+
+    def __init__(self, local_feature: nn.Module, matcher: SuperGlue, match_config: Dict, use_cuda_graph: bool = True,
+                 capacity: Optional[int] = None) -> None:
+        super().__init__()
+        if not isinstance(matcher, SuperGlue):
+            raise TypeError('openglue_b200.ImagePairMatcher takes an openglue_b200.SuperGlue as its matcher')
+        if not callable(getattr(local_feature, 'extract_padded', None)):
+            raise TypeError('openglue_b200.ImagePairMatcher takes a front-end with extract_padded (OpenCVSIFT, SuperPointNet[Bn])')
+        self.local_feature = local_feature
+        self.matcher = matcher
+        self.laf_converter = get_laf_to_sideinfo_converter(match_config['superglue']['laf_to_sideinfo_method'])
+        self.log_response = bool(match_config['superglue'].get('log_transform_response', False))
+        self.match_threshold = float(match_config['inference']['match_threshold'])
+        self.capacity = capacity
+        self.use_cuda_graph = use_cuda_graph
+        self._graphs: Dict[tuple, tuple] = {}
+        self.max_graphs = 4
+        self.eval()
+
+    def _chain(self, image0: torch.Tensor, image1: torch.Tensor, K: int) -> Dict[str, torch.Tensor]:
+        dev = image0.device
+        B = image0.shape[0]
+        data, out = {}, {}
+        for i, img in ((0, image0), (1, image1)):
+            lafs, resp, desc, num, over = self.local_feature.extract_padded(img, K)
+            f = prepare_features_output(lafs, resp, desc, self.laf_converter, log_response=self.log_response)
+            size = torch.empty(B, 2, dtype=torch.float32, device=dev)        # (W, H) per pair, filled on the device
+            size[:, 0] = float(img.shape[3])
+            size[:, 1] = float(img.shape[2])
+            data.update({f'keypoints{i}': f['keypoints'], f'side_info{i}': f['side_info'], f'local_descriptors{i}': desc,
+                         f'num_keypoints{i}': num, f'image{i}_size': size})
+            out.update({f'lafs{i}': lafs, f'keypoints{i}': f['keypoints'], f'num_keypoints{i}': num, f'overflow{i}': over})
+        res = self.matcher.run(data, want_matches=True, want_context=False, match_threshold=self.match_threshold)
+        m0, s0, m1, s1 = res['matches0'], res['matching_scores0'], res['matches1'], res['matching_scores1']
+        with torch.cuda.device(dev):
+            _cabi.check(_cabi.lib().og_mask_empty_pairs(ptr(out['num_keypoints0']), ptr(out['num_keypoints1']), B, K, K, ptr(m0), ptr(s0),
+                                                        ptr(m1), ptr(s1), stream(dev)), 'og_mask_empty_pairs')
+        out.update(matches0=m0, matching_scores0=s0, matches1=m1, matching_scores1=s1)
+        return out
+
+    def _versions(self) -> tuple:
+        return (getattr(self.matcher, '_alloc_gen', 0), self.matcher._weights_version(), _frontend_version(self.local_feature))
+
+    def _run_graph(self, image0: torch.Tensor, image1: torch.Tensor, K: int) -> Dict[str, torch.Tensor]:
+        """Replay (capturing on first use) the CUDA graph for these shapes; the images are copied into its static buffers."""
+        dev = image0.device
+        key = (tuple(image0.shape), tuple(image1.shape), image0.dtype, image1.dtype, K, str(dev), self.matcher._precision(),
+               self.match_threshold)
+        entry = self._graphs.get(key)
+        if entry is not None and entry[4] != self._versions():
+            del self._graphs[key]                # buffers or weights the graph reads were replaced: capture again
+            entry = None
+        if entry is None:
+            static0, static1 = torch.empty_like(image0), torch.empty_like(image1)
+            static0.copy_(image0)
+            static1.copy_(image1)
+            self._chain(static0, static1, K)                                    # warm-up: weights, workspaces, kernel attributes
+            torch.cuda.synchronize(dev)
+            # the front-end's cached workspaces are baked into the graph: hold them even if the front-end drops them later
+            held = tuple(getattr(self.local_feature, '_ws', {}).values())
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                out = self._chain(static0, static1, K)
+            while len(self._graphs) >= self.max_graphs:                         # bounded memory: drop the oldest shape
+                del self._graphs[next(iter(self._graphs))]
+            entry = self._graphs[key] = (graph, static0, static1, out, self._versions(), held)
+        graph, static0, static1, out = entry[:4]
+        static0.copy_(image0)
+        static1.copy_(image1)
+        graph.replay()
+        return out
+
+    @torch.no_grad()
+    def forward(self, image0: torch.Tensor, image1: torch.Tensor, borrow: bool = False) -> Dict[str, torch.Tensor]:
+        """``borrow=True`` (CUDA-graph mode): return the graph's own output buffers instead of copies; the next call on this
+        matcher overwrites them (use it when the results are consumed on the same stream right away)."""
+        for i, img in ((0, image0), (1, image1)):
+            if not torch.is_tensor(img) or img.dim() != 4 or img.shape[1] != 1:
+                raise ValueError(f'image{i} must be [B, 1, H, W], got {tuple(img.shape) if torch.is_tensor(img) else type(img)}')
+        if image0.shape[0] != image1.shape[0] or image0.shape[0] < 1:
+            raise ValueError(f'image0 and image1 must hold the same number of images, got {image0.shape[0]} and {image1.shape[0]}')
+        K = padded_capacity(self.local_feature.max_keypoints, self.capacity)
+        if image0.device.type != 'cuda' or image1.device != image0.device:
+            raise RuntimeError('openglue_b200.ImagePairMatcher needs both images on one CUDA device (sm_90a); there is no CPU path')
+        with torch.cuda.device(image0.device):
+            if not self.use_cuda_graph:
+                return self._chain(image0, image1, K)
+            out = self._run_graph(image0, image1, K)
+        return out if borrow else {k: v.clone() for k, v in out.items()}

@@ -6,8 +6,10 @@ checkpoints load), same ``forward(image [B,1,H,W]) -> (lafs [B,N,2,3], scores [B
 All arithmetic runs in ``libopenglue_b200.so`` (``csrc/superpoint.cuh`` + the tensor-core GEMM): activations are NHWC, a 3x3
 convolution is an im2col gather + one GEMM with bias / ReLU fused (3xTF32 wgmma; the 1-channel input layer and ``precision='fp32'``
 run the exact fp32 kernel), then max-pool, channel norm, cell softmax, pixel heat map + non-maximum suppression + threshold + border
-removal, ordered compaction, top-k and bilinear descriptor sampling as one kernel each.  The only host step is reading the
-per-image keypoint counts (the reference's ``torch.nonzero`` synchronises in the same place) to size the output.
+removal, ordered compaction, top-k and bilinear descriptor sampling as one kernel each.  The only host step of ``forward`` is
+reading the per-image keypoint counts (the reference's ``torch.nonzero`` synchronises in the same place) to size the output;
+``extract_padded`` sizes its outputs by a fixed capacity instead and keeps the counts on the device, so it never synchronises
+and can be captured into a CUDA graph.
 ``SuperPointNetBn`` (BatchNorm variant, model.py:132-199: conv -> BatchNorm2d -> ReLU, also behind the two 1x1 heads) is the
 same kernel schedule on folded weights: in eval mode ``BN(W x + b) = (g / sqrt(var + eps)) W x + (b - mean) g / sqrt(var + eps) + beta``,
 folded once in float64 on the host.  There is no CPU path.
@@ -23,6 +25,7 @@ import torch.nn as nn
 from . import _cabi
 from ._cabi import ptr
 from ._ops import _Ops
+from .features import padded_capacity
 
 __all__ = ['SuperPointNet', 'SuperPointNetBn']
 
@@ -126,6 +129,72 @@ class SuperPointNet(nn.Module):
             self.last_probs = probs.view(B, hc, wc, 65)                  # kept for inspection / tests
         return probs, coarse
 
+    @torch.no_grad()
+    def extract_padded(self, image: torch.Tensor, capacity: Optional[int] = None):
+        """``forward`` for a batch whose images keep their own keypoint counts, without a host synchronisation.
+
+        image [B,1,H,W] -> (lafs [B,K,2,3], scores [B,K], descriptors [B,K,D], num_keypoints [B] int32, overflow [B] int32), all
+        on the image's device, K = ``capacity`` (default ``max_keypoints``).  Rows [0, num_keypoints[b]) of image b are what
+        ``forward(image[b:b+1])`` returns (its own top-k, raster order when it keeps every keypoint; no ``min_stack``); the rows
+        past them are 0, as ``pad_features`` writes them.
+
+        ``overflow[b] = 1`` where ``forward`` would raise or K cuts the image: more non-maximum-suppression survivors than the
+        16384 candidates an image holds (the first 16384 in raster order are used), or more kept keypoints than K (the first K
+        in output order are kept and num_keypoints[b] = K).  Check it whenever the results are next read on the host."""
+        K = padded_capacity(self.max_keypoints, capacity)
+        if image.dim() != 4 or image.shape[1] != 1 or image.shape[2] % 8 or image.shape[3] % 8:
+            raise ValueError('image must be [B, 1, H, W] with H, W multiples of 8')
+        if image.device.type != 'cuda':
+            raise RuntimeError('openglue_b200.SuperPointNet needs CUDA tensors (sm_90a); there is no CPU path')
+        H, W = image.shape[2], image.shape[3]
+        probs, coarse = self._network(image)
+        return self._keypoints_padded(probs, coarse, H, W, K)
+
+    def _candidates(self, probs: torch.Tensor, H: int, W: int, ops: _Ops):
+        """heat map, NMS, threshold and borders, then the ordered compaction: (cand_idx, cand_score [B, cap], count [B], cap)"""
+        dev = probs.device
+        hc, wc = H // 8, W // 8
+        B = probs.shape[0] // (hc * wc)
+        lib, st = ops.lib, ops.st()
+        heat = ops.empty(B, H, W)
+        _cabi.check(lib.og_sp_heat_nms(ptr(probs), B, hc, wc, int(self.nms_kernel), float(self.keypoint_threshold), int(self.remove_borders_size),
+                                       ptr(heat), st), 'og_sp_heat_nms')
+        cap = min(H * W, _MAX_CAND)
+        cand_idx = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        cand_score = ops.empty(B, cap)
+        count = torch.empty(B, dtype=torch.int32, device=dev)
+        _cabi.check(lib.og_sp_compact(ptr(heat), B, H * W, cap, ptr(cand_idx), ptr(cand_score), ptr(count), st),
+                    'og_sp_compact')
+        return cand_idx, cand_score, count, cap
+
+    def _keypoints_padded(self, probs: torch.Tensor, coarse: torch.Tensor, H: int, W: int, K: int):
+        """The post-processing of extract_padded from the layers' outputs (as _keypoints), at K rows per image"""
+        dev = probs.device
+        hc, wc = H // 8, W // 8
+        B = probs.shape[0] // (hc * wc)
+        d = self.descriptor_dim
+        ops = self._ops(dev)
+        lib = ops.lib
+        i32 = dict(dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            st = ops.st()
+            cand_idx, cand_score, count, cap = self._candidates(probs, H, W, ops)
+            n_out, mode, overflow = torch.empty(B, **i32), torch.empty(B, **i32), torch.zeros(B, **i32)
+            _cabi.check(lib.og_keypoint_counts(ptr(count), B, cap, int(self.max_keypoints), K, ptr(n_out), ptr(mode), ptr(overflow), st),
+                        'og_keypoint_counts')
+            # the outputs start at 0: select and sampling write rows [0, n_out[b]) only
+            kpts, scores, desc = ops.zeros(B, K, 2), ops.zeros(B, K), ops.zeros(B, K, d)
+            # max_count = cap: the sort's shared memory covers any count the device holds
+            _cabi.check(lib.og_sp_select(ptr(cand_idx), ptr(cand_score), ptr(count), ptr(n_out), ptr(mode), B, cap, W, K, cap, ptr(kpts), ptr(scores), st),
+                        'og_sp_select')
+            _cabi.check(lib.og_sp_sample_desc(ptr(coarse), B, hc, wc, d, ptr(kpts), ptr(n_out), K, K, 8, ptr(desc), st), 'og_sp_sample_desc')
+            real = (torch.arange(K, device=dev) < n_out[:, None]).float()
+            lafs = ops.zeros(B, K, 2, 3)                                 # identity frame + position on the real rows (model.py:119-127)
+            lafs[:, :, 0, 0] = real
+            lafs[:, :, 1, 1] = real
+            lafs[:, :, :, 2] = kpts
+        return lafs, scores, desc, n_out, overflow
+
     def _keypoints(self, probs: torch.Tensor, coarse: torch.Tensor, H: int, W: int):
         """The post-processing of forward (model.py:84-129) from the layers' outputs: probs [B hc wc, 65] and coarse [B hc wc, D]
         (NHWC, hc = H / 8, wc = W / 8, CUDA float32) -> (lafs [B,N,2,3], scores [B,N], descriptors [B,N,D])."""
@@ -136,15 +205,7 @@ class SuperPointNet(nn.Module):
         lib = ops.lib
         with torch.cuda.device(dev):
             st = ops.st()
-            heat = ops.empty(B, H, W)
-            _cabi.check(lib.og_sp_heat_nms(ptr(probs), B, hc, wc, int(self.nms_kernel), float(self.keypoint_threshold), int(self.remove_borders_size),
-                                           ptr(heat), st), 'og_sp_heat_nms')
-            cap = min(H * W, _MAX_CAND)
-            cand_idx = torch.empty(B, cap, dtype=torch.int32, device=dev)
-            cand_score = ops.empty(B, cap)
-            count = torch.empty(B, dtype=torch.int32, device=dev)
-            _cabi.check(lib.og_sp_compact(ptr(heat), B, H * W, cap, ptr(cand_idx), ptr(cand_score), ptr(count), st),
-                        'og_sp_compact')
+            cand_idx, cand_score, count, cap = self._candidates(probs, H, W, ops)
             counts = count.tolist()                                      # the one host synchronisation (the reference's nonzero)
             if max(counts) > cap:
                 raise RuntimeError(f'{max(counts)} keypoints survive non-maximum suppression in one image (capacity {cap}): raise keypoint_threshold')
