@@ -492,6 +492,23 @@ int og_softmax_bwd_rows_padded(const float* P, float* dP, int64_t ld, int batch,
 int og_kenc_input_padded(const float* kpts, const float* side, int batch, int cap, const int* lengths, int side_info_size,
                          const float* pair_wh, float* out, void* stream);
 int og_mask_padded_rows(const float* src, int batch, int cap, int cols, const int* lengths, float* dst, void* stream);
+/* Guarded forms: the skip of the reference's training_step (models/matching_module.py:96-97) decided on the device, so that a
+ * training step from images runs without a host synchronisation.  `skip` is a device int32 flag; a skipped step changes no
+ * training state.
+ *   og_train_guard          skip = 1 when some lengths[i] <= 0 (an image without keypoints: the reference's `data is None`) or
+ *                           when the B row lengths or the B column lengths total fewer than 2 (BatchNorm1d's "more than 1 value
+ *                           per channel"), else 0.  lengths [2B] device int32: n_0 .. n_{B-1}, m_0 .. m_{B-1}.
+ *   og_bn_train_fwd_guarded og_bn_train_fwd_padded (og_bn_train_fwd over batch x cap rows when lengths is NULL) with: running_mean /
+ *                           running_var left untouched when *skip != 0; num_batches_tracked (int64, optional) += 1 - *skip on
+ *                           the device.  y, save_mean and save_invstd are written either way.  skip NULL: never skipped.
+ *   og_train_skip_outputs   when *skip != 0: loss[0 .. nloss) = NaN, x[0 .. n) = 0 (gradients); nothing otherwise.  nloss <= 256.
+ * With skip NULL or *skip == 0 every guarded form equals its unguarded entry point bit for bit.                         */
+int og_train_guard(const int* lengths, int B, int* skip, void* stream);
+int og_bn_train_fwd_guarded(const float* a, int64_t lda, int batch, int cap, const int* lengths, int cols, int relu, const float* gamma,
+                            const float* beta, float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
+                            float* running_mean, float* running_var, const int* skip, int64_t* num_batches_tracked, float* workspace,
+                            void* stream);
+int og_train_skip_outputs(const int* skip, float* loss, int nloss, float* x, int64_t n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * SuperPoint front-end operators (SURVEY.md section 8, row f4): SuperPointNet.forward (models/features/superpoint/model.py:61-129)
@@ -637,6 +654,8 @@ int og_homography_pairs(const uint8_t* rgb, int B, int H, int W, int offset, con
  * step_size = -lr / bc1 in fp64, rounded once to fp32.
  * OG_EINVAL without touching the GPU: null pointers, nseg or ntiles <= 0, max_norm <= 0, beta outside [0, 1), eps < 0,
  * lr_gamma <= 0, a small workspace (OG_EWORKSPACE).
+ * og_clip_adam_step_guarded: the same step behind a device int32 flag `skip` (NULL: og_clip_adam_step).  When *skip != 0
+ * only the gradients are written, with 0: parameters, moments, step counts, lr, grad_norm and sched_steps keep their bits.
  * og_adam_schedule (tests): the same device-derived scalars for steps 1 .. nsteps from an initial lr:
  * lr_out[k] = the lr of step k + 1, step_size[k] / bc2_sqrt[k] its fp32 scalars.                        */
 #define OG_OPTIM_TILE 2048
@@ -657,6 +676,9 @@ int64_t og_optim_state_bytes(void);
 int64_t og_optim_workspace_bytes(int nseg);
 int og_clip_adam_step(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
                       double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes, void* stream);
+int og_clip_adam_step_guarded(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
+                              double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes,
+                              const int* skip, void* stream);
 int og_adam_schedule(int64_t nsteps, double lr, double lr_gamma, double beta1, double beta2, double* lr_out, float* step_size,
                      float* bc2_sqrt, void* stream);
 

@@ -17,6 +17,7 @@ and the steps either side of those:
     OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
     ImagePairMatcher(local_feature, superglue, match_config)(image0, image1) -> padded matches   (batches of pairs, one CUDA graph)
     synthesize_homography_pairs(images_u8, offset, warp_offset, generator)   (the homography-pretraining dataset's pairs, batched)
+    ImagePairTrainStep(local_feature, superglue, config, optimizer)(batch)   (training_step from images, one CUDA graph)
 """
 from .gt_matches import generate_gt_matches  # noqa: F401
 from .homography import synthesize_homography_pairs  # noqa: F401
@@ -28,5 +29,6 @@ from .sinkhorn import matching_log_probs  # noqa: F401
 from .superglue import MatchingCore, PendingMatches, SuperGlue  # noqa: F401
 from .sift import OpenCVSIFT, sift_create_torch  # noqa: F401
 from .superpoint import SuperPointNet, SuperPointNetBn  # noqa: F401
+from .training import ImagePairTrainStep  # noqa: F401
 
 __version__ = '0.1.0'

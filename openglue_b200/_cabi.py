@@ -132,6 +132,9 @@ SYMBOLS = {
     'og_softmax_bwd_rows_padded': (_I, [_P, _P, _L, _I, _L, _I, _F, _P, _P]),
     'og_kenc_input_padded': (_I, [_P, _P, _I, _I, _P, _I, _P, _P, _P]),
     'og_mask_padded_rows': (_I, [_P, _I, _I, _I, _P, _P, _P]),
+    'og_train_guard': (_I, [_P, _I, _P, _P]),
+    'og_bn_train_fwd_guarded': (_I, [_P, _L, _I, _I, _P, _I, _I, _P, _P, _F, _F, _P, _L, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'og_train_skip_outputs': (_I, [_P, _P, _I, _P, _L, _P]),
     # SuperPoint front-end operators (row f4)
     'og_sp_im2col3x3': (_I, [_P, _I, _I, _I, _I, _P, _P]),
     'og_sp_maxpool2x2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
@@ -161,6 +164,7 @@ SYMBOLS = {
     'og_optim_state_bytes': (_L, []),
     'og_optim_workspace_bytes': (_L, [_I]),
     'og_clip_adam_step': (_I, [_P, _I, _L, _D, _D, _D, _D, _D, _P, _P, _L, _P]),
+    'og_clip_adam_step_guarded': (_I, [_P, _I, _L, _D, _D, _D, _D, _D, _P, _P, _L, _P, _P]),
     'og_adam_schedule': (_I, [_L, _D, _D, _D, _D, _P, _P, _P, _P]),
 }
 

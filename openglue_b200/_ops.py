@@ -177,10 +177,18 @@ class _Ops:
         _cabi.check(self.lib.og_mix_param_grad(ptr(csum), ptr(mix), ptr(out), d, self.st()), 'og_mix_param_grad')
         return out
 
-    def bn_fwd(self, a, gamma, beta, eps, momentum, running_mean, running_var, lens=None):
-        """``lens``: statistics over the real rows of every pair (rows [B, cap])"""
+    def bn_fwd(self, a, gamma, beta, eps, momentum, running_mean, running_var, lens=None, skip=None, num_batches_tracked=None):
+        """``lens``: statistics over the real rows of every pair (rows [B, cap]).  ``skip`` (device int32 flag): the guarded form,
+        which leaves the running statistics untouched when the flag is set and adds 1 - skip to ``num_batches_tracked``."""
         rows, cols = a.shape
         y, mean, invstd = self.empty(rows, cols), self.empty(cols), self.empty(cols)
+        if skip is not None:
+            B = 1 if lens is None else lens.numel()
+            _cabi.check(self.lib.og_bn_train_fwd_guarded(ptr(a), a.stride(0), B, rows // B, ptr(lens), cols, 1, ptr(gamma), ptr(beta), float(eps),
+                                                         float(momentum), ptr(y), cols, ptr(mean), ptr(invstd), ptr(running_mean),
+                                                         ptr(running_var), ptr(skip), ptr(num_batches_tracked), ptr(self.ws(cols)), self.st()),
+                        'og_bn_train_fwd_guarded')
+            return y, mean, invstd
         if lens is not None:
             B = lens.numel()
             _cabi.check(self.lib.og_bn_train_fwd_padded(ptr(a), a.stride(0), B, rows // B, ptr(lens), cols, 1, ptr(gamma), ptr(beta), float(eps),

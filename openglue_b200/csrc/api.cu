@@ -649,7 +649,8 @@ int og_colsum(const float* x, int64_t ldx, const float* y, int64_t ldy, const fl
 
 static int bn_train_fwd_impl(const float* a_, int64_t lda, int rows, int cols, int relu, const float* gamma, const float* beta,
                              float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
-                             float* running_mean, float* running_var, float* workspace, const int* len, int cap, void* stream) {
+                             float* running_mean, float* running_var, float* workspace, const int* len, int cap, const int* skip,
+                             long long* num_batches_tracked, void* stream) {
   OG_CHECK_ARG(a_ && gamma && beta && y && save_mean && save_invstd && workspace, "bn_train_fwd: null pointer");
   OG_CHECK_ARG(rows > 0 && cols > 0, "bn_train_fwd: bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
@@ -662,7 +663,7 @@ static int bn_train_fwd_impl(const float* a_, int64_t lda, int rows, int cols, i
   r.mu = save_mean; r.out0 = var;
   if ((rc = colreduce_launch<2>(r, st)) != OG_OK) return rc;
   if ((rc = OG_LAUNCH(bn_finish_stats_kernel, cdiv(cols, 256), 256, 0, st, save_mean, var, cols, rows, len, cap, eps, momentum, save_invstd,
-                      running_mean, running_var)) != OG_OK) return rc;
+                      running_mean, running_var, skip, num_batches_tracked)) != OG_OK) return rc;
   return OG_LAUNCH(bn_apply_kernel, eltwise_grid((int64_t)rows * cols), 256, 0, st, a_, lda, rows, cols, relu, save_mean, save_invstd, gamma,
                    beta, y, ldy);
 }
@@ -671,7 +672,7 @@ int og_bn_train_fwd(const float* a_, int64_t lda, int rows, int cols, int relu, 
                     float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
                     float* running_mean, float* running_var, float* workspace, void* stream) {
   return bn_train_fwd_impl(a_, lda, rows, cols, relu, gamma, beta, eps, momentum, y, ldy, save_mean, save_invstd, running_mean, running_var,
-                           workspace, nullptr, rows, stream);
+                           workspace, nullptr, rows, nullptr, nullptr, stream);
 }
 
 int og_bn_train_fwd_padded(const float* a_, int64_t lda, int batch, int cap, const int* lengths, int cols, int relu, const float* gamma,
@@ -679,7 +680,29 @@ int og_bn_train_fwd_padded(const float* a_, int64_t lda, int batch, int cap, con
                            float* running_mean, float* running_var, float* workspace, void* stream) {
   OG_CHECK_ARG(lengths && batch > 0 && cap > 0 && (int64_t)batch * cap <= INT32_MAX, "bn_train_fwd_padded: bad lengths or sizes");
   return bn_train_fwd_impl(a_, lda, batch * cap, cols, relu, gamma, beta, eps, momentum, y, ldy, save_mean, save_invstd, running_mean,
-                           running_var, workspace, lengths, cap, stream);
+                           running_var, workspace, lengths, cap, nullptr, nullptr, stream);
+}
+
+int og_bn_train_fwd_guarded(const float* a_, int64_t lda, int batch, int cap, const int* lengths, int cols, int relu, const float* gamma,
+                            const float* beta, float eps, float momentum, float* y, int64_t ldy, float* save_mean, float* save_invstd,
+                            float* running_mean, float* running_var, const int* skip, int64_t* num_batches_tracked, float* workspace,
+                            void* stream) {
+  OG_CHECK_ARG(batch > 0 && cap > 0 && (int64_t)batch * cap <= INT32_MAX, "bn_train_fwd_guarded: bad sizes");
+  return bn_train_fwd_impl(a_, lda, batch * cap, cols, relu, gamma, beta, eps, momentum, y, ldy, save_mean, save_invstd, running_mean,
+                           running_var, workspace, lengths, cap, skip, reinterpret_cast<long long*>(num_batches_tracked), stream);
+}
+
+int og_train_guard(const int* lengths, int B, int* skip, void* stream) {
+  OG_CHECK_ARG(lengths && skip, "train_guard: null pointer");
+  OG_CHECK_ARG(B > 0 && B <= INT32_MAX / 2, "train_guard: B = %d must be positive", B);
+  return OG_LAUNCH(train_guard_kernel, 1, 32, 0, (cudaStream_t)stream, lengths, B, skip);
+}
+
+int og_train_skip_outputs(const int* skip, float* loss, int nloss, float* x, int64_t n, void* stream) {
+  OG_CHECK_ARG(skip && (loss || nloss == 0) && (x || n == 0), "train_skip_outputs: null pointer");
+  OG_CHECK_ARG(nloss >= 0 && nloss <= 256 && n >= 0, "train_skip_outputs: bad sizes");
+  if (nloss == 0 && n == 0) return OG_OK;
+  return OG_LAUNCH(train_skip_outputs_kernel, std::max(eltwise_grid(n), 1u), 256, 0, (cudaStream_t)stream, skip, loss, nloss, x, n);
 }
 
 static int bn_train_bwd_impl(const float* dy, int64_t lddy, const float* a_, int64_t lda, int rows, int cols, int relu,
@@ -1020,8 +1043,9 @@ int64_t og_optim_workspace_bytes(int nseg) { return nseg > 0 ? optim_workspace_b
 
 static bool unit_beta(double b) { return b >= 0.0 && b < 1.0; }
 
-int og_clip_adam_step(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
-                      double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes, void* stream) {
+static int clip_adam_impl(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
+                          double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes,
+                          const int* skip, void* stream) {
   OG_CHECK_ARG(segments && state && workspace, "clip_adam_step: null pointer");
   OG_CHECK_ARG(nseg > 0 && ntiles > 0, "clip_adam_step: nseg = %d and ntiles = %lld must be positive", nseg, (long long)ntiles);
   OG_CHECK_ARG(max_norm > 0.0, "clip_adam_step: max_norm = %g must be positive", max_norm);
@@ -1030,7 +1054,18 @@ int og_clip_adam_step(const og_optim_segment* segments, int nseg, int64_t ntiles
   OG_CHECK_ARG(lr_gamma > 0.0, "clip_adam_step: lr_gamma = %g must be positive", lr_gamma);
   if (workspace_bytes < optim_workspace_bytes(nseg)) return fail(OG_EWORKSPACE, "clip_adam_step: workspace too small");
   const OptHyper h = {beta1, beta2, eps, max_norm, lr_gamma};
-  return optim_step_launch(segments, nseg, ntiles, h, state, workspace, (cudaStream_t)stream);
+  return optim_step_launch(segments, nseg, ntiles, h, state, workspace, skip, (cudaStream_t)stream);
+}
+
+int og_clip_adam_step(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
+                      double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes, void* stream) {
+  return clip_adam_impl(segments, nseg, ntiles, beta1, beta2, eps, max_norm, lr_gamma, state, workspace, workspace_bytes, nullptr, stream);
+}
+
+int og_clip_adam_step_guarded(const og_optim_segment* segments, int nseg, int64_t ntiles, double beta1, double beta2, double eps,
+                              double max_norm, double lr_gamma, og_optim_state* state, void* workspace, int64_t workspace_bytes,
+                              const int* skip, void* stream) {
+  return clip_adam_impl(segments, nseg, ntiles, beta1, beta2, eps, max_norm, lr_gamma, state, workspace, workspace_bytes, skip, stream);
 }
 
 int og_adam_schedule(int64_t nsteps, double lr, double lr_gamma, double beta1, double beta2, double* lr_out, float* step_size,

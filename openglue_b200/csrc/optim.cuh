@@ -8,6 +8,9 @@
 //                        CTA to finish sums the partials in CTA order (deterministic, no float atomics), writes the norm and the
 //                        clip coefficient to the state block, advances every segment's step count and derives its Adam scalars;
 //   optim_update_kernel  launched with PDL after it: one fused pass per element (clip, m, v, p), then lr <- lr * gamma.
+// A nullable `skip` (int32 on the device, og_clip_adam_step_guarded) skips the step when it reads non-zero: the norm kernel writes
+// nothing, the update kernel only zeroes the gradients (parameters, moments, step counts, lr and sched_steps keep their bits).
+// A null `skip` or *skip == 0 is the step above, bit for bit.
 // HBM-bound: the norm reads 4 B per parameter, the update reads p, g, m, v and writes p, m, v (and g where clipping changes it).
 #pragma once
 #include "common.cuh"
@@ -57,8 +60,10 @@ __device__ __forceinline__ float clip_coefficient(float norm, double max_norm) {
 }
 
 __global__ void __launch_bounds__(OPT_THREADS) optim_norm_kernel(const og_optim_segment* __restrict__ segs, int nseg, int64_t ntiles,
-                                                                 OptHyper h, og_optim_state* state, double* partial, float2* scal) {
+                                                                 OptHyper h, og_optim_state* state, double* partial, float2* scal,
+                                                                 const int* skip) {
   tc::launch_dependents();                                    // the update kernel's CTAs may become resident; they wait for us
+  if (skip && *skip) return;                                  // a skipped step: no norm, no step count, the counter stays 0
   __shared__ double red[OPT_THREADS / 32];
   __shared__ bool last;
   double acc = 0.0;
@@ -126,8 +131,17 @@ struct AdamElt {
 };
 
 __global__ void __launch_bounds__(OPT_THREADS) optim_update_kernel(const og_optim_segment* __restrict__ segs, int nseg, int64_t ntiles,
-                                                                   OptHyper h, og_optim_state* state, const float2* __restrict__ scal) {
+                                                                   OptHyper h, og_optim_state* state, const float2* __restrict__ scal,
+                                                                   const int* skip) {
   tc::grid_dependency_wait();                                 // the norm kernel has completed: coefficient, steps and scalars are final
+  if (skip && *skip) {                                        // a skipped step leaves zero gradients and nothing else
+    for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+      const og_optim_segment& s = segs[optim_find_segment(segs, nseg, t)];
+      const int64_t base = (t - s.tile0) * OPT_TILE, end = min(base + OPT_TILE, s.numel);
+      for (int64_t j = base + threadIdx.x; j < end; j += OPT_THREADS) s.grad[j] = 0.f;
+    }
+    return;
+  }
   AdamElt op;
   op.coef = state->clip_coef;
   op.w1 = (float)(1.0 - h.beta1);
@@ -198,13 +212,13 @@ inline unsigned optim_update_grid(int64_t ntiles) {
 }
 
 inline int optim_step_launch(const og_optim_segment* segs, int nseg, int64_t ntiles, const OptHyper& h, og_optim_state* state,
-                             void* ws, cudaStream_t stream) {
+                             void* ws, const int* skip, cudaStream_t stream) {
   double* partial = static_cast<double*>(ws);
   float2* scal = reinterpret_cast<float2*>(partial + OPT_NORM_CTAS);
-  int rc = OG_LAUNCH(optim_norm_kernel, OPT_NORM_CTAS, OPT_THREADS, 0, stream, segs, nseg, ntiles, h, state, partial, scal);
+  int rc = OG_LAUNCH(optim_norm_kernel, OPT_NORM_CTAS, OPT_THREADS, 0, stream, segs, nseg, ntiles, h, state, partial, scal, skip);
   if (rc != OG_OK) return rc;
   return launch("optim_update_kernel", optim_update_kernel, LaunchAttr::pdl, dim3(optim_update_grid(ntiles)), dim3(OPT_THREADS), 0,
-                stream, segs, nseg, ntiles, h, state, (const float2*)scal);
+                stream, segs, nseg, ntiles, h, state, (const float2*)scal, skip);
 }
 
 // Test path of the device-derived scalars: the lr schedule of steps 1 .. n (lr_out[k] = the lr step k + 1 uses, one thread,

@@ -157,15 +157,22 @@ inline int colreduce_launch(ColReduceArgs a, cudaStream_t st) {
 // BatchNorm1d with batch statistics (torch.nn.functional.batch_norm, training=True): y = gamma (r - mu) / sqrt(var + eps) + beta,
 // r = relu(a) when the ReLU in front of the norm is fused in; var is the biased variance; the running statistics move by
 // `momentum` towards (mu, unbiased var).  A padded batch (len set) counts its real rows, sum_b len[b] (ColReduceArgs).
+// Guarded form (og_bn_train_fwd_guarded): a nullable device flag `skip` leaves the running statistics untouched when it reads
+// non-zero, and a nullable `num_batches_tracked` is incremented by 1 - *skip (by 1 without a flag) - BatchNorm1d's counter kept
+// on the device.  Null pointers give the unguarded arithmetic.
 __global__ void __launch_bounds__(256) bn_finish_stats_kernel(const float* __restrict__ mean, const float* __restrict__ var, int cols, int rows_all,
                                                               const int* __restrict__ len, int cap, float eps, float momentum,
                                                               float* __restrict__ invstd, float* __restrict__ running_mean,
-                                                              float* __restrict__ running_var) {
+                                                              float* __restrict__ running_var, const int* __restrict__ skip,
+                                                              long long* __restrict__ num_batches_tracked) {
   const int c = blockIdx.x * 256 + threadIdx.x;
   if (c >= cols) return;
+  const bool skipped = skip && *skip;
+  if (num_batches_tracked && c == 0 && !skipped) *num_batches_tracked += 1;
   const int rows = padded_count(len, rows_all, cap);
   const float v = var[c];
   invstd[c] = __fdiv_rn(1.f, __fsqrt_rn(v + eps));
+  if (skipped) return;
   if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean[c];
   if (running_var) {
     const float unbiased = rows > 1 ? v * __fdiv_rn((float)rows, (float)(rows - 1)) : v;
@@ -289,6 +296,33 @@ __global__ void __launch_bounds__(256) mix_param_grad_kernel(const float* __rest
   if (c >= d) return;
   const float al = __fdiv_rn(1.f, 1.f + expf(-mix[c]));
   dmix[c] = colsum[c] * al * (1.f - al);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// the skip of the reference's training_step (models/matching_module.py:96-97), decided on the device.  lengths [2B]: n_0 .. n_{B-1},
+// m_0 .. m_{B-1} as the front-ends wrote them.  skip = 1 when an image has no keypoint (the reference's `data is None`) or when one
+// side's real rows total fewer than 2 (what BatchNorm1d raises on: one value per channel), else 0.  One warp.
+__global__ void __launch_bounds__(32) train_guard_kernel(const int* __restrict__ lengths, int B, int* __restrict__ skip) {
+  const int lane = threadIdx.x;
+  bool empty = false;
+  unsigned tot[2] = {0u, 0u};                                 // saturated at 2: only "fewer than 2" matters
+  for (int i = lane; i < 2 * B; i += 32) {
+    const int l = lengths[i];
+    empty |= l <= 0;
+    unsigned& t = tot[i >= B];
+    t = min(t + (unsigned)max(l, 0), 2u);
+  }
+  empty = __any_sync(0xffffffffu, empty);
+  const unsigned s0 = __reduce_add_sync(0xffffffffu, tot[0]), s1 = __reduce_add_sync(0xffffffffu, tot[1]);
+  if (lane == 0) *skip = (empty || s0 < 2u || s1 < 2u) ? 1 : 0;
+}
+// a skipped step's outputs: loss[0 .. nloss) = NaN and x[0 .. n) = 0 when *skip != 0; nothing is written otherwise
+__global__ void __launch_bounds__(256) train_skip_outputs_kernel(const int* __restrict__ skip, float* __restrict__ loss, int nloss,
+                                                                 float* __restrict__ x, int64_t n) {
+  if (!*skip) return;
+  const int64_t i0 = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (i0 < nloss) loss[i0] = CUDART_NAN_F;
+  for (int64_t i = i0; i < n; i += (int64_t)gridDim.x * 256) x[i] = 0.f;
 }
 
 }  // namespace og

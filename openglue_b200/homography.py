@@ -35,18 +35,7 @@ def synthesize_homography_pairs(images_u8: torch.Tensor, offset: int, warp_offse
     ``warp_offset`` [B, 4, 2] integers in [-offset, offset): (x, y) of the corners (off, off), (off, H-off-1), (W-off-1, off),
     (W-off-1, H-off-1), in the reference's order; None draws them uniformly, as the reference's ``np.random.randint`` does, with
     ``torch.randint`` on ``generator``'s device (the images' device when None)."""
-    if not torch.is_tensor(images_u8) or images_u8.dtype != torch.uint8:
-        raise TypeError(f'images_u8 must be a uint8 tensor, got {getattr(images_u8, "dtype", type(images_u8))}')
-    if images_u8.dim() != 4 or images_u8.shape[3] != 3:
-        raise ValueError(f'images_u8 must be [B, H, W, 3] RGB, got {tuple(images_u8.shape)}')
-    B, H, W, _ = images_u8.shape
-    if isinstance(offset, bool) or int(offset) != offset:
-        raise TypeError(f'offset must be an integer, got {offset!r}')
-    offset = int(offset)
-    if B < 1 or B > 65535:
-        raise ValueError(f'the batch must hold 1 .. 65535 images, got {B}')
-    if offset < 1 or 2 * offset >= min(H, W):
-        raise ValueError(f'offset must be >= 1 with 2 * offset < min(H, W) = {min(H, W)}, got {offset}')
+    B, H, W, offset = _check_images(images_u8, offset)
     if warp_offset is not None:
         if not torch.is_tensor(warp_offset) or warp_offset.dtype.is_floating_point or warp_offset.dtype.is_complex \
                 or warp_offset.dtype == torch.bool:
@@ -62,7 +51,31 @@ def synthesize_homography_pairs(images_u8: torch.Tensor, offset: int, warp_offse
     if warp_offset is None:
         gdev = generator.device if generator is not None else dev
         warp_offset = torch.randint(-offset, offset, (B, 4, 2), generator=generator, device=gdev, dtype=torch.int32)
-    warp_offset = warp_offset.to(device=dev, dtype=torch.int32).contiguous()
+    return _pairs(images_u8, offset, warp_offset.to(device=dev, dtype=torch.int32).contiguous())
+
+
+def _check_images(images_u8: torch.Tensor, offset: int):
+    """-> (B, H, W, offset) of a valid images_u8 [B, H, W, 3] uint8 and offset; raises before any launch otherwise"""
+    if not torch.is_tensor(images_u8) or images_u8.dtype != torch.uint8:
+        raise TypeError(f'images_u8 must be a uint8 tensor, got {getattr(images_u8, "dtype", type(images_u8))}')
+    if images_u8.dim() != 4 or images_u8.shape[3] != 3:
+        raise ValueError(f'images_u8 must be [B, H, W, 3] RGB, got {tuple(images_u8.shape)}')
+    B, H, W, _ = images_u8.shape
+    if isinstance(offset, bool) or int(offset) != offset:
+        raise TypeError(f'offset must be an integer, got {offset!r}')
+    offset = int(offset)
+    if B < 1 or B > 65535:
+        raise ValueError(f'the batch must hold 1 .. 65535 images, got {B}')
+    if offset < 1 or 2 * offset >= min(H, W):
+        raise ValueError(f'offset must be >= 1 with 2 * offset < min(H, W) = {min(H, W)}, got {offset}')
+    return B, H, W, offset
+
+
+def _pairs(images_u8: torch.Tensor, offset: int, warp_offset: torch.Tensor) -> dict:
+    """The launch of synthesize_homography_pairs on checked arguments (``warp_offset``: int32 [B, 4, 2] on the images' device,
+    in range): no host synchronisation, so it can be captured in a CUDA graph."""
+    B, H, W, _ = images_u8.shape
+    dev = images_u8.device
     images_u8 = images_u8.detach().contiguous()
     h, w = H - 2 * offset, W - 2 * offset
     image0 = torch.empty(B, 1, h, w, dtype=torch.float32, device=dev)

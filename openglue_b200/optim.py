@@ -16,7 +16,7 @@ by the reference) are not built.  There is no CPU path.
 from __future__ import annotations
 
 import math
-from typing import Dict, List
+from typing import Dict, List, Optional
 
 import torch
 
@@ -35,6 +35,11 @@ class ClippedAdam(torch.optim.Optimizer):
     them), and the learning rate in float64.  Parameters whose ``.grad`` is None are skipped and their step does not advance,
     as in torch.  ``last_grad_norm`` is a 0-dim device tensor holding what ``clip_grad_norm_`` returned for the last step (a
     view that the next step overwrites).
+
+    ``step(skip=flag)`` (a device int32 [] flag, as ``og_train_guard`` writes it) is the same step behind the flag: when it reads
+    non-zero the gradients are zeroed and nothing else changes - parameters, moments, step counts, lr and the scheduler's count
+    keep their bits - without a host synchronisation.  Which parameters then have Adam state is known on the device only;
+    ``state_dict()`` reads it from their step counts.
 
     ``get_last_lr()``, ``state_dict()`` and ``load_state_dict()`` synchronise with the device.  ``state_dict()`` returns
     ``{'optimizer': ..., 'lr_scheduler': ...}`` in exactly the layout of torch's ``Adam.state_dict()`` / ``StepLR.state_dict()``,
@@ -89,6 +94,7 @@ class ClippedAdam(torch.optim.Optimizer):
             self._state = torch.zeros(3, dtype=torch.float64, device=dev)
             self._state[0].fill_(lr)
         self._stepped = [False] * len(ps)          # which parameters have Adam state (torch creates it at their first step)
+        self._unsure = set()                       # parameters first stepped behind a device flag: state iff their step count > 0
         self._key = None                           # (index, param pointer, grad pointer) of the uploaded segment table
         self._table = self._table_host = self._ws = None
         self._nseg = self._ntiles = 0
@@ -147,7 +153,9 @@ class ClippedAdam(torch.optim.Optimizer):
         self._nseg, self._ntiles = len(idx), tile
 
     @torch.no_grad()
-    def step(self, closure=None):
+    def step(self, closure=None, skip: Optional[torch.Tensor] = None):
+        if skip is not None and (not torch.is_tensor(skip) or skip.dtype != torch.int32 or skip.device != self.dev or skip.numel() != 1):
+            raise ValueError(f'ClippedAdam.step: skip must be a one-element int32 tensor on {self.dev}')
         loss = None
         if closure is not None:                    # Lightning's automatic optimisation: forward + backward run inside the closure
             with torch.enable_grad():
@@ -156,6 +164,8 @@ class ClippedAdam(torch.optim.Optimizer):
         idx = [i for i, p in enumerate(ps) if p.grad is not None]
         with torch.cuda.device(self.dev):
             if not idx:                            # Adam skips every parameter; StepLR still steps
+                if skip is not None:
+                    raise ValueError('ClippedAdam.step(skip=...) needs at least one parameter with a gradient')
                 self._lr.mul_(self.lr_gamma)
                 self._sched_steps.add_(1)
                 return loss
@@ -171,19 +181,29 @@ class ClippedAdam(torch.optim.Optimizer):
                 self._key = key
             b1, b2 = self.param_groups[0]['betas']
             lib = _cabi.lib()
-            rc = lib.og_clip_adam_step(ptr(self._table), self._nseg, self._ntiles, b1, b2, self.param_groups[0]['eps'], self.grad_clip,
-                                       self.lr_gamma, ptr(self._state), ptr(self._ws), self._ws.numel(), stream(self.dev))
-            _cabi.check(rc, 'og_clip_adam_step')
+            if skip is None:
+                rc = lib.og_clip_adam_step(ptr(self._table), self._nseg, self._ntiles, b1, b2, self.param_groups[0]['eps'], self.grad_clip,
+                                           self.lr_gamma, ptr(self._state), ptr(self._ws), self._ws.numel(), stream(self.dev))
+                _cabi.check(rc, 'og_clip_adam_step')
+            else:
+                rc = lib.og_clip_adam_step_guarded(ptr(self._table), self._nseg, self._ntiles, b1, b2, self.param_groups[0]['eps'],
+                                                   self.grad_clip, self.lr_gamma, ptr(self._state), ptr(self._ws), self._ws.numel(),
+                                                   ptr(skip), stream(self.dev))
+                _cabi.check(rc, 'og_clip_adam_step_guarded')
         self._last_idx = idx
-        self._stepped_now(idx)
+        self._stepped_now(idx, guarded=skip is not None)
         return loss
 
-    def _stepped_now(self, idx: List[int]) -> None:
+    def _stepped_now(self, idx: List[int], guarded: bool = False) -> None:
         """Parameters ``idx`` were just updated (by step() or a graph replay that contains it): they have Adam state, and
-        their version counters move so that caches keyed on them (SuperGlue's packed weights) see the new values."""
+        their version counters move so that caches keyed on them (SuperGlue's packed weights) see the new values.  ``guarded``:
+        the step may have been skipped on the device, so a parameter without state gets it only if its step count moved."""
         ps = self.param_groups[0]['params']
         for i in idx:
-            self._stepped[i] = True
+            if guarded and not self._stepped[i]:
+                self._unsure.add(i)
+            else:
+                self._stepped[i] = True
         torch.autograd.graph.increment_version([ps[i] for i in idx])
 
     def _snapshot(self):
@@ -212,6 +232,10 @@ class ClippedAdam(torch.optim.Optimizer):
         lr = float(self._lr.item())
         steps = self._steps.cpu()
         self.param_groups[0]['lr'] = lr
+        for i in list(self._unsure):               # a step behind a device flag counted only if it was not skipped
+            if float(steps[i]) > 0:
+                self._stepped[i] = True
+                self._unsure.discard(i)
         states = [{'step': steps[i].clone(), 'exp_avg': self._exp_avg[i], 'exp_avg_sq': self._exp_avg_sq[i]} if self._stepped[i] else None
                   for i in range(len(self._stepped))]
         return _torch_state_dicts(self._torch_pair(lr), states, int(self._sched_steps.item()))
@@ -236,6 +260,7 @@ class ClippedAdam(torch.optim.Optimizer):
         me['initial_lr'] = float(ag.get('initial_lr', ag['lr']))
         self.lr_gamma = float(sch_sd['gamma'])
         steps = torch.zeros(len(me['params']), dtype=torch.float32)
+        self._unsure = set()
         with torch.cuda.device(self.dev):
             for i, p in enumerate(me['params']):
                 st = adam.state.get(p)

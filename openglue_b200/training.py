@@ -20,7 +20,7 @@ the padding's contents never reach a result, and every gradient at a padding row
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -28,15 +28,16 @@ from . import _cabi
 from ._ops import _Ops, _pad4  # noqa: F401  (tests build their torch double of the kernels on _Ops' composite helpers)
 from .superglue import is_padded, padded_inputs
 
-__all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep']
+__all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep', 'ImagePairTrainStep']
 
 
 class _BN:
     """One BatchNorm1d call site: parameters, running buffers and what the backward pass needs."""
 
-    def __init__(self, mod: torch.nn.BatchNorm1d, lens: Optional[torch.Tensor] = None):
+    def __init__(self, mod: torch.nn.BatchNorm1d, lens: Optional[torch.Tensor] = None, skip: Optional[torch.Tensor] = None):
         self.mod = mod
         self.pk = {} if lens is None else {'lens': lens}           # padded batch: statistics over the real rows of every pair
+        self.skip = skip                                           # device flag: a skipped step moves no running buffer
 
     def forward(self, ops: _Ops, a: torch.Tensor) -> torch.Tensor:
         m = self.mod
@@ -44,6 +45,11 @@ class _BN:
         if m.momentum is None:
             raise NotImplementedError('BatchNorm1d(momentum=None) (cumulative average) is not built')
         track = m.track_running_stats and m.running_mean is not None
+        if self.skip is not None:                                  # num_batches_tracked += 1 - skip on the device
+            y, self.mean, self.invstd = ops.bn_fwd(a, m.weight, m.bias, m.eps, m.momentum, m.running_mean if track else None,
+                                                   m.running_var if track else None, skip=self.skip,
+                                                   num_batches_tracked=m.num_batches_tracked if track else None, **self.pk)
+            return y
         y, self.mean, self.invstd = ops.bn_fwd(a, m.weight, m.bias, m.eps, m.momentum, m.running_mean if track else None,
                                                m.running_var if track else None, **self.pk)
         if track:
@@ -62,9 +68,12 @@ class TrainStep:
     A padded batch (``num_keypoints0`` / ``num_keypoints1``, per-pair ``image0_size`` / ``image1_size`` optional, validated by
     :func:`~openglue_b200.superglue.padded_inputs`) gives each pair's outputs on its own block: ``scores[b, :n_b+1, :m_b+1]``
     (dustbins at n_b, m_b) and ``-inf`` elsewhere, context descriptors 0 past the lengths.  ``backward`` reads ``dscores`` on
-    those blocks and ``dctx`` on the real columns only; the local-descriptor gradients are 0 on the padding rows."""
+    those blocks and ``dctx`` on the real columns only; the local-descriptor gradients are 0 on the padding rows.
 
-    def __init__(self, model, data: dict, ops=None):
+    ``skip`` (device int32 [] flag, as ``og_train_guard`` writes it): the BatchNorm running statistics and ``num_batches_tracked``
+    move only when it reads 0; the outputs are computed either way."""
+
+    def __init__(self, model, data: dict, ops=None, skip: Optional[torch.Tensor] = None):
         model._check_head_dim()                         # before the forward pass moves any BatchNorm running buffer
         self.model = model
         cfg = model.config
@@ -86,6 +95,7 @@ class TrainStep:
             prec = model._precision()
             ops = _Ops(self.dev, _cabi.OG_PREC_FP32 if prec == _cabi.OG_PREC_FP32 else _cabi.OG_PREC_TF32X3)
         self.ops = ops                                  # (tests inject a torch double of the kernels to check this schedule on the CPU)
+        self.skip = skip
         f = lambda t, last: self._prep(t, last)
         self.kpts = [f(data['keypoints0'], 2), f(data['keypoints1'], 2)]
         self.side = [f(data['side_info0'], self.S), f(data['side_info1'], self.S)]
@@ -171,7 +181,7 @@ class TrainStep:
                     h = ops.kenc_input(self.kpts[i], self.side[i], rows, self.S, self.wh[i][0], self.wh[i][1])
                 rec = []
                 for j in range(nl - 1):
-                    conv, bn = enc[3 * j], _BN(enc[3 * j + 2], self._len(i))
+                    conv, bn = enc[3 * j], _BN(enc[3 * j + 2], self._len(i), self.skip)
                     a = ops.linear(h, self._w2(conv), conv.bias)
                     rec.append((h, bn))
                     h = bn.forward(ops, a)
@@ -225,7 +235,7 @@ class TrainStep:
         c1 = ops.axpby(xq, msg, 1.0, -1.0) if self.use_offset else xq
         fc = mod.fc
         a = ops.linear(c1, self._w2(fc[0]), fc[0].bias, A2=msg)
-        bn = _BN(fc[2], self._len(iq))
+        bn = _BN(fc[2], self._len(iq), self.skip)
         hbn = bn.forward(ops, a)
         out = ops.linear(hbn, self._w2(fc[3]), fc[3].bias, R=xq)
         self.calls.append(dict(name=name, mod=mod, xq=xq, xkv=xkv, iq=iq, ikv=ikv, q=q, k=k, v=v, o=o, msg=msg, c1=c1, bn=bn, hbn=hbn, **kl))
@@ -527,3 +537,282 @@ class GraphedTrainStep:
         if self.optimizer is not None:                                   # the kernels wrote the parameters through raw pointers
             self.optimizer._stepped_now(self._opt_idx)
         return {'loss': self.loss[0], 'metric_loss': self.loss[1]}
+
+
+# transformation type -> {tensor key: shape with B, h, w filled in by _transformation}
+_TF_KEYS = {'perspective': ('H',), '3d_reprojection': ('K0', 'K1', 'R', 'T', 'depth0', 'depth1')}
+
+
+class ImagePairTrainStep:
+    """The reference's ``training_step`` from images (models/matching_module.py:71-105 with features computed online, as
+    ``train.py`` and ``pretrain_homography.py`` run it), replayed as one CUDA graph::
+
+        opt = ClippedAdam.from_config(superglue, config['train'])
+        step = ImagePairTrainStep(local_feature, superglue.train(), config, optimizer=opt)
+        out = step(batch)                      # batch: 'image0' [B,1,H0,W0], 'image1' [B,1,H1,W1], 'transformation'
+        out = step.pretrain(images_u8, offset) # homography pretraining: uint8 RGB [B,H,W,3] -> synthesized pairs -> the same step
+
+    One call runs ``extract_padded`` on both images (K rows per image, ``capacity`` or the front-end's ``max_keypoints``),
+    ``prepare_features_output``, the per-pair image sizes, ``gt_matches`` with the device counts, the padded :class:`TrainStep`
+    forward, ``criterion``, the backward pass, the gradients into ``p.grad`` and, with ``optimizer`` (a
+    :class:`~openglue_b200.optim.ClippedAdam`), its step.  Without an optimiser the call ends with the gradients in ``p.grad``.
+    ``batch['transformation']`` is ``{'type': ['perspective'] * B, 'H' [B,3,3]}`` or ``{'type': ['3d_reprojection'] * B, 'K0',
+    'K1', 'R' [B,3,3], 'T' [B,3], 'depth0' [B,h0,w0], 'depth1' [B,h1,w1]}`` (depth images, as MegaDepth's loader gives them).
+    ``pretrain(images_u8, offset)`` draws each image's corner offsets with ``torch.randint`` on the default CUDA generator (new ones
+    on every replay; ``torch.cuda.manual_seed`` reproduces them), synthesizes the pairs (``synthesize_homography_pairs``) and runs
+    the same step.
+
+    The reference skips a batch in which an image has no keypoint (``data is None``); a batch in which one side's real rows total
+    fewer than 2 makes ``BatchNorm1d`` raise there.  Both are decided here on the device (``og_train_guard``): such a batch is
+    skipped - parameters, BatchNorm buffers and optimiser state keep their bits, ``p.grad`` is 0, the loss is NaN and
+    ``skipped`` is 1 - with no host synchronisation.
+
+    Returns device tensors: ``loss``, ``metric_loss`` (0-dim), ``skipped`` (int32, 0-dim), ``num_keypoints0`` /
+    ``num_keypoints1`` and ``overflow0`` / ``overflow1`` (int32 [B]: the front-end's flags, an image cut to K rows trains on its
+    first K) and, from ``pretrain``, ``warp_offset`` (int32 [B,4,2]) - copies, or the graph's own buffers with ``borrow=True``
+    (overwritten by the next call).
+
+    ``use_cuda_graph=True`` captures one graph per (image shapes and dtypes, K, transformation type and tensor shapes, precision,
+    device) after one eager warm-up run, which is not a training step: the BatchNorm buffers, the parameters and the optimiser
+    state are restored after it.  A graph is captured again when a parameter, buffer or gradient of the matcher is reallocated
+    or a weight of the front-end changes; at most ``max_graphs`` are kept.  ``use_cuda_graph=False`` runs the same chain
+    eagerly, with the same results bit for bit.
+
+    Not built: ``train.margin`` (the metric loss on padded batches), colour augmentation (``train.augmentations.name`` other
+    than ``'none'``) and fine-tuning the front-end (``features.finetune``)."""
+
+    _OUT_KEYS = ('loss', 'metric_loss', 'skipped', 'num_keypoints0', 'num_keypoints1', 'overflow0', 'overflow1')
+
+    def __init__(self, local_feature: torch.nn.Module, superglue, config: dict, optimizer=None, capacity: Optional[int] = None,
+                 use_cuda_graph: bool = True):
+        from .features import get_laf_to_sideinfo_converter
+        from .optim import ClippedAdam
+        from .superglue import SuperGlue
+        if not isinstance(superglue, SuperGlue):
+            raise TypeError('openglue_b200.ImagePairTrainStep trains an openglue_b200.SuperGlue')
+        if not superglue.training:
+            raise RuntimeError('ImagePairTrainStep runs the training-mode step: call superglue.train() first')
+        if not callable(getattr(local_feature, 'extract_padded', None)):
+            raise TypeError('openglue_b200.ImagePairTrainStep takes a front-end with extract_padded (OpenCVSIFT, SuperPointNet[Bn])')
+        if (config.get('features') or {}).get('finetune', False):
+            raise NotImplementedError('fine-tuning the front-end (features.finetune) is not built: openglue_b200 front-ends run in eval mode')
+        train = config['train']
+        if train.get('margin') is not None:
+            raise NotImplementedError('criterion(margin=...) on a padded batch (num_keypoints0 / num_keypoints1) is not built')
+        aug = (train.get('augmentations') or {}).get('name', 'none')
+        if aug != 'none':
+            raise NotImplementedError(f"train.augmentations.name = {aug!r}: colour augmentation is not built (only 'none')")
+        if optimizer is not None and not isinstance(optimizer, ClippedAdam):
+            raise TypeError('ImagePairTrainStep runs the optimiser step of openglue_b200.ClippedAdam only '
+                            f'(got {type(optimizer).__name__}): pass optimizer=None and step other optimisers after the call')
+        superglue._check_head_dim()
+        sg_cfg = config['superglue']
+        self.laf_converter = get_laf_to_sideinfo_converter(sg_cfg['laf_to_sideinfo_method'])
+        side = superglue.config['positional_encoding'].get('side_info_size', 1)
+        if side != 1 + self.laf_converter.side_info_dim:
+            raise ValueError(f"side_info_size {side} of the matcher does not fit laf_to_sideinfo_method "
+                             f"{sg_cfg['laf_to_sideinfo_method']!r} (1 + {self.laf_converter.side_info_dim} columns)")
+        d = superglue.config['descriptor_dim']
+        fd = getattr(local_feature, 'descriptor_dim', 128)                 # OpenCVSIFT: 128
+        if fd != d:
+            raise ValueError(f'the front-end describes keypoints in {fd} dimensions, the matcher takes {d}')
+        self.log_response = bool(sg_cfg.get('log_transform_response', False))
+        self.positive_threshold = float(train['gt_positive_threshold'])  # as in the reference, the labels do not depend on them
+        self.negative_threshold = train.get('gt_negative_threshold')
+        self.nll_weight = float(train.get('nll_weight', 1.0))
+        self.metric_weight = float(train.get('metric_weight', 0.0))      # multiplies metric_loss = 0 (margin None)
+        local_feature.eval()                                               # matching_module.py:77-78
+        self.local_feature, self.superglue, self.optimizer = local_feature, superglue, optimizer
+        self.capacity, self.use_cuda_graph = capacity, use_cuda_graph
+        self.params = list(superglue.named_parameters())
+        self._grads = None                                                 # one zero-padded buffer behind every p.grad
+        self._graphs: Dict[tuple, tuple] = {}
+        self.max_graphs = 4
+
+    # ------------------------------------------------------------------ the chain
+    def _bind_grads(self, dev) -> None:
+        """p.grad = views of one buffer (16-byte aligned slices), so that a skipped step zeroes every gradient in one launch"""
+        if self._grads is None or self._grads[0].device != dev or any(p.device != dev for _, p in self.params):
+            sizes = [(p.numel() + 3) // 4 * 4 for _, p in self.params]
+            flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
+            views, off = [], 0
+            for (_, p), n in zip(self.params, sizes):
+                views.append(flat[off:off + p.numel()].view(p.shape))
+                off += n
+            self._grads = (flat, views)
+        for (_, p), g in zip(self.params, self._grads[1]):
+            if p.grad is not g:
+                p.grad = g
+
+    def _chain(self, image0: torch.Tensor, image1: torch.Tensor, tf: dict, K: int) -> Dict[str, torch.Tensor]:
+        from .features import prepare_features_output
+        from .gt_matches import gt_matches
+        from .losses import _run as criterion_run
+        dev = image0.device
+        B = image0.shape[0]
+        lib, st = _cabi.lib(), _cabi.stream(dev)
+        data, out = {}, {}
+        for i, img in ((0, image0), (1, image1)):
+            lafs, resp, desc, num, over = self.local_feature.extract_padded(img, K)
+            f = prepare_features_output(lafs, resp, desc, self.laf_converter, log_response=self.log_response)
+            size = torch.empty(B, 2, dtype=torch.float32, device=dev)         # (W, H) per pair, filled on the device
+            size[:, 0] = float(img.shape[3])
+            size[:, 1] = float(img.shape[2])
+            data.update({f'keypoints{i}': f['keypoints'], f'side_info{i}': f['side_info'], f'local_descriptors{i}': desc,
+                         f'num_keypoints{i}': num, f'image{i}_size': size})
+            out.update({f'num_keypoints{i}': num, f'overflow{i}': over})
+        lens = torch.cat([out['num_keypoints0'], out['num_keypoints1']])
+        skip = torch.empty((), dtype=torch.int32, device=dev)
+        _cabi.check(lib.og_train_guard(_cabi.ptr(lens), B, _cabi.ptr(skip), st), 'og_train_guard')
+        gt0, gt1 = gt_matches(data['keypoints0'], data['keypoints1'], tf, lens)
+        y_true = {'gt_matches0': gt0, 'gt_matches1': gt1, 'num_keypoints0': out['num_keypoints0'], 'num_keypoints1': out['num_keypoints1']}
+        step = TrainStep(self.superglue, data, skip=skip)
+        scores, _, _ = step.forward()
+        loss, dscores = criterion_run(y_true, {'scores': scores}, True, self.nll_weight)
+        grads = step.backward(dscores)
+        for name, p in self.params:
+            p.grad.copy_(grads[name].reshape(p.shape))
+        flat = self._grads[0]
+        if self.optimizer is None:                                         # loss = NaN and every p.grad = 0 when skipped
+            _cabi.check(lib.og_train_skip_outputs(_cabi.ptr(skip), _cabi.ptr(loss), 2, _cabi.ptr(flat), flat.numel(), st), 'og_train_skip_outputs')
+        else:                                                              # the guarded optimiser step zeroes the gradients
+            _cabi.check(lib.og_train_skip_outputs(_cabi.ptr(skip), _cabi.ptr(loss), 2, None, 0, st), 'og_train_skip_outputs')
+            self.optimizer.step(skip=skip)
+        out.update(loss=loss[0], metric_loss=loss[1], skipped=skip)
+        return out
+
+    # ------------------------------------------------------------------ arguments
+    def _K(self) -> int:
+        from .features import padded_capacity
+        return padded_capacity(self.local_feature.max_keypoints, self.capacity)
+
+    def _check_model(self, dev) -> None:
+        for _, p in self.params:
+            if p.device != dev or p.dtype != torch.float32:
+                raise RuntimeError('openglue_b200 training needs float32 parameters on the device of the images')
+        if not self.superglue.training:
+            raise RuntimeError('ImagePairTrainStep runs the training-mode step: call superglue.train() first')
+        if self.optimizer is not None and self.optimizer.dev != dev:
+            raise RuntimeError(f'the optimiser holds its state on {self.optimizer.dev}, the images are on {dev}')
+
+    @staticmethod
+    def _images(image0, image1) -> None:
+        for i, img in ((0, image0), (1, image1)):
+            if not torch.is_tensor(img) or img.dim() != 4 or img.shape[1] != 1:
+                raise ValueError(f'image{i} must be [B, 1, H, W], got {tuple(img.shape) if torch.is_tensor(img) else type(img)}')
+        if image0.shape[0] != image1.shape[0] or image0.shape[0] < 1:
+            raise ValueError(f'image0 and image1 must hold the same number of images, got {image0.shape[0]} and {image1.shape[0]}')
+
+    @staticmethod
+    def _transformation(tf: dict, B: int) -> Tuple[str, Dict[str, torch.Tensor]]:
+        """-> (type, {key: tensor}) of batch['transformation'], shapes checked (depth: images [B, h, w])"""
+        kind = tf['type'][0] if isinstance(tf['type'], (list, tuple)) else tf['type']
+        if kind not in _TF_KEYS:
+            raise ValueError(f'Unknown transformation type {kind}.')
+        want = {'H': (B, 3, 3), 'K0': (B, 3, 3), 'K1': (B, 3, 3), 'R': (B, 3, 3), 'T': (B, 3)}
+        out = {}
+        for k in _TF_KEYS[kind]:
+            t = tf[k]
+            if not torch.is_tensor(t):
+                raise TypeError(f'transformation[{k!r}] must be a tensor')
+            ok = tuple(t.shape) == want[k] if k in want else (t.dim() == 3 and t.shape[0] == B)
+            if not ok:
+                raise ValueError(f"transformation[{k!r}] has shape {tuple(t.shape)}, expected {want.get(k, f'[{B}, h, w]')}")
+            out[k] = t
+        return kind, out
+
+    # ------------------------------------------------------------------ graphs
+    def _versions(self) -> tuple:
+        from .features import _frontend_version
+        sg = [t.data_ptr() for t in list(self.superglue.parameters()) + list(self.superglue.buffers())]
+        grads = [None if p.grad is None else p.grad.data_ptr() for _, p in self.params]
+        return tuple(sg), tuple(grads), _frontend_version(self.local_feature)
+
+    def _run(self, key: tuple, inputs: Dict[str, torch.Tensor], chain) -> Dict[str, torch.Tensor]:
+        """Replay (capturing on first use) the graph of ``chain(static inputs)`` for ``key``; the inputs are copied into its
+        static buffers.  Eager when use_cuda_graph is False."""
+        dev = self.superglue.dustbin_score.device
+        self._bind_grads(dev)
+        if not self.use_cuda_graph:
+            return chain(inputs)
+        opt, model = self.optimizer, self.superglue
+        entry = self._graphs.get(key)
+        if entry is not None and entry[3] != self._versions():
+            del self._graphs[key]                       # storage or weights the graph reads were replaced: capture again
+            entry = None
+        if entry is None:
+            static = {k: torch.empty(v.shape, dtype=torch.float32 if v.is_floating_point() else v.dtype, device=dev)
+                      for k, v in inputs.items()}
+            for k, v in inputs.items():
+                static[k].copy_(v)
+            saved = [b.clone() for b in model.buffers()]                   # the warm-up run is not a training step
+            saved_opt = None if opt is None else opt._snapshot()
+            chain(static)                                                  # warm-up: weights, workspaces, kernel attributes
+            torch.cuda.synchronize(dev)
+            for b, s in zip(model.buffers(), saved):
+                b.copy_(s)
+            if opt is not None:                                            # parameters and optimiser state
+                opt._restore(saved_opt)
+            # the front-end's cached workspaces and packed weights are baked into the graph: hold them
+            held = (tuple(getattr(self.local_feature, '_ws', {}).values()), getattr(self.local_feature, '_packed', None))
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                out = chain(static)
+            if opt is not None:                                            # the capture ran nothing
+                opt._stepped = list(saved_opt[-1])
+            while len(self._graphs) >= self.max_graphs:                    # bounded memory: drop the oldest shape
+                del self._graphs[next(iter(self._graphs))]
+            entry = self._graphs[key] = (graph, static, out, self._versions(), held, None if opt is None else opt._last_idx)
+        graph, static, out = entry[:3]
+        for k, v in inputs.items():
+            static[k].copy_(v, non_blocking=True)
+        graph.replay()
+        if opt is not None:                                                # the kernels wrote the parameters through raw pointers
+            opt._stepped_now(entry[5], guarded=True)
+        return out
+
+    # ------------------------------------------------------------------ public
+    def __call__(self, batch: dict, borrow: bool = False) -> Dict[str, torch.Tensor]:
+        """One training step on ``batch`` (``image0``, ``image1``, ``transformation``).  ``borrow=True`` (CUDA-graph mode): the graph's
+        own output buffers instead of copies."""
+        image0, image1 = batch['image0'], batch['image1']
+        self._images(image0, image1)
+        B = image0.shape[0]
+        kind, tf = self._transformation(batch['transformation'], B)
+        K = self._K()
+        if image0.device.type != 'cuda' or image1.device != image0.device:
+            raise RuntimeError('openglue_b200.ImagePairTrainStep needs both images on one CUDA device (sm_90a); there is no CPU path')
+        dev = image0.device
+        self._check_model(dev)
+        inputs = {'image0': image0, 'image1': image1, **tf}
+
+        def chain(x):
+            t = {'type': [kind] * B, **{k: x[k] for k in tf}}
+            return self._chain(x['image0'], x['image1'], t, K)
+        key = (tuple(image0.shape), tuple(image1.shape), image0.dtype, image1.dtype, K, kind,
+               tuple((k, tuple(v.shape)) for k, v in tf.items()), self.superglue._precision(), str(dev))
+        with torch.cuda.device(dev):
+            out = self._run(key, inputs, chain)
+        return out if borrow or not self.use_cuda_graph else {k: v.clone() for k, v in out.items()}
+
+    def pretrain(self, images_u8: torch.Tensor, offset: int, borrow: bool = False) -> Dict[str, torch.Tensor]:
+        """Homography pretraining (``pretrain_homography.py``): ``synthesize_homography_pairs(images_u8, offset)`` with offsets drawn
+        on the device, then the step; the result also holds ``warp_offset`` [B, 4, 2]."""
+        from .homography import _check_images, _pairs
+        B, _, _, offset = _check_images(images_u8, offset)
+        K = self._K()
+        if images_u8.device.type != 'cuda':
+            raise RuntimeError('openglue_b200: images_u8 must be a CUDA tensor (sm_90a); there is no CPU path')
+        dev = images_u8.device
+        self._check_model(dev)
+
+        def chain(x):
+            wo = torch.randint(-offset, offset, (B, 4, 2), device=dev, dtype=torch.int32)   # the default generator: graph-safe
+            pairs = _pairs(x['images_u8'], offset, wo)
+            out = self._chain(pairs['image0'], pairs['image1'], pairs['transformation'], K)
+            out['warp_offset'] = wo
+            return out
+        key = ('pretrain', tuple(images_u8.shape), offset, K, self.superglue._precision(), str(dev))
+        with torch.cuda.device(dev):
+            out = self._run(key, {'images_u8': images_u8}, chain)
+        return out if borrow or not self.use_cuda_graph else {k: v.clone() for k, v in out.items()}
