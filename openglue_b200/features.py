@@ -24,7 +24,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 import torch.nn as nn
 
-from . import _cabi
+from . import _cabi, _graphs
 from ._cabi import ptr, stream
 from .superglue import SuperGlue
 
@@ -242,6 +242,39 @@ def _frontend_version(module: nn.Module) -> tuple:
     return tuple((t.data_ptr(), t._version) for t in list(module.parameters()) + list(module.buffers()))
 
 
+def _frontend_storage(module: nn.Module) -> tuple:
+    """The front-end's cached workspaces and packed weights: a captured graph reads them, so it holds them even if the
+    front-end drops them later"""
+    return tuple(getattr(module, '_ws', {}).values()), getattr(module, '_packed', None)
+
+
+def _check_image_pair(image0, image1) -> None:
+    for i, img in ((0, image0), (1, image1)):
+        if not torch.is_tensor(img) or img.dim() != 4 or img.shape[1] != 1:
+            raise ValueError(f'image{i} must be [B, 1, H, W], got {tuple(img.shape) if torch.is_tensor(img) else type(img)}')
+    if image0.shape[0] != image1.shape[0] or image0.shape[0] < 1:
+        raise ValueError(f'image0 and image1 must hold the same number of images, got {image0.shape[0]} and {image1.shape[0]}')
+
+
+def _image_pair_inputs(local_feature: nn.Module, laf_converter: LAFConverter, log_response: bool, image0: torch.Tensor,
+                       image1: torch.Tensor, K: int) -> Tuple[Dict[str, torch.Tensor], Dict[str, torch.Tensor]]:
+    """The image-pair front-end: ``extract_padded`` on both images (K rows each), ``prepare_features_output`` and the per-pair
+    image sizes -> (the padded matcher inputs, {``lafs{i}``, ``keypoints{i}``, ``num_keypoints{i}``, ``overflow{i}``})."""
+    dev = image0.device
+    B = image0.shape[0]
+    data, feats = {}, {}
+    for i, img in ((0, image0), (1, image1)):
+        lafs, resp, desc, num, over = local_feature.extract_padded(img, K)
+        f = prepare_features_output(lafs, resp, desc, laf_converter, log_response=log_response)
+        size = torch.empty(B, 2, dtype=torch.float32, device=dev)        # (W, H) per pair, filled on the device
+        size[:, 0] = float(img.shape[3])
+        size[:, 1] = float(img.shape[2])
+        data.update({f'keypoints{i}': f['keypoints'], f'side_info{i}': f['side_info'], f'local_descriptors{i}': desc,
+                     f'num_keypoints{i}': num, f'image{i}_size': size})
+        feats.update({f'lafs{i}': lafs, f'keypoints{i}': f['keypoints'], f'num_keypoints{i}': num, f'overflow{i}': over})
+    return data, feats
+
+
 class ImagePairMatcher(nn.Module):
     """Batches of image pairs to matches with no host synchronisation, replayed as one CUDA graph by default.
 
@@ -279,23 +312,14 @@ class ImagePairMatcher(nn.Module):
         self.match_threshold = float(match_config['inference']['match_threshold'])
         self.capacity = capacity
         self.use_cuda_graph = use_cuda_graph
-        self._graphs: Dict[tuple, tuple] = {}
+        self._graphs: Dict[tuple, _graphs.Entry] = {}
         self.max_graphs = 4
         self.eval()
 
     def _chain(self, image0: torch.Tensor, image1: torch.Tensor, K: int) -> Dict[str, torch.Tensor]:
         dev = image0.device
         B = image0.shape[0]
-        data, out = {}, {}
-        for i, img in ((0, image0), (1, image1)):
-            lafs, resp, desc, num, over = self.local_feature.extract_padded(img, K)
-            f = prepare_features_output(lafs, resp, desc, self.laf_converter, log_response=self.log_response)
-            size = torch.empty(B, 2, dtype=torch.float32, device=dev)        # (W, H) per pair, filled on the device
-            size[:, 0] = float(img.shape[3])
-            size[:, 1] = float(img.shape[2])
-            data.update({f'keypoints{i}': f['keypoints'], f'side_info{i}': f['side_info'], f'local_descriptors{i}': desc,
-                         f'num_keypoints{i}': num, f'image{i}_size': size})
-            out.update({f'lafs{i}': lafs, f'keypoints{i}': f['keypoints'], f'num_keypoints{i}': num, f'overflow{i}': over})
+        data, out = _image_pair_inputs(self.local_feature, self.laf_converter, self.log_response, image0, image1, K)
         res = self.matcher.run(data, want_matches=True, want_context=False, match_threshold=self.match_threshold)
         m0, s0, m1, s1 = res['matches0'], res['matching_scores0'], res['matches1'], res['matching_scores1']
         with torch.cuda.device(dev):
@@ -312,39 +336,15 @@ class ImagePairMatcher(nn.Module):
         dev = image0.device
         key = (tuple(image0.shape), tuple(image1.shape), image0.dtype, image1.dtype, K, str(dev), self.matcher._precision(),
                self.match_threshold)
-        entry = self._graphs.get(key)
-        if entry is not None and entry[4] != self._versions():
-            del self._graphs[key]                # buffers or weights the graph reads were replaced: capture again
-            entry = None
-        if entry is None:
-            static0, static1 = torch.empty_like(image0), torch.empty_like(image1)
-            static0.copy_(image0)
-            static1.copy_(image1)
-            self._chain(static0, static1, K)                                    # warm-up: weights, workspaces, kernel attributes
-            torch.cuda.synchronize(dev)
-            # the front-end's cached workspaces are baked into the graph: hold them even if the front-end drops them later
-            held = tuple(getattr(self.local_feature, '_ws', {}).values())
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = self._chain(static0, static1, K)
-            while len(self._graphs) >= self.max_graphs:                         # bounded memory: drop the oldest shape
-                del self._graphs[next(iter(self._graphs))]
-            entry = self._graphs[key] = (graph, static0, static1, out, self._versions(), held)
-        graph, static0, static1, out = entry[:4]
-        static0.copy_(image0)
-        static1.copy_(image1)
-        graph.replay()
-        return out
+        return _graphs.run(self._graphs, self.max_graphs, key, self._versions, {'image0': image0, 'image1': image1},
+                           lambda s: self._chain(s['image0'], s['image1'], K), dev, f32=False,
+                           hold=lambda: _frontend_storage(self.local_feature))
 
     @torch.no_grad()
     def forward(self, image0: torch.Tensor, image1: torch.Tensor, borrow: bool = False) -> Dict[str, torch.Tensor]:
         """``borrow=True`` (CUDA-graph mode): return the graph's own output buffers instead of copies; the next call on this
         matcher overwrites them (use it when the results are consumed on the same stream right away)."""
-        for i, img in ((0, image0), (1, image1)):
-            if not torch.is_tensor(img) or img.dim() != 4 or img.shape[1] != 1:
-                raise ValueError(f'image{i} must be [B, 1, H, W], got {tuple(img.shape) if torch.is_tensor(img) else type(img)}')
-        if image0.shape[0] != image1.shape[0] or image0.shape[0] < 1:
-            raise ValueError(f'image0 and image1 must hold the same number of images, got {image0.shape[0]} and {image1.shape[0]}')
+        _check_image_pair(image0, image1)
         K = padded_capacity(self.local_feature.max_keypoints, self.capacity)
         if image0.device.type != 'cuda' or image1.device != image0.device:
             raise RuntimeError('openglue_b200.ImagePairMatcher needs both images on one CUDA device (sm_90a); there is no CPU path')

@@ -17,7 +17,7 @@ from typing import Dict, Optional
 import torch
 import torch.nn as nn
 
-from . import _cabi
+from . import _cabi, _graphs
 from ._cabi import ptr, stream
 from .packing import pack_weights
 
@@ -80,6 +80,21 @@ def padded_inputs(data: dict, B: int, n: int, m: int) -> Dict[str, torch.Tensor]
             w, h = SuperGlue._image_wh(data, idx)
             out[f'image{idx}_size'] = torch.tensor([[w, h]], dtype=torch.float32).expand(B, 2)
     return out
+
+
+_MATCHER_KEYS = ('keypoints0', 'keypoints1', 'side_info0', 'side_info1', 'local_descriptors0', 'local_descriptors1')
+
+
+def _matcher_inputs(data: dict):
+    """A batch as the inputs of a captured matcher step -> ({name: tensor}, key constants): the six per-keypoint tensors plus a
+    padded batch's lengths and per-pair sizes (:func:`padded_inputs`); a uniform batch's image sizes, plain floats baked into
+    the graph, are the constants ``{'image0_size': (W, H), 'image1_size': (W, H)}``, read next to the tensors."""
+    tensors = {k: data[k] for k in _MATCHER_KEYS}
+    if is_padded(data):
+        k0, k1 = tensors['keypoints0'], tensors['keypoints1']
+        tensors.update(padded_inputs(data, k0.shape[0], k0.shape[1], k1.shape[1]))
+        return tensors, {}
+    return tensors, {'image0_size': SuperGlue._image_wh(data, 0), 'image1_size': SuperGlue._image_wh(data, 1)}
 
 
 # The autograd drop-in's outputs feed losses written against the reference layout, which read every pair's dustbins at
@@ -391,58 +406,24 @@ class MatchingCore(nn.Module):
         self.match_threshold = float(match_threshold)           # per core; the shared SuperGlue's config is not touched
         self.device = torch.device(device) if device is not None else None
         self.use_cuda_graph = use_cuda_graph
-        self._graphs: Dict[tuple, tuple] = {}
+        self._graphs: Dict[tuple, _graphs.Entry] = {}
         self.max_graphs = 4                                     # captured shapes kept (alternating shapes do not re-capture)
 
-    _TENSOR_KEYS = ('keypoints0', 'keypoints1', 'side_info0', 'side_info1', 'local_descriptors0', 'local_descriptors1')
+    _TENSOR_KEYS = _MATCHER_KEYS
     _OUT_KEYS = ('matches0', 'matching_scores0', 'matches1', 'matching_scores1')
 
     def _run_graph(self, data: dict, dev: torch.device) -> Dict[str, torch.Tensor]:
         """Replay (capturing on first use) the CUDA graph for this shape; inputs are copied into its static buffers."""
-        shapes = tuple(tuple(data[k].shape) for k in self._TENSOR_KEYS)
-        extra = {}
-        if is_padded(data):                      # lengths and sizes go through static buffers: not part of the key
-            k0, k1 = data['keypoints0'], data['keypoints1']
-            extra = padded_inputs(data, k0.shape[0], k0.shape[1], k1.shape[1])
-            sizes = 'padded'
-        else:
-            sizes = (SuperGlue._image_wh(data, 0), SuperGlue._image_wh(data, 1))   # plain floats (collated sizes are tensors)
+        sg = self.superglue
+        inputs, consts = _matcher_inputs(data)
         # the precision picks the captured kernels and packed-weight forms: a switch in config['precision'] repacks only at the
-        # next run, so the alloc-gen check below cannot see it yet
-        key = (shapes, sizes, str(dev), self.superglue._weights_version(), self.superglue._precision(), self.match_threshold)
-        entry = self._graphs.get(key)
-        if entry is not None and entry[3] != getattr(self.superglue, '_alloc_gen', 0):
-            # the SuperGlue's workspace / packed weights were reallocated since this graph was captured (a bigger call
-            # on the same module, another core sharing it): its kernels would read and write freed blocks
-            del self._graphs[key]
-            entry = None
-        if entry is None:
-            static = dict(data)
-            if extra:                                                                # sizes come from image*_size alone
-                static.pop('image0', None)
-                static.pop('image1', None)
-            for k in self._TENSOR_KEYS:
-                static[k] = torch.empty(data[k].shape, dtype=torch.float32, device=dev)
-                static[k].copy_(data[k], non_blocking=True)
-            for k, v in extra.items():
-                static[k] = torch.empty(v.shape, dtype=v.dtype, device=dev)
-                static[k].copy_(v, non_blocking=True)
-            run = lambda: self.superglue.run(static, want_matches=True, want_context=False, match_threshold=self.match_threshold)
-            run()                                                                    # warm-up: builds weights, workspace, attributes
-            torch.cuda.synchronize(dev)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = run()
-            while len(self._graphs) >= self.max_graphs:                              # bounded memory: drop the oldest shape
-                del self._graphs[next(iter(self._graphs))]
-            entry = self._graphs[key] = (graph, static, out, getattr(self.superglue, '_alloc_gen', 0))
-        graph, static, out, _ = entry
-        for k in self._TENSOR_KEYS:
-            static[k].copy_(data[k], non_blocking=True)
-        for k, v in extra.items():
-            static[k].copy_(v, non_blocking=True)
-        graph.replay()
-        return out
+        # next run, so the version cannot see it yet
+        key = (tuple(tuple(data[k].shape) for k in _MATCHER_KEYS), tuple(consts.values()), str(dev), sg._precision(),
+               self.match_threshold)
+        # workspace / packed weights reallocated (by a bigger call, or another core sharing the SuperGlue) or weights changed
+        version = lambda: (getattr(sg, '_alloc_gen', 0), sg._weights_version())
+        chain = lambda s: sg.run({**s, **consts}, want_matches=True, want_context=False, match_threshold=self.match_threshold)
+        return _graphs.run(self._graphs, self.max_graphs, key, version, inputs, chain, dev, f32=True)
 
     def forward(self, data: dict, want_scores: bool = False, borrow: bool = False) -> Dict[str, torch.Tensor]:
         """``borrow=True`` (device input, CUDA-graph mode): return the graph's own output buffers instead of copies; they are

@@ -24,9 +24,11 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from . import _cabi
+from . import _cabi, _graphs
 from ._ops import _Ops, _pad4  # noqa: F401  (tests build their torch double of the kernels on _Ops' composite helpers)
-from .superglue import is_padded, padded_inputs
+from .features import (_check_image_pair, _frontend_storage, _frontend_version, _image_pair_inputs,
+                       get_laf_to_sideinfo_converter, padded_capacity)
+from .superglue import _MATCHER_KEYS, _matcher_inputs, is_padded, padded_inputs
 
 __all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep', 'ImagePairTrainStep']
 
@@ -415,6 +417,56 @@ def train_forward(model, data: dict) -> Dict[str, torch.Tensor]:
     return {'context_descriptors0': c0, 'context_descriptors1': c1, 'scores': scores}
 
 
+def _bind_grads(params, grads, dev):
+    """p.grad = views of one buffer (16-byte aligned slices) -> (buffer, views), passed back in as ``grads``: a skipped step zeroes
+    every gradient in one launch, and a captured graph's gradients stay where ``p.grad`` points after ``zero_grad()``"""
+    if grads is None or grads[0].device != dev or any(p.device != dev for _, p in params):
+        sizes = [(p.numel() + 3) // 4 * 4 for _, p in params]
+        flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
+        views, off = [], 0
+        for (_, p), n in zip(params, sizes):
+            views.append(flat[off:off + p.numel()].view(p.shape))
+            off += n
+        grads = (flat, views)
+    for (_, p), g in zip(params, grads[1]):
+        if p.grad is not g:
+            p.grad = g
+    return grads
+
+
+def _pointers(model, params) -> tuple:
+    """The storage of the parameters, buffers and gradients a captured step reads; not their versions, which every step bumps"""
+    return (tuple(t.data_ptr() for t in list(model.parameters()) + list(model.buffers())),
+            tuple(None if p.grad is None else p.grad.data_ptr() for _, p in params))
+
+
+class _WarmupGuard:
+    """The warm-up run before a capture is not a training step: the BatchNorm buffers and, with an optimiser, the parameters
+    and its state are put back after it.  ``guarded``: the replayed optimiser step may have been skipped on the device."""
+
+    def __init__(self, model, optimizer, guarded: bool):
+        self.model, self.opt, self.guarded = model, optimizer, guarded
+
+    def save(self) -> None:
+        self._saved = [b.clone() for b in self.model.buffers()], None if self.opt is None else self.opt._snapshot()
+
+    def restore(self) -> None:
+        for b, s in zip(self.model.buffers(), self._saved[0]):
+            b.copy_(s)
+        if self.opt is not None:
+            self.opt._restore(self._saved[1])
+
+    def captured(self):
+        snap, self._saved = self._saved[1], None
+        if self.opt is not None:                                         # the capture ran nothing: no parameter has new state
+            self.opt._stepped = list(snap[-1])
+            return self.opt._last_idx
+
+    def replayed(self, idx) -> None:
+        if self.opt is not None:                                         # the kernels wrote the parameters through raw pointers
+            self.opt._stepped_now(idx, guarded=self.guarded)
+
+
 class GraphedTrainStep:
     """The whole training step of one batch shape - train-mode forward, ``criterion``, backward, gradients into ``param.grad`` and,
     with ``optimizer`` (a :class:`~openglue_b200.optim.ClippedAdam`), the optimiser step - captured ONCE into a CUDA graph and
@@ -431,8 +483,10 @@ class GraphedTrainStep:
     buffers, and with ``optimizer`` the parameters and its state, are restored after it, so the first replay is step 1.
 
     The graph reads the parameters and BatchNorm buffers in place (so optimiser steps and running statistics carry over) and the
-    inputs from static copies.  Re-create the object when shapes change or parameters are re-allocated (``.to()``, ``load_state_dict``
-    keeps storage and is fine).  Results are bit-identical to the eager step (same kernels, same order).
+    inputs from static copies.  Every call must keep the captured shapes and, for a uniform batch, the captured image sizes, which
+    the graph bakes in: another shape or size raises ``ValueError``.  ``p.grad`` is bound again on every call (``zero_grad()``
+    may have set it to None), and the step is captured again when a parameter, buffer or gradient is re-allocated (``p.data =
+    ...``; ``load_state_dict`` keeps storage).  Results are bit-identical to the eager step (same kernels, same order).
 
     ``margin`` / ``metric_weight`` (the reference's ``train.margin`` / ``train.metric_weight``, matching_module.py:101-105): with a
     margin the graph also computes ``metric_loss`` on the context descriptors (``og_metric_loss_fwd``) and backpropagates
@@ -443,8 +497,6 @@ class GraphedTrainStep:
     ``image1_size`` optional): the lengths and sizes live in static device buffers like the other inputs, so one capture per
     capacity (B, N, M) replays every set of lengths; the step is :class:`TrainStep`'s padded step with :func:`criterion`'s
     per-pair loss.  ``margin`` is not built for padded batches."""
-
-    _KEYS = ('keypoints0', 'keypoints1', 'side_info0', 'side_info1', 'local_descriptors0', 'local_descriptors1')
 
     def __init__(self, model, data: dict, y_true: dict, nll_weight: float = 1.0, optimizer=None, margin: Optional[float] = None,
                  metric_weight: float = 0.0):
@@ -459,34 +511,22 @@ class GraphedTrainStep:
         if optimizer is not None and not isinstance(optimizer, ClippedAdam):
             raise TypeError('GraphedTrainStep captures the optimiser step of openglue_b200.ClippedAdam only '
                             f'(got {type(optimizer).__name__}): run other optimisers after the replay')
-        self.model, self.dev, self.optimizer = model, dev, optimizer
-        self.static = dict(data)
-        for k in self._KEYS:
-            self.static[k] = data[k].detach().float().contiguous().clone()
-        self.gt = {k: y_true[k].to(device=dev, dtype=torch.int64).contiguous().clone() for k in ('gt_matches0', 'gt_matches1')}
         self.padded = is_padded(data)
-        if self.padded:                                                  # lengths and sizes through static buffers: any set replays
-            if margin is not None:
-                raise NotImplementedError('GraphedTrainStep(margin=...) on a padded batch (num_keypoints0 / num_keypoints1) is not built')
-            self.static.pop('image0', None)
-            self.static.pop('image1', None)
-            for k, v in self._extra(data).items():
-                self.static[k] = v.to(dev).clone()
-            self.gt.update({k: self.static[k] for k in ('num_keypoints0', 'num_keypoints1')})
+        if self.padded and margin is not None:
+            raise NotImplementedError('GraphedTrainStep(margin=...) on a padded batch (num_keypoints0 / num_keypoints1) is not built')
+        self.model, self.dev, self.optimizer = model, dev, optimizer
         self.params = list(model.named_parameters())
-        for _, p in self.params:
-            if p.grad is None:
-                p.grad = torch.zeros_like(p)
+        self._guard = _WarmupGuard(model, optimizer, guarded=False)
+        inputs, self._key, consts = self._inputs(data, y_true)
 
-        def run():
-            step = TrainStep(model, self.static)
+        def chain(s):                         # s: the static inputs; a padded batch's labels read its lengths there too
+            step = TrainStep(model, {**s, **consts})
             scores, c0, c1 = step.forward()
-            loss, dscores = criterion_run(self.gt, {'scores': scores}, True, float(nll_weight))
+            loss, dscores = criterion_run(s, {'scores': scores}, True, float(nll_weight))
             if margin is None:
                 grads = step.backward(dscores)
             else:                                                        # metric_loss into loss[1]; its gradient scaled as autograd
-                _, _, dc0, dc1 = _metric_run(self.gt['gt_matches0'], self.gt['gt_matches1'], c0, c1, float(margin), True, 1.0,
-                                             out=loss[1:])
+                _, _, dc0, dc1 = _metric_run(s['gt_matches0'], s['gt_matches1'], c0, c1, float(margin), True, 1.0, out=loss[1:])
                 for dc in (dc0, dc1):                                    # scales the eager step's unit gradients (one rounding)
                     step.ops.axpby(dc, None, float(metric_weight), 0.0, out=dc)
                 grads = step.backward(dscores, dc0, dc1)
@@ -494,49 +534,36 @@ class GraphedTrainStep:
                 p.grad.copy_(grads[name].reshape(p.shape))
             if optimizer is not None:
                 optimizer.step()
-            return loss, scores
-
+            return loss
+        self._chain = chain
+        self._grads = _bind_grads(self.params, None, dev)
         with torch.cuda.device(dev):
-            saved = [b.clone() for b in model.buffers()]                # the warm-up run must not count as a training step
-            saved_opt = None if optimizer is None else optimizer._snapshot()
-            cur = torch.cuda.current_stream(dev)
-            side = torch.cuda.Stream(dev)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                run()                                                    # builds function attributes, allocator pools
-            cur.wait_stream(side)
-            torch.cuda.synchronize(dev)
-            for b, s in zip(model.buffers(), saved):
-                b.copy_(s)
-            if optimizer is not None:
-                optimizer._restore(saved_opt)
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self.loss, self.scores = run()
-            if optimizer is not None:                                    # the capture ran nothing: no parameter has state yet
-                self._opt_idx = optimizer._last_idx
-                optimizer._stepped = list(saved_opt[-1])
+            self._graphs = {self._key: _graphs.capture(inputs, chain, dev, f32=True, version=self._version, guard=self._guard)}
 
-    def _extra(self, data):
-        k0, k1 = data['keypoints0'], data['keypoints1']
-        return padded_inputs(data, k0.shape[0], k0.shape[1], k1.shape[1])
+    def _inputs(self, data: dict, y_true: dict):
+        """-> (static inputs, key, key constants) of a batch"""
+        tensors, consts = _matcher_inputs(data)
+        # labels as int64, whatever dtype they come in: og_metric_loss_fwd reads the static buffer as int64
+        tensors.update({k: y_true[k].to(torch.int64) for k in ('gt_matches0', 'gt_matches1')})
+        return tensors, (tuple(tuple(data[k].shape) for k in _MATCHER_KEYS), tuple(consts.values())), consts
+
+    def _version(self) -> tuple:
+        return _pointers(self.model, self.params)
 
     def __call__(self, data: dict, y_true: dict) -> Dict[str, torch.Tensor]:
         if is_padded(data) != self.padded:
             raise ValueError('the batch must be padded (num_keypoints0 / num_keypoints1) exactly when the captured one was')
-        for k in self._KEYS:
-            if tuple(data[k].shape) != tuple(self.static[k].shape):
-                raise ValueError(f'{k}: shape {tuple(data[k].shape)} differs from the captured {tuple(self.static[k].shape)}')
-            self.static[k].copy_(data[k], non_blocking=True)
-        if self.padded:
-            for k, v in self._extra(data).items():
-                self.static[k].copy_(v, non_blocking=True)
-        for k in ('gt_matches0', 'gt_matches1'):
-            self.gt[k].copy_(y_true[k], non_blocking=True)
-        self.graph.replay()
-        if self.optimizer is not None:                                   # the kernels wrote the parameters through raw pointers
-            self.optimizer._stepped_now(self._opt_idx)
-        return {'loss': self.loss[0], 'metric_loss': self.loss[1]}
+        inputs, key, _ = self._inputs(data, y_true)
+        for k, shape, want in zip(_MATCHER_KEYS, key[0], self._key[0]):
+            if shape != want:
+                raise ValueError(f'{k}: shape {shape} differs from the captured {want}')
+        if key[1] != self._key[1]:
+            raise ValueError(f'image sizes (W, H) {key[1]} differ from the captured {self._key[1]}: a uniform batch bakes them into '
+                             'the graph')
+        self._grads = _bind_grads(self.params, self._grads, self.dev)
+        with torch.cuda.device(self.dev):
+            loss = _graphs.run(self._graphs, 1, self._key, self._version, inputs, self._chain, self.dev, f32=True, guard=self._guard)
+        return {'loss': loss[0], 'metric_loss': loss[1]}
 
 
 # transformation type -> {tensor key: shape with B, h, w filled in by _transformation}
@@ -585,7 +612,6 @@ class ImagePairTrainStep:
 
     def __init__(self, local_feature: torch.nn.Module, superglue, config: dict, optimizer=None, capacity: Optional[int] = None,
                  use_cuda_graph: bool = True):
-        from .features import get_laf_to_sideinfo_converter
         from .optim import ClippedAdam
         from .superglue import SuperGlue
         if not isinstance(superglue, SuperGlue):
@@ -626,41 +652,19 @@ class ImagePairTrainStep:
         self.capacity, self.use_cuda_graph = capacity, use_cuda_graph
         self.params = list(superglue.named_parameters())
         self._grads = None                                                 # one zero-padded buffer behind every p.grad
-        self._graphs: Dict[tuple, tuple] = {}
+        self._guard = _WarmupGuard(superglue, optimizer, guarded=True)
+        self._graphs: Dict[tuple, _graphs.Entry] = {}
         self.max_graphs = 4
 
     # ------------------------------------------------------------------ the chain
-    def _bind_grads(self, dev) -> None:
-        """p.grad = views of one buffer (16-byte aligned slices), so that a skipped step zeroes every gradient in one launch"""
-        if self._grads is None or self._grads[0].device != dev or any(p.device != dev for _, p in self.params):
-            sizes = [(p.numel() + 3) // 4 * 4 for _, p in self.params]
-            flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
-            views, off = [], 0
-            for (_, p), n in zip(self.params, sizes):
-                views.append(flat[off:off + p.numel()].view(p.shape))
-                off += n
-            self._grads = (flat, views)
-        for (_, p), g in zip(self.params, self._grads[1]):
-            if p.grad is not g:
-                p.grad = g
-
     def _chain(self, image0: torch.Tensor, image1: torch.Tensor, tf: dict, K: int) -> Dict[str, torch.Tensor]:
-        from .features import prepare_features_output
         from .gt_matches import gt_matches
         from .losses import _run as criterion_run
         dev = image0.device
         B = image0.shape[0]
         lib, st = _cabi.lib(), _cabi.stream(dev)
-        data, out = {}, {}
-        for i, img in ((0, image0), (1, image1)):
-            lafs, resp, desc, num, over = self.local_feature.extract_padded(img, K)
-            f = prepare_features_output(lafs, resp, desc, self.laf_converter, log_response=self.log_response)
-            size = torch.empty(B, 2, dtype=torch.float32, device=dev)         # (W, H) per pair, filled on the device
-            size[:, 0] = float(img.shape[3])
-            size[:, 1] = float(img.shape[2])
-            data.update({f'keypoints{i}': f['keypoints'], f'side_info{i}': f['side_info'], f'local_descriptors{i}': desc,
-                         f'num_keypoints{i}': num, f'image{i}_size': size})
-            out.update({f'num_keypoints{i}': num, f'overflow{i}': over})
+        data, feats = _image_pair_inputs(self.local_feature, self.laf_converter, self.log_response, image0, image1, K)
+        out = {k: feats[k] for k in ('num_keypoints0', 'num_keypoints1', 'overflow0', 'overflow1')}
         lens = torch.cat([out['num_keypoints0'], out['num_keypoints1']])
         skip = torch.empty((), dtype=torch.int32, device=dev)
         _cabi.check(lib.og_train_guard(_cabi.ptr(lens), B, _cabi.ptr(skip), st), 'og_train_guard')
@@ -683,7 +687,6 @@ class ImagePairTrainStep:
 
     # ------------------------------------------------------------------ arguments
     def _K(self) -> int:
-        from .features import padded_capacity
         return padded_capacity(self.local_feature.max_keypoints, self.capacity)
 
     def _check_model(self, dev) -> None:
@@ -694,14 +697,6 @@ class ImagePairTrainStep:
             raise RuntimeError('ImagePairTrainStep runs the training-mode step: call superglue.train() first')
         if self.optimizer is not None and self.optimizer.dev != dev:
             raise RuntimeError(f'the optimiser holds its state on {self.optimizer.dev}, the images are on {dev}')
-
-    @staticmethod
-    def _images(image0, image1) -> None:
-        for i, img in ((0, image0), (1, image1)):
-            if not torch.is_tensor(img) or img.dim() != 4 or img.shape[1] != 1:
-                raise ValueError(f'image{i} must be [B, 1, H, W], got {tuple(img.shape) if torch.is_tensor(img) else type(img)}')
-        if image0.shape[0] != image1.shape[0] or image0.shape[0] < 1:
-            raise ValueError(f'image0 and image1 must hold the same number of images, got {image0.shape[0]} and {image1.shape[0]}')
 
     @staticmethod
     def _transformation(tf: dict, B: int) -> Tuple[str, Dict[str, torch.Tensor]]:
@@ -723,60 +718,24 @@ class ImagePairTrainStep:
 
     # ------------------------------------------------------------------ graphs
     def _versions(self) -> tuple:
-        from .features import _frontend_version
-        sg = [t.data_ptr() for t in list(self.superglue.parameters()) + list(self.superglue.buffers())]
-        grads = [None if p.grad is None else p.grad.data_ptr() for _, p in self.params]
-        return tuple(sg), tuple(grads), _frontend_version(self.local_feature)
+        return _pointers(self.superglue, self.params), _frontend_version(self.local_feature)
 
     def _run(self, key: tuple, inputs: Dict[str, torch.Tensor], chain) -> Dict[str, torch.Tensor]:
         """Replay (capturing on first use) the graph of ``chain(static inputs)`` for ``key``; the inputs are copied into its
         static buffers.  Eager when use_cuda_graph is False."""
         dev = self.superglue.dustbin_score.device
-        self._bind_grads(dev)
+        self._grads = _bind_grads(self.params, self._grads, dev)
         if not self.use_cuda_graph:
             return chain(inputs)
-        opt, model = self.optimizer, self.superglue
-        entry = self._graphs.get(key)
-        if entry is not None and entry[3] != self._versions():
-            del self._graphs[key]                       # storage or weights the graph reads were replaced: capture again
-            entry = None
-        if entry is None:
-            static = {k: torch.empty(v.shape, dtype=torch.float32 if v.is_floating_point() else v.dtype, device=dev)
-                      for k, v in inputs.items()}
-            for k, v in inputs.items():
-                static[k].copy_(v)
-            saved = [b.clone() for b in model.buffers()]                   # the warm-up run is not a training step
-            saved_opt = None if opt is None else opt._snapshot()
-            chain(static)                                                  # warm-up: weights, workspaces, kernel attributes
-            torch.cuda.synchronize(dev)
-            for b, s in zip(model.buffers(), saved):
-                b.copy_(s)
-            if opt is not None:                                            # parameters and optimiser state
-                opt._restore(saved_opt)
-            # the front-end's cached workspaces and packed weights are baked into the graph: hold them
-            held = (tuple(getattr(self.local_feature, '_ws', {}).values()), getattr(self.local_feature, '_packed', None))
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = chain(static)
-            if opt is not None:                                            # the capture ran nothing
-                opt._stepped = list(saved_opt[-1])
-            while len(self._graphs) >= self.max_graphs:                    # bounded memory: drop the oldest shape
-                del self._graphs[next(iter(self._graphs))]
-            entry = self._graphs[key] = (graph, static, out, self._versions(), held, None if opt is None else opt._last_idx)
-        graph, static, out = entry[:3]
-        for k, v in inputs.items():
-            static[k].copy_(v, non_blocking=True)
-        graph.replay()
-        if opt is not None:                                                # the kernels wrote the parameters through raw pointers
-            opt._stepped_now(entry[5], guarded=True)
-        return out
+        return _graphs.run(self._graphs, self.max_graphs, key, self._versions, inputs, chain, dev, f32=True,
+                           hold=lambda: _frontend_storage(self.local_feature), guard=self._guard)
 
     # ------------------------------------------------------------------ public
     def __call__(self, batch: dict, borrow: bool = False) -> Dict[str, torch.Tensor]:
         """One training step on ``batch`` (``image0``, ``image1``, ``transformation``).  ``borrow=True`` (CUDA-graph mode): the graph's
         own output buffers instead of copies."""
         image0, image1 = batch['image0'], batch['image1']
-        self._images(image0, image1)
+        _check_image_pair(image0, image1)
         B = image0.shape[0]
         kind, tf = self._transformation(batch['transformation'], B)
         K = self._K()
