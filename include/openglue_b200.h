@@ -562,8 +562,15 @@ int og_sp_sample_desc(const float* coarse, int B, int Hc, int Wc, int D, const f
  *   og_sift_fast_atan2       out[i] = cv2's fastAtan2(y[i], x[i]) in degrees: fused = cv::hal::fastAtan2's vector form, 0 = the
  *                            scalar one (cv2.fastAtan2)
  *   og_sift_gaussian_taps    host only: cv2's float Gaussian kernel for sigma (taps computed in double, rounded to float); returns the
- *                            number of taps, or OG_EUNSUPPORTED when it exceeds cap                                                  */
+ *                            number of taps, or OG_EUNSUPPORTED when it exceeds cap
+ *   og_sift_workspace_layout host only: where og_sift_detect keeps each stage's results in its workspace, for reading them back.
+ *                            out[0] = the octave count nO; out[1 + 4 o ..] = h, w, Gaussian offset, DoG offset of octave o (levels
+ *                            [6][B][h][w] and [5][B][h][w] float32); then the byte offsets of the located extrema (the SiftLoc
+ *                            records of csrc/sift.cuh, [B][cap]), the raw keypoints ([B][cap][5] float32), their octave words
+ *                            ([B][cap] int32) and the counts (int32: located [B], then raw keypoints [B]), and the workspace
+ *                            size.  Returns the number of entries written (1 + 4 nO + 5), or < 0 when n is too small       */
 int64_t og_sift_workspace_bytes(int B, int H, int W, int cap);
+int og_sift_workspace_layout(int B, int H, int W, int cap, int64_t* out, int n);
 int og_sift_detect(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,
                    int* count, void* stream);
 int og_sift_detect_padded(const void* image, int dtype, int B, int H, int W, int cap, void* ws, int64_t ws_bytes, float* kp, int* octave,

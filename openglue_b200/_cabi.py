@@ -145,6 +145,7 @@ SYMBOLS = {
     'og_sp_sample_desc': (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P]),
     # OpenCV SIFT front-end (row f7)
     'og_sift_workspace_bytes': (_L, [_I, _I, _I, _I]),
+    'og_sift_workspace_layout': (_I, [_I, _I, _I, _I, _P, _I]),
     'og_sift_detect': (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P, _P]),
     'og_sift_detect_padded': (_I, [_P, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P, _P, _P]),
     'og_sift_select_workspace_bytes': (_L, [_I, _I]),

@@ -864,6 +864,22 @@ int64_t og_sift_workspace_bytes(int B, int H, int W, int cap) {
   if (!sift_layout(B, H, W, cap, L)) return fail(OG_EUNSUPPORTED, "sift: a %d x %d image has no octave or more than %d", H, W, SIFT_MAX_OCTAVES);
   return L.total;
 }
+int og_sift_workspace_layout(int B, int H, int W, int cap, int64_t* out, int n) {
+  OG_CHECK_ARG(out, "sift_workspace_layout: null pointer");
+  const int64_t bytes = og_sift_workspace_bytes(B, H, W, cap);
+  if (bytes < 0) return (int)bytes;
+  SiftLayout L;
+  sift_layout(B, H, W, cap, L);
+  const int need = 1 + 4 * L.nO + 5;
+  OG_CHECK_ARG(n >= need, "sift_workspace_layout: %d entries, %d needed", n, need);
+  int i = 0;
+  out[i++] = L.nO;
+  for (int o = 0; o < L.nO; ++o) {
+    out[i++] = L.h[o]; out[i++] = L.w[o]; out[i++] = L.gauss_off[o]; out[i++] = L.dog_off[o];
+  }
+  out[i++] = L.loc_off; out[i++] = L.kp_off; out[i++] = L.oct_off; out[i++] = L.cnt_off; out[i++] = L.total;
+  return i;
+}
 int og_sift_gaussian_taps(double sigma, float* taps, int cap) {
   OG_CHECK_ARG(taps && sigma > 0 && cap > 0, "sift_gaussian_taps: bad arguments");
   const int n = sift_gaussian_taps(sigma, taps, cap);

@@ -61,6 +61,7 @@ struct SiftTaps { float k[SIFT_MAX_TAPS]; int n; };
 // A located extremum before orientation assignment: octave o (0 = the upsampled image), layer, pixel, cv2's packed octave word
 // and the keypoint in base-image coordinates as adjustLocalExtrema forms it.
 struct SiftLoc { int o, layer, r, c, octw; float x, y, size, response; };
+static_assert(sizeof(SiftLoc) == 36, "SiftLoc is read back as a 36-byte record (tests/test_sift_stages.py)");
 
 // ---------------------------------------------------------------------------------------------------------------------
 // cv2's fastAtan2 (degrees in [0, 360)): the polynomial of cv::hal::fastAtan2.  fused = the vector loop's form (v_fma), else the
