@@ -585,6 +585,42 @@ int og_sift_fast_atan2(const float* y, const float* x, int64_t n, int fused, flo
 int og_sift_gaussian_taps(double sigma, float* taps, int cap);
 
 /* ---------------------------------------------------------------------------------------------
+ * kornia's DoG SIFT front-end (the reference's SIFT, models/features/sift.py on base.py: ScaleSpaceDetector + run_nms + LAFDescriptor
+ * of kornia 0.6.3; csrc/kornia_sift.cuh).  B same-size float32 images [B, H, W] in [0, 1]; num_features (<= 8192) keypoints per image
+ * leave the detector.  Every stage is its own call, so a caller (or a test) can feed any stage its own inputs.
+ *   og_ksift_workspace_bytes   the workspace of pyramid / detect / describe (same B, H, W, num_features): octaves, responses,
+ *                              the selection state and the patch pyramid; < 0 when the image is not supported
+ *   og_ksift_workspace_layout  host only: out[0] = the octave count nO; out[1 + 5 o ..] = h, w, and the byte offsets of the Gaussian
+ *                              levels ([B][6][h][w]), the DoG ([B][5][h][w]) and the voxel responses ([B][5][h][w]) of octave o; then
+ *                              the patch-pyramid level count nP and per level h, w, byte offset (-1: level 0 is the image); then
+ *                              the workspace size.  Returns the number of entries written
+ *   og_ksift_pyramid           ScalePyramid(3, 1.6, 32, double_image=True) and BlobDoG into ws
+ *   og_ksift_detect            from the DoG in ws: conv_quad_interp3d on DoG and -DoG, the per-octave top-k of every voxel (response
+ *                              desc, voxel index asc), laf_is_inside_image, the global top-k (response desc, octave asc, per-octave
+ *                              rank asc) -> lafs [B, num_features, 2, 3] in image pixels (before orientation), resp [B, num_features],
+ *                              count [B] (rows past it are 0)
+ *   og_ksift_select_workspace_bytes / og_ksift_select
+ *                              base.py's run_nms on detector outputs lafs [B, cap, 2, 3], resp [B, cap], count [B] of H x W images:
+ *                              nms = 0 keeps every output; otherwise the float32 key sort (equal keys by index), unique positions,
+ *                              nms2d(nms_diameter, odd) on the scattered scores, then the first min(survivors, max_keypoints)
+ *                              survivors in detector order (their top-k; max_keypoints <= 0: no cap), survivors = the batch minimum
+ *                              when min_stack -> sel [B, cap] detector indices, n_sel [B]
+ *   og_ksift_describe          rows j < n[b] of lafs_out [B, out_cap, 2, 3], scores, desc [B, out_cap, 128] and angle (optional,
+ *                              [B, out_cap]: LAFOrienter's dominant orientation in radians) for detector output sel[b][j] (sel NULL:
+ *                              j): LAFOrienter(19) unless upright, then SIFTDescriptor(41, rootsift) on kornia's pyrdown patch pyramid
+ *                              of image; rows past n[b] are written as 0                                                       */
+int64_t og_ksift_workspace_bytes(int B, int H, int W, int num_features);
+int og_ksift_workspace_layout(int B, int H, int W, int num_features, int64_t* out, int n);
+int og_ksift_pyramid(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, void* stream);
+int og_ksift_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream);
+int64_t og_ksift_select_workspace_bytes(int B, int cap);
+int og_ksift_select(const float* lafs, const float* resp, const int* count, int B, int H, int W, int cap, int nms, int nms_diameter,
+                    int max_keypoints, int min_stack, void* work, int64_t work_bytes, int* sel, int* n_sel, void* stream);
+int og_ksift_describe(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs,
+                      const float* resp, int cap, const int* sel, const int* n, int out_cap, int upright, int rootsift, float* lafs_out,
+                      float* scores, float* desc, float* angle, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Local features -> matcher inputs, and matches -> the compact match list of stand-alone inference.
  *   og_prepare_features  prepare_features_output (models/features/utils.py:54-65) with the LAF -> side-information converter
  *                        superglue.laf_to_sideinfo_method names (models/laf_converter.py:108-128).  One thread per keypoint.

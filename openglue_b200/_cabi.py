@@ -154,6 +154,13 @@ SYMBOLS = {
     'og_sift_rootsift_laf': (_I, [_P, _P, _L, _I, _P, _P, _P, _P]),
     'og_sift_fast_atan2': (_I, [_P, _P, _L, _I, _P, _P]),
     'og_sift_gaussian_taps': (_I, [_D, _P, _I]),
+    'og_ksift_workspace_bytes': (_L, [_I, _I, _I, _I]),
+    'og_ksift_workspace_layout': (_I, [_I, _I, _I, _I, _P, _I]),
+    'og_ksift_pyramid': (_I, [_P, _I, _I, _I, _I, _P, _L, _P]),
+    'og_ksift_detect': (_I, [_I, _I, _I, _I, _P, _L, _P, _P, _P, _P]),
+    'og_ksift_select_workspace_bytes': (_L, [_I, _I]),
+    'og_ksift_select': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P]),
+    'og_ksift_describe': (_I, [_P, _I, _I, _I, _I, _P, _L, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
     # local features -> matcher inputs, matches -> compact list
     'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

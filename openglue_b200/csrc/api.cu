@@ -15,6 +15,7 @@
 #include "train_ops.cuh"
 #include "superpoint.cuh"
 #include "sift.cuh"
+#include "kornia_sift.cuh"
 #include "features.cuh"
 #include "homography.cuh"
 #include "optim.cuh"
@@ -1023,6 +1024,167 @@ int og_match_compact(const int64_t* matches0, const float* mscores0, const float
   OG_CHECK_ARG(B > 0 && n > 0 && m > 0 && (int64_t)B * n <= INT32_MAX - 1024, "match_compact: bad sizes");
   return OG_LAUNCH(match_compact_kernel, 1, 1024, 0, (cudaStream_t)stream, matches0, mscores0, lafs0, lafs1, B * n, n, m, pair, ij, confidence,
                    out_lafs0, out_lafs1, out_kpts0, out_kpts1, total);
+}
+
+// ---- kornia SIFT front-end (csrc/kornia_sift.cuh) ----
+static int ks_check_sizes(int B, int H, int W, int k, KsLayout& L, const char* who) {
+  if (B <= 0 || B > 65535 || H <= 0 || W <= 0 || k <= 0) return fail(OG_EINVAL, "%s: bad sizes", who);
+  if (k > KS_MAX_FEATURES) return fail(OG_EUNSUPPORTED, "%s: num_features %d above %d", who, k, KS_MAX_FEATURES);
+  if (min(H, W) < 2 || (int64_t)5 * 4 * H * W > 0xffffffffLL) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image is not supported", who, H, W);
+  if (!ks_layout(B, H, W, k, L)) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image has more than %d octaves", who, H, W, KS_MAX_OCTAVES);
+  return OG_OK;
+}
+int64_t og_ksift_workspace_bytes(int B, int H, int W, int num_features) {
+  KsLayout L;
+  if (const int rc = ks_check_sizes(B, H, W, num_features, L, "ksift_workspace_bytes")) return rc;
+  return L.bytes;
+}
+int og_ksift_workspace_layout(int B, int H, int W, int num_features, int64_t* out, int n) {
+  OG_CHECK_ARG(out, "ksift_workspace_layout: null pointer");
+  KsLayout L;
+  if (const int rc = ks_check_sizes(B, H, W, num_features, L, "ksift_workspace_layout")) return rc;
+  const int need = 1 + 5 * L.nO + 1 + 3 * L.np + 1;
+  OG_CHECK_ARG(n >= need, "ksift_workspace_layout: %d entries, %d needed", n, need);
+  int i = 0;
+  out[i++] = L.nO;
+  for (int o = 0; o < L.nO; ++o) {
+    out[i++] = L.oct[o].h; out[i++] = L.oct[o].w;
+    out[i++] = 4 * L.oct[o].gauss; out[i++] = 4 * L.oct[o].dog; out[i++] = 4 * L.oct[o].resp;
+  }
+  out[i++] = L.np;
+  for (int l = 0; l < L.np; ++l) { out[i++] = L.ph[l]; out[i++] = L.pw[l]; out[i++] = l == 0 ? -1 : 4 * L.pyr[l]; }
+  out[i++] = L.bytes;
+  return i;
+}
+static int ks_blur(float* ws_f, const KsLayout& L, int B, int h, int w, const float* src, int64_t src_stride, double sigma,
+                   float* dst, int64_t dst_stride, cudaStream_t st) {
+  KsTaps t;
+  const int k = ks_kernel_size(sigma, h, w);
+  if (k > KS_MAX_TAPS) return fail(OG_EUNSUPPORTED, "ksift: sigma %g needs more than %d taps", sigma, KS_MAX_TAPS);
+  ks_gaussian_taps(k, sigma, t);
+  const int64_t plane = (int64_t)h * w;
+  float* tmp = ws_f + L.tmp;
+  if (const int rc = OG_LAUNCH(ks_blur_kernel, sift_grid(B * plane), 256, 0, st, src, src_stride, B, h, w, t, 0, tmp, plane)) return rc;
+  return OG_LAUNCH(ks_blur_kernel, sift_grid(B * plane), 256, 0, st, (const float*)tmp, plane, B, h, w, t, 1, dst, dst_stride);
+}
+static int ks_args(void* ws, int64_t ws_bytes, int B, int H, int W, int k, KsLayout& L, const char* who) {
+  OG_CHECK_ARG(ws, "%s: null workspace", who);
+  if (const int rc = ks_check_sizes(B, H, W, k, L, who)) return rc;
+  OG_CHECK_ARG(ws_bytes >= L.bytes, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes, (long long)L.bytes);
+  return OG_OK;
+}
+int og_ksift_pyramid(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, void* stream) {
+  KsLayout L;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "ksift_pyramid")) return rc;
+  OG_CHECK_ARG(image, "ksift_pyramid: null image");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* f = static_cast<float*>(ws);
+  const KsOctave& o0 = L.oct[0];
+  const int64_t p0 = (int64_t)o0.h * o0.w;
+  float* g0 = f + o0.gauss;
+  if (const int rc = OG_LAUNCH(ks_upsample_kernel, sift_grid(B * p0), 256, 0, st, image, B, H, W, g0)) return rc;
+  // the upsampled image has sigma 1.0; the first level is blurred to 1.6
+  double cur = 1.6;
+  if (const int rc = ks_blur(f, L, B, o0.h, o0.w, g0, KS_LEVELS * p0, std::max(std::sqrt(1.6 * 1.6 - 1.0), 0.01), g0, KS_LEVELS * p0, st)) return rc;
+  const double step = std::pow(2.0, 1.0 / 3.0);
+  for (int o = 0; o < L.nO; ++o) {
+    const KsOctave& oc = L.oct[o];
+    const int64_t plane = (int64_t)oc.h * oc.w;
+    float* g = f + oc.gauss;
+    if (o > 0) {
+      const KsOctave& pv = L.oct[o - 1];
+      if (const int rc = OG_LAUNCH(ks_subsample_kernel, sift_grid(B * plane), 256, 0, st, (const float*)(f + pv.gauss), B, pv.h, pv.w,
+                                   oc.h, oc.w, g)) return rc;
+    }
+    cur = 1.6;
+    for (int l = 1; l < KS_LEVELS; ++l) {
+      const double sigma = cur * std::sqrt(step * step - 1.0);
+      if (const int rc = ks_blur(f, L, B, oc.h, oc.w, g + (l - 1) * plane, KS_LEVELS * plane, sigma, g + l * plane, KS_LEVELS * plane, st)) return rc;
+      cur *= step;
+    }
+    if (const int rc = OG_LAUNCH(ks_dog_kernel, sift_grid(B * KS_DOG * plane), 256, 0, st, (const float*)g, B, (int)plane, f + oc.dog)) return rc;
+  }
+  return OG_OK;
+}
+int og_ksift_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream) {
+  KsLayout L;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "ksift_detect")) return rc;
+  OG_CHECK_ARG(lafs && resp && count, "ksift_detect: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* f = static_cast<float*>(ws);
+  char* c = static_cast<char*>(ws);
+  const int segs = B * L.nO, k = L.k;
+  KsSel* sel = reinterpret_cast<KsSel*>(c + L.state);
+  unsigned int* hist = reinterpret_cast<unsigned int*>(c + L.hist);
+  unsigned long long* cand = reinterpret_cast<unsigned long long*>(c + L.cand);
+  int* cnt = reinterpret_cast<int*>(c + L.count);
+  if (const int rc = OG_LAUNCH(ks_select_init_kernel, cdiv(segs, 128), 128, 0, st, L, segs, sel, hist, cnt)) return rc;
+  for (int o = 0; o < L.nO; ++o) {
+    const KsOctave& oc = L.oct[o];
+    const int64_t per = (int64_t)KS_DOG * oc.h * oc.w;
+    if (const int rc = OG_LAUNCH(ks_response_kernel, sift_grid(B * per), 256, 0, st, (const float*)(f + oc.dog), B, oc.h, oc.w, f + oc.resp)) return rc;
+    const dim3 grid((unsigned)std::min<int64_t>(cdiv((int)std::min<int64_t>(per, INT_MAX), 2048), 512), B);
+    for (int pass = 0; pass < 8; ++pass) {
+      if (const int rc = OG_LAUNCH(ks_hist_kernel, grid, 256, 0, st, (const float*)(f + oc.resp), per, o, L.nO, (const KsSel*)sel, hist)) return rc;
+      if (const int rc = OG_LAUNCH(ks_pick_kernel, cdiv(B, 128), 128, 0, st, B, o, L.nO, sel, hist)) return rc;
+    }
+    if (const int rc = OG_LAUNCH(ks_compact_kernel, grid, 256, 0, st, (const float*)(f + oc.resp), per, o, L.nO, (const KsSel*)sel, k, cand, cnt)) return rc;
+  }
+  const size_t smem = (size_t)pow2_ceil(k) * 8;
+  if (const int rc = smem_opt_in<ks_octave_list_kernel<512>>((int)((size_t)KS_MAX_FEATURES * 8))) return rc;
+  KsCand* list = reinterpret_cast<KsCand*>(c + L.list);
+  KsCand* scratch = reinterpret_cast<KsCand*>(c + L.scratch);
+  if (const int rc = OG_LAUNCH(ks_octave_list_kernel<512>, segs, 512, smem, st, (const float*)f, L, B, H, W, (const int*)cnt, scratch, list,
+                               (const unsigned long long*)cand)) return rc;
+  if (const int rc = OG_LAUNCH(ks_merge_kernel, dim3(cdiv(k, 256), L.nO, B), 256, 0, st, (const KsCand*)list, (const int*)cnt, L.nO, k,
+                               lafs, resp, count)) return rc;
+  return OG_LAUNCH(ks_det_tail_kernel, dim3(cdiv(k, 256), B), 256, 0, st, (const int*)count, k, lafs, resp);
+}
+int64_t og_ksift_select_workspace_bytes(int B, int cap) {
+  if (B <= 0 || B > 65535 || cap <= 0 || cap > KS_MAX_FEATURES) return fail(OG_EINVAL, "ksift_select_workspace_bytes: bad sizes");
+  return align_up((int64_t)B * cap, 256) + (int64_t)B * 4;
+}
+int og_ksift_select(const float* lafs, const float* resp, const int* count, int B, int H, int W, int cap, int nms, int nms_diameter,
+                    int max_keypoints, int min_stack, void* work, int64_t work_bytes, int* sel, int* n_sel, void* stream) {
+  OG_CHECK_ARG(lafs && resp && count && work && sel && n_sel, "ksift_select: null pointer");
+  OG_CHECK_ARG(H > 0 && W > 0, "ksift_select: bad image size");
+  OG_CHECK_ARG(!nms || (nms_diameter > 0 && nms_diameter % 2 == 1), "ksift_select: nms_diameter must be odd and positive, got %d", nms_diameter);
+  const int64_t need = og_ksift_select_workspace_bytes(B, cap);
+  if (need < 0) return (int)need;
+  OG_CHECK_ARG(work_bytes >= need, "ksift_select: workspace of %lld bytes, %lld needed", (long long)work_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned char* keep = static_cast<unsigned char*>(work);
+  int* kept = reinterpret_cast<int*>(keep + align_up((int64_t)B * cap, 256));
+  const size_t smem = (size_t)pow2_ceil(cap) * 16;
+  if (const int rc = smem_opt_in<ks_nms_kernel<1024>>((int)((size_t)KS_MAX_FEATURES * 16))) return rc;
+  if (const int rc = OG_LAUNCH(ks_nms_kernel<1024>, B, 1024, smem, st, lafs, resp, count, cap, H, W, nms_diameter / 2, nms, keep, kept)) return rc;
+  return OG_LAUNCH(ks_select_kernel, B, 1024, 0, st, (const unsigned char*)keep, (const int*)kept, B, cap, max_keypoints, min_stack, sel, n_sel);
+}
+int og_ksift_describe(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs,
+                      const float* resp, int cap, const int* sel, const int* n, int out_cap, int upright, int rootsift, float* lafs_out,
+                      float* scores, float* desc, float* angle, void* stream) {
+  KsLayout L;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "ksift_describe")) return rc;
+  OG_CHECK_ARG(image && lafs && resp && n && lafs_out && scores && desc, "ksift_describe: null pointer");
+  OG_CHECK_ARG(cap > 0 && out_cap > 0 && out_cap <= 65535, "ksift_describe: bad capacities");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* f = static_cast<float*>(ws);
+  KsPyr P{};
+  P.n = L.np;
+  for (int l = 0; l < L.np; ++l) {
+    P.h[l] = L.ph[l]; P.w[l] = L.pw[l];
+    P.p[l] = l == 0 ? image : f + L.pyr[l];
+    if (l == 0) continue;
+    if (L.ph[l] < 1 || L.pw[l] < 1) { P.n = l; break; }
+    const int64_t m = (int64_t)B * L.ph[l - 1] * L.pw[l - 1];
+    if (const int rc = OG_LAUNCH(ks_pyrdown_blur_kernel, sift_grid(m), 256, 0, st, P.p[l - 1], B, L.ph[l - 1], L.pw[l - 1], f + L.tmp)) return rc;
+    if (const int rc = OG_LAUNCH(ks_pyrdown_resize_kernel, sift_grid((int64_t)B * L.ph[l] * L.pw[l]), 256, 0, st, (const float*)(f + L.tmp), B,
+                                 L.ph[l - 1], L.pw[l - 1], L.ph[l], L.pw[l], f + L.pyr[l])) return rc;
+  }
+  KsDescConst* K = reinterpret_cast<KsDescConst*>(static_cast<char*>(ws) + L.consts);
+  if (const int rc = OG_LAUNCH(ks_desc_const_kernel, 1, 32, 0, st, K)) return rc;
+  return OG_LAUNCH(ks_describe_kernel<256>, dim3(out_cap, B), 256, 0, st, P, H, W, lafs, resp, cap, sel, n, out_cap, upright, rootsift,
+                   (const KsDescConst*)K, lafs_out, scores, desc, angle);
 }
 
 int og_keypoint_counts(const int* count, int B, int cap, int max_keypoints, int K, int* n_out, int* mode, int* overflow, void* stream) {

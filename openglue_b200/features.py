@@ -278,7 +278,7 @@ def _image_pair_inputs(local_feature: nn.Module, laf_converter: LAFConverter, lo
 class ImagePairMatcher(nn.Module):
     """Batches of image pairs to matches with no host synchronisation, replayed as one CUDA graph by default.
 
-    ``local_feature``: an ``OpenCVSIFT`` or ``SuperPointNet`` / ``SuperPointNetBn``; ``matcher``: an ``openglue_b200.SuperGlue``;
+    ``local_feature``: an ``OpenCVSIFT``, ``SIFT`` or ``SuperPointNet`` / ``SuperPointNetBn``; ``matcher``: an ``openglue_b200.SuperGlue``;
     ``match_config``: ``OpenGlueMatcher``'s (``superglue.laf_to_sideinfo_method``, optional ``superglue.log_transform_response``,
     ``inference.match_threshold``).  ``capacity``: the keypoint rows K per image (default: the front-end's ``max_keypoints``).
 
@@ -304,7 +304,7 @@ class ImagePairMatcher(nn.Module):
         if not isinstance(matcher, SuperGlue):
             raise TypeError('openglue_b200.ImagePairMatcher takes an openglue_b200.SuperGlue as its matcher')
         if not callable(getattr(local_feature, 'extract_padded', None)):
-            raise TypeError('openglue_b200.ImagePairMatcher takes a front-end with extract_padded (OpenCVSIFT, SuperPointNet[Bn])')
+            raise TypeError('openglue_b200.ImagePairMatcher takes a front-end with extract_padded (OpenCVSIFT, SIFT, SuperPointNet[Bn])')
         self.local_feature = local_feature
         self.matcher = matcher
         self.laf_converter = get_laf_to_sideinfo_converter(match_config['superglue']['laf_to_sideinfo_method'])

@@ -619,7 +619,7 @@ class ImagePairTrainStep:
         if not superglue.training:
             raise RuntimeError('ImagePairTrainStep runs the training-mode step: call superglue.train() first')
         if not callable(getattr(local_feature, 'extract_padded', None)):
-            raise TypeError('openglue_b200.ImagePairTrainStep takes a front-end with extract_padded (OpenCVSIFT, SuperPointNet[Bn])')
+            raise TypeError('openglue_b200.ImagePairTrainStep takes a front-end with extract_padded (OpenCVSIFT, SIFT, SuperPointNet[Bn])')
         if (config.get('features') or {}).get('finetune', False):
             raise NotImplementedError('fine-tuning the front-end (features.finetune) is not built: openglue_b200 front-ends run in eval mode')
         train = config['train']
