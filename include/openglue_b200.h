@@ -621,6 +621,36 @@ int og_ksift_describe(const float* image, int B, int H, int W, int num_features,
                       float* scores, float* desc, float* angle, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * kornia's GFTT / AffNet / HardNet front-end (the reference's GFTTAffNetHardNet, models/features/hardnet.py on base.py, kornia 0.6.3;
+ * csrc/kornia_gftt.cuh).  Same images and num_features as og_ksift_*; selection is og_ksift_select.  The two patch CNNs are run by
+ * the caller between the describe stages (NHWC im2col: og_sp_im2col3x3 / og_kgftt_im2col3x3_s2, then og_linear_auto_fwd), over
+ * chunks of output rows [r0, r0 + rows) of the [B, out_cap] output, so their scratch is bounded by the chunk size.
+ *   og_kgftt_workspace_bytes / og_kgftt_workspace_layout   as og_ksift_*; octave 0 is H x W and the second volume of each octave
+ *                              holds the GFTT responses of all 6 Gaussian levels ([B][6][h][w])
+ *   og_kgftt_pyramid           ScalePyramid(3, 1.6, 32, double_image=False), CornerGFTT on every level (times sigma^4), and the
+ *                              pyrdown patch pyramid of image, into ws
+ *   og_kgftt_detect            conv_quad_interp3d (maxima only) on levels 0 .. 4 of the responses, then og_ksift_detect's top-k,
+ *                              border test and merge -> lafs [B, num_features, 2, 3] (before AffNet), resp, count [B]
+ *   og_kgftt_affnet_patches    patches [rows, 32, 32]: AffNet's standardised input ((x - mean) / (std + 1e-6), Bessel's std) on
+ *                              make_upright of detector output sel[b][j] (sel NULL: j), zeros for rows with j >= n[b]
+ *   og_kgftt_frames            from AffNet's 8x8-conv output xy [rows, 3] (before tanh): the affine LAF (preserve_orientation),
+ *                              LAFOrienter(19) unless upright -> lafs_out, scores, angle (optional) rows of [B, out_cap], and
+ *                              patches [rows, 32, 32], HardNet's standardised input on the final LAF; rows past n[b] are 0
+ *   og_kgftt_im2col3x3_s2      3x3, stride 2, pad 1 im2col on NHWC: out [B ceil(H/2) ceil(W/2), 9 C], columns (3 ky + kx) C + c
+ *   og_kgftt_desc_finish       desc [B, out_cap, 128]: rows j < n[b] divided by max(||row||_2, 1e-12) (F.normalize), others 0  */
+int64_t og_kgftt_workspace_bytes(int B, int H, int W, int num_features);
+int og_kgftt_workspace_layout(int B, int H, int W, int num_features, int64_t* out, int n);
+int og_kgftt_pyramid(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, void* stream);
+int og_kgftt_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream);
+int og_kgftt_affnet_patches(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs, int cap,
+                            const int* sel, const int* n, int out_cap, int r0, int rows, float* patches, void* stream);
+int og_kgftt_frames(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs, const float* resp,
+                    int cap, const int* sel, const int* n, int out_cap, int r0, int rows, const float* xy, int upright, float* lafs_out,
+                    float* scores, float* angle, float* patches, void* stream);
+int og_kgftt_im2col3x3_s2(const float* x, int B, int H, int W, int C, float* out, void* stream);
+int og_kgftt_desc_finish(float* desc, int B, int out_cap, const int* n, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Local features -> matcher inputs, and matches -> the compact match list of stand-alone inference.
  *   og_prepare_features  prepare_features_output (models/features/utils.py:54-65) with the LAF -> side-information converter
  *                        superglue.laf_to_sideinfo_method names (models/laf_converter.py:108-128).  One thread per keypoint.

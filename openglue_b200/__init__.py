@@ -14,6 +14,7 @@ and the steps either side of those:
     SuperPointNet(max_keypoints, ...)(image) -> (lafs, scores, descriptors)   (the detector / descriptor front-end; SuperPointNetBn: its BatchNorm variant)
     OpenCVSIFT(max_keypoints, nms_diameter, rootsift)(image) -> (lafs, scores, descriptors)   (OPENCV_SIFT: cv2's SIFT + radius NMS + RootSIFT)
     SIFT(max_keypoints=8000, nms_diameter=9, upright, rootsift)(images) -> (lafs, responses, descriptors)   (SIFT: kornia's DoG detector + run_nms + RootSIFT)
+    GFTTAffNetHardNet(max_keypoints=8000, nms_diameter=9, upright, weights=...)(images) -> (lafs, responses, descriptors)   (GFTT + AffNet + run_nms + HardNet)
     prepare_features_output(lafs, responses, desc, get_laf_to_sideinfo_converter(method), ...)   (front-end output -> SuperGlue input)
     OpenGlueMatcher(local_feature, superglue, match_config)(data) -> compact match list   (stand-alone image-pair inference)
     ImagePairMatcher(local_feature, superglue, match_config)(image0, image1) -> padded matches   (batches of pairs, one CUDA graph)
@@ -30,6 +31,7 @@ from .sinkhorn import matching_log_probs  # noqa: F401
 from .superglue import MatchingCore, PendingMatches, SuperGlue  # noqa: F401
 from .sift import OpenCVSIFT, sift_create_torch  # noqa: F401
 from .kornia_sift import SIFT  # noqa: F401
+from .gftt_hardnet import GFTTAffNetHardNet  # noqa: F401
 from .superpoint import SuperPointNet, SuperPointNetBn  # noqa: F401
 from .training import ImagePairTrainStep  # noqa: F401
 

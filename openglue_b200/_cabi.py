@@ -161,6 +161,15 @@ SYMBOLS = {
     'og_ksift_select_workspace_bytes': (_L, [_I, _I]),
     'og_ksift_select': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P, _P, _P]),
     'og_ksift_describe': (_I, [_P, _I, _I, _I, _I, _P, _L, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
+    # kornia GFTT / AffNet / HardNet front-end
+    'og_kgftt_workspace_bytes': (_L, [_I, _I, _I, _I]),
+    'og_kgftt_workspace_layout': (_I, [_I, _I, _I, _I, _P, _I]),
+    'og_kgftt_pyramid': (_I, [_P, _I, _I, _I, _I, _P, _L, _P]),
+    'og_kgftt_detect': (_I, [_I, _I, _I, _I, _P, _L, _P, _P, _P, _P]),
+    'og_kgftt_affnet_patches': (_I, [_P, _I, _I, _I, _I, _P, _L, _P, _I, _P, _P, _I, _I, _I, _P, _P]),
+    'og_kgftt_frames': (_I, [_P, _I, _I, _I, _I, _P, _L, _P, _P, _I, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P]),
+    'og_kgftt_im2col3x3_s2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
+    'og_kgftt_desc_finish': (_I, [_P, _I, _I, _P, _P]),
     # local features -> matcher inputs, matches -> compact list
     'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -16,6 +16,7 @@
 #include "superpoint.cuh"
 #include "sift.cuh"
 #include "kornia_sift.cuh"
+#include "kornia_gftt.cuh"
 #include "features.cuh"
 #include "homography.cuh"
 #include "optim.cuh"
@@ -1073,6 +1074,25 @@ static int ks_args(void* ws, int64_t ws_bytes, int B, int H, int W, int k, KsLay
   OG_CHECK_ARG(ws_bytes >= L.bytes, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes, (long long)L.bytes);
   return OG_OK;
 }
+// The Gaussian levels 1 .. 5 of octave o (and its level 0, the previous octave's level 3 at [::2, ::2], for o > 0)
+static int ks_octave_levels(float* f, const KsLayout& L, int B, int o, cudaStream_t st) {
+  const KsOctave& oc = L.oct[o];
+  const int64_t plane = (int64_t)oc.h * oc.w;
+  float* g = f + oc.gauss;
+  if (o > 0) {
+    const KsOctave& pv = L.oct[o - 1];
+    if (const int rc = OG_LAUNCH(ks_subsample_kernel, sift_grid(B * plane), 256, 0, st, (const float*)(f + pv.gauss), B, pv.h, pv.w,
+                                 oc.h, oc.w, g)) return rc;
+  }
+  const double step = std::pow(2.0, 1.0 / 3.0);
+  double cur = 1.6;
+  for (int l = 1; l < KS_LEVELS; ++l) {
+    const double sigma = cur * std::sqrt(step * step - 1.0);
+    if (const int rc = ks_blur(f, L, B, oc.h, oc.w, g + (l - 1) * plane, KS_LEVELS * plane, sigma, g + l * plane, KS_LEVELS * plane, st)) return rc;
+    cur *= step;
+  }
+  return OG_OK;
+}
 int og_ksift_pyramid(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, void* stream) {
   KsLayout L;
   if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "ksift_pyramid")) return rc;
@@ -1084,33 +1104,19 @@ int og_ksift_pyramid(const float* image, int B, int H, int W, int num_features, 
   float* g0 = f + o0.gauss;
   if (const int rc = OG_LAUNCH(ks_upsample_kernel, sift_grid(B * p0), 256, 0, st, image, B, H, W, g0)) return rc;
   // the upsampled image has sigma 1.0; the first level is blurred to 1.6
-  double cur = 1.6;
   if (const int rc = ks_blur(f, L, B, o0.h, o0.w, g0, KS_LEVELS * p0, std::max(std::sqrt(1.6 * 1.6 - 1.0), 0.01), g0, KS_LEVELS * p0, st)) return rc;
-  const double step = std::pow(2.0, 1.0 / 3.0);
   for (int o = 0; o < L.nO; ++o) {
     const KsOctave& oc = L.oct[o];
     const int64_t plane = (int64_t)oc.h * oc.w;
-    float* g = f + oc.gauss;
-    if (o > 0) {
-      const KsOctave& pv = L.oct[o - 1];
-      if (const int rc = OG_LAUNCH(ks_subsample_kernel, sift_grid(B * plane), 256, 0, st, (const float*)(f + pv.gauss), B, pv.h, pv.w,
-                                   oc.h, oc.w, g)) return rc;
-    }
-    cur = 1.6;
-    for (int l = 1; l < KS_LEVELS; ++l) {
-      const double sigma = cur * std::sqrt(step * step - 1.0);
-      if (const int rc = ks_blur(f, L, B, oc.h, oc.w, g + (l - 1) * plane, KS_LEVELS * plane, sigma, g + l * plane, KS_LEVELS * plane, st)) return rc;
-      cur *= step;
-    }
-    if (const int rc = OG_LAUNCH(ks_dog_kernel, sift_grid(B * KS_DOG * plane), 256, 0, st, (const float*)g, B, (int)plane, f + oc.dog)) return rc;
+    if (const int rc = ks_octave_levels(f, L, B, o, st)) return rc;
+    if (const int rc = OG_LAUNCH(ks_dog_kernel, sift_grid(B * KS_DOG * plane), 256, 0, st, (const float*)(f + oc.gauss), B, (int)plane,
+                                 f + oc.dog)) return rc;
   }
   return OG_OK;
 }
-int og_ksift_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream) {
-  KsLayout L;
-  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "ksift_detect")) return rc;
-  OG_CHECK_ARG(lafs && resp && count, "ksift_detect: null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
+// The detector on the volumes in ws: the responses of every voxel (SIFT: extrema of DoG and -DoG; GFTT: maxima of levels 0 .. 4),
+// the exact per-octave top-k, the border test and the global top-k
+static int ks_detect(const KsLayout& L, int B, int H, int W, bool gftt, void* ws, float* lafs, float* resp, int* count, cudaStream_t st) {
   float* f = static_cast<float*>(ws);
   char* c = static_cast<char*>(ws);
   const int segs = B * L.nO, k = L.k;
@@ -1122,7 +1128,11 @@ int og_ksift_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_
   for (int o = 0; o < L.nO; ++o) {
     const KsOctave& oc = L.oct[o];
     const int64_t per = (int64_t)KS_DOG * oc.h * oc.w;
-    if (const int rc = OG_LAUNCH(ks_response_kernel, sift_grid(B * per), 256, 0, st, (const float*)(f + oc.dog), B, oc.h, oc.w, f + oc.resp)) return rc;
+    if (gftt) {
+      if (const int rc = OG_LAUNCH(kg_response_kernel, sift_grid(B * per), 256, 0, st, (const float*)(f + oc.dog), B, oc.h, oc.w, f + oc.resp)) return rc;
+    } else {
+      if (const int rc = OG_LAUNCH(ks_response_kernel, sift_grid(B * per), 256, 0, st, (const float*)(f + oc.dog), B, oc.h, oc.w, f + oc.resp)) return rc;
+    }
     const dim3 grid((unsigned)std::min<int64_t>(cdiv((int)std::min<int64_t>(per, INT_MAX), 2048), 512), B);
     for (int pass = 0; pass < 8; ++pass) {
       if (const int rc = OG_LAUNCH(ks_hist_kernel, grid, 256, 0, st, (const float*)(f + oc.resp), per, o, L.nO, (const KsSel*)sel, hist)) return rc;
@@ -1131,14 +1141,26 @@ int og_ksift_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_
     if (const int rc = OG_LAUNCH(ks_compact_kernel, grid, 256, 0, st, (const float*)(f + oc.resp), per, o, L.nO, (const KsSel*)sel, k, cand, cnt)) return rc;
   }
   const size_t smem = (size_t)pow2_ceil(k) * 8;
-  if (const int rc = smem_opt_in<ks_octave_list_kernel<512>>((int)((size_t)KS_MAX_FEATURES * 8))) return rc;
   KsCand* list = reinterpret_cast<KsCand*>(c + L.list);
   KsCand* scratch = reinterpret_cast<KsCand*>(c + L.scratch);
-  if (const int rc = OG_LAUNCH(ks_octave_list_kernel<512>, segs, 512, smem, st, (const float*)f, L, B, H, W, (const int*)cnt, scratch, list,
-                               (const unsigned long long*)cand)) return rc;
+  if (gftt) {
+    if (const int rc = smem_opt_in<ks_octave_list_kernel<512, 1>>((int)((size_t)KS_MAX_FEATURES * 8))) return rc;
+    if (const int rc = OG_LAUNCH((ks_octave_list_kernel<512, 1>), segs, 512, smem, st, (const float*)f, L, B, H, W, (const int*)cnt, scratch,
+                                 list, (const unsigned long long*)cand)) return rc;
+  } else {
+    if (const int rc = smem_opt_in<ks_octave_list_kernel<512>>((int)((size_t)KS_MAX_FEATURES * 8))) return rc;
+    if (const int rc = OG_LAUNCH(ks_octave_list_kernel<512>, segs, 512, smem, st, (const float*)f, L, B, H, W, (const int*)cnt, scratch, list,
+                                 (const unsigned long long*)cand)) return rc;
+  }
   if (const int rc = OG_LAUNCH(ks_merge_kernel, dim3(cdiv(k, 256), L.nO, B), 256, 0, st, (const KsCand*)list, (const int*)cnt, L.nO, k,
                                lafs, resp, count)) return rc;
   return OG_LAUNCH(ks_det_tail_kernel, dim3(cdiv(k, 256), B), 256, 0, st, (const int*)count, k, lafs, resp);
+}
+int og_ksift_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream) {
+  KsLayout L;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "ksift_detect")) return rc;
+  OG_CHECK_ARG(lafs && resp && count, "ksift_detect: null pointer");
+  return ks_detect(L, B, H, W, false, ws, lafs, resp, count, (cudaStream_t)stream);
 }
 int64_t og_ksift_select_workspace_bytes(int B, int cap) {
   if (B <= 0 || B > 65535 || cap <= 0 || cap > KS_MAX_FEATURES) return fail(OG_EINVAL, "ksift_select_workspace_bytes: bad sizes");
@@ -1160,6 +1182,28 @@ int og_ksift_select(const float* lafs, const float* resp, const int* count, int 
   if (const int rc = OG_LAUNCH(ks_nms_kernel<1024>, B, 1024, smem, st, lafs, resp, count, cap, H, W, nms_diameter / 2, nms, keep, kept)) return rc;
   return OG_LAUNCH(ks_select_kernel, B, 1024, 0, st, (const unsigned char*)keep, (const int*)kept, B, cap, max_keypoints, min_stack, sel, n_sel);
 }
+// kornia's pyrdown patch pyramid: level 0 is the image, level l > 0 in ws
+static KsPyr ks_patch_pyramid(const KsLayout& L, const float* image, void* ws) {
+  float* f = static_cast<float*>(ws);
+  KsPyr P{};
+  P.n = L.np;
+  for (int l = 0; l < L.np; ++l) {
+    P.h[l] = L.ph[l]; P.w[l] = L.pw[l];
+    P.p[l] = l == 0 ? image : f + L.pyr[l];
+    if (l > 0 && (L.ph[l] < 1 || L.pw[l] < 1)) { P.n = l; break; }
+  }
+  return P;
+}
+static int ks_build_patch_pyramid(const KsLayout& L, int B, const KsPyr& P, void* ws, cudaStream_t st) {
+  float* f = static_cast<float*>(ws);
+  for (int l = 1; l < P.n; ++l) {
+    const int64_t m = (int64_t)B * L.ph[l - 1] * L.pw[l - 1];
+    if (const int rc = OG_LAUNCH(ks_pyrdown_blur_kernel, sift_grid(m), 256, 0, st, P.p[l - 1], B, L.ph[l - 1], L.pw[l - 1], f + L.tmp)) return rc;
+    if (const int rc = OG_LAUNCH(ks_pyrdown_resize_kernel, sift_grid((int64_t)B * L.ph[l] * L.pw[l]), 256, 0, st, (const float*)(f + L.tmp), B,
+                                 L.ph[l - 1], L.pw[l - 1], L.ph[l], L.pw[l], f + L.pyr[l])) return rc;
+  }
+  return OG_OK;
+}
 int og_ksift_describe(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs,
                       const float* resp, int cap, const int* sel, const int* n, int out_cap, int upright, int rootsift, float* lafs_out,
                       float* scores, float* desc, float* angle, void* stream) {
@@ -1168,23 +1212,120 @@ int og_ksift_describe(const float* image, int B, int H, int W, int num_features,
   OG_CHECK_ARG(image && lafs && resp && n && lafs_out && scores && desc, "ksift_describe: null pointer");
   OG_CHECK_ARG(cap > 0 && out_cap > 0 && out_cap <= 65535, "ksift_describe: bad capacities");
   cudaStream_t st = (cudaStream_t)stream;
-  float* f = static_cast<float*>(ws);
-  KsPyr P{};
-  P.n = L.np;
-  for (int l = 0; l < L.np; ++l) {
-    P.h[l] = L.ph[l]; P.w[l] = L.pw[l];
-    P.p[l] = l == 0 ? image : f + L.pyr[l];
-    if (l == 0) continue;
-    if (L.ph[l] < 1 || L.pw[l] < 1) { P.n = l; break; }
-    const int64_t m = (int64_t)B * L.ph[l - 1] * L.pw[l - 1];
-    if (const int rc = OG_LAUNCH(ks_pyrdown_blur_kernel, sift_grid(m), 256, 0, st, P.p[l - 1], B, L.ph[l - 1], L.pw[l - 1], f + L.tmp)) return rc;
-    if (const int rc = OG_LAUNCH(ks_pyrdown_resize_kernel, sift_grid((int64_t)B * L.ph[l] * L.pw[l]), 256, 0, st, (const float*)(f + L.tmp), B,
-                                 L.ph[l - 1], L.pw[l - 1], L.ph[l], L.pw[l], f + L.pyr[l])) return rc;
-  }
+  const KsPyr P = ks_patch_pyramid(L, image, ws);
+  if (const int rc = ks_build_patch_pyramid(L, B, P, ws, st)) return rc;
   KsDescConst* K = reinterpret_cast<KsDescConst*>(static_cast<char*>(ws) + L.consts);
   if (const int rc = OG_LAUNCH(ks_desc_const_kernel, 1, 32, 0, st, K)) return rc;
   return OG_LAUNCH(ks_describe_kernel<256>, dim3(out_cap, B), 256, 0, st, P, H, W, lafs, resp, cap, sel, n, out_cap, upright, rootsift,
                    (const KsDescConst*)K, lafs_out, scores, desc, angle);
+}
+
+// ---- kornia GFTT / AffNet / HardNet front-end (csrc/kornia_gftt.cuh) ----
+static int kg_check_sizes(int B, int H, int W, int k, KsLayout& L, const char* who) {
+  if (B <= 0 || B > 65535 || H <= 0 || W <= 0 || k <= 0) return fail(OG_EINVAL, "%s: bad sizes", who);
+  if (k > KS_MAX_FEATURES) return fail(OG_EUNSUPPORTED, "%s: num_features %d above %d", who, k, KS_MAX_FEATURES);
+  if (min(H, W) < 2 || (int64_t)6 * H * W > 0xffffffffLL) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image is not supported", who, H, W);
+  if (!ks_layout(B, H, W, k, L, false, KS_LEVELS)) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image has more than %d octaves", who, H, W, KS_MAX_OCTAVES);
+  return OG_OK;
+}
+static int kg_args(const void* ws, int64_t ws_bytes, int B, int H, int W, int k, KsLayout& L, const char* who) {
+  OG_CHECK_ARG(ws, "%s: null workspace", who);
+  if (const int rc = kg_check_sizes(B, H, W, k, L, who)) return rc;
+  OG_CHECK_ARG(ws_bytes >= L.bytes, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes, (long long)L.bytes);
+  return OG_OK;
+}
+int64_t og_kgftt_workspace_bytes(int B, int H, int W, int num_features) {
+  KsLayout L;
+  if (const int rc = kg_check_sizes(B, H, W, num_features, L, "kgftt_workspace_bytes")) return rc;
+  return L.bytes;
+}
+int og_kgftt_workspace_layout(int B, int H, int W, int num_features, int64_t* out, int n) {
+  OG_CHECK_ARG(out, "kgftt_workspace_layout: null pointer");
+  KsLayout L;
+  if (const int rc = kg_check_sizes(B, H, W, num_features, L, "kgftt_workspace_layout")) return rc;
+  const int need = 1 + 5 * L.nO + 1 + 3 * L.np + 1;
+  OG_CHECK_ARG(n >= need, "kgftt_workspace_layout: %d entries, %d needed", n, need);
+  int i = 0;
+  out[i++] = L.nO;
+  for (int o = 0; o < L.nO; ++o) {
+    out[i++] = L.oct[o].h; out[i++] = L.oct[o].w;
+    out[i++] = 4 * L.oct[o].gauss; out[i++] = 4 * L.oct[o].dog; out[i++] = 4 * L.oct[o].resp;
+  }
+  out[i++] = L.np;
+  for (int l = 0; l < L.np; ++l) { out[i++] = L.ph[l]; out[i++] = L.pw[l]; out[i++] = l == 0 ? -1 : 4 * L.pyr[l]; }
+  out[i++] = L.bytes;
+  return i;
+}
+int og_kgftt_pyramid(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, void* stream) {
+  KsLayout L;
+  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_pyramid")) return rc;
+  OG_CHECK_ARG(image, "kgftt_pyramid: null image");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* f = static_cast<float*>(ws);
+  const KsOctave& o0 = L.oct[0];
+  const int64_t p0 = (int64_t)o0.h * o0.w;
+  // the input has sigma 0.5; the first level is blurred to 1.6
+  if (const int rc = ks_blur(f, L, B, H, W, image, p0, std::max(std::sqrt(1.6 * 1.6 - 0.25), 0.01), f + o0.gauss, KS_LEVELS * p0, st)) return rc;
+  KgGftt g;
+  KsTaps t;
+  ks_gaussian_taps(7, 1.0, t);
+  for (int i = 0; i < 7; ++i) for (int j = 0; j < 7; ++j) g.k2[i * 7 + j] = t.k[i] * t.k[j];
+  const double step = std::pow(2.0, 1.0 / 3.0);
+  double cur = 1.6;
+  for (int l = 0; l < KS_LEVELS; ++l) { g.s4[l] = powf((float)cur, 4.f); cur *= step; }     // the level sigmas, float32, to the 4th
+  for (int o = 0; o < L.nO; ++o) {
+    const KsOctave& oc = L.oct[o];
+    if (const int rc = ks_octave_levels(f, L, B, o, st)) return rc;
+    const dim3 grid(cdiv(oc.w, KG_TILE), cdiv(oc.h, KG_TILE), B * KS_LEVELS);
+    if (const int rc = OG_LAUNCH(kg_gftt_kernel, grid, dim3(KG_TILE, KG_TILE), 0, st, (const float*)(f + oc.gauss), oc.h, oc.w, g, f + oc.dog)) return rc;
+  }
+  const KsPyr P = ks_patch_pyramid(L, image, ws);
+  if (const int rc = ks_build_patch_pyramid(L, B, P, ws, st)) return rc;
+  return OG_LAUNCH(ks_desc_const_kernel, 1, 32, 0, st, reinterpret_cast<KsDescConst*>(static_cast<char*>(ws) + L.consts));
+}
+int og_kgftt_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream) {
+  KsLayout L;
+  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_detect")) return rc;
+  OG_CHECK_ARG(lafs && resp && count, "kgftt_detect: null pointer");
+  return ks_detect(L, B, H, W, true, ws, lafs, resp, count, (cudaStream_t)stream);
+}
+static int kg_rows_args(const float* image, const float* lafs, const int* n, int cap, int out_cap, int B, int r0, int rows, const char* who) {
+  OG_CHECK_ARG(image && lafs && n, "%s: null pointer", who);
+  OG_CHECK_ARG(cap > 0 && out_cap > 0 && rows >= 0 && r0 >= 0 && (int64_t)r0 + rows <= (int64_t)B * out_cap && (int64_t)B * out_cap <= INT32_MAX,
+               "%s: bad rows [%d, %d + %d) of %d x %d", who, r0, r0, rows, B, out_cap);
+  return OG_OK;
+}
+int og_kgftt_affnet_patches(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs, int cap,
+                            const int* sel, const int* n, int out_cap, int r0, int rows, float* patches, void* stream) {
+  KsLayout L;
+  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_affnet_patches")) return rc;
+  if (const int rc = kg_rows_args(image, lafs, n, cap, out_cap, B, r0, rows, "kgftt_affnet_patches")) return rc;
+  OG_CHECK_ARG(patches, "kgftt_affnet_patches: null pointer");
+  if (rows == 0) return OG_OK;
+  return OG_LAUNCH(kg_affnet_patch_kernel<256>, rows, 256, 0, (cudaStream_t)stream, ks_patch_pyramid(L, image, ws), H, W, lafs, cap, sel, n, out_cap,
+                   r0, patches);
+}
+int og_kgftt_frames(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs, const float* resp,
+                    int cap, const int* sel, const int* n, int out_cap, int r0, int rows, const float* xy, int upright, float* lafs_out,
+                    float* scores, float* angle, float* patches, void* stream) {
+  KsLayout L;
+  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_frames")) return rc;
+  if (const int rc = kg_rows_args(image, lafs, n, cap, out_cap, B, r0, rows, "kgftt_frames")) return rc;
+  OG_CHECK_ARG(resp && xy && lafs_out && scores && patches, "kgftt_frames: null pointer");
+  if (rows == 0) return OG_OK;
+  const KsDescConst* K = reinterpret_cast<const KsDescConst*>(static_cast<const char*>(ws) + L.consts);
+  return OG_LAUNCH(kg_frame_kernel<256>, rows, 256, 0, (cudaStream_t)stream, ks_patch_pyramid(L, image, ws), H, W, lafs, resp, cap, sel, n,
+                   out_cap, r0, xy, upright, K, lafs_out, scores, angle, patches);
+}
+int og_kgftt_im2col3x3_s2(const float* x, int B, int H, int W, int C, float* out, void* stream) {
+  OG_CHECK_ARG(x && out && B > 0 && H > 0 && W > 0 && C > 0, "kgftt_im2col3x3_s2: bad arguments");
+  const int64_t cols = (int64_t)B * ((H + 1) / 2) * ((W + 1) / 2) * 9 * ((C % 4 == 0) ? C / 4 : C);
+  return OG_LAUNCH(kg_im2col3x3_s2_kernel, sp_grid(cols), 256, 0, (cudaStream_t)stream, x, B, H, W, C, out);
+}
+int og_kgftt_desc_finish(float* desc, int B, int out_cap, const int* n, void* stream) {
+  OG_CHECK_ARG(desc && n && B > 0 && out_cap > 0, "kgftt_desc_finish: bad arguments");
+  const int64_t rows = (int64_t)B * out_cap;
+  return OG_LAUNCH(kg_desc_finish_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, desc, B, out_cap, n);
 }
 
 int og_keypoint_counts(const int* count, int B, int cap, int max_keypoints, int K, int* n_out, int* mode, int* overflow, void* stream) {

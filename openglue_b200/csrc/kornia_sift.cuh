@@ -43,11 +43,13 @@ struct KsLayout {
   int64_t bytes;
 };
 
-// Octave sizes: 2H x 2W, then [::2, ::2] while the smaller side stays above 32 (ScalePyramid.forward)
-inline bool ks_layout(int B, int H, int W, int k, KsLayout& L) {
+// Octave sizes: 2H x 2W (H x W without double_image), then [::2, ::2] while the smaller side stays above 32
+// (ScalePyramid.forward).  The per-octave volume the detector reads ("dog") has vol_levels levels: the 5 DoG levels of SIFT, or
+// the GFTT responses of all 6 Gaussian levels.
+inline bool ks_layout(int B, int H, int W, int k, KsLayout& L, bool double_image = true, int vol_levels = KS_DOG) {
   L = KsLayout{};
   L.k = k;
-  int h = 2 * H, w = 2 * W;
+  int h = double_image ? 2 * H : H, w = double_image ? 2 * W : W;
   int64_t f = 0;
   for (;;) {
     if (L.nO == KS_MAX_OCTAVES) return false;
@@ -55,13 +57,13 @@ inline bool ks_layout(int B, int H, int W, int k, KsLayout& L) {
     o.h = h; o.w = w;
     const int64_t plane = (int64_t)B * h * w;
     o.gauss = f; f += KS_LEVELS * plane;
-    o.dog = f; f += KS_DOG * plane;
+    o.dog = f; f += vol_levels * plane;
     o.resp = f; f += KS_DOG * plane;
     const int nh = (h + 1) / 2, nw = (w + 1) / 2;
     if (min(nh, nw) <= 32) break;
     h = nh; w = nw;
   }
-  L.tmp = f; f += (int64_t)B * 2 * H * 2 * W;
+  L.tmp = f; f += (int64_t)B * L.oct[0].h * L.oct[0].w;
   // patch pyramid for 19-pixel patches (the deeper of the two): level k + 1 exists while level k's smaller side is >= 19
   int ph = H, pw = W;
   L.np = 1; L.ph[0] = H; L.pw[0] = W; L.pyr[0] = -1;
@@ -329,7 +331,8 @@ struct KsCand { float resp, scale, x, y; };     // a detector candidate in image
 
 // One segment per CTA: sorts its candidates (response desc, voxel asc), builds their LAFs, zeroes the responses of LAFs that
 // touch the octave border, maps them to the image, and sorts again by (zeroed response desc, rank asc): list[s][0 .. n)
-template <int THREADS>
+// GFTT: the volume holds 6 levels per image, of which the first 5 enter the interpolation, and only maxima count.
+template <int THREADS, int GFTT = 0>
 __global__ void __launch_bounds__(THREADS) ks_octave_list_kernel(const float* __restrict__ ws_f, KsLayout L, int B, int H, int W,
                                                                  const int* __restrict__ count, KsCand* __restrict__ scratch,
                                                                  KsCand* __restrict__ list, const unsigned long long* __restrict__ cand) {
@@ -343,13 +346,13 @@ __global__ void __launch_bounds__(THREADS) ks_octave_list_kernel(const float* __
   __syncthreads();
   cta_bitonic_sort<THREADS>(n2, [&](int lo, int hi) { return key[lo] > key[hi]; },
                             [&](int lo, int hi) { const auto t = key[lo]; key[lo] = key[hi]; key[hi] = t; });
-  const float* dog = ws_f + oc.dog + (int64_t)b * KS_DOG * oc.h * oc.w;
+  const float* dog = ws_f + oc.dog + (int64_t)b * (GFTT ? KS_LEVELS : KS_DOG) * oc.h * oc.w;
   // laf_to_boundary_points(12): the centre, then (sin t, cos t) at torch.linspace(0, 2 pi, 11)
   const float mo = (float)min(oc.h - 1, oc.w - 1), mi = (float)min(H - 1, W - 1);
   for (int j = threadIdx.x; j < n; j += THREADS) {
     const uint32_t idx = 0xffffffffu - (uint32_t)(key[j] & 0xffffffffull);
     const int x = (int)(idx % oc.w), y = (int)((idx / oc.w) % oc.h), l = (int)(idx / ((uint32_t)oc.h * oc.w));
-    const KsPoint p = ks_point(dog, oc.h, oc.w, l, y, x);
+    const KsPoint p = GFTT ? ks_quad_interp(dog, 1.f, oc.h, oc.w, l, y, x) : ks_point(dog, oc.h, oc.w, l, y, x);
     const float sigma = __fmul_rn(1.6f, exp2f(__fdiv_rn(p.s, 3.f)));
     const float sc = __fmul_rn(6.0f, sigma);
     bool good = p.x >= 0.f && p.x <= (float)oc.w && p.y >= 0.f && p.y <= (float)oc.h;
@@ -647,6 +650,84 @@ __device__ void ks_patch(const KsPyr& P, int b, int H, int W, const float a[6], 
   }
 }
 
+// LAFOrienter(19) on the LAF a (every thread of the CTA, a in registers, la its shared copy): the dominant orientation of its
+// 19-pixel patch; a <- set_laf_orientation(a, rad2deg(angle) + get_laf_orientation(a)).  Returns the angle (radians).
+template <int THREADS>
+__device__ float ks_orient(const KsPyr& P, int b, int H, int W, const KsDescConst* __restrict__ K, float a[6], float* patch, float* wa,
+                           float* wb, unsigned char* bin, float* hist, float* la) {
+  ks_patch<KS_ORI_PS>(P, b, H, W, a, patch);
+  __syncthreads();
+  constexpr int N = KS_ORI_PS * KS_ORI_PS;
+  const float two_pi = __fmul_rn(2.f, KS_PI);
+  for (int i = threadIdx.x; i < N; i += THREADS) {
+    const int r = i / KS_ORI_PS, c = i % KS_ORI_PS;
+    auto P_ = [&](int rr, int cc) { return patch[min(max(rr, 0), KS_ORI_PS - 1) * KS_ORI_PS + min(max(cc, 0), KS_ORI_PS - 1)]; };
+    // normalised Sobel (taps / 8), replicate border
+    float gx = __fmul_rn(-0.125f, P_(r - 1, c - 1));
+    gx = __fadd_rn(gx, __fmul_rn(0.125f, P_(r - 1, c + 1)));
+    gx = __fadd_rn(gx, __fmul_rn(-0.25f, P_(r, c - 1)));
+    gx = __fadd_rn(gx, __fmul_rn(0.25f, P_(r, c + 1)));
+    gx = __fadd_rn(gx, __fmul_rn(-0.125f, P_(r + 1, c - 1)));
+    gx = __fadd_rn(gx, __fmul_rn(0.125f, P_(r + 1, c + 1)));
+    float gy = __fmul_rn(-0.125f, P_(r - 1, c - 1));
+    gy = __fadd_rn(gy, __fmul_rn(-0.25f, P_(r - 1, c)));
+    gy = __fadd_rn(gy, __fmul_rn(-0.125f, P_(r - 1, c + 1)));
+    gy = __fadd_rn(gy, __fmul_rn(0.125f, P_(r + 1, c - 1)));
+    gy = __fadd_rn(gy, __fmul_rn(0.25f, P_(r + 1, c)));
+    gy = __fadd_rn(gy, __fmul_rn(0.125f, P_(r + 1, c + 1)));
+    const float mag = __fmul_rn(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), 1e-8f)), K->ori_w[i]);
+    const float ori = __fadd_rn(atan2f(gy, __fadd_rn(gx, 1e-8f)), two_pi);
+    const float ob = __fdiv_rn(__fmul_rn((float)KS_ORI_BINS, __fadd_rn(ori, KS_PI)), two_pi);
+    const float f = floorf(ob);
+    const float w1 = __fsub_rn(ob, f);
+    int b0 = (int)f % KS_ORI_BINS;
+    bin[i] = (unsigned char)b0;
+    wa[i] = __fmul_rn(__fsub_rn(1.f, w1), mag);
+    wb[i] = __fmul_rn(w1, mag);
+  }
+  __syncthreads();
+  if (threadIdx.x < KS_ORI_BINS) {              // adaptive_avg_pool2d: the bin's sum over the patch in raster order / N
+    const int q = threadIdx.x;
+    float s = 0.f;
+    for (int i = 0; i < N; ++i) {
+      const int b0 = bin[i], b1 = (b0 + 1) % KS_ORI_BINS;
+      s = __fadd_rn(s, __fadd_rn(b0 == q ? wa[i] : 0.f, b1 == q ? wb[i] : 0.f));
+    }
+    hist[q] = __fdiv_rn(s, (float)N);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float best = -CUDART_INF_F;
+    int bi = 0;
+    for (int q = 0; q < KS_ORI_BINS; ++q) {       // circular conv1d [0.33, 0.34, 0.33], then the first maximum
+      const float v = __fadd_rn(__fadd_rn(__fmul_rn(0.33f, hist[(q + KS_ORI_BINS - 1) % KS_ORI_BINS]), __fmul_rn(0.34f, hist[q])),
+                                __fmul_rn(0.33f, hist[(q + 1) % KS_ORI_BINS]));
+      if (v > best) { best = v; bi = q; }
+    }
+    const float an = -__fsub_rn(__fdiv_rn(__fmul_rn(two_pi, (float)bi), (float)KS_ORI_BINS), KS_PI);
+    // set_laf_orientation(laf, rad2deg(an) + prev): rotate_laf(make_upright(laf), new - prev)
+    const float prev = __fdiv_rn(__fmul_rn(180.f, atan2f(a[1], a[0])), KS_PI);
+    const float nd = __fadd_rn(__fdiv_rn(__fmul_rn(180.f, an), KS_PI), prev);
+    const float rad = __fdiv_rn(__fmul_rn(__fsub_rn(nd, prev), KS_PI), 180.f);
+    const float cs = cosf(rad), sn = sinf(rad);
+    const float det = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a[0], a[4]), __fmul_rn(a[3], a[1])), 1e-10f)));
+    const float b2a2 = __fadd_rn(sqrtf(__fadd_rn(__fmul_rn(a[1], a[1]), __fmul_rn(a[0], a[0]))), 1e-9f);
+    const float u00 = __fmul_rn(det, __fdiv_rn(b2a2, det)), u01 = 0.f;
+    const float u10 = __fmul_rn(det, __fdiv_rn(__fadd_rn(__fmul_rn(a[4], a[1]), __fmul_rn(a[3], a[0])), __fmul_rn(b2a2, det)));
+    const float u11 = __fmul_rn(det, __fdiv_rn(det, b2a2));
+    la[0] = __fadd_rn(__fmul_rn(u00, cs), __fmul_rn(u01, -sn));
+    la[1] = __fadd_rn(__fmul_rn(u00, sn), __fmul_rn(u01, cs));
+    la[3] = __fadd_rn(__fmul_rn(u10, cs), __fmul_rn(u11, -sn));
+    la[4] = __fadd_rn(__fmul_rn(u10, sn), __fmul_rn(u11, cs));
+    hist[0] = an;
+  }
+  __syncthreads();
+  const float ang = hist[0];
+  for (int e = 0; e < 6; ++e) a[e] = la[e];
+  __syncthreads();
+  return ang;
+}
+
 // One CTA per output row (j, b): orientation (unless upright) and the SIFT descriptor of LAF sel[b][j] of lafs_in; rows past
 // n[b] are written as zeros.
 
@@ -677,78 +758,7 @@ __global__ void __launch_bounds__(THREADS) ks_describe_kernel(KsPyr P, int H, in
   float a[6];
   for (int e = 0; e < 6; ++e) a[e] = la[e];
   float ang = 0.f;
-  if (!upright) {
-    ks_patch<KS_ORI_PS>(P, b, H, W, a, patch);
-    __syncthreads();
-    constexpr int N = KS_ORI_PS * KS_ORI_PS;
-    const float two_pi = __fmul_rn(2.f, KS_PI);
-    for (int i = threadIdx.x; i < N; i += THREADS) {
-      const int r = i / KS_ORI_PS, c = i % KS_ORI_PS;
-      auto P_ = [&](int rr, int cc) { return patch[min(max(rr, 0), KS_ORI_PS - 1) * KS_ORI_PS + min(max(cc, 0), KS_ORI_PS - 1)]; };
-      // normalised Sobel (taps / 8), replicate border
-      float gx = __fmul_rn(-0.125f, P_(r - 1, c - 1));
-      gx = __fadd_rn(gx, __fmul_rn(0.125f, P_(r - 1, c + 1)));
-      gx = __fadd_rn(gx, __fmul_rn(-0.25f, P_(r, c - 1)));
-      gx = __fadd_rn(gx, __fmul_rn(0.25f, P_(r, c + 1)));
-      gx = __fadd_rn(gx, __fmul_rn(-0.125f, P_(r + 1, c - 1)));
-      gx = __fadd_rn(gx, __fmul_rn(0.125f, P_(r + 1, c + 1)));
-      float gy = __fmul_rn(-0.125f, P_(r - 1, c - 1));
-      gy = __fadd_rn(gy, __fmul_rn(-0.25f, P_(r - 1, c)));
-      gy = __fadd_rn(gy, __fmul_rn(-0.125f, P_(r - 1, c + 1)));
-      gy = __fadd_rn(gy, __fmul_rn(0.125f, P_(r + 1, c - 1)));
-      gy = __fadd_rn(gy, __fmul_rn(0.25f, P_(r + 1, c)));
-      gy = __fadd_rn(gy, __fmul_rn(0.125f, P_(r + 1, c + 1)));
-      const float mag = __fmul_rn(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), 1e-8f)), K->ori_w[i]);
-      const float ori = __fadd_rn(atan2f(gy, __fadd_rn(gx, 1e-8f)), two_pi);
-      const float ob = __fdiv_rn(__fmul_rn((float)KS_ORI_BINS, __fadd_rn(ori, KS_PI)), two_pi);
-      const float f = floorf(ob);
-      const float w1 = __fsub_rn(ob, f);
-      int b0 = (int)f % KS_ORI_BINS;
-      bin[i] = (unsigned char)b0;
-      wa[i] = __fmul_rn(__fsub_rn(1.f, w1), mag);
-      wb[i] = __fmul_rn(w1, mag);
-    }
-    __syncthreads();
-    if (threadIdx.x < KS_ORI_BINS) {              // adaptive_avg_pool2d: the bin's sum over the patch in raster order / N
-      const int q = threadIdx.x;
-      float s = 0.f;
-      for (int i = 0; i < N; ++i) {
-        const int b0 = bin[i], b1 = (b0 + 1) % KS_ORI_BINS;
-        s = __fadd_rn(s, __fadd_rn(b0 == q ? wa[i] : 0.f, b1 == q ? wb[i] : 0.f));
-      }
-      hist[q] = __fdiv_rn(s, (float)N);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float best = -CUDART_INF_F;
-      int bi = 0;
-      for (int q = 0; q < KS_ORI_BINS; ++q) {       // circular conv1d [0.33, 0.34, 0.33], then the first maximum
-        const float v = __fadd_rn(__fadd_rn(__fmul_rn(0.33f, hist[(q + KS_ORI_BINS - 1) % KS_ORI_BINS]), __fmul_rn(0.34f, hist[q])),
-                                  __fmul_rn(0.33f, hist[(q + 1) % KS_ORI_BINS]));
-        if (v > best) { best = v; bi = q; }
-      }
-      const float an = -__fsub_rn(__fdiv_rn(__fmul_rn(two_pi, (float)bi), (float)KS_ORI_BINS), KS_PI);
-      // set_laf_orientation(laf, rad2deg(an) + prev): rotate_laf(make_upright(laf), new - prev)
-      const float prev = __fdiv_rn(__fmul_rn(180.f, atan2f(a[1], a[0])), KS_PI);
-      const float nd = __fadd_rn(__fdiv_rn(__fmul_rn(180.f, an), KS_PI), prev);
-      const float rad = __fdiv_rn(__fmul_rn(__fsub_rn(nd, prev), KS_PI), 180.f);
-      const float cs = cosf(rad), sn = sinf(rad);
-      const float det = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a[0], a[4]), __fmul_rn(a[3], a[1])), 1e-10f)));
-      const float b2a2 = __fadd_rn(sqrtf(__fadd_rn(__fmul_rn(a[1], a[1]), __fmul_rn(a[0], a[0]))), 1e-9f);
-      const float u00 = __fmul_rn(det, __fdiv_rn(b2a2, det)), u01 = 0.f;
-      const float u10 = __fmul_rn(det, __fdiv_rn(__fadd_rn(__fmul_rn(a[4], a[1]), __fmul_rn(a[3], a[0])), __fmul_rn(b2a2, det)));
-      const float u11 = __fmul_rn(det, __fdiv_rn(det, b2a2));
-      la[0] = __fadd_rn(__fmul_rn(u00, cs), __fmul_rn(u01, -sn));
-      la[1] = __fadd_rn(__fmul_rn(u00, sn), __fmul_rn(u01, cs));
-      la[3] = __fadd_rn(__fmul_rn(u10, cs), __fmul_rn(u11, -sn));
-      la[4] = __fadd_rn(__fmul_rn(u10, sn), __fmul_rn(u11, cs));
-      hist[0] = an;
-    }
-    __syncthreads();
-    ang = hist[0];
-    for (int e = 0; e < 6; ++e) a[e] = la[e];
-    __syncthreads();
-  }
+  if (!upright) ang = ks_orient<THREADS>(P, b, H, W, K, a, patch, wa, wb, bin, hist, la);
   ks_patch<KS_DESC_PS>(P, b, H, W, a, patch);
   __syncthreads();
   constexpr int N = KS_DESC_PS * KS_DESC_PS;
