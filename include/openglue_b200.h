@@ -651,6 +651,35 @@ int og_kgftt_im2col3x3_s2(const float* x, int B, int H, int W, int C, float* out
 int og_kgftt_desc_finish(float* desc, int B, int out_cap, const int* n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * The DoG / AffNet / OriNet / HardNet front-end (the reference's OPENCVDoGAffNetHardNet, models/features/opencv/dog_affnet_harnet.py:
+ * cv2 SIFT keypoints, kornia_moons' LAFs, kornia 0.6.3's AffNet, OriNet and HardNet; csrc/dog_affnet.cuh).  Detection and selection
+ * are og_sift_detect (dtype 1) and og_sift_select; these stages describe the selected keypoints from the float image [B, H, W].
+ * The three CNNs are run by the caller between the stages (as og_kgftt_*), over chunks of output rows [r0, r0 + rows) of the
+ * [B, out_cap] output.  lafs [B, out_cap, 2, 3] carries each row's LAF between the stages: each stage reads its rows and rewrites them.
+ *   og_dogaff_workspace_bytes / og_dogaff_workspace_layout   the float image's pyrdown patch pyramid for 32-pixel patches.
+ *                              layout (host only): out[0] = levels np; out[1 + 3 l ..] = h, w, byte offset of level l (-1: the
+ *                              image); then the workspace bytes.  Returns the entries written.
+ *   og_dogaff_pyramid          builds the patch pyramid of image into ws
+ *   og_dogaff_affnet_patches   row (b, j), j < n[b]: keypoint kp[b, sel[b, j]] (kp [B, cap, 5] = x, y, size, angle, response) ->
+ *                              lafs = laf_from_opencv_SIFT_kpts (mrSize 6), scores = response, patches [rows, 32, 32] = AffNet's
+ *                              standardised input on make_upright(laf); rows past n[b] are 0
+ *   og_dogaff_frames           from AffNet's 8x8-conv output xy [rows, 3] (before tanh): lafs <- the affine LAF (preserve_orientation),
+ *                              patches = OriNet's standardised input on it
+ *   og_dogaff_orinet_head      from OriNet's last 3x3-conv activations act [rows, 8, 8, 64] (NHWC, 16-byte aligned), the head's
+ *                              weight [2, 8, 8, 64] ((ky, kx, c) order, 8-byte aligned) and bias [2]: Conv2d(64, 2, 8, padding=1),
+ *                              tanh, mean, angle = atan2(y0 + 1e-8, y1 + 1e-8); lafs <- set_laf_orientation(laf, rad2deg(angle) +
+ *                              get_laf_orientation(laf)), angle [B, out_cap], patches = HardNet's standardised input on the new LAF */
+int64_t og_dogaff_workspace_bytes(int B, int H, int W);
+int og_dogaff_workspace_layout(int B, int H, int W, int64_t* out, int n);
+int og_dogaff_pyramid(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, void* stream);
+int og_dogaff_affnet_patches(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, const float* kp, int cap, const int* sel,
+                             const int* n, int out_cap, int r0, int rows, float* lafs, float* scores, float* patches, void* stream);
+int og_dogaff_frames(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, const int* n, int out_cap, int r0, int rows,
+                     const float* xy, float* lafs, float* patches, void* stream);
+int og_dogaff_orinet_head(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, const int* n, int out_cap, int r0, int rows,
+                          const float* act, const float* weight, const float* bias, float* lafs, float* angle, float* patches, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Local features -> matcher inputs, and matches -> the compact match list of stand-alone inference.
  *   og_prepare_features  prepare_features_output (models/features/utils.py:54-65) with the LAF -> side-information converter
  *                        superglue.laf_to_sideinfo_method names (models/laf_converter.py:108-128).  One thread per keypoint.

@@ -170,6 +170,13 @@ SYMBOLS = {
     'og_kgftt_frames': (_I, [_P, _I, _I, _I, _I, _P, _L, _P, _P, _I, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P]),
     'og_kgftt_im2col3x3_s2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
     'og_kgftt_desc_finish': (_I, [_P, _I, _I, _P, _P]),
+    # DoG (cv2) / AffNet / OriNet / HardNet front-end
+    'og_dogaff_workspace_bytes': (_L, [_I, _I, _I]),
+    'og_dogaff_workspace_layout': (_I, [_I, _I, _I, _P, _I]),
+    'og_dogaff_pyramid': (_I, [_P, _I, _I, _I, _P, _L, _P]),
+    'og_dogaff_affnet_patches': (_I, [_P, _I, _I, _I, _P, _L, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
+    'og_dogaff_frames': (_I, [_P, _I, _I, _I, _P, _L, _P, _I, _I, _I, _P, _P, _P, _P]),
+    'og_dogaff_orinet_head': (_I, [_P, _I, _I, _I, _P, _L, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     # local features -> matcher inputs, matches -> compact list
     'og_prepare_features': (_I, [_P, _P, _L, _I, _I, _P, _P, _P]),
     'og_match_compact': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

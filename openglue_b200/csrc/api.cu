@@ -17,6 +17,7 @@
 #include "sift.cuh"
 #include "kornia_sift.cuh"
 #include "kornia_gftt.cuh"
+#include "dog_affnet.cuh"
 #include "features.cuh"
 #include "homography.cuh"
 #include "optim.cuh"
@@ -1326,6 +1327,78 @@ int og_kgftt_desc_finish(float* desc, int B, int out_cap, const int* n, void* st
   OG_CHECK_ARG(desc && n && B > 0 && out_cap > 0, "kgftt_desc_finish: bad arguments");
   const int64_t rows = (int64_t)B * out_cap;
   return OG_LAUNCH(kg_desc_finish_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, desc, B, out_cap, n);
+}
+
+// ---- DoG (cv2) / AffNet / OriNet / HardNet front-end (csrc/dog_affnet.cuh) ----
+// The workspace holds the float image's pyrdown patch pyramid for 32-pixel patches and the blur's scratch
+static int kd_layout(int B, int H, int W, KsLayout& L, const char* who) {
+  if (B <= 0 || B > 65535 || H <= 0 || W <= 0) return fail(OG_EINVAL, "%s: bad sizes", who);
+  if (min(H, W) < 2 || (int64_t)H * W > 0x7fffffffLL) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image is not supported", who, H, W);
+  L = KsLayout{};
+  int64_t f = 0;
+  L.tmp = f; f += (int64_t)B * H * W;
+  if (!ks_patch_levels(B, H, W, KG_PS, L, f)) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image has too many pyramid levels", who, H, W);
+  L.bytes = align_up(f * 4, 256);
+  return OG_OK;
+}
+static int kd_args(const float* image, const void* ws, int64_t ws_bytes, int B, int H, int W, KsLayout& L, const char* who) {
+  OG_CHECK_ARG(image && ws, "%s: null image or workspace", who);
+  if (const int rc = kd_layout(B, H, W, L, who)) return rc;
+  OG_CHECK_ARG(ws_bytes >= L.bytes, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes, (long long)L.bytes);
+  return OG_OK;
+}
+int64_t og_dogaff_workspace_bytes(int B, int H, int W) {
+  KsLayout L;
+  if (const int rc = kd_layout(B, H, W, L, "dogaff_workspace_bytes")) return rc;
+  return L.bytes;
+}
+int og_dogaff_workspace_layout(int B, int H, int W, int64_t* out, int n) {
+  OG_CHECK_ARG(out, "dogaff_workspace_layout: null pointer");
+  KsLayout L;
+  if (const int rc = kd_layout(B, H, W, L, "dogaff_workspace_layout")) return rc;
+  const int need = 1 + 3 * L.np + 1;
+  OG_CHECK_ARG(n >= need, "dogaff_workspace_layout: %d entries, %d needed", n, need);
+  int i = 0;
+  out[i++] = L.np;
+  for (int l = 0; l < L.np; ++l) { out[i++] = L.ph[l]; out[i++] = L.pw[l]; out[i++] = l == 0 ? -1 : 4 * L.pyr[l]; }
+  out[i++] = L.bytes;
+  return i;
+}
+int og_dogaff_pyramid(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, void* stream) {
+  KsLayout L;
+  if (const int rc = kd_args(image, ws, ws_bytes, B, H, W, L, "dogaff_pyramid")) return rc;
+  return ks_build_patch_pyramid(L, B, ks_patch_pyramid(L, image, ws), ws, (cudaStream_t)stream);
+}
+int og_dogaff_affnet_patches(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, const float* kp, int cap, const int* sel,
+                             const int* n, int out_cap, int r0, int rows, float* lafs, float* scores, float* patches, void* stream) {
+  KsLayout L;
+  if (const int rc = kd_args(image, ws, ws_bytes, B, H, W, L, "dogaff_affnet_patches")) return rc;
+  if (const int rc = kg_rows_args(image, kp, n, cap, out_cap, B, r0, rows, "dogaff_affnet_patches")) return rc;
+  OG_CHECK_ARG(sel && lafs && scores && patches, "dogaff_affnet_patches: null pointer");
+  if (rows == 0) return OG_OK;
+  return OG_LAUNCH(kd_affnet_patch_kernel<256>, rows, 256, 0, (cudaStream_t)stream, ks_patch_pyramid(L, image, ws), H, W, kp, cap, sel, n,
+                   out_cap, r0, lafs, scores, patches);
+}
+int og_dogaff_frames(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, const int* n, int out_cap, int r0, int rows,
+                     const float* xy, float* lafs, float* patches, void* stream) {
+  KsLayout L;
+  if (const int rc = kd_args(image, ws, ws_bytes, B, H, W, L, "dogaff_frames")) return rc;
+  if (const int rc = kg_rows_args(image, lafs, n, 1, out_cap, B, r0, rows, "dogaff_frames")) return rc;
+  OG_CHECK_ARG(xy && patches, "dogaff_frames: null pointer");
+  if (rows == 0) return OG_OK;
+  return OG_LAUNCH(kd_frame_kernel<256>, rows, 256, 0, (cudaStream_t)stream, ks_patch_pyramid(L, image, ws), H, W, n, out_cap, r0, xy, lafs,
+                   patches);
+}
+int og_dogaff_orinet_head(const float* image, int B, int H, int W, void* ws, int64_t ws_bytes, const int* n, int out_cap, int r0, int rows,
+                          const float* act, const float* weight, const float* bias, float* lafs, float* angle, float* patches, void* stream) {
+  KsLayout L;
+  if (const int rc = kd_args(image, ws, ws_bytes, B, H, W, L, "dogaff_orinet_head")) return rc;
+  if (const int rc = kg_rows_args(image, lafs, n, 1, out_cap, B, r0, rows, "dogaff_orinet_head")) return rc;
+  OG_CHECK_ARG(act && weight && bias && angle && patches, "dogaff_orinet_head: null pointer");
+  OG_CHECK_ARG(((uintptr_t)act % 16) == 0 && ((uintptr_t)weight % 8) == 0, "dogaff_orinet_head: act must be 16-byte and weight 8-byte aligned");
+  if (rows == 0) return OG_OK;
+  return OG_LAUNCH(kd_orinet_head_kernel, rows, 256, 0, (cudaStream_t)stream, ks_patch_pyramid(L, image, ws), H, W, n, out_cap, r0, act, weight,
+                   bias, lafs, angle, patches);
 }
 
 int og_keypoint_counts(const int* count, int B, int cap, int max_keypoints, int K, int* n_out, int* mode, int* overflow, void* stream) {

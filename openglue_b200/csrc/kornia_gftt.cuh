@@ -143,6 +143,32 @@ __global__ void __launch_bounds__(THREADS) kg_affnet_patch_kernel(KsPyr P, int H
   kg_standardize<THREADS>(patch, red, o);
 }
 
+// LAFAffNetShapeEstimator(preserve_orientation=True) after the network: v [3] (AffNet's 8x8-conv output, before tanh) and the
+// input LAF d -> the affine LAF a at d's centre, with d's orientation
+__device__ __forceinline__ void kg_affine_frame(const float* v, const float d[6], float a[6]) {
+  const float t0 = tanhf(v[0]), t1 = tanhf(v[1]), t2 = tanhf(v[2]);   // AdaptiveAvgPool2d(1) of a 1x1 map: the value itself
+  // new_laf = [[1 + t0, 0 t0], [t1, 1 + t2]] at the original centre
+  const float nl[6] = {__fadd_rn(1.f, t0), __fmul_rn(0.f, t0), d[2], t1, __fadd_rn(1.f, t2), d[5]};
+  const float scale_orig = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(d[0], d[4]), __fmul_rn(d[3], d[1])), 1e-10f)));
+  const float ori_orig = __fdiv_rn(__fmul_rn(180.f, atan2f(d[1], d[0])), KS_PI);
+  const float ellipse = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(nl[0], nl[4]), __fmul_rn(nl[3], nl[1])), 1e-10f)));
+  const float coef = __fdiv_rn(scale_orig, ellipse);
+  float u[6], s[6];
+  kg_upright(nl, u);                                    // scale_laf(make_upright(new_laf), scale_orig / ellipse_scale)
+  s[0] = __fmul_rn(u[0], coef); s[1] = __fmul_rn(u[1], coef); s[2] = u[2];
+  s[3] = __fmul_rn(u[3], coef); s[4] = __fmul_rn(u[4], coef); s[5] = u[5];
+  // set_laf_orientation(s, ori_orig) = rotate_laf(make_upright(s), ori_orig - get_laf_orientation(s))
+  const float cur = __fdiv_rn(__fmul_rn(180.f, atan2f(s[1], s[0])), KS_PI);
+  const float rad = __fdiv_rn(__fmul_rn(__fsub_rn(ori_orig, cur), KS_PI), 180.f);
+  const float cs = cosf(rad), sn = sinf(rad);
+  kg_upright(s, u);
+  a[0] = __fadd_rn(__fmul_rn(u[0], cs), __fmul_rn(u[1], -sn));
+  a[1] = __fadd_rn(__fmul_rn(u[0], sn), __fmul_rn(u[1], cs));
+  a[3] = __fadd_rn(__fmul_rn(u[3], cs), __fmul_rn(u[4], -sn));
+  a[4] = __fadd_rn(__fmul_rn(u[3], sn), __fmul_rn(u[4], cs));
+  a[2] = d[2]; a[5] = d[5];
+}
+
 // After AffNet's CNN, chunk rows [r0, r0 + gridDim.x): xy [rows][3] (before tanh) and the detector LAF -> the affine LAF
 // (LAFAffNetShapeEstimator with preserve_orientation), then LAFOrienter(19) unless upright; writes the row's LAF, score and angle
 // and HardNet's standardised patch on the final LAF (out [rows][32][32]).  Rows past n[b] get zeros.
@@ -170,30 +196,7 @@ __global__ void __launch_bounds__(THREADS) kg_frame_kernel(KsPyr P, int H, int W
   }
   float d[6], a[6];
   for (int e = 0; e < 6; ++e) d[e] = lafs_in[((int64_t)b * cap_in + src) * 6 + e];
-  {
-    const float* v = xy + (int64_t)blockIdx.x * 3;
-    const float t0 = tanhf(v[0]), t1 = tanhf(v[1]), t2 = tanhf(v[2]);   // AdaptiveAvgPool2d(1) of a 1x1 map: the value itself
-    // new_laf = [[1 + t0, 0 t0], [t1, 1 + t2]] at the original centre
-    const float nl[6] = {__fadd_rn(1.f, t0), __fmul_rn(0.f, t0), d[2], t1, __fadd_rn(1.f, t2), d[5]};
-    const float scale_orig = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(d[0], d[4]), __fmul_rn(d[3], d[1])), 1e-10f)));
-    const float ori_orig = __fdiv_rn(__fmul_rn(180.f, atan2f(d[1], d[0])), KS_PI);
-    const float ellipse = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(nl[0], nl[4]), __fmul_rn(nl[3], nl[1])), 1e-10f)));
-    const float coef = __fdiv_rn(scale_orig, ellipse);
-    float u[6], s[6];
-    kg_upright(nl, u);                                    // scale_laf(make_upright(new_laf), scale_orig / ellipse_scale)
-    s[0] = __fmul_rn(u[0], coef); s[1] = __fmul_rn(u[1], coef); s[2] = u[2];
-    s[3] = __fmul_rn(u[3], coef); s[4] = __fmul_rn(u[4], coef); s[5] = u[5];
-    // set_laf_orientation(s, ori_orig) = rotate_laf(make_upright(s), ori_orig - get_laf_orientation(s))
-    const float cur = __fdiv_rn(__fmul_rn(180.f, atan2f(s[1], s[0])), KS_PI);
-    const float rad = __fdiv_rn(__fmul_rn(__fsub_rn(ori_orig, cur), KS_PI), 180.f);
-    const float cs = cosf(rad), sn = sinf(rad);
-    kg_upright(s, u);
-    a[0] = __fadd_rn(__fmul_rn(u[0], cs), __fmul_rn(u[1], -sn));
-    a[1] = __fadd_rn(__fmul_rn(u[0], sn), __fmul_rn(u[1], cs));
-    a[3] = __fadd_rn(__fmul_rn(u[3], cs), __fmul_rn(u[4], -sn));
-    a[4] = __fadd_rn(__fmul_rn(u[3], sn), __fmul_rn(u[4], cs));
-    a[2] = d[2]; a[5] = d[5];
-  }
+  kg_affine_frame(xy + (int64_t)blockIdx.x * 3, d, a);
   if (threadIdx.x < 6) la[threadIdx.x] = a[threadIdx.x];
   __syncthreads();
   float ang = 0.f;

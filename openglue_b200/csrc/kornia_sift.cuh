@@ -43,6 +43,21 @@ struct KsLayout {
   int64_t bytes;
 };
 
+// The pyrdown patch pyramid of an H x W image for patches of ps pixels: level k + 1 exists while level k's smaller side is >= ps.
+// Sets L.np, L.ph, L.pw and L.pyr (float offsets from f, which it advances).
+inline bool ks_patch_levels(int B, int H, int W, int ps, KsLayout& L, int64_t& f) {
+  int ph = H, pw = W;
+  L.np = 1; L.ph[0] = H; L.pw[0] = W; L.pyr[0] = -1;
+  while (min(ph, pw) >= ps) {
+    if (L.np == KS_MAX_PATCH_LEVELS) return false;
+    ph /= 2; pw /= 2;
+    L.ph[L.np] = ph; L.pw[L.np] = pw;
+    L.pyr[L.np] = f; f += (int64_t)B * max(ph, 1) * max(pw, 1);
+    ++L.np;
+  }
+  return true;
+}
+
 // Octave sizes: 2H x 2W (H x W without double_image), then [::2, ::2] while the smaller side stays above 32
 // (ScalePyramid.forward).  The per-octave volume the detector reads ("dog") has vol_levels levels: the 5 DoG levels of SIFT, or
 // the GFTT responses of all 6 Gaussian levels.
@@ -64,16 +79,8 @@ inline bool ks_layout(int B, int H, int W, int k, KsLayout& L, bool double_image
     h = nh; w = nw;
   }
   L.tmp = f; f += (int64_t)B * L.oct[0].h * L.oct[0].w;
-  // patch pyramid for 19-pixel patches (the deeper of the two): level k + 1 exists while level k's smaller side is >= 19
-  int ph = H, pw = W;
-  L.np = 1; L.ph[0] = H; L.pw[0] = W; L.pyr[0] = -1;
-  while (min(ph, pw) >= KS_ORI_PS) {
-    if (L.np == KS_MAX_PATCH_LEVELS) return false;
-    ph /= 2; pw /= 2;
-    L.ph[L.np] = ph; L.pw[L.np] = pw;
-    L.pyr[L.np] = f; f += (int64_t)B * max(ph, 1) * max(pw, 1);
-    ++L.np;
-  }
+  // patch pyramid for 19-pixel patches (the deeper of the two)
+  if (!ks_patch_levels(B, H, W, KS_ORI_PS, L, f)) return false;
   int64_t b = align_up(f * 4, 256);
   const int segs = B * L.nO;
   L.state = b; b = align_up(b + (int64_t)segs * 32, 256);
@@ -650,6 +657,24 @@ __device__ void ks_patch(const KsPyr& P, int b, int H, int W, const float a[6], 
   }
 }
 
+// LAFOrienter's composition for the angle an (radians) found on the LAF a: set_laf_orientation(a, rad2deg(an) + prev), i.e.
+// rotate_laf(make_upright(a), new - prev) with prev = get_laf_orientation(a).  Writes the new 2x2 part to la[0, 1, 3, 4].
+__device__ __forceinline__ void ks_set_orientation(const float a[6], float an, float* la) {
+  const float prev = __fdiv_rn(__fmul_rn(180.f, atan2f(a[1], a[0])), KS_PI);
+  const float nd = __fadd_rn(__fdiv_rn(__fmul_rn(180.f, an), KS_PI), prev);
+  const float rad = __fdiv_rn(__fmul_rn(__fsub_rn(nd, prev), KS_PI), 180.f);
+  const float cs = cosf(rad), sn = sinf(rad);
+  const float det = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a[0], a[4]), __fmul_rn(a[3], a[1])), 1e-10f)));
+  const float b2a2 = __fadd_rn(sqrtf(__fadd_rn(__fmul_rn(a[1], a[1]), __fmul_rn(a[0], a[0]))), 1e-9f);
+  const float u00 = __fmul_rn(det, __fdiv_rn(b2a2, det)), u01 = 0.f;
+  const float u10 = __fmul_rn(det, __fdiv_rn(__fadd_rn(__fmul_rn(a[4], a[1]), __fmul_rn(a[3], a[0])), __fmul_rn(b2a2, det)));
+  const float u11 = __fmul_rn(det, __fdiv_rn(det, b2a2));
+  la[0] = __fadd_rn(__fmul_rn(u00, cs), __fmul_rn(u01, -sn));
+  la[1] = __fadd_rn(__fmul_rn(u00, sn), __fmul_rn(u01, cs));
+  la[3] = __fadd_rn(__fmul_rn(u10, cs), __fmul_rn(u11, -sn));
+  la[4] = __fadd_rn(__fmul_rn(u10, sn), __fmul_rn(u11, cs));
+}
+
 // LAFOrienter(19) on the LAF a (every thread of the CTA, a in registers, la its shared copy): the dominant orientation of its
 // 19-pixel patch; a <- set_laf_orientation(a, rad2deg(angle) + get_laf_orientation(a)).  Returns the angle (radians).
 template <int THREADS>
@@ -705,20 +730,7 @@ __device__ float ks_orient(const KsPyr& P, int b, int H, int W, const KsDescCons
       if (v > best) { best = v; bi = q; }
     }
     const float an = -__fsub_rn(__fdiv_rn(__fmul_rn(two_pi, (float)bi), (float)KS_ORI_BINS), KS_PI);
-    // set_laf_orientation(laf, rad2deg(an) + prev): rotate_laf(make_upright(laf), new - prev)
-    const float prev = __fdiv_rn(__fmul_rn(180.f, atan2f(a[1], a[0])), KS_PI);
-    const float nd = __fadd_rn(__fdiv_rn(__fmul_rn(180.f, an), KS_PI), prev);
-    const float rad = __fdiv_rn(__fmul_rn(__fsub_rn(nd, prev), KS_PI), 180.f);
-    const float cs = cosf(rad), sn = sinf(rad);
-    const float det = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a[0], a[4]), __fmul_rn(a[3], a[1])), 1e-10f)));
-    const float b2a2 = __fadd_rn(sqrtf(__fadd_rn(__fmul_rn(a[1], a[1]), __fmul_rn(a[0], a[0]))), 1e-9f);
-    const float u00 = __fmul_rn(det, __fdiv_rn(b2a2, det)), u01 = 0.f;
-    const float u10 = __fmul_rn(det, __fdiv_rn(__fadd_rn(__fmul_rn(a[4], a[1]), __fmul_rn(a[3], a[0])), __fmul_rn(b2a2, det)));
-    const float u11 = __fmul_rn(det, __fdiv_rn(det, b2a2));
-    la[0] = __fadd_rn(__fmul_rn(u00, cs), __fmul_rn(u01, -sn));
-    la[1] = __fadd_rn(__fmul_rn(u00, sn), __fmul_rn(u01, cs));
-    la[3] = __fadd_rn(__fmul_rn(u10, cs), __fmul_rn(u11, -sn));
-    la[4] = __fadd_rn(__fmul_rn(u10, sn), __fmul_rn(u11, cs));
+    ks_set_orientation(a, an, la);
     hist[0] = an;
   }
   __syncthreads();

@@ -243,9 +243,10 @@ def _frontend_version(module: nn.Module) -> tuple:
 
 
 def _frontend_storage(module: nn.Module) -> tuple:
-    """The front-end's cached workspaces and packed weights: a captured graph reads them, so it holds them even if the
-    front-end drops them later"""
-    return tuple(getattr(module, '_ws', {}).values()), getattr(module, '_packed', None)
+    """The cached workspaces and packed weights of the front-end and of every module inside it (``DoGOpenCVAffNetHardNet``
+    detects through its own ``OpenCVSIFT``): a captured graph reads them, so it holds them even if a module drops them later"""
+    mods = list(module.modules())
+    return tuple(v for m in mods for v in getattr(m, '_ws', {}).values()), tuple(getattr(m, '_packed', None) for m in mods)
 
 
 def _check_image_pair(image0, image1) -> None:

@@ -16,7 +16,6 @@ from ``weights=`` or from the files kornia caches under ``torch.hub.get_dir()/ch
 """
 from __future__ import annotations
 
-import os
 from typing import List, Optional, Tuple
 
 import torch
@@ -25,18 +24,14 @@ import torch.nn as nn
 from . import _cabi
 from ._cabi import ptr, stream
 from ._ops import _Ops
+from ._patch_cnn import AFFNET_CONVS, CHUNK, HARDNET_CONVS, HEAD, PS  # noqa: F401
+from ._patch_cnn import AffNet as _AffNet, HardNet as _HardNet, fold as _fold, state_dict_of as _state_dict_of  # noqa: F401
+from ._patch_cnn import cnn_buffers, load_networks, nhwc_head, run_cnn, weights_key
 from .features import padded_capacity
 
 __all__ = ['GFTTAffNetHardNet']
 
 MAX_FEATURES = 8192                 # keypoints per image the detector and run_nms sort in one CTA's shared memory
-PS = 32
-CHUNK = 128                         # patches per CNN pass: the scratch is CHUNK * 1.34 MB (im2col of HardNet's 32x32x32 layer)
-# (features index, in channels, out channels, stride) of the 3x3 convolutions; each is followed by BatchNorm2d(affine=False), ReLU
-AFFNET_CONVS = [(0, 1, 16, 1), (3, 16, 16, 1), (6, 16, 32, 2), (9, 32, 32, 1), (12, 32, 64, 2), (15, 64, 64, 1)]
-HARDNET_CONVS = [(0, 1, 32, 1), (3, 32, 32, 1), (6, 32, 64, 2), (9, 64, 64, 1), (12, 64, 128, 2), (15, 128, 128, 1)]
-HEAD = 19                           # the 8x8 convolution of both networks (index 18 is Dropout)
-BN_EPS = 1e-5
 # the files kornia 0.6.3 caches in torch.hub.get_dir()/checkpoints, and where it fetches them from
 CHECKPOINTS = {
     'affnet': ('AffNet.pth', 'https://github.com/ducha-aiki/affnet/raw/master/pretrained/AffNet.pth'),
@@ -44,31 +39,6 @@ CHECKPOINTS = {
                 'https://github.com/DagnyT/hardnet/raw/master/pretrained/train_liberty_with_aug/checkpoint_liberty_with_aug.pth'),
 }
 ORIENT_SMOOTH = (0.33, 0.34, 0.33)  # PatchDominantGradientOrientation's fixed angular smoothing
-
-
-def _conv_stack(convs):
-    layers = []
-    for _, ci, co, s in convs:
-        layers += [nn.Conv2d(ci, co, kernel_size=3, stride=s, padding=1, bias=False), nn.BatchNorm2d(co, affine=False), nn.ReLU()]
-    return layers
-
-
-class _AffNet(nn.Module):
-    """LAFAffNetShapeEstimator's parameters (``features.<i>``)"""
-
-    def __init__(self):
-        super().__init__()
-        self.features = nn.Sequential(*_conv_stack(AFFNET_CONVS), nn.Dropout(0.25), nn.Conv2d(64, 3, kernel_size=8, bias=True), nn.Tanh(),
-                                      nn.AdaptiveAvgPool2d(1))
-
-
-class _HardNet(nn.Module):
-    """HardNet's parameters (``features.<i>``)"""
-
-    def __init__(self):
-        super().__init__()
-        self.features = nn.Sequential(*_conv_stack(HARDNET_CONVS), nn.Dropout(0.3), nn.Conv2d(128, 128, kernel_size=8, bias=False),
-                                      nn.BatchNorm2d(128, affine=False))
 
 
 class _AngleDetector(nn.Module):
@@ -84,26 +54,6 @@ class _Orienter(nn.Module):
     def __init__(self):
         super().__init__()
         self.angle_detector = _AngleDetector()
-
-
-def _fold(conv_w: torch.Tensor, bn: nn.BatchNorm2d, bias: Optional[torch.Tensor] = None):
-    """eval-mode BatchNorm2d(affine=False) after a convolution, folded in float64: (W / s, (b - mean) / s), s = sqrt(var + eps);
-    the weight as [Cout, (ky, kx, Cin)] for NHWC im2col"""
-    s = torch.sqrt(bn.running_var.detach().double() + bn.eps)
-    w = conv_w.detach().double() / s.view(-1, 1, 1, 1)
-    b = ((bias.detach().double() if bias is not None else 0.0) - bn.running_mean.detach().double()) / s
-    co = w.shape[0]
-    return w.permute(0, 2, 3, 1).reshape(co, -1).float().contiguous(), b.float().contiguous()
-
-
-def _state_dict_of(src, name: str) -> dict:
-    if isinstance(src, (str, os.PathLike)):
-        # kornia's checkpoints hold training state beside the tensors, so they need the full unpickler, as kornia loads them
-        src = torch.load(os.fspath(src), map_location='cpu', weights_only=False)
-    if not isinstance(src, dict):
-        raise TypeError(f'weights[{name!r}] must be a checkpoint path or a state dict, got {type(src)}')
-    sd = src.get('state_dict', src)
-    return {k: v for k, v in sd.items() if k.startswith('features.')}
 
 
 class GFTTAffNetHardNet(nn.Module):
@@ -153,26 +103,11 @@ class GFTTAffNetHardNet(nn.Module):
     # ------------------------------------------------------------------ weights
     def load_weights(self, weights=None) -> None:
         """Loads AffNet and HardNet from ``weights`` (see the class) or from kornia's cache; never downloads."""
-        if weights is None:
-            root = os.path.join(torch.hub.get_dir(), 'checkpoints')
-            weights = {}
-            for name, (fname, url) in CHECKPOINTS.items():
-                path = os.path.join(root, fname)
-                if not os.path.isfile(path):
-                    raise FileNotFoundError(f'{path} not found: GFTTAffNetHardNet reads the {name} weights kornia caches there and never '
-                                            f'downloads; fetch {url} into {root}, or pass weights={{"affnet": ..., "hardnet": ...}}')
-                weights[name] = path
-        if set(weights) != {'affnet', 'hardnet'}:
-            raise ValueError(f"weights must have the keys 'affnet' and 'hardnet', got {sorted(weights)}")
-        for name, net in (('affnet', self.detector.aff), ('hardnet', self.descriptor.descriptor)):
-            res = net.load_state_dict(_state_dict_of(weights[name], name), strict=False)
-            missing = [k for k in res.missing_keys if not k.endswith('num_batches_tracked')]   # older checkpoints lack the counter
-            if missing or res.unexpected_keys:
-                raise KeyError(f'{name} weights: missing {missing}, unexpected {res.unexpected_keys}')
+        load_networks('GFTTAffNetHardNet', weights, CHECKPOINTS, {'affnet': self.detector.aff, 'hardnet': self.descriptor.descriptor})
 
     def _weights(self):
         """The networks' GEMM weights, packed once per parameter / buffer version: {name: [(W [Cout, K], bias [Cout])]}"""
-        key = tuple((t._version, t.data_ptr()) for t in list(self.parameters()) + list(self.buffers()))
+        key = weights_key(self)
         if self._packed is None or self._packed[0] != key:
             if not self.upright:
                 w = self.detector.ori.angle_detector.angular_smooth.weight.detach().flatten().tolist()
@@ -184,8 +119,7 @@ class GFTTAffNetHardNet(nn.Module):
                 layers = [_fold(net[i].weight, net[i + 1]) for i, *_ in convs]
                 head = net[HEAD]
                 if name == 'affnet':
-                    layers.append((head.weight.detach().permute(0, 2, 3, 1).reshape(3, -1).float().contiguous(),
-                                   head.bias.detach().float().contiguous()))
+                    layers.append(nhwc_head(head))
                 else:
                     layers.append(_fold(head.weight, net[HEAD + 1]))
                 packed[name] = layers
@@ -219,12 +153,7 @@ class GFTTAffNetHardNet(nn.Module):
         return self._ws[key]
 
     def _cnn_buffers(self, dev):
-        """patches [CHUNK, 32, 32], im2col [CHUNK * 32 * 32 * 9 * 32], two activations [CHUNK * 32 * 32 * 32], xy [CHUNK, 3]"""
-        key = ('cnn', dev)
-        if key not in self._ws:
-            f = lambda n: torch.empty(n, dtype=torch.float32, device=dev)
-            self._ws[key] = (f(CHUNK * PS * PS), f(CHUNK * PS * PS * 9 * 32), f(CHUNK * PS * PS * 32), f(CHUNK * PS * PS * 32), f(CHUNK * 3))
-        return self._ws[key]
+        return cnn_buffers(self._ws, dev)
 
     @staticmethod
     def _image(images: torch.Tensor) -> torch.Tensor:
@@ -258,22 +187,7 @@ class GFTTAffNetHardNet(nn.Module):
         return ws, det_lafs, det_resp, sel, n_sel
 
     def _cnn(self, ops: _Ops, layers, x: torch.Tensor, rows: int, convs, col, acts, out: torch.Tensor):
-        """One patch CNN on rows NHWC patches x [rows, 32, 32, 1]: 3x3 convolutions with folded BatchNorm and ReLU, then the 8x8
-        convolution as one GEMM over the flattened 8x8xC activations into out [rows, Cout]"""
-        lib, st = ops.lib, ops.st()
-        h = w = PS
-        for li, (_, ci, co, s) in enumerate(convs):
-            wt, b = layers[li]
-            if s == 1:
-                _cabi.check(lib.og_sp_im2col3x3(ptr(x), rows, h, w, ci, ptr(col), st), 'og_sp_im2col3x3')
-            else:
-                _cabi.check(lib.og_kgftt_im2col3x3_s2(ptr(x), rows, h, w, ci, ptr(col), st), 'og_kgftt_im2col3x3_s2')
-                h, w = (h + 1) // 2, (w + 1) // 2
-            a = col[:rows * h * w * 9 * ci].view(rows * h * w, 9 * ci)
-            y = acts[li % 2][:rows * h * w * co].view(rows * h * w, co)
-            x = ops.linear(a, wt, b, relu=True, out=y)
-        wt, b = layers[-1]
-        ops.linear(x.view(rows, -1), wt, b, out=out)
+        run_cnn(ops, layers, x, rows, convs, col, acts, out)
 
     def _describe(self, img, ws, det_lafs, det_resp, sel, n, out_cap):
         B, _, H, W = img.shape
