@@ -323,9 +323,7 @@ def extract_patches_from_pyramid(img: torch.Tensor, laf: torch.Tensor, PS: int) 
     _, ch, h, w = img.shape
     B, N = laf.shape[:2]
     nlaf = normalize_laf(laf, h, w)
-    scale = 2.0 * get_laf_scale(denormalize_laf(nlaf, h, w)) / float(PS)
-    max_level = min(h, w) // PS
-    pyr_idx = scale.log2().clamp(min=0.0, max=max(0, max_level - 1)).long()
+    pyr_idx = patch_pyramid_level(laf, h, w, PS)
     cur, level = img, 0
     out = torch.zeros(B, N, ch, PS, PS).to(nlaf)
     while True:
@@ -346,6 +344,15 @@ def extract_patches_from_pyramid(img: torch.Tensor, laf: torch.Tensor, PS: int) 
         cur = pyrdown(cur)
         level += 1
     return out
+
+
+def patch_pyramid_level(laf: torch.Tensor, h: int, w: int, PS: int) -> torch.Tensor:
+    """The pyrdown level extract_patches_from_pyramid samples each LAF [B, N, 2, 3] of an h x w image from, in the LAF's dtype:
+    log2(2 scale / PS) clamped to [0, min(h, w) // PS - 1], [B, N, 1, 1] int64.  Levels at or past patch_pyramid_levels are not
+    visited, and their patches stay zero."""
+    scale = 2.0 * get_laf_scale(denormalize_laf(normalize_laf(laf, h, w), h, w)) / float(PS)
+    max_level = min(h, w) // PS
+    return scale.log2().clamp(min=0.0, max=max(0, max_level - 1)).long()
 
 
 def patch_pyramid_levels(h: int, w: int, PS: int) -> int:

@@ -48,6 +48,27 @@ def test_oracle_float32_against_float64_stage_by_stage():
     assert float((a32.double() - a64).abs().max()) <= 1e-5
 
 
+def test_patch_pyramid_level_float32_against_float64():
+    """the level of LAFs at scale 16 2^k (1 + d): float32 and float64 agree away from the boundaries and differ by at most one level
+    next to them; the clamp to min(h, w) // 32 - 1 holds in both; the levels are the ones extract_patches_from_pyramid samples"""
+    H, W = 160, 171
+    d = torch.tensor([-1e-2, -4e-4, -2.0 ** -22, 0.0, 2.0 ** -22, 4e-4, 1e-2], dtype=torch.float64)
+    s = (16.0 * 2.0 ** torch.arange(6, dtype=torch.float64)[:, None] * (1 + d)).flatten()
+    laf = torch.zeros(1, s.numel(), 2, 3, dtype=torch.float64)
+    laf[0, :, 0, 0], laf[0, :, 1, 1], laf[0, :, 0, 2], laf[0, :, 1, 2] = s, s, 80.0, 70.0
+    l64 = KO.patch_pyramid_level(laf, H, W, 32).flatten()
+    l32 = KO.patch_pyramid_level(laf.float(), H, W, 32).flatten()
+    far = (d.abs() >= 4e-4).repeat(6)
+    assert torch.equal(l32[far], l64[far]) and int((l32 - l64).abs().max()) <= 1
+    assert int(l64.max()) == min(H, W) // 32 - 1 and int(l64.min()) == 0
+    k = torch.log2(s / 16).floor().clamp(0, 4).long()                 # the nominal level of each row
+    assert torch.equal(l64[far], k[far])
+    img = torch.rand(1, 1, H, W, dtype=torch.float64, generator=torch.Generator().manual_seed(0))
+    p = KO.extract_patches_from_pyramid(img, laf, 32).flatten(2)
+    past = l64 >= KO.patch_pyramid_levels(H, W, 32)                    # levels never visited: zero patches
+    assert bool(past.any()) and not p[0, past].any() and bool((p[0, ~past].abs().amax(1) > 0).all())
+
+
 def test_fixture_consistency():
     for name in ['ksift_tiny', 'ksift_small', 'ksift_odd', 'ksift_warp', 'ksift_uniform', 'ksift_pair']:
         fx = _fx(name)
