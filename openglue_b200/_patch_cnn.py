@@ -1,6 +1,6 @@
 """What the kornia patch-CNN front-ends (``GFTTAffNetHardNet``, ``DoGOpenCVAffNetHardNet``) share: kornia's AffNet / OriNet /
-HardNet layer tables, the eval-mode BatchNorm fold, checkpoint reading, and the CNNs as NHWC im2col + the Hopper GEMM over chunks of
-``CHUNK`` patches."""
+HardNet layer tables and checkpoint files, the eval-mode BatchNorm fold, checkpoint reading, the packed-weight cache, and the CNNs
+as NHWC im2col + the Hopper GEMM over chunks of ``CHUNK`` patches."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,9 @@ import torch.nn as nn
 
 from . import _cabi
 from ._cabi import ptr
+from ._frontend import FrontEnd
 from ._ops import _Ops
+from .features import weights_key
 
 PS = 32
 CHUNK = 128                         # patches per CNN pass: the scratch is CHUNK * 1.34 MB (im2col of HardNet's 32x32x32 layer)
@@ -21,6 +23,13 @@ AFFNET_CONVS = [(0, 1, 16, 1), (3, 16, 16, 1), (6, 16, 32, 2), (9, 32, 32, 1), (
 HARDNET_CONVS = [(0, 1, 32, 1), (3, 32, 32, 1), (6, 32, 64, 2), (9, 64, 64, 1), (12, 64, 128, 2), (15, 128, 128, 1)]
 HEAD = 19                           # the 8x8 convolution of the networks (index 18 is Dropout)
 BN_EPS = 1e-5
+# the files kornia 0.6.3 caches in torch.hub.get_dir()/checkpoints, and where it fetches them from
+CHECKPOINTS = {
+    'affnet': ('AffNet.pth', 'https://github.com/ducha-aiki/affnet/raw/master/pretrained/AffNet.pth'),
+    'orinet': ('OriNet.pth', 'https://github.com/ducha-aiki/affnet/raw/master/pretrained/OriNet.pth'),
+    'hardnet': ('checkpoint_liberty_with_aug.pth',
+                'https://github.com/DagnyT/hardnet/raw/master/pretrained/train_liberty_with_aug/checkpoint_liberty_with_aug.pth'),
+}
 
 
 def conv_stack(convs):
@@ -96,11 +105,6 @@ def load_networks(owner: str, weights, checkpoints: dict, nets: dict) -> None:
             raise KeyError(f'{name} weights: missing {missing}, unexpected {res.unexpected_keys}')
 
 
-def weights_key(module: nn.Module):
-    """Changes whenever a parameter or buffer of ``module`` is written or replaced"""
-    return tuple((t._version, t.data_ptr()) for t in list(module.parameters()) + list(module.buffers()))
-
-
 def cnn_buffers(ws: dict, dev):
     """patches [CHUNK, 32, 32], im2col [CHUNK * 32 * 32 * 9 * 32], two activations [CHUNK * 32 * 32 * 32], xy [CHUNK, 3], cached in
     ``ws`` under ('cnn', dev)"""
@@ -132,3 +136,24 @@ def run_cnn(ops: _Ops, layers, x: torch.Tensor, rows: int, convs, col, acts, out
     wt, b = layers[len(convs)]
     ops.linear(x.view(rows, -1), wt, b, out=out)
     return out
+
+
+class CNNFrontEnd(FrontEnd):
+    """A front-end that describes through the patch CNNs: ``precision`` picks the GEMM, ``_pack()`` gives the networks' GEMM
+    layers ({name: [(W [Cout, K], bias [Cout])]}), and the networks run on their running BatchNorm statistics only"""
+
+    def _ops(self, dev) -> _Ops:
+        return _Ops(dev, _cabi.OG_PREC_FP32 if self.precision == 'fp32' else _cabi.OG_PREC_TF32X3)
+
+    def _weights_on(self, dev):
+        """``_pack()`` on dev, once per parameter / buffer version"""
+        key = (weights_key(self), dev)
+        if self._packed is None or self._packed[0] != key:
+            self._packed = (key, {name: [(w.to(dev), b.to(dev)) for w, b in layers] for name, layers in self._pack().items()})
+        return self._packed[1]
+
+    def train(self, mode: bool = True):
+        if mode:
+            raise RuntimeError(f'openglue_b200.{type(self).__name__} is an inference front-end (its networks run on their running '
+                               'BatchNorm statistics); fine-tuning them is not built')
+        return super().train(mode)

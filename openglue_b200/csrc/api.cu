@@ -1041,12 +1041,10 @@ int64_t og_ksift_workspace_bytes(int B, int H, int W, int num_features) {
   if (const int rc = ks_check_sizes(B, H, W, num_features, L, "ksift_workspace_bytes")) return rc;
   return L.bytes;
 }
-int og_ksift_workspace_layout(int B, int H, int W, int num_features, int64_t* out, int n) {
-  OG_CHECK_ARG(out, "ksift_workspace_layout: null pointer");
-  KsLayout L;
-  if (const int rc = ks_check_sizes(B, H, W, num_features, L, "ksift_workspace_layout")) return rc;
+// og_ksift_workspace_layout / og_kgftt_workspace_layout: the octaves, the patch pyramid and the total size of L into out[0, n)
+static int ks_write_layout(const KsLayout& L, int64_t* out, int n, const char* who) {
   const int need = 1 + 5 * L.nO + 1 + 3 * L.np + 1;
-  OG_CHECK_ARG(n >= need, "ksift_workspace_layout: %d entries, %d needed", n, need);
+  OG_CHECK_ARG(n >= need, "%s: %d entries, %d needed", who, n, need);
   int i = 0;
   out[i++] = L.nO;
   for (int o = 0; o < L.nO; ++o) {
@@ -1057,6 +1055,12 @@ int og_ksift_workspace_layout(int B, int H, int W, int num_features, int64_t* ou
   for (int l = 0; l < L.np; ++l) { out[i++] = L.ph[l]; out[i++] = L.pw[l]; out[i++] = l == 0 ? -1 : 4 * L.pyr[l]; }
   out[i++] = L.bytes;
   return i;
+}
+int og_ksift_workspace_layout(int B, int H, int W, int num_features, int64_t* out, int n) {
+  OG_CHECK_ARG(out, "ksift_workspace_layout: null pointer");
+  KsLayout L;
+  if (const int rc = ks_check_sizes(B, H, W, num_features, L, "ksift_workspace_layout")) return rc;
+  return ks_write_layout(L, out, n, "ksift_workspace_layout");
 }
 static int ks_blur(float* ws_f, const KsLayout& L, int B, int h, int w, const float* src, int64_t src_stride, double sigma,
                    float* dst, int64_t dst_stride, cudaStream_t st) {
@@ -1069,9 +1073,12 @@ static int ks_blur(float* ws_f, const KsLayout& L, int B, int h, int w, const fl
   if (const int rc = OG_LAUNCH(ks_blur_kernel, sift_grid(B * plane), 256, 0, st, src, src_stride, B, h, w, t, 0, tmp, plane)) return rc;
   return OG_LAUNCH(ks_blur_kernel, sift_grid(B * plane), 256, 0, st, (const float*)tmp, plane, B, h, w, t, 1, dst, dst_stride);
 }
-static int ks_args(void* ws, int64_t ws_bytes, int B, int H, int W, int k, KsLayout& L, const char* who) {
+// A workspace of ws_bytes at ws for a front-end whose sizes `check` accepts (ks_check_sizes: kornia SIFT, kg_check_sizes: GFTT)
+typedef int (*KsSizeCheck)(int B, int H, int W, int k, KsLayout& L, const char* who);
+static int ks_args(const void* ws, int64_t ws_bytes, int B, int H, int W, int k, KsLayout& L, const char* who,
+                   KsSizeCheck check = ks_check_sizes) {
   OG_CHECK_ARG(ws, "%s: null workspace", who);
-  if (const int rc = ks_check_sizes(B, H, W, k, L, who)) return rc;
+  if (const int rc = check(B, H, W, k, L, who)) return rc;
   OG_CHECK_ARG(ws_bytes >= L.bytes, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes, (long long)L.bytes);
   return OG_OK;
 }
@@ -1229,12 +1236,6 @@ static int kg_check_sizes(int B, int H, int W, int k, KsLayout& L, const char* w
   if (!ks_layout(B, H, W, k, L, false, KS_LEVELS)) return fail(OG_EUNSUPPORTED, "%s: a %d x %d image has more than %d octaves", who, H, W, KS_MAX_OCTAVES);
   return OG_OK;
 }
-static int kg_args(const void* ws, int64_t ws_bytes, int B, int H, int W, int k, KsLayout& L, const char* who) {
-  OG_CHECK_ARG(ws, "%s: null workspace", who);
-  if (const int rc = kg_check_sizes(B, H, W, k, L, who)) return rc;
-  OG_CHECK_ARG(ws_bytes >= L.bytes, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes, (long long)L.bytes);
-  return OG_OK;
-}
 int64_t og_kgftt_workspace_bytes(int B, int H, int W, int num_features) {
   KsLayout L;
   if (const int rc = kg_check_sizes(B, H, W, num_features, L, "kgftt_workspace_bytes")) return rc;
@@ -1244,22 +1245,11 @@ int og_kgftt_workspace_layout(int B, int H, int W, int num_features, int64_t* ou
   OG_CHECK_ARG(out, "kgftt_workspace_layout: null pointer");
   KsLayout L;
   if (const int rc = kg_check_sizes(B, H, W, num_features, L, "kgftt_workspace_layout")) return rc;
-  const int need = 1 + 5 * L.nO + 1 + 3 * L.np + 1;
-  OG_CHECK_ARG(n >= need, "kgftt_workspace_layout: %d entries, %d needed", n, need);
-  int i = 0;
-  out[i++] = L.nO;
-  for (int o = 0; o < L.nO; ++o) {
-    out[i++] = L.oct[o].h; out[i++] = L.oct[o].w;
-    out[i++] = 4 * L.oct[o].gauss; out[i++] = 4 * L.oct[o].dog; out[i++] = 4 * L.oct[o].resp;
-  }
-  out[i++] = L.np;
-  for (int l = 0; l < L.np; ++l) { out[i++] = L.ph[l]; out[i++] = L.pw[l]; out[i++] = l == 0 ? -1 : 4 * L.pyr[l]; }
-  out[i++] = L.bytes;
-  return i;
+  return ks_write_layout(L, out, n, "kgftt_workspace_layout");
 }
 int og_kgftt_pyramid(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, void* stream) {
   KsLayout L;
-  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_pyramid")) return rc;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_pyramid", kg_check_sizes)) return rc;
   OG_CHECK_ARG(image, "kgftt_pyramid: null image");
   cudaStream_t st = (cudaStream_t)stream;
   float* f = static_cast<float*>(ws);
@@ -1286,7 +1276,7 @@ int og_kgftt_pyramid(const float* image, int B, int H, int W, int num_features, 
 }
 int og_kgftt_detect(int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, float* lafs, float* resp, int* count, void* stream) {
   KsLayout L;
-  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_detect")) return rc;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_detect", kg_check_sizes)) return rc;
   OG_CHECK_ARG(lafs && resp && count, "kgftt_detect: null pointer");
   return ks_detect(L, B, H, W, true, ws, lafs, resp, count, (cudaStream_t)stream);
 }
@@ -1299,7 +1289,7 @@ static int kg_rows_args(const float* image, const float* lafs, const int* n, int
 int og_kgftt_affnet_patches(const float* image, int B, int H, int W, int num_features, void* ws, int64_t ws_bytes, const float* lafs, int cap,
                             const int* sel, const int* n, int out_cap, int r0, int rows, float* patches, void* stream) {
   KsLayout L;
-  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_affnet_patches")) return rc;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_affnet_patches", kg_check_sizes)) return rc;
   if (const int rc = kg_rows_args(image, lafs, n, cap, out_cap, B, r0, rows, "kgftt_affnet_patches")) return rc;
   OG_CHECK_ARG(patches, "kgftt_affnet_patches: null pointer");
   if (rows == 0) return OG_OK;
@@ -1310,7 +1300,7 @@ int og_kgftt_frames(const float* image, int B, int H, int W, int num_features, v
                     int cap, const int* sel, const int* n, int out_cap, int r0, int rows, const float* xy, int upright, float* lafs_out,
                     float* scores, float* angle, float* patches, void* stream) {
   KsLayout L;
-  if (const int rc = kg_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_frames")) return rc;
+  if (const int rc = ks_args(ws, ws_bytes, B, H, W, num_features, L, "kgftt_frames", kg_check_sizes)) return rc;
   if (const int rc = kg_rows_args(image, lafs, n, cap, out_cap, B, r0, rows, "kgftt_frames")) return rc;
   OG_CHECK_ARG(resp && xy && lafs_out && scores && patches, "kgftt_frames: null pointer");
   if (rows == 0) return OG_OK;

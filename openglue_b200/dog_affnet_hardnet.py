@@ -18,29 +18,19 @@ kornia caches under ``torch.hub.get_dir()/checkpoints``.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Tuple
-
 import torch
 import torch.nn as nn
 
-from . import _cabi
-from ._cabi import ptr, stream
-from ._ops import _Ops
-from ._patch_cnn import AFFNET_CONVS, CHUNK, HARDNET_CONVS, HEAD, AffNet, HardNet
-from ._patch_cnn import cnn_buffers, conv_stack, fold, load_networks, nhwc_head, run_cnn, weights_key
-from .features import padded_capacity
+from . import _cabi, _patch_cnn
+from ._cabi import ptr
+from ._patch_cnn import AFFNET_CONVS, CHUNK, HARDNET_CONVS, HEAD, AffNet, CNNFrontEnd, HardNet
+from ._patch_cnn import cnn_buffers, conv_stack, fold, load_networks, nhwc_head
 from .sift import DEFAULT_CAPACITY, OpenCVSIFT
 
 __all__ = ['DoGOpenCVAffNetHardNet']
 
 ORINET_CONVS = AFFNET_CONVS             # OriNet's 3x3 stack has AffNet's shapes
-# the files kornia 0.6.3 caches in torch.hub.get_dir()/checkpoints, and where it fetches them from
-CHECKPOINTS = {
-    'affnet': ('AffNet.pth', 'https://github.com/ducha-aiki/affnet/raw/master/pretrained/AffNet.pth'),
-    'orinet': ('OriNet.pth', 'https://github.com/ducha-aiki/affnet/raw/master/pretrained/OriNet.pth'),
-    'hardnet': ('checkpoint_liberty_with_aug.pth',
-                'https://github.com/DagnyT/hardnet/raw/master/pretrained/train_liberty_with_aug/checkpoint_liberty_with_aug.pth'),
-}
+CHECKPOINTS = {k: _patch_cnn.CHECKPOINTS[k] for k in ('affnet', 'orinet', 'hardnet')}
 
 
 class _OriNet(nn.Module):
@@ -58,7 +48,7 @@ class _Orienter(nn.Module):
         self.angle_detector = _OriNet()
 
 
-class DoGOpenCVAffNetHardNet(nn.Module):
+class DoGOpenCVAffNetHardNet(CNNFrontEnd):
     """``DoGOpenCVAffNetHardNet(max_keypoints=-1, nms_diameter=9., *, weights=None, precision='tf32x3', capacity=65536)``: the
     reference's constructor, plus where the pretrained networks come from, the GEMM precision and ``OpenCVSIFT``'s bound on the
     keypoints per image before NMS.  ``forward(image [1,1,H,W] float in [0, 1], or uint8 / 255)`` returns ``(lafs [1,N,2,3],
@@ -71,6 +61,8 @@ class DoGOpenCVAffNetHardNet(nn.Module):
     ``FileNotFoundError`` when one is absent.  The networks are registered under the reference module's names
     (``affnet.features.<i>.*``, ``orinet.angle_detector.features.<i>.*``, ``hardnet.features.<i>.*``), so a reference module's
     ``state_dict()`` loads."""
+
+    _cv2_detector = True
 
     def __init__(self, max_keypoints: int = -1, nms_diameter: float = 9., *, weights=None, precision: str = 'tf32x3',
                  capacity: int = DEFAULT_CAPACITY):
@@ -85,7 +77,6 @@ class DoGOpenCVAffNetHardNet(nn.Module):
         self.orinet = _Orienter()
         self.hardnet = HardNet()
         self.eval()
-        self._ws, self._packed = {}, None
         self.load_weights(weights)
 
     @property
@@ -101,61 +92,39 @@ class DoGOpenCVAffNetHardNet(nn.Module):
         load_networks('DoGOpenCVAffNetHardNet', weights, CHECKPOINTS,
                       {'affnet': self.affnet, 'orinet': self.orinet.angle_detector, 'hardnet': self.hardnet})
 
-    def _weights_on(self, dev):
-        """The networks' weights on dev, packed once per parameter / buffer version: {name: [(W [Cout, K], bias [Cout])]}; OriNet's
-        head as [2, (ky, kx, c)] for og_dogaff_orinet_head"""
-        key = (weights_key(self), dev)
-        if self._packed is None or self._packed[0] != key:
-            packed = {}
-            for name, net, convs in (('affnet', self.affnet.features, AFFNET_CONVS), ('orinet', self.orinet.angle_detector.features, ORINET_CONVS),
-                                     ('hardnet', self.hardnet.features, HARDNET_CONVS)):
-                layers = [fold(net[i].weight, net[i + 1]) for i, *_ in convs]
-                layers.append(fold(net[HEAD].weight, net[HEAD + 1]) if name == 'hardnet' else nhwc_head(net[HEAD]))
-                packed[name] = [(w.to(dev), b.to(dev)) for w, b in layers]
-            self._packed = (key, packed)
-        return self._packed[1]
-
-    def train(self, mode: bool = True):
-        if mode:
-            raise RuntimeError('openglue_b200.DoGOpenCVAffNetHardNet is the inference front-end (its networks run on their running '
-                               'BatchNorm statistics); fine-tuning them is not built')
-        return super().train(mode)
+    def _pack(self):
+        """OriNet's head as [2, (ky, kx, c)] for og_dogaff_orinet_head"""
+        packed = {}
+        for name, net, convs in (('affnet', self.affnet.features, AFFNET_CONVS),
+                                 ('orinet', self.orinet.angle_detector.features, ORINET_CONVS),
+                                 ('hardnet', self.hardnet.features, HARDNET_CONVS)):
+            layers = [fold(net[i].weight, net[i + 1]) for i, *_ in convs]
+            layers.append(fold(net[HEAD].weight, net[HEAD + 1]) if name == 'hardnet' else nhwc_head(net[HEAD]))
+            packed[name] = layers
+        return packed
 
     # ------------------------------------------------------------------ device work
-    def _workspace(self, dev, B, H, W):
-        key = (dev, B, H, W)
-        if key not in self._ws:
-            sizes = [k for k in self._ws if k[0] != 'cnn']
-            while len(sizes) >= 2:                                      # the two image sizes of a pair batch stay cached
-                del self._ws[sizes.pop(0)]
-            n = _cabi.check_size(_cabi.lib().og_dogaff_workspace_bytes(B, H, W), 'og_dogaff_workspace_bytes')
-            self._ws[key] = torch.empty(n, dtype=torch.uint8, device=dev)
-        return self._ws[key]
+    def _workspace_bytes(self, lib, B, H, W):
+        return {'og_dogaff_workspace_bytes': lib.og_dogaff_workspace_bytes(B, H, W)}
 
-    @staticmethod
-    def _image(images) -> torch.Tensor:
-        if not torch.is_tensor(images):
-            raise TypeError(f'images must be a CUDA tensor [B, 1, H, W]; numpy input (the reference\'s CPU path) is not supported, '
-                            f'got {type(images)}')
-        if images.dim() != 4 or images.shape[1] != 1:
-            raise ValueError(f'images must be [B, 1, H, W], got {tuple(images.shape)}')
-        if images.device.type != 'cuda':
-            raise RuntimeError('openglue_b200.DoGOpenCVAffNetHardNet needs CUDA tensors (sm_90a); there is no CPU path')
-        if images.dtype == torch.uint8:
-            return (images.float() / 255.).contiguous()
-        if not images.is_floating_point():
-            raise ValueError(f'images must be float in [0, 1] or uint8, got {images.dtype}')
-        return images.detach().float().contiguous()
+    def _detect_select(self, img: torch.Tensor, min_stack: bool, overflow=None):
+        """``OpenCVSIFT``'s detection and selection, on the float image it quantises as the reference does"""
+        return self._sift._detect_select(img, min_stack, overflow)
 
-    def _describe(self, img, kp, sel, n, out_cap):
-        """Rows [0, n[b]) of the [B, out_cap] outputs from the selected keypoints kp[b, sel[b, j]]: (lafs, scores, desc, angles)"""
+    def _describe_selected(self, img, det, n, K, n_max, padded):
+        return self._describe(img, det.kp, det.sel, n, K)[:3]
+
+    def _describe(self, img, kp, sel, n, out_cap, tap=None):
+        """The selected keypoints kp[b, sel[b, j]], j < n[b], in chunks of CHUNK: kornia_moons' LAF and AffNet's patch, AffNet,
+        the affine frame and OriNet's patch, OriNet and its head with HardNet's patch, HardNet; then the descriptors'
+        normalisation.  ``tap(stage, r0, rows, t)``, when given, sees each chunk's patches after the stage that cuts them
+        ('affnet', 'orinet', 'hardnet'): (lafs, scores, desc, angles)"""
         B, _, H, W = img.shape
         dev = img.device
-        f32 = dict(dtype=torch.float32, device=dev)
-        lafs, scores, desc = torch.empty(B, out_cap, 2, 3, **f32), torch.empty(B, out_cap, **f32), torch.empty(B, out_cap, 128, **f32)
-        angles = torch.empty(B, out_cap, **f32)
+        lafs, scores, desc = self._outputs(B, out_cap, dev)
+        angles = torch.empty(B, out_cap, dtype=torch.float32, device=dev)
         lib = _cabi.lib()
-        ops = _Ops(dev, _cabi.OG_PREC_FP32 if self.precision == 'fp32' else _cabi.OG_PREC_TF32X3)
+        ops = self._ops(dev)
         st = ops.st()
         wts = self._weights_on(dev)
         ws = self._workspace(dev, B, H, W)
@@ -168,61 +137,19 @@ class DoGOpenCVAffNetHardNet(nn.Module):
         d2 = desc.view(rows_all, 128)
         for r0 in range(0, rows_all, CHUNK):
             rows = min(CHUNK, rows_all - r0)
-            _cabi.check(lib.og_dogaff_affnet_patches(*args, ptr(kp), cap, ptr(sel), ptr(n), out_cap, r0, rows, ptr(lafs), ptr(scores),
-                                                     ptr(patches), st), 'og_dogaff_affnet_patches')
-            run_cnn(ops, wts['affnet'], patches, rows, AFFNET_CONVS, col, (act0, act1), xy[:rows * 3].view(rows, 3))
+            _cabi.check(lib.og_dogaff_affnet_patches(*args, ptr(kp), cap, ptr(sel), ptr(n), out_cap, r0, rows, ptr(lafs),
+                                                     ptr(scores), ptr(patches), st), 'og_dogaff_affnet_patches')
+            if tap is not None:
+                tap('affnet', r0, rows, patches)
+            _patch_cnn.run_cnn(ops, wts['affnet'], patches, rows, AFFNET_CONVS, col, (act0, act1), xy[:rows * 3].view(rows, 3))
             _cabi.check(lib.og_dogaff_frames(*args, ptr(n), out_cap, r0, rows, ptr(xy), ptr(lafs), ptr(patches), st), 'og_dogaff_frames')
-            act = run_cnn(ops, wts['orinet'], patches, rows, ORINET_CONVS, col, (act0, act1), None)
-            _cabi.check(lib.og_dogaff_orinet_head(*args, ptr(n), out_cap, r0, rows, ptr(act), ptr(ori_w), ptr(ori_b), ptr(lafs), ptr(angles),
-                                                  ptr(patches), st), 'og_dogaff_orinet_head')
-            run_cnn(ops, wts['hardnet'], patches, rows, HARDNET_CONVS, col, (act0, act1), d2[r0:r0 + rows])
+            if tap is not None:
+                tap('orinet', r0, rows, patches)
+            act = _patch_cnn.run_cnn(ops, wts['orinet'], patches, rows, ORINET_CONVS, col, (act0, act1), None)
+            _cabi.check(lib.og_dogaff_orinet_head(*args, ptr(n), out_cap, r0, rows, ptr(act), ptr(ori_w), ptr(ori_b), ptr(lafs),
+                                                  ptr(angles), ptr(patches), st), 'og_dogaff_orinet_head')
+            if tap is not None:
+                tap('hardnet', r0, rows, patches)
+            _patch_cnn.run_cnn(ops, wts['hardnet'], patches, rows, HARDNET_CONVS, col, (act0, act1), d2[r0:r0 + rows])
         _cabi.check(lib.og_kgftt_desc_finish(ptr(desc), B, out_cap, ptr(n), st), 'og_kgftt_desc_finish')
         return lafs, scores, desc, angles
-
-    @torch.no_grad()
-    def _run(self, images):
-        img = self._image(images)
-        B = img.shape[0]
-        with torch.cuda.device(img.device):
-            _, kp, _, count, sel, n_sel = self._sift._detect_select(img, 1)
-            counts = torch.cat([count, n_sel]).tolist()                 # the one host synchronisation: the output sizes
-            if max(counts[:B]) > self.capacity:
-                raise RuntimeError(f'{max(counts[:B])} SIFT keypoints in one image exceed the capacity {self.capacity}: raise '
-                                   f'DoGOpenCVAffNetHardNet(capacity=...)')
-            n = counts[B:]
-            lafs, scores, desc, _ = self._describe(img, kp, sel, n_sel, max(max(n), 1))
-        return [(lafs[b:b + 1, :k], scores[b:b + 1, :k], desc[b:b + 1, :k]) for b, k in enumerate(n)]
-
-    def forward(self, image: torch.Tensor, mask=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-        """The reference's ``detect_and_compute`` of one image; ``mask`` is ignored, as in the reference."""
-        image = self._image(image)
-        assert image.size(0) == 1                                       # as the reference (dog_affnet_harnet.py)
-        return self._run(image)[0]
-
-    def extract_batch(self, images: torch.Tensor) -> List[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
-        """B same-size images through one launch per stage: a list of B ``(lafs [1,N_b,2,3], scores [1,N_b], descriptors
-        [1,N_b,128])``, each equal to ``forward`` of that image."""
-        return self._run(images)
-
-    @torch.no_grad()
-    def extract_padded(self, images: torch.Tensor, capacity: Optional[int] = None):
-        """``extract_batch`` at a fixed capacity, without a host synchronisation.
-
-        images [B,1,H,W] -> (lafs [B,K,2,3], scores [B,K], descriptors [B,K,128], num_keypoints [B] int32, overflow [B] int32), all
-        on the images' device, K = ``capacity`` (default ``max_keypoints``).  Rows [0, num_keypoints[b]) of image b are
-        ``extract_batch``'s rows for it, the rows past them are 0.  ``overflow[b] = 1`` where ``extract_batch`` would raise (more
-        keypoints before NMS than ``self.capacity``; the selection then runs on those that fitted) or K cuts the image (the first K
-        rows in response order are kept)."""
-        K = padded_capacity(self.max_keypoints, capacity)
-        img = self._image(images)
-        B = img.shape[0]
-        dev = img.device
-        i32 = dict(dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            overflow = torch.empty(B, **i32)
-            _, kp, _, _, sel, n_sel = self._sift._detect_select(img, 1, overflow)
-            num = torch.empty(B, **i32)
-            _cabi.check(_cabi.lib().og_keypoint_counts(ptr(n_sel), B, K, -1, K, ptr(num), None, ptr(overflow), stream(dev)),
-                        'og_keypoint_counts')
-            lafs, scores, desc, _ = self._describe(img, kp, sel, num, K)
-        return lafs, scores, desc, num, overflow

@@ -237,9 +237,10 @@ class OpenGlueMatcher(nn.Module):
         return compact_matches(res['matches0'], res['matching_scores0'], lafs0, lafs1)
 
 
-def _frontend_version(module: nn.Module) -> tuple:
-    """Storage and version of every parameter and buffer: a captured graph has the front-end's packed weights baked in"""
-    return tuple((t.data_ptr(), t._version) for t in list(module.parameters()) + list(module.buffers()))
+def weights_key(module: nn.Module) -> tuple:
+    """Changes whenever a parameter or buffer of ``module`` is written or replaced: the key of its packed weights, and of a
+    captured graph that has a front-end's packed weights baked in"""
+    return tuple((t._version, t.data_ptr()) for t in list(module.parameters()) + list(module.buffers()))
 
 
 def _frontend_storage(module: nn.Module) -> tuple:
@@ -279,7 +280,8 @@ def _image_pair_inputs(local_feature: nn.Module, laf_converter: LAFConverter, lo
 class ImagePairMatcher(nn.Module):
     """Batches of image pairs to matches with no host synchronisation, replayed as one CUDA graph by default.
 
-    ``local_feature``: an ``OpenCVSIFT``, ``SIFT`` or ``SuperPointNet`` / ``SuperPointNetBn``; ``matcher``: an ``openglue_b200.SuperGlue``;
+    ``local_feature``: an ``OpenCVSIFT``, ``SIFT``, ``GFTTAffNetHardNet``, ``DoGOpenCVAffNetHardNet`` or ``SuperPointNet`` /
+    ``SuperPointNetBn``; ``matcher``: an ``openglue_b200.SuperGlue``;
     ``match_config``: ``OpenGlueMatcher``'s (``superglue.laf_to_sideinfo_method``, optional ``superglue.log_transform_response``,
     ``inference.match_threshold``).  ``capacity``: the keypoint rows K per image (default: the front-end's ``max_keypoints``).
 
@@ -305,7 +307,8 @@ class ImagePairMatcher(nn.Module):
         if not isinstance(matcher, SuperGlue):
             raise TypeError('openglue_b200.ImagePairMatcher takes an openglue_b200.SuperGlue as its matcher')
         if not callable(getattr(local_feature, 'extract_padded', None)):
-            raise TypeError('openglue_b200.ImagePairMatcher takes a front-end with extract_padded (OpenCVSIFT, SIFT, SuperPointNet[Bn])')
+            raise TypeError('openglue_b200.ImagePairMatcher takes a front-end with extract_padded (OpenCVSIFT, SIFT, GFTTAffNetHardNet, '
+                            'DoGOpenCVAffNetHardNet, SuperPointNet[Bn])')
         self.local_feature = local_feature
         self.matcher = matcher
         self.laf_converter = get_laf_to_sideinfo_converter(match_config['superglue']['laf_to_sideinfo_method'])
@@ -330,7 +333,7 @@ class ImagePairMatcher(nn.Module):
         return out
 
     def _versions(self) -> tuple:
-        return (getattr(self.matcher, '_alloc_gen', 0), self.matcher._weights_version(), _frontend_version(self.local_feature))
+        return (getattr(self.matcher, '_alloc_gen', 0), self.matcher._weights_version(), weights_key(self.local_feature))
 
     def _run_graph(self, image0: torch.Tensor, image1: torch.Tensor, K: int) -> Dict[str, torch.Tensor]:
         """Replay (capturing on first use) the CUDA graph for these shapes; the images are copied into its static buffers."""

@@ -25,7 +25,7 @@ import torch.nn as nn
 from . import _cabi
 from ._cabi import ptr
 from ._ops import _Ops
-from .features import padded_capacity
+from .features import padded_capacity, weights_key
 
 __all__ = ['SuperPointNet', 'SuperPointNetBn']
 
@@ -58,7 +58,7 @@ class SuperPointNet(nn.Module):
         return m.weight.detach(), m.bias.detach()
 
     def _weights(self):
-        key = tuple((p._version, p.data_ptr()) for p in list(self.parameters()) + list(self.buffers()))
+        key = weights_key(self)
         if self._packed is None or self._packed[0] != key:
             w = {}
             for name, m in self.named_children():

@@ -26,8 +26,8 @@ import torch
 
 from . import _cabi, _graphs
 from ._ops import _Ops, _pad4  # noqa: F401  (tests build their torch double of the kernels on _Ops' composite helpers)
-from .features import (_check_image_pair, _frontend_storage, _frontend_version, _image_pair_inputs,
-                       get_laf_to_sideinfo_converter, padded_capacity)
+from .features import (_check_image_pair, _frontend_storage, _image_pair_inputs, get_laf_to_sideinfo_converter, padded_capacity,
+                       weights_key)
 from .superglue import _MATCHER_KEYS, _matcher_inputs, is_padded, padded_inputs
 
 __all__ = ['TrainStep', 'train_forward', 'GraphedTrainStep', 'ImagePairTrainStep']
@@ -619,7 +619,8 @@ class ImagePairTrainStep:
         if not superglue.training:
             raise RuntimeError('ImagePairTrainStep runs the training-mode step: call superglue.train() first')
         if not callable(getattr(local_feature, 'extract_padded', None)):
-            raise TypeError('openglue_b200.ImagePairTrainStep takes a front-end with extract_padded (OpenCVSIFT, SIFT, SuperPointNet[Bn])')
+            raise TypeError('openglue_b200.ImagePairTrainStep takes a front-end with extract_padded (OpenCVSIFT, SIFT, GFTTAffNetHardNet, '
+                            'DoGOpenCVAffNetHardNet, SuperPointNet[Bn])')
         if (config.get('features') or {}).get('finetune', False):
             raise NotImplementedError('fine-tuning the front-end (features.finetune) is not built: openglue_b200 front-ends run in eval mode')
         train = config['train']
@@ -718,7 +719,7 @@ class ImagePairTrainStep:
 
     # ------------------------------------------------------------------ graphs
     def _versions(self) -> tuple:
-        return _pointers(self.superglue, self.params), _frontend_version(self.local_feature)
+        return _pointers(self.superglue, self.params), weights_key(self.local_feature)
 
     def _run(self, key: tuple, inputs: Dict[str, torch.Tensor], chain) -> Dict[str, torch.Tensor]:
         """Replay (capturing on first use) the graph of ``chain(static inputs)`` for ``key``; the inputs are copied into its

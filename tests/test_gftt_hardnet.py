@@ -18,6 +18,7 @@ from oracle import kornia_gftt_oracle as KG  # noqa: E402
 from oracle import kornia_sift_oracle as KO  # noqa: E402
 from oracle.gen_golden_gftt_hardnet import load_fixture  # noqa: E402
 from openglue_b200 import GFTTAffNetHardNet, ImagePairMatcher, ImagePairTrainStep, _cabi  # noqa: E402
+from openglue_b200 import _patch_cnn as PC  # noqa: E402
 from openglue_b200 import gftt_hardnet as GH  # noqa: E402
 from openglue_b200._cabi import ptr  # noqa: E402
 from openglue_b200._ops import _Ops  # noqa: E402
@@ -181,12 +182,12 @@ def test_cnns_against_float64_convolutions(precision):
     ops = _Ops(dev, _cabi.OG_PREC_FP32 if precision == 'fp32' else _cabi.OG_PREC_TF32X3)
     rows = 200 if GH.CHUNK >= 200 else GH.CHUNK
     x = KG.normalize_input(torch.rand(rows, 1, 32, 32, generator=torch.Generator().manual_seed(3)))
-    patches, col, a0, a1, _ = m._cnn_buffers(dev)
+    patches, col, a0, a1, _ = PC.cnn_buffers(m._ws, dev)
     patches[:rows * 1024].copy_(x.flatten())
     aff64, hard64 = KG.features_in(torch.float64)
     for name, net, convs, nout in (('affnet', aff64, GH.AFFNET_CONVS, 3), ('hardnet', hard64, GH.HARDNET_CONVS, 128)):
         out = torch.empty(rows, nout, device=dev)
-        m._cnn(ops, m._weights_on(dev)[name], patches, rows, convs, col, (a0, a1), out)
+        PC.run_cnn(ops, m._weights_on(dev)[name], patches, rows, convs, col, (a0, a1), out)
         torch.cuda.synchronize()
         with torch.no_grad():
             want = net[:19](x.double())

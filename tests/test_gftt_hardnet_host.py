@@ -17,6 +17,7 @@ from oracle import kornia_gftt_oracle as KG  # noqa: E402
 from oracle import kornia_sift_oracle as KO  # noqa: E402
 from oracle.gen_golden_gftt_hardnet import load_fixture  # noqa: E402
 from openglue_b200 import GFTTAffNetHardNet  # noqa: E402
+from openglue_b200 import _patch_cnn as PC  # noqa: E402
 from openglue_b200 import gftt_hardnet as GH  # noqa: E402
 
 REF = os.environ.get('OG_REFERENCE_ROOT', '/root/reference')
@@ -90,19 +91,19 @@ def test_fixtures_equal_a_fresh_run_of_the_reference():
 
 def test_batchnorm_fold_equals_conv_then_batchnorm():
     sd = KG.synthetic_hardnet_state_dict()
-    net = GH._HardNet()
+    net = PC.HardNet()
     net.load_state_dict(sd)
     x = torch.randn(3, 32, 10, 10, generator=torch.Generator().manual_seed(0), dtype=torch.float64)
     conv, bn = net.features[3], net.features[4]
     want = F.batch_norm(F.conv2d(x, conv.weight.double(), padding=1), bn.running_mean.double(), bn.running_var.double(), eps=bn.eps)
-    w, b = GH._fold(conv.weight, bn)
+    w, b = PC.fold(conv.weight, bn)
     cols = F.unfold(x, 3, padding=1).view(3, 32, 9, 100).permute(0, 3, 2, 1).reshape(3, 100, 9 * 32)    # (ky, kx, c) columns
     got = (cols @ w.double().t() + b.double()).permute(0, 2, 1).reshape(3, 32, 10, 10)
     assert float((got - want).abs().max()) <= 1e-5 * float(want.abs().max())
     head, hbn = net.features[19], net.features[20]
     y = torch.randn(2, 128, 8, 8, dtype=torch.float64)
     want = F.batch_norm(F.conv2d(y, head.weight.double()), hbn.running_mean.double(), hbn.running_var.double(), eps=hbn.eps).flatten(1)
-    w, b = GH._fold(head.weight, hbn)
+    w, b = PC.fold(head.weight, hbn)
     got = y.permute(0, 2, 3, 1).reshape(2, -1) @ w.double().t() + b.double()
     assert float((got - want).abs().max()) <= 1e-5 * float(want.abs().max())
 
@@ -112,6 +113,21 @@ def test_batchnorm_fold_equals_conv_then_batchnorm():
 def test_argument_refusals(kwargs):
     with pytest.raises(ValueError):
         GFTTAffNetHardNet(**kwargs, weights=_weights())
+
+
+def test_input_refusals():
+    import numpy as np
+    m = GFTTAffNetHardNet(max_keypoints=64, weights=_weights())
+    with pytest.raises(TypeError):
+        m(np.zeros((1, 1, 32, 32), np.float32))
+    with pytest.raises(ValueError):
+        m(torch.zeros(1, 3, 32, 32))
+    with pytest.raises(RuntimeError, match='GFTTAffNetHardNet needs CUDA'):
+        m(torch.zeros(1, 1, 32, 32))
+    with pytest.raises(RuntimeError, match='CUDA'):
+        m.extract_padded(torch.zeros(2, 1, 32, 32), 16)
+    with pytest.raises(RuntimeError):
+        m.train()
 
 
 def test_weights_load_from_kornia_layout_reference_modules_and_files(tmp_path):

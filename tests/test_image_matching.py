@@ -199,8 +199,7 @@ def test_sift_overflow_flags_only_the_images_over_capacity():
         for got, want in zip((lafs, scores, desc), s):
             assert torch.equal(got[b, :k], want[0, :k]), b                     # the first K in response order
     # the capacity before NMS: the selection runs on the keypoints that fitted, the images below it are unchanged
-    sift._run(imgs, want_raw=True)
-    raw = sift.last_raw['count'].tolist()
+    raw = sift._detect_select(sift._image(imgs)).count.tolist()
     small = OpenCVSIFT(max_keypoints=-1, capacity=sorted(raw)[1])
     lafs, scores, desc, num, over = small.extract_padded(imgs, 8192)
     assert over.tolist() == [int(x > small.capacity) for x in raw] and sum(over.tolist()) == 1

@@ -137,6 +137,8 @@ def test_arguments_are_checked():
         s.extract_padded(torch.rand(1, 1, 64, 64))
     with pytest.raises(ValueError):
         s(torch.rand(1, 3, 64, 64))
+    with pytest.raises(TypeError):
+        s(torch.rand(1, 1, 64, 64).numpy())
 
 
 def test_workspace_queries():

@@ -352,72 +352,22 @@ def _det_table(B, H, W, cap, seed):
     return lafs, r, torch.stack([x, y, s / 6, t, r], -1)
 
 
-def _loop_gftt(m, img, lafs, resp, sel, n, out_cap):
-    """GFTTAffNetHardNet._describe's chunk loop, keeping every chunk's AffNet and HardNet patches and the angles"""
-    B, _, H, W = img.shape
-    dev = img.device
-    ws = _gftt_ws(m, img)
-    k = m.max_keypoints
-    ops = _Ops(dev, PREC[m.precision])
-    wts = m._weights_on(dev)
-    patches, col, a0, a1, xy = cnn_buffers({}, dev)
+def _describe(m, img, args, n, out_cap):
+    """The module's _describe of the selected rows (``args``: what it takes before n), keeping through its tap every chunk's patches
+    of each stage ('p_affnet', 'p_orinet', 'p_hardnet') and the angles"""
+    B = img.shape[0]
     R = B * out_cap
-    o = dict(lafs=torch.empty(B, out_cap, 2, 3, device=dev), scores=torch.empty(B, out_cap, device=dev),
-             angles=torch.empty(B, out_cap, device=dev), desc=torch.empty(B, out_cap, 128, device=dev),
-             p_aff=torch.empty(R, PS, PS, device=dev), p_hard=torch.empty(R, PS, PS, device=dev))
-    for r0 in range(0, R, CHUNK):
-        rows = min(CHUNK, R - r0)
-        _cabi.check(_lib().og_kgftt_affnet_patches(ptr(img), B, H, W, k, ptr(ws), ws.numel(), ptr(lafs), k, ptr(sel), ptr(n), out_cap, r0, rows,
-                                                   ptr(patches), _st()), 'og_kgftt_affnet_patches')
-        o['p_aff'][r0:r0 + rows] = patches[:rows * PS * PS].view(rows, PS, PS)
-        run_cnn(ops, wts['affnet'], patches, rows, AFFNET_CONVS, col, (a0, a1), xy[:rows * 3].view(rows, 3))
-        _cabi.check(_lib().og_kgftt_frames(ptr(img), B, H, W, k, ptr(ws), ws.numel(), ptr(lafs), ptr(resp), k, ptr(sel), ptr(n), out_cap, r0, rows,
-                                           ptr(xy), int(m.upright), ptr(o['lafs']), ptr(o['scores']), ptr(o['angles']), ptr(patches), _st()),
-                    'og_kgftt_frames')
-        o['p_hard'][r0:r0 + rows] = patches[:rows * PS * PS].view(rows, PS, PS)
-        run_cnn(ops, wts['hardnet'], patches, rows, HARDNET_CONVS, col, (a0, a1), o['desc'].view(R, 128)[r0:r0 + rows])
-    _cabi.check(_lib().og_kgftt_desc_finish(ptr(o['desc']), B, out_cap, ptr(n), _st()), 'og_kgftt_desc_finish')
-    want = m._describe(img, ws, lafs, resp, sel, n, out_cap)
-    torch.cuda.synchronize()
-    for key, t in zip(('lafs', 'scores', 'desc'), want):
-        assert torch.equal(o[key], t), key                              # the loop is the module's
-    return {key: t.cpu() for key, t in o.items()}
+    o = {}
 
-
-def _loop_dog(m, img, kp, sel, n, out_cap):
-    """DoGOpenCVAffNetHardNet._describe's chunk loop, keeping every chunk's AffNet, OriNet and HardNet patches"""
-    B, _, H, W = img.shape
-    dev = img.device
-    ops = _Ops(dev, PREC[m.precision])
-    wts = m._weights_on(dev)
-    ws = m._workspace(dev, B, H, W)
-    patches, col, a0, a1, xy = cnn_buffers({}, dev)
-    cap = m.capacity
-    args = (ptr(img), B, H, W, ptr(ws), ws.numel())
-    _cabi.check(_lib().og_dogaff_pyramid(*args, _st()), 'og_dogaff_pyramid')
-    ori_w, ori_b = wts['orinet'][-1]
-    R = B * out_cap
-    o = dict(lafs=torch.empty(B, out_cap, 2, 3, device=dev), scores=torch.empty(B, out_cap, device=dev),
-             angles=torch.empty(B, out_cap, device=dev), desc=torch.empty(B, out_cap, 128, device=dev),
-             p_aff=torch.empty(R, PS, PS, device=dev), p_ori=torch.empty(R, PS, PS, device=dev), p_hard=torch.empty(R, PS, PS, device=dev))
-    for r0 in range(0, R, CHUNK):
-        rows = min(CHUNK, R - r0)
-        _cabi.check(_lib().og_dogaff_affnet_patches(*args, ptr(kp), cap, ptr(sel), ptr(n), out_cap, r0, rows, ptr(o['lafs']), ptr(o['scores']),
-                                                    ptr(patches), _st()), 'og_dogaff_affnet_patches')
-        o['p_aff'][r0:r0 + rows] = patches[:rows * PS * PS].view(rows, PS, PS)
-        run_cnn(ops, wts['affnet'], patches, rows, AFFNET_CONVS, col, (a0, a1), xy[:rows * 3].view(rows, 3))
-        _cabi.check(_lib().og_dogaff_frames(*args, ptr(n), out_cap, r0, rows, ptr(xy), ptr(o['lafs']), ptr(patches), _st()), 'og_dogaff_frames')
-        o['p_ori'][r0:r0 + rows] = patches[:rows * PS * PS].view(rows, PS, PS)
-        act = run_cnn(ops, wts['orinet'], patches, rows, AFFNET_CONVS, col, (a0, a1), None)
-        _cabi.check(_lib().og_dogaff_orinet_head(*args, ptr(n), out_cap, r0, rows, ptr(act), ptr(ori_w), ptr(ori_b), ptr(o['lafs']), ptr(o['angles']),
-                                                 ptr(patches), _st()), 'og_dogaff_orinet_head')
-        o['p_hard'][r0:r0 + rows] = patches[:rows * PS * PS].view(rows, PS, PS)
-        run_cnn(ops, wts['hardnet'], patches, rows, HARDNET_CONVS, col, (a0, a1), o['desc'].view(R, 128)[r0:r0 + rows])
-    _cabi.check(_lib().og_kgftt_desc_finish(ptr(o['desc']), B, out_cap, ptr(n), _st()), 'og_kgftt_desc_finish')
-    want = m._describe(img, kp, sel, n, out_cap)
+    def tap(stage, r0, rows, t):
+        if stage == 'angles':
+            o['angles'] = t.clone()
+        else:
+            p = o.setdefault(f'p_{stage}', torch.full((R, PS, PS), float('nan'), device=DEV))
+            p[r0:r0 + rows] = t[:rows * PS * PS].view(rows, PS, PS)
+    out = m._describe(img, *args, n, out_cap, tap)
     torch.cuda.synchronize()
-    for key, t in zip(('lafs', 'scores', 'desc', 'angles'), want):
-        assert torch.equal(o[key], t), key                              # the loop is the module's
+    o.update(zip(('lafs', 'scores', 'desc', 'angles'), out))            # DoG returns the angles, GFTT gives them to the tap
     return {key: t.cpu() for key, t in o.items()}
 
 
@@ -433,13 +383,14 @@ def test_row_mapping_across_images_and_chunks(front):
     n = torch.tensor(COUNTS, dtype=torch.int32)
     if front == 'gftt':
         m = _gftt_model(CAP_IN)
-        run = lambda im, src, s, nn, oc: _loop_gftt(m, im, src[0].to(DEV).contiguous(), src[1].to(DEV).contiguous(), s, nn, oc)
+        run = lambda im, src, s, nn, oc: _describe(m, im, (_gftt_ws(m, im), src[0].to(DEV).contiguous(), src[1].to(DEV).contiguous(), s),
+                                                   nn, oc)
         src = (lafs, resp)
         pick = lambda b, idx: (lafs[b:b + 1, idx], resp[b:b + 1, idx])
     else:
         m = _dog_model(capacity=CAP_IN)
         assert m.capacity == CAP_IN
-        run = lambda im, src, s, nn, oc: _loop_dog(m, im, src.to(DEV).contiguous(), s, nn, oc)
+        run = lambda im, src, s, nn, oc: _describe(m, im, (src.to(DEV).contiguous(), s), nn, oc)
         src = kp
         pick = lambda b, idx: kp[b:b + 1, idx]
     got = run(img, src, sel.to(DEV), n.to(DEV), OUT_CAP)

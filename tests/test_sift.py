@@ -176,6 +176,8 @@ def test_module_refuses_cpu_and_batches_in_forward():
         m(torch.zeros(1, 1, 64, 64))
     with pytest.raises(AssertionError):
         m(torch.zeros(2, 1, 64, 64))
+    with pytest.raises(TypeError):
+        m(np.zeros((64, 64), np.uint8))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -188,20 +190,18 @@ def _detect_all(fx):
     lib = cab.lib()
     img = torch.from_numpy(fx['image']).to(DEV)[None, None]
     m = OpenCVSIFT(max_keypoints=-1, nms_diameter=0.0)                   # nms off, no top-k: sel = every keypoint by response
-    m._run(img, want_raw=True)
-    r = m.last_raw
-    n = int(r['count'][0])
+    r = m._detect_select(m._image(img))
+    n = int(r.count[0])
     H, W = img.shape[2:]
-    ws, _ = m._workspace(img.device, 1, H, W)
     sel = torch.arange(m.capacity, dtype=torch.int32, device=DEV)[None]
     n_sel = torch.tensor([n], dtype=torch.int32, device=DEV)
     oc = max(n, 1)
     out = [torch.empty(1, oc, *s, device=DEV) for s in ((2, 3), (), (128,), (128,))]
     st = cab.stream()
-    cab.check(lib.og_sift_describe(cab.ptr(ws), 1, H, W, m.capacity, cab.ptr(r['kp']), cab.ptr(r['octave']), cab.ptr(sel), cab.ptr(n_sel), oc, n, 1,
+    cab.check(lib.og_sift_describe(cab.ptr(r.ws), 1, H, W, m.capacity, cab.ptr(r.kp), cab.ptr(r.octave), cab.ptr(sel), cab.ptr(n_sel), oc, n, 1,
                                    *[cab.ptr(t) for t in out], st), 'og_sift_describe')
-    kp = r['kp'][0, :n].cpu().numpy()
-    return dict(pt=kp[:, :2], size=kp[:, 2], angle=kp[:, 3], response=kp[:, 4], octave=r['octave'][0, :n].cpu().numpy(),
+    kp = r.kp[0, :n].cpu().numpy()
+    return dict(pt=kp[:, :2], size=kp[:, 2], angle=kp[:, 3], response=kp[:, 4], octave=r.octave[0, :n].cpu().numpy(),
                 raw=out[3][0, :n].cpu().numpy())
 
 

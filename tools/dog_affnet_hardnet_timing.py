@@ -23,7 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from openglue_b200 import DoGOpenCVAffNetHardNet  # noqa: E402
-from openglue_b200 import dog_affnet_hardnet as DA  # noqa: E402
+from openglue_b200 import _patch_cnn as PC  # noqa: E402
 from oracle import dog_affnet_oracle as KD  # noqa: E402
 from oracle import kornia_gftt_oracle as KG  # noqa: E402
 from tools.kornia_sift_timing import texture, timed  # noqa: E402
@@ -47,15 +47,15 @@ def main():
         n = [int(t[0].shape[1]) for t in fe.extract_batch(img)]
         t_fwd = timed(run, args.reps)
         t_pad = timed(lambda: fe.extract_padded(img, NF), args.reps)
-        cnn = DA.run_cnn
-        DA.run_cnn = lambda ops, layers, x, rows, convs, col, acts, out: acts[1] if out is None else out   # all but the CNNs
+        cnn = PC.run_cnn
+        PC.run_cnn = lambda ops, layers, x, rows, convs, col, acts, out: acts[1] if out is None else out   # all but the CNNs
         t_rest = timed(run, args.reps)
-        DA.run_cnn = cnn
+        PC.run_cnn = cnn
         row = dict(B=B, keypoints_per_image=sum(n) / B, forward_ms_per_image=t_fwd / B, extract_padded_ms_per_image=t_pad / B,
                    cnn_share=1 - t_rest / t_fwd)
         if B == 1:
-            _, kp, _, _, sel, n_sel = fe._sift._detect_select(img, 1)
-            kp1 = kp[0, sel[0, :int(n_sel[0])].long()][None].contiguous()
+            det = fe._detect_select(img, True)
+            kp1 = det.kp[0, det.sel[0, :int(det.n_sel[0])].long()][None].contiguous()
             with torch.no_grad():
                 row['oracle_f32_cuda_describe_ms'] = timed(lambda: KD.describe(img, kp1), args.oracle_reps, warmup=1)
             try:
