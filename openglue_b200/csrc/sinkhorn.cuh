@@ -50,7 +50,7 @@ struct SinkArgs {
   float* hist_u;                         // optional [B][iters][n+1]: u_t of every iteration  (kept for the backward pass,
   float* hist_v;                         // optional [B][iters+1][m+1]: v_t, row 0 = v_0 = 0   csrc/sinkhorn_bwd.cuh)
   const int* len_n;                      // padded batch (null otherwise): pair b has len_n[b] rows and len_m[b] columns of the
-  const int* len_m;                      // capacity n x m (clamped into [1, n] / [1, m])
+  const int* len_m;                      // capacity n x m (clamped into [1, n] / [1, m]); S outside that block is never read
 };
 
 constexpr int SINK_WARPS = 8;
@@ -149,8 +149,8 @@ struct SinkRowRing {
   const Args& a;
   const float* seg;                                    // this warp's column segment of row 0 of the pair
   int first, end_real, n, c0, lane;                    // first row of the warp; rows >= end_real do not exist in memory; row n: dustbin
-  uint32_t bytes, consumed;                            // bytes of a segment: 0 when it lies beyond the last column
-  bool full;                                           // the whole segment lies inside the row (warp-uniform)
+  uint32_t bytes, consumed;                            // bytes of a segment: 0 when it lies beyond the pair's last column
+  bool full;                                           // the whole segment lies inside the pair's row (warp-uniform)
   float dz;                                            // the dustbin score divided by reg, Z = M / reg
   uint64_t policy;
 
@@ -163,7 +163,7 @@ struct SinkRowRing {
     end_real = min(s.r1, s.n);
     n = s.n;
     c0 = s.c0; lane = s.lane;
-    const int seg_cols = min(a.m, c0 + C) - c0;        // <= 0: this warp's segment lies beyond the last column
+    const int seg_cols = min(s.m, c0 + C) - c0;        // <= 0: this warp's segment lies beyond the pair's last column
     bytes = seg_cols > 0 ? (uint32_t)(((seg_cols + 3) / 4) * 16) : 0u;     // <= 4 * (lds - c0): inside the padded row
     full = seg_cols == C;
     consumed = 0;
@@ -197,8 +197,9 @@ struct SinkRowRing {
     }
   }
 
-  // This warp's segment of row `row` in registers (columns >= a.m zero, divided by reg), and the slot refilled with the row SLOTS
-  // ahead.  The dustbin row is the constant dustbin score.
+  // This warp's segment of row `row` in registers (columns >= m zero, divided by reg), and the slot refilled with the row SLOTS
+  // ahead.  The dustbin row is the constant dustbin score.  In a padded batch the columns m .. a.m - 1 of a row are padding of any
+  // bits (NaN + -inf would be NaN), so they are neither copied nor read.
   __device__ __forceinline__ void take(int row, float4 (&z)[V]) {
     if (row >= n) {
 #pragma unroll
@@ -216,14 +217,14 @@ struct SinkRowRing {
     if (full) {                                        // no masks (the common case)
 #pragma unroll
       for (int k = 0; k < V; ++k) z[k] = src[lane + 32 * k];
-    } else {
+    } else {                                           // the pair's columns, reloaded: this path is rare and keeps no register
+      const int m = padded_length(a.len_m, blockIdx.x / a.SP, a.m);
 #pragma unroll
       for (int k = 0; k < V; ++k) {
         const int idx = lane + 32 * k;
         const int c = c0 + 4 * idx;
-        const int m = a.m;
         float4 q = (c < m) ? src[idx] : make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c < m && c + 3 >= m) {                     // the float4 that straddles column m: its tail is row padding (any bits)
+        if (c < m && c + 3 >= m) {                     // the float4 that straddles column m: its tail is padding (any bits)
           if (c + 1 >= m) q.y = 0.f;
           if (c + 2 >= m) q.z = 0.f;
           q.w = 0.f;
@@ -345,7 +346,7 @@ __device__ __forceinline__ void sink_fwd_rows(const SinkArgs& a, const SinkPair&
   for (int r = 0; r < NR; ++r) mx[r] = (sub == 0) ? t_m : -CUDART_INF_F;
 #pragma unroll
   for (int k = 0; k < V; ++k) {
-    const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(v_s + c0 + 4 * (lane + 32 * k));   // columns >= m: finite z + (-inf) = -inf, e = 0
+    const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(v_s + c0 + 4 * (lane + 32 * k));   // columns >= m: z = 0 (SinkRowRing), 0 + (-inf) = -inf, e = 0
 #pragma unroll
     for (int r = 0; r < NR; ++r) {
       z[r][2 * k] = add2(z[r][2 * k], vv.x); z[r][2 * k + 1] = add2(z[r][2 * k + 1], vv.y);

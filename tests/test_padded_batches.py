@@ -235,9 +235,11 @@ def _sinkhorn_padded(S, dust, lens, iters, reg):
     return scores.cpu()
 
 
+@pytest.mark.parametrize('fill', ['randn', float('nan'), float('inf'), -float('inf'), 1e30])
 @pytest.mark.parametrize('resident', [1, 0])
 @pytest.mark.parametrize('N,M', [(300, 500), (200, 1000), (150, 2000), (100, 4000), (60, 8192)])
-def test_sinkhorn_lengths_against_oracle(N, M, resident):
+def test_sinkhorn_lengths_against_oracle(N, M, resident, fill):
+    """fill: what S holds outside each pair's block (rows >= n_b, columns m_b .. M - 1), never read"""
     lib = _cabi.lib()
     prev = lib.og_set_sinkhorn_resident(resident)
     try:
@@ -245,7 +247,11 @@ def test_sinkhorn_lengths_against_oracle(N, M, resident):
         g = torch.Generator().manual_seed(N + M)
         S = torch.randn(len(ns), N, M, generator=g) * 3
         dust = torch.tensor([0.7])
-        got = _sinkhorn_padded(S, dust, ns + ms, 50, 1.0)
+        Sp = S.clone()
+        if fill != 'randn':
+            for b, (n, m) in enumerate(zip(ns, ms)):
+                Sp[b, n:], Sp[b, :, m:] = fill, fill
+        got = _sinkhorn_padded(Sp, dust, ns + ms, 50, 1.0)
         for b, (n, m) in enumerate(zip(ns, ms)):
             ref = O.matching_log_probs(S[b:b + 1, :n, :m].double(), dust.double()[0], 50, 1.0)[0]
             assert (got[b, :n + 1, :m + 1].double() - ref).abs().max() <= 1e-3
