@@ -12,21 +12,16 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 import time
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from openglue_b200 import DoGOpenCVAffNetHardNet  # noqa: E402
-from openglue_b200 import _patch_cnn as PC  # noqa: E402
-from oracle import dog_affnet_oracle as KD  # noqa: E402
-from oracle import kornia_gftt_oracle as KG  # noqa: E402
-from tools.kornia_sift_timing import texture, timed  # noqa: E402
+from gpu_timing import card, events_ms  # first: it makes the package and the oracle importable
+from kornia_sift_timing import texture
+from openglue_b200 import DoGOpenCVAffNetHardNet
+from openglue_b200 import _patch_cnn as PC
+from oracle import dog_affnet_oracle as KD
+from oracle import kornia_gftt_oracle as KG
 
 NF = 2048
 
@@ -37,7 +32,6 @@ def main():
     ap.add_argument('--oracle-reps', type=int, default=2)
     args = ap.parse_args()
     dev = 'cuda:0'
-    card = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip()
     w = {'affnet': KG.synthetic_affnet_state_dict(), 'orinet': KD.synthetic_orinet_state_dict(), 'hardnet': KG.synthetic_hardnet_state_dict()}
     fe = DoGOpenCVAffNetHardNet(max_keypoints=NF, weights=w)
     rows = []
@@ -45,11 +39,11 @@ def main():
         img = texture(B, 720, 960, 7, dev)
         run = (lambda: fe(img)) if B == 1 else (lambda: fe.extract_batch(img))
         n = [int(t[0].shape[1]) for t in fe.extract_batch(img)]
-        t_fwd = timed(run, args.reps)
-        t_pad = timed(lambda: fe.extract_padded(img, NF), args.reps)
+        t_fwd = events_ms(run, args.reps, warmup=2)
+        t_pad = events_ms(lambda: fe.extract_padded(img, NF), args.reps, warmup=2)
         cnn = PC.run_cnn
         PC.run_cnn = lambda ops, layers, x, rows, convs, col, acts, out: acts[1] if out is None else out   # all but the CNNs
-        t_rest = timed(run, args.reps)
+        t_rest = events_ms(run, args.reps, warmup=2)
         PC.run_cnn = cnn
         row = dict(B=B, keypoints_per_image=sum(n) / B, forward_ms_per_image=t_fwd / B, extract_padded_ms_per_image=t_pad / B,
                    cnn_share=1 - t_rest / t_fwd)
@@ -57,7 +51,7 @@ def main():
             det = fe._detect_select(img, True)
             kp1 = det.kp[0, det.sel[0, :int(det.n_sel[0])].long()][None].contiguous()
             with torch.no_grad():
-                row['oracle_f32_cuda_describe_ms'] = timed(lambda: KD.describe(img, kp1), args.oracle_reps, warmup=1)
+                row['oracle_f32_cuda_describe_ms'] = events_ms(lambda: KD.describe(img, kp1), args.oracle_reps, warmup=1)
             try:
                 import cv2
                 u8 = (img[0, 0].cpu().numpy() * 255).astype('uint8')
@@ -71,7 +65,7 @@ def main():
                 row['cv2_host_detect_ms'] = None
         rows.append(row)
         print(json.dumps(row))
-    print(json.dumps(dict(card=card, image='960x720', max_keypoints=NF, rows=rows)))
+    print(json.dumps(dict(card=card(), image='960x720', max_keypoints=NF, rows=rows)))
 
 
 if __name__ == '__main__':

@@ -14,8 +14,7 @@ import os
 import subprocess
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from gpu_timing import card, events_ms
 
 PEAK = {'f16': 989e12, 'tf32': 495e12}
 N, PAIRS, D = 2048, 16, 256
@@ -101,14 +100,7 @@ def measure(iters=50):
             call = lambda: lib.og_linear_f16_fwd(C.byref(a), _p(Wh), _p(Wl), _p(meta), _p(amax), _p(amax_out), _p(scale), *outs, 0, _st())
         for _ in range(5):
             _cabi.check(call(), name)
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            call()
-        e1.record()
-        torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / iters
+        ms = events_ms(call, iters)
         flop = 2.0 * batch * rows * K * nout
         out.append({'shape': name, 'rows': batch * rows, 'K': K, 'nout': nout, 'form': form, 'ms': round(ms, 4),
                     'tflops': round(flop / ms / 1e9, 1), 'mma_share': round(3 * flop / (ms * 1e-3) / PEAK[form], 3),
@@ -125,10 +117,7 @@ def main():
     if args.json:
         print(json.dumps(measure()))
         return
-    import torch
-    name = torch.cuda.get_device_name(0)
-    q = subprocess.run(['nvidia-smi', '--query-gpu=power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True, text=True)
-    print(json.dumps({'device': name, 'power_limit_and_max_sm_clock': q.stdout.strip()}))
+    print(json.dumps({'card': card()}))
     runs = {'this': measure()}
     if args.against:
         env = dict(os.environ, OG_LIB=os.path.abspath(args.against))

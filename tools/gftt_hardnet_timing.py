@@ -10,19 +10,14 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from openglue_b200 import GFTTAffNetHardNet  # noqa: E402
-from openglue_b200 import _patch_cnn as PC  # noqa: E402
-from oracle import kornia_gftt_oracle as KG  # noqa: E402
-from tools.kornia_sift_timing import texture, timed  # noqa: E402
+from gpu_timing import card, events_ms  # first: it makes the package and the oracle importable
+from kornia_sift_timing import texture
+from openglue_b200 import GFTTAffNetHardNet
+from openglue_b200 import _patch_cnn as PC
+from oracle import kornia_gftt_oracle as KG
 
 
 def main():
@@ -31,24 +26,23 @@ def main():
     ap.add_argument('--oracle-reps', type=int, default=2)
     args = ap.parse_args()
     dev = 'cuda:0'
-    card = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip()
     w = {'affnet': KG.synthetic_affnet_state_dict(), 'hardnet': KG.synthetic_hardnet_state_dict()}
     fe = GFTTAffNetHardNet(max_keypoints=1024, weights=w)
     rows = []
     for B in (1, 16):
         img = texture(B, 720, 960, 7, dev)
-        t_fwd = timed(lambda: fe(img), args.reps)
-        t_pad = timed(lambda: fe.extract_padded(img), args.reps)
+        t_fwd = events_ms(lambda: fe(img), args.reps, warmup=2)
+        t_pad = events_ms(lambda: fe.extract_padded(img), args.reps, warmup=2)
         cnn = PC.run_cnn
         PC.run_cnn = lambda ops, layers, x, rows, convs, col, acts, out: out     # everything but the CNN GEMMs and im2col
-        t_rest = timed(lambda: fe(img), args.reps)
+        t_rest = events_ms(lambda: fe(img), args.reps, warmup=2)
         PC.run_cnn = cnn
         with torch.no_grad():
-            t_or = timed(lambda: KG.run(img, 1024), args.oracle_reps, warmup=1) if B == 1 else None
+            t_or = events_ms(lambda: KG.run(img, 1024), args.oracle_reps, warmup=1) if B == 1 else None
         rows.append(dict(B=B, forward_ms_per_image=t_fwd / B, extract_padded_ms_per_image=t_pad / B, cnn_share=1 - t_rest / t_fwd,
                          oracle_f32_cuda_ms_per_image=None if t_or is None else t_or / B))
         print(json.dumps(rows[-1]))
-    print(json.dumps(dict(card=card, image='960x720', max_keypoints=1024, rows=rows)))
+    print(json.dumps(dict(card=card(), image='960x720', max_keypoints=1024, rows=rows)))
 
 
 if __name__ == '__main__':

@@ -14,35 +14,11 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'oracle'))
-
-
-def _gpu():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return {'name': torch.cuda.get_device_name(0), 'nvidia_smi': q}
-
-
-def _time(fn, iters):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters
+from gpu_timing import card, rounds_ms
 
 
 def _images(B, seed, dev):
@@ -67,7 +43,7 @@ def main():
     from openglue_b200.synthetic import default_config, synthetic_state_dict
     dev = torch.device('cuda:0')
     mc = {'superglue': {'laf_to_sideinfo_method': 'none'}, 'inference': {'match_threshold': 0.2}}
-    result = {'gpu': _gpu(), 'iters': args.iters, 'rounds': args.rounds, 'image': [720, 960], 'results': []}
+    result = {'card': card(), 'iters': args.iters, 'rounds': args.rounds, 'image': [720, 960], 'results': []}
     for name in ('sift', 'superpoint'):
         if name == 'sift':
             fe, D = OpenCVSIFT(max_keypoints=2048), 128
@@ -93,13 +69,9 @@ def main():
             }
             for fn in forms.values():                                          # warm-up (and the one capture)
                 fn()
-            torch.cuda.synchronize()
             out = eager(i0, i1)
             counts = (out['num_keypoints0'].tolist(), out['num_keypoints1'].tolist())
-            times = {k: [] for k in forms}
-            for _ in range(args.rounds):
-                for k, fn in forms.items():
-                    times[k].append(_time(fn, args.iters))
+            times = rounds_ms(forms, args.iters, args.rounds)
             row = {'features': name, 'batch': B, 'keypoints0': counts[0], 'keypoints1': counts[1],
                    'overflow': int(out['overflow0'].sum() + out['overflow1'].sum())}
             for k, v in times.items():

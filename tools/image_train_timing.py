@@ -14,39 +14,15 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'oracle'))
+from gpu_timing import card, rounds_ms
 
 CONFIG = {'superglue': {'laf_to_sideinfo_method': 'none', 'log_transform_response': False},
           'train': {'gt_positive_threshold': 2, 'gt_negative_threshold': 7, 'margin': None, 'nll_weight': 1.0, 'metric_weight': 0.0,
                     'augmentations': {'name': 'none'}, 'lr': 1e-4, 'grad_clip': 10.0, 'scheduler_gamma': 0.999994}}
-
-
-def _gpu():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return {'name': torch.cuda.get_device_name(0), 'nvidia_smi': q}
-
-
-def _time(fn, iters):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters
 
 
 def _rgb(B, dev):
@@ -76,7 +52,7 @@ def main():
     B, offset = args.batch, 256
     imgs = _rgb(B, dev)
     conv = get_laf_to_sideinfo_converter('none')
-    result = {'gpu': _gpu(), 'iters': args.iters, 'rounds': args.rounds, 'batch': B, 'image': [1232, 1472], 'offset': offset, 'results': []}
+    result = {'card': card(), 'iters': args.iters, 'rounds': args.rounds, 'batch': B, 'image': [1232, 1472], 'offset': offset, 'results': []}
     for name in ('superpoint', 'sift'):
         if name == 'sift':
             fe, D, K = OpenCVSIFT(max_keypoints=2048), 128, 2048
@@ -115,16 +91,11 @@ def main():
         forms = {'hand': hand, 'eager': lambda: eager.pretrain(imgs, offset), 'graph': lambda: graph.pretrain(imgs, offset, borrow=True)}
         for fn in forms.values():                                              # warm-up (and the one capture)
             fn()
-        torch.cuda.synchronize()
         out = eager.pretrain(imgs, offset)
         row = {'features': name, 'keypoints_capacity': K, 'keypoints0': out['num_keypoints0'].tolist(),
                'keypoints1': out['num_keypoints1'].tolist(), 'overflow': int(out['overflow0'].sum() + out['overflow1'].sum()),
                'skipped': int(out['skipped'])}
-        times = {k: [] for k in forms}
-        for _ in range(args.rounds):
-            for k, fn in forms.items():
-                times[k].append(_time(fn, args.iters))
-        for k, v in times.items():
+        for k, v in rounds_ms(forms, args.iters, args.rounds).items():
             row[f'{k}_ms'] = round(statistics.median(v), 3)
             row[f'{k}_rounds_ms'] = [round(x, 3) for x in v]
         result['results'].append(row)

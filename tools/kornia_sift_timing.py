@@ -9,17 +9,12 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from openglue_b200 import SIFT  # noqa: E402
-from oracle import kornia_sift_oracle as KO  # noqa: E402
+from gpu_timing import card, events_ms  # first: it makes the package and the oracle importable
+from openglue_b200 import SIFT
+from oracle import kornia_sift_oracle as KO
 
 
 def texture(B, H, W, seed, dev):
@@ -29,19 +24,6 @@ def texture(B, H, W, seed, dev):
         n = torch.rand(B, 1, H // s + 2, W // s + 2, generator=g, device=dev)
         x += torch.nn.functional.interpolate(n, size=(H, W), mode='bicubic', align_corners=False) * (s / 64.0)
     return (x / x.amax()).clamp(0, 1)
-
-
-def timed(fn, reps, warmup=2):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(reps):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / reps
 
 
 def oracle_forward(img, nf):
@@ -56,19 +38,18 @@ def main():
     ap.add_argument('--oracle-reps', type=int, default=2)
     args = ap.parse_args()
     dev = 'cuda:0'
-    card = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip()
     sift = SIFT(max_keypoints=1024)
     rows = []
     for B in (1, 16):
         img = texture(B, 720, 960, 7, dev)
-        t_fwd = timed(lambda: sift(img), args.reps)
-        t_pad = timed(lambda: sift.extract_padded(img), args.reps)
+        t_fwd = events_ms(lambda: sift(img), args.reps, warmup=2)
+        t_pad = events_ms(lambda: sift.extract_padded(img), args.reps, warmup=2)
         with torch.no_grad():
-            t_or = timed(lambda: oracle_forward(img, 1024), args.oracle_reps, warmup=1) if B == 1 else None
+            t_or = events_ms(lambda: oracle_forward(img, 1024), args.oracle_reps, warmup=1) if B == 1 else None
         rows.append(dict(B=B, forward_ms_per_image=t_fwd / B, extract_padded_ms_per_image=t_pad / B,
                          oracle_f32_cuda_ms_per_image=None if t_or is None else t_or / B))
         print(json.dumps(rows[-1]))
-    print(json.dumps(dict(card=card, image='960x720', max_keypoints=1024, rows=rows)))
+    print(json.dumps(dict(card=card(), image='960x720', max_keypoints=1024, rows=rows)))
 
 
 if __name__ == '__main__':

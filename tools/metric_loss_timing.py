@@ -16,14 +16,11 @@ import copy
 import json
 import os
 import statistics
-import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-from train_step_timing import _gpu, _labels, _time  # noqa: E402
+from gpu_timing import card, rounds_ms
+from train_step_timing import _labels
 
 
 def _criterion_case(B, n, m, d, seed, dev):
@@ -54,7 +51,7 @@ def main():
     from openglue_b200.synthetic import default_config, synthetic_pairs, synthetic_state_dict
     from openglue_b200.training import GraphedTrainStep
     dev = torch.device('cuda:0')
-    res = {'gpu': _gpu(), 'iters': args.iters, 'rounds': args.rounds, 'criterion': {}, 'train_step': {}}
+    res = {'card': card(), 'iters': args.iters, 'rounds': args.rounds, 'criterion': {}, 'train_step': {}}
 
     for B, N in ((4, 1024), (16, 2048)):
         y_true, y_pred = _criterion_case(B, N, N, 256, 0, dev)
@@ -64,12 +61,9 @@ def main():
         fwd = lambda: criterion(y_true, y_pred, margin=0.5)
         grad = lambda: criterion(y_true, yg, margin=0.5)
         for f in (plain, fwd, grad):
-            _time(f, 2)
-        tp, tf, tg = [], [], []
-        for _ in range(args.rounds):
-            tp.append(_time(plain, args.iters))
-            tf.append(_time(fwd, args.iters))
-            tg.append(_time(grad, args.iters))
+            for _ in range(2):
+                f()
+        tp, tf, tg = rounds_ms({'plain': plain, 'fwd': fwd, 'grad': grad}, args.iters, args.rounds).values()
         res['criterion'][f'{B}x{N}x{N} d=256'] = {'margin_none_ms': statistics.median(tp), 'margin_ms': statistics.median(tf),
                                                    'margin_with_grad_ms': statistics.median(tg), 'rounds_ms': [tp, tf, tg]}
         del y_true, y_pred, yg
@@ -94,11 +88,9 @@ def main():
         step_b = GraphedTrainStep(mb, data, y_true, optimizer=opt(mb), margin=0.5, metric_weight=0.5)
         fa, fb = (lambda: step_a(data, y_true)), (lambda: step_b(data, y_true))
         for f in (fa, fb):
-            _time(f, 3)
-        ta, tb = [], []
-        for _ in range(args.rounds):
-            ta.append(_time(fa, args.iters))
-            tb.append(_time(fb, args.iters))
+            for _ in range(3):
+                f()
+        ta, tb = rounds_ms({'a': fa, 'b': fb}, args.iters, args.rounds).values()
         res['train_step'][f'B={B}'] = {'no_margin_ms': ta, 'margin_ms': tb, 'median_no_margin_ms': statistics.median(ta),
                                        'median_margin_ms': statistics.median(tb)}
         del step_a, step_b, ma, mb

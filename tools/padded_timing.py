@@ -10,17 +10,11 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
 import statistics
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'tools'))
-
-from sift_timing import gpu_info  # noqa: E402
+from gpu_timing import card, events_ms
 
 B, CAP, D, STAGES, ITERS = 16, 2048, 256, 9, 100
 
@@ -31,22 +25,6 @@ def length_sets():
     skew0, skew1 = torch.randint(128, 513, (B,), generator=g), torch.randint(128, 513, (B,), generator=g)
     skew0[0] = skew1[0] = CAP
     return {'uniform_1024_2048': uniform, 'skewed': (skew0, skew1)}
-
-
-def time_ms(fn, iters: int, warmup: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    rounds = []
-    for _ in range(3):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        ev[0].record()
-        for _ in range(iters):
-            fn()
-        ev[1].record()
-        ev[1].synchronize()
-        rounds.append(ev[0].elapsed_time(ev[1]) / iters)
-    return statistics.median(rounds)
 
 
 def main():
@@ -66,25 +44,25 @@ def main():
     model.load_state_dict(synthetic_state_dict(cfg, seed=0))
     model = model.to(dev)
     full = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in synthetic_pairs(B, CAP, CAP, D, 1, seed=1).items()}
-    info = dict(gpu_info(), precision=args.precision, batch=B, capacity=CAP, descriptor_dim=D, stages=STAGES, sinkhorn_iters=ITERS,
+    info = dict(card=card(), precision=args.precision, batch=B, capacity=CAP, descriptor_dim=D, stages=STAGES, sinkhorn_iters=ITERS,
                 iters=args.iters)
     eager = MatchingCore(model)
     graphed = MatchingCore(model, use_cuda_graph=True)
     graphed.max_graphs = 2 * B + 2                       # one graph per pair shape at B = 1, and the batches
 
-    print(json.dumps(dict(info, mode='uniform_full_capacity_eager', ms=time_ms(lambda: eager(full), args.iters, args.warmup))), flush=True)
-    print(json.dumps(dict(info, mode='uniform_full_capacity_graph', ms=time_ms(lambda: graphed(full), args.iters, args.warmup))), flush=True)
+    def report(forms, **what):                           # each form on its own: warm-up, then the median of three rounds
+        for mode, fn in forms.items():
+            ms = statistics.median([events_ms(fn, args.iters, args.warmup), events_ms(fn, args.iters), events_ms(fn, args.iters)])
+            print(json.dumps(dict(info, **what, mode=mode, ms=ms)), flush=True)
+
+    report({'uniform_full_capacity_eager': lambda: eager(full), 'uniform_full_capacity_graph': lambda: graphed(full)})
     for name, (n0, n1) in length_sets().items():
         padded = dict(full, num_keypoints0=n0, num_keypoints1=n1)
         pairs = [{k: (v[b:b + 1, :(n0 if k.endswith('0') else n1)[b]] if torch.is_tensor(v) else v) for k, v in full.items()}
                  for b in range(B)]
-        res = {'padded_eager': time_ms(lambda: eager(padded), args.iters, args.warmup),
-               'padded_graph': time_ms(lambda: graphed(padded), args.iters, args.warmup),
-               'one_at_a_time_eager': time_ms(lambda: [eager(p) for p in pairs], args.iters, args.warmup),
-               'one_at_a_time_graph': time_ms(lambda: [graphed(p) for p in pairs], args.iters, args.warmup)}
-        for mode, ms in res.items():
-            print(json.dumps(dict(info, lengths=name, mean_n=float(n0.float().mean()), mean_m=float(n1.float().mean()), mode=mode, ms=ms)),
-                  flush=True)
+        report({'padded_eager': lambda: eager(padded), 'padded_graph': lambda: graphed(padded),
+                'one_at_a_time_eager': lambda: [eager(p) for p in pairs], 'one_at_a_time_graph': lambda: [graphed(p) for p in pairs]},
+               lengths=name, mean_n=float(n0.float().mean()), mean_m=float(n1.float().mean()))
 
 
 if __name__ == '__main__':

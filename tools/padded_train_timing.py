@@ -12,33 +12,11 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-
-def _gpu():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return {'name': torch.cuda.get_device_name(0), 'nvidia_smi': q}
-
-
-def _time(fn, iters):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters
+from gpu_timing import card, rounds_ms
 
 
 def main():
@@ -84,12 +62,8 @@ def main():
         forms[name] = (lambda s=step, d=data, yy=y: s(d, yy))
         for _ in range(3):
             forms[name]()
-    torch.cuda.synchronize()
-    ms = {k: [] for k in forms}
-    for _ in range(args.rounds):
-        for k, fn in forms.items():
-            ms[k].append(_time(fn, args.iters))
-    res = {'gpu': _gpu(), 'batch': B, 'capacity': N, 'lengths0': n0.tolist(), 'lengths1': n1.tolist(),
+    ms = rounds_ms(forms, args.iters, args.rounds)
+    res = {'card': card(), 'batch': B, 'capacity': N, 'lengths0': n0.tolist(), 'lengths1': n1.tolist(),
            'kept_keypoints': {'padded': int(n0.sum() + n1.sum()), 'min_stack': B * (a + b), 'full': 2 * B * N},
            'config': 'd 256, 9 stages, 4 heads, 20 Sinkhorn iterations, tf32x3, GraphedTrainStep + ClippedAdam',
            'ms_per_iteration_median': {k: statistics.median(v) for k, v in ms.items()}, 'ms_per_iteration_rounds': ms}

@@ -10,15 +10,12 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from gpu_timing import card, events_ms
 
 
 def image(seed: int, H: int = 720, W: int = 960) -> torch.Tensor:
@@ -30,52 +27,27 @@ def image(seed: int, H: int = 720, W: int = 960) -> torch.Tensor:
     return ((x - x.min()) / (x.max() - x.min())).clamp(0, 1)
 
 
-def gpu_info() -> dict:
-    try:
-        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = [s.strip() for s in out.split(',')]
-        return {'gpu': name, 'power_limit': power, 'max_sm_clock': clock}
-    except Exception:                                          # noqa: BLE001
-        return {'gpu': torch.cuda.get_device_name(0)}
-
-
-def time_gpu(fn, iters: int, warmup: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    ev[0].record()
-    for _ in range(iters):
-        fn()
-    ev[1].record()
-    torch.cuda.synchronize()
-    return ev[0].elapsed_time(ev[1]) / iters
-
-
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--reference', default=os.environ.get('OG_REFERENCE_ROOT', '/root/reference'))
     a = ap.parse_args()
-    info = {}
     if torch.cuda.is_available():
         from openglue_b200 import OpenCVSIFT
-        info = gpu_info()
+        info = {'card': card()}
         m = OpenCVSIFT(max_keypoints=2048, nms_diameter=9., rootsift=True)
         one = image(0).cuda()
         batch = torch.cat([image(s) for s in range(16)]).cuda()
         n = m(one)[1].shape[1]
-        ms1 = time_gpu(lambda: m(one), a.iters, a.warmup)
+        ms1 = events_ms(lambda: m(one), a.iters, a.warmup)
         print(json.dumps({'what': 'OpenCVSIFT.forward', 'batch': 1, 'H': 720, 'W': 960, 'keypoints': n, 'ms_per_image': round(ms1, 3), **info}))
-        ms16 = time_gpu(lambda: m.extract_batch(batch), max(2, a.iters // 4), 1)
+        ms16 = events_ms(lambda: m.extract_batch(batch), max(2, a.iters // 4), 1)
         print(json.dumps({'what': 'OpenCVSIFT.extract_batch', 'batch': 16, 'H': 720, 'W': 960, 'ms_per_image': round(ms16 / 16, 3), **info}))
     else:
         print(json.dumps({'what': 'OpenCVSIFT', 'gpu': 'not measured (no CUDA device)'}))
     try:
         import cv2  # noqa: F401
-        sys.path.insert(0, os.path.join(ROOT, 'oracle'))
         os.environ['OG_REFERENCE_ROOT'] = a.reference
         from gen_golden_sift import import_reference
         sift_create, _ = import_reference()

@@ -21,9 +21,9 @@ import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from openglue_b200 import _cabi  # noqa: E402
-from openglue_b200._cabi import ptr, stream  # noqa: E402
+from gpu_timing import card, events_ms  # first: it makes the package importable
+from openglue_b200 import _cabi
+from openglue_b200._cabi import ptr, stream
 
 # (label, pairs, n, m, iterations)
 SHAPES = [('C3', 16, 2048, 2048, 100), ('C2', 32, 1024, 1024, 100), ('C5', 1, 4096, 1024, 50), ('C1', 1, 512, 512, 20),
@@ -67,13 +67,7 @@ def measure(launches, rounds, quiet=False):
         for _ in range(rounds):
             for mode in (1, 0):
                 lib.og_set_sinkhorn_resident(mode)
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(launches):
-                    run(mode, outs[mode])
-                e1.record()
-                e1.synchronize()
-                times[mode].append(e0.elapsed_time(e1) / launches)
+                times[mode].append(events_ms(lambda: run(mode, outs[mode]), launches))
         lib.og_set_sinkhorn_resident(1)
         r = {'shape': label, 'pairs': B, 'n': n, 'm': m, 'iters': T,
              'ms_resident': statistics.median(times[1]), 'ms_streaming': statistics.median(times[0]),
@@ -105,9 +99,8 @@ def main():
     if args.json:
         print(json.dumps(measure(args.launches, args.rounds, quiet=True)))
         return
-    smi = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                         capture_output=True, text=True).stdout.strip()
-    print('device:', smi)
+    gpu = card()
+    print(json.dumps({'card': gpu}))
     results = measure(args.launches, args.rounds)
     against = None
     if args.against:
@@ -124,7 +117,7 @@ def main():
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, 'sinkhorn_timing.json'), 'w') as f:
-            json.dump({'device': smi, 'launches': args.launches, 'rounds': args.rounds, 'results': results,
+            json.dump({'card': gpu, 'launches': args.launches, 'rounds': args.rounds, 'results': results,
                        'against': args.against, 'against_results': against}, f, indent=1)
 
 

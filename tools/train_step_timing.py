@@ -15,32 +15,10 @@ import copy
 import json
 import os
 import statistics
-import subprocess
-import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-
-def _gpu():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return {'name': torch.cuda.get_device_name(0), 'nvidia_smi': q}
-
-
-def _time(fn, iters):
-    """ms per call: CUDA events around `iters` calls"""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / iters
+from gpu_timing import card, rounds_ms
 
 
 def _labels(pairs, dev):
@@ -70,7 +48,7 @@ def main():
     dev = torch.device('cuda:0')
     cfg = default_config(descriptor_dim=256, num_stages=9, num_heads=4, num_iters=20)
     sd = synthetic_state_dict(cfg, seed=0)
-    res = {'gpu': _gpu(), 'config': 'd=256, 9 stages, 4 heads, 20 Sinkhorn iterations, tf32x3 training GEMMs',
+    res = {'card': card(), 'config': 'd=256, 9 stages, 4 heads, 20 Sinkhorn iterations, tf32x3 training GEMMs',
            'keypoints': args.keypoints, 'iters': args.iters, 'rounds': args.rounds, 'train_step': {}, 'optimizer_alone': {}}
 
     def model():
@@ -100,11 +78,9 @@ def main():
             step_b(data, y_true)
 
         for f in (form_a, form_b):
-            _time(f, 3)
-        ta, tb = [], []
-        for _ in range(args.rounds):
-            ta.append(_time(form_a, args.iters))
-            tb.append(_time(form_b, args.iters))
+            for _ in range(3):
+                f()
+        ta, tb = rounds_ms({'a': form_a, 'b': form_b}, args.iters, args.rounds).values()
         res['train_step'][f'B={B}'] = {'a_graph_plus_eager_torch_optimizer_ms': ta, 'b_graph_with_clipped_adam_ms': tb,
                                        'median_a_ms': statistics.median(ta), 'median_b_ms': statistics.median(tb)}
         del step_a, step_b, ma, mb, adam, sched, pa
@@ -132,12 +108,9 @@ def main():
     with torch.cuda.graph(graph):
         ours.step()
     for f in (torch_seq, ours.step, graph.replay):
-        _time(f, 3)
-    tt, to, tg = [], [], []
-    for _ in range(args.rounds):
-        tt.append(_time(torch_seq, args.iters * 5))
-        to.append(_time(ours.step, args.iters * 5))
-        tg.append(_time(graph.replay, args.iters * 5))
+        for _ in range(3):
+            f()
+    tt, to, tg = rounds_ms({'torch': torch_seq, 'eager': ours.step, 'graph': graph.replay}, args.iters * 5, args.rounds).values()
     hbm = 36 * n                                        # norm pass 4 B + fused pass 32 B per parameter (from shapes)
     res['optimizer_alone'] = {'parameters': n, 'torch_foreach_clip_adam_steplr_ms': tt, 'clipped_adam_eager_ms': to,
                               'clipped_adam_graph_replay_ms': tg, 'bytes_per_step': hbm,
